@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- benchmark of the protocol.Decoder hot path on B200 (BASELINE.json configs 2-5).
+"""bench.py -- benchmark of the protocol.Decoder hot path on H100 (BASELINE.json configs 2-5).
 
 Metric (BASELINE.json): IQ Msamples/s decoded (1 sample = I byte + Q byte) on synthetic uint8 IQ
 with injected ERT packets.
 
-  python bench.py --gpus N --steps K --warmup W            our arm (libertgpu.so, sm_100a)
+  python bench.py --gpus N --steps K --warmup W            our arm (libertgpu.so, sm_90a)
   python bench.py --impl reference --gpus N --steps K ...  CPU arm: the reference's algorithm on
                                                            the box's host cores (oracle port: Go
                                                            is not in this image, see DESIGN.md)
@@ -29,6 +29,11 @@ One JSON line is printed by rank 0.  `value` = whole-job Msamples/s with the IQ 
 timed region); `roofline` = the demod kernel against the measured HBM copy bandwidth;
 `cpu_baseline` = the CPU restatement timed on this box (bounded sample); `sustained` = the same
 step repeated for >= 2 s.
+
+`--dump-outputs DIR` writes, after the timed steps of every workload, the candidate records the last
+timed step returned (block, idx, preamble_id, check_mask, flags, bytes, r900_digits) as
+DIR/<workload>_<field>.npy in float64 / float32, so that two builds can be compared output for output.
+The workloads share 64 MB; a workload with more records than its share writes a fixed, seeded sample.
 """
 from __future__ import annotations
 
@@ -73,6 +78,8 @@ def parse_args():
     ap.add_argument("--skip-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-threads", type=int, default=0, help="reference arm: threads (default: every CPU the process may use)")
     ap.add_argument("--no-numa-bind", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's candidate records of every workload as DIR/<workload>_<field>.npy")
     return ap.parse_args()
 
 
@@ -88,14 +95,14 @@ def workload_config(name, w, nbytes_per_gpu, world, bs, pkl):
         "msgtype": w["msgtype"], "chip_length": CHIP_LENGTH, "block_size": bs, "bytes_per_gpu": nbytes_per_gpu,
         "blocks_per_gpu": blocks_per_gpu, "total_bytes": nbytes_per_gpu * world, "seed": w["seed"],
         "halo_blocks": max(p.halo_blocks for p in plans),
-        "l2": "input per step exceeds the 126 MB L2: no flush needed",
+        "l2": "input per step exceeds the 50 MB L2: no flush needed",
         "sharding": "contiguous block-aligned shards + halo, no collective on the data path",
     }
 
 
 # ----------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """SM clock and throttle reasons DURING the timed region (B200_PROFILING.md): NVML polled every
+    """SM clock and throttle reasons DURING the timed region: NVML polled every
     ~0.5 ms from a thread, with the `nvidia-smi -lms` recipe as fallback."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
@@ -421,6 +428,8 @@ def measure(job, args, barrier, sampler, stream, with_e2e, sustained_s):
     ms_total, launches, t_wall0, t_wall1 = timed(args.steps)
     out = {"ms_total": ms_total, "launches": launches, "n_pkts": n_pkts,
            "clocks": sampler.window(t_wall0, t_wall1) if sampler else None}
+    if args.dump_outputs:
+        out["outputs"] = h.fetch(1 << 20)   # what the last timed step returns to its caller
     # timed region 2: the same K steps with CUDA events recorded by the library around each stage (the roofline's
     # kernel time); the events sit between the kernels, so this pass runs them strictly one after another
     h.set_stage_timing(True)
@@ -488,6 +497,37 @@ def measure(job, args, barrier, sampler, stream, with_e2e, sustained_s):
     return out
 
 
+DUMP_LIMIT_BYTES = 64_000_000
+
+
+def dump_outputs(dirname, prefix, got, limit=None):
+    """The candidate records as DIR/<prefix>_<field>.npy: integer fields as float64 (exact), byte arrays as float32.
+    Above `limit` bytes (default DUMP_LIMIT_BYTES) a fixed, seeded sample of whole records is written, in stream order."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    fields = {"block": np.float64, "idx": np.float64, "preamble_id": np.float64, "check_mask": np.float64,
+              "flags": np.float64, "bytes": np.float32, "r900_digits": np.float32}
+    row_bytes = sum(np.dtype(t).itemsize * int(np.prod(got.dtype[f].shape or (1,))) for f, t in fields.items())
+    keep = max(0, (limit or DUMP_LIMIT_BYTES) - 256 * len(fields)) // row_bytes   # .npy headers are < 256 bytes
+    if len(got) > keep:
+        got = got[np.sort(np.random.default_rng(0).choice(len(got), keep, replace=False))]
+    for f, t in fields.items():
+        np.save(os.path.join(dirname, f"{prefix}_{f}.npy"), got[f].astype(t))
+
+
+def gpu_identity(index):
+    """Name and power limit of the GPU the numbers were measured on."""
+    import torch
+    ident = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        q = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        ident["power_limit_w"] = float(q.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return ident
+
+
 def reduce_over_ranks(world, vals_max, vals_sum):
     import torch
     import torch.distributed as dist
@@ -508,15 +548,7 @@ def summarise(job, args, raw, world, peak, peak_src):
     dm = raw["stage_ms"]["demod"]
     achieved = 2.0 * job.nsamples / (dm * 1e-3) / 1e9   # 2 algorithmic bytes per sample (SURVEY.md 8d), this rank's launch
     step_bw = 2.0 * job.nsamples / (ms_per_step * 1e-3) / 1e9
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "demod_traffic.json")
-    if os.path.exists(tp):
-        try:
-            tj = json.load(open(tp))
-            traffic = tj.get("dram_bytes_per_sample", 0) * job.nsamples or None
-            traffic_src = f"from profile: {tj.get('source', 'profiles/demod_traffic.json')} (dram bytes per sample x samples per launch), not captured in this run"
-        except Exception:
-            traffic = None
+    traffic, traffic_src = None, "not measured: no hardware counters are read by this benchmark"
     kern = job.h.demod_kernel_name()
     res = {
         "name": job.name, "metric": metric_name(job.w), "value": round(value, 1), "unit": UNIT,
@@ -585,7 +617,8 @@ def run_b200(args):
     pp = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pp):
         peaks = json.load(open(pp))
-    peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)") if "hbm_gbs" in peaks else (6650.0, "fallback (B200_PROFILING.md)")
+    peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)") if "hbm_gbs" in peaks else \
+        (3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured")
 
     names = [args.config]
     if not args.no_extras and args.config == "scm1g":
@@ -597,6 +630,9 @@ def run_b200(args):
         job = Job(name, args, world, rank, local)
         head = i == 0
         raw = measure(job, args, barrier, sampler, stream, with_e2e=head, sustained_s=args.sustained_seconds if head else 0.0)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, name if world == 1 else f"{name}_rank{rank}", raw.pop("outputs"),
+                         DUMP_LIMIT_BYTES // (len(names) * world))
         mx = [raw["ms_total"], raw.get("e2e_s", 0.0), raw.get("e2e_pageable_s", 0.0), raw["sustained"]["ms_total"] if "sustained" in raw else 0.0]
         sm = [float(raw["n_pkts"])]
         mx, sm = reduce_over_ranks(world, mx, sm)
@@ -638,7 +674,7 @@ def run_b200(args):
             "pkts_per_s": head["pkts_per_s"], "pkts_per_step": head["pkts_per_step"],
             "e2e": head.get("e2e"), "gpu_launches": head["gpu_launches"], "stage_ms": head["stage_ms"],
             "roofline": head["roofline"], "clocks": head["clocks"], "sustained": head.get("sustained"),
-            "numa": numa,
+            "numa": numa, "gpu": gpu_identity(local),
         }
         if cpu:
             line["cpu_baseline"] = cpu

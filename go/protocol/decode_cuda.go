@@ -1,7 +1,7 @@
 //go:build cuda
 
 // decode_cuda.go -- drop-in replacement for rtlamr's protocol/decode.go that runs the Decoder hot
-// path (magnitude, matched filter, quantize, pack, preamble search, slice, CRC screen) on a B200
+// path (magnitude, matched filter, quantize, pack, preamble search, slice, CRC screen) on an H100
 // through libertgpu.so (include/ertgpu.h).
 //
 // How to use it (see INTEGRATION.md):
@@ -16,7 +16,7 @@
 // INTEGRATION.md) because its DSP half also moved to the GPU.
 //
 // STATUS: EXPERIMENTAL.  Written without a Go toolchain at hand (none in the build image): this file has
-// never been compiled; parity_test.go next to it is the first thing to run where Go and a B200 exist.
+// never been compiled; parity_test.go next to it is the first thing to run where Go and an H100 exist.
 // The C++ mirror in rtlamr_b200/host/ exercises the same call sequence in the parity tests.
 //
 // Two things a maintainer must know:

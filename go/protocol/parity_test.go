@@ -5,7 +5,7 @@
 // 1. On any Go machine, produce the dump with the unmodified reference (go/goldengen/README.md):
 //      GOLDEN_IN=assets/sample.bin GOLDEN_OUT=go_dump_sample_cl78_scm.jsonl GOLDEN_MSGTYPES=scm GOLDEN_CL=78 \
 //        go test ./protocol -run TestDumpGolden -count=1            (build WITHOUT -tags cuda)
-// 2. On a B200 machine, with decode_cuda.go in place:
+// 2. On an H100 machine, with decode_cuda.go in place:
 //      ERT_GOLDEN=go_dump_sample_cl78_scm.jsonl ERT_GOLDEN_IN=assets/sample.bin \
 //        go test -tags cuda ./protocol -run TestCudaParity -count=1
 //
@@ -14,7 +14,7 @@
 // for other chip lengths the stock byte pre-filter drops candidates, decode.go:256,271, and the stock list must
 // be a SUBSET), and the Quantized / packed / Signal / csum taps are bit-identical at the dumped blocks.
 //
-// Written without a Go toolchain at hand; compiled and run only where Go and a B200 exist.
+// Written without a Go toolchain at hand; compiled and run only where Go and an H100 exist.
 package protocol
 
 import (

@@ -1,5 +1,5 @@
 /*
- * ertgpu.h -- C ABI of libertgpu.so: a Blackwell (sm_100a) implementation of the
+ * ertgpu.h -- C ABI of libertgpu.so: a Hopper (sm_90a) implementation of the
  * rtlamr `protocol.Decoder` hot path (uint8 IQ -> magnitude -> Manchester
  * matched filter -> quantize -> pack -> preamble search -> slice -> CRC screen).
  *

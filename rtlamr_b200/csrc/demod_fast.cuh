@@ -102,71 +102,6 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
     return v;
 }
 
-// packed fp32 pairs (sm_100 FADD2): lane-wise IEEE round-to-nearest, no flush-to-zero, so each half is
-// bit-identical to a scalar add.rn.f32
-__device__ __forceinline__ uint64_t pack2(float lo, float hi) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ uint64_t sub2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-
-// ---- Tensor Memory as a per-thread scratchpad (no MMA anywhere) --------------------------------------------
-// TMEM is 128 lanes x 512 columns of 32 bits per SM; a warp reaches the 32 lanes of quarter (warp % 4) and
-// `tcgen05.ld/st.32x32b.xN` move N consecutive columns of lane i to/from N registers of thread i.  That is
-// exactly a private array per thread that costs no registers and no shared-memory bandwidth: the demod
-// kernel keeps the chip-sum ring there (VAR bit 3), which brings it under the 168 registers a third warp
-// per scheduler needs.  Measured (tools/tmem_probe.cu, B200): 170 B/cycle/SM loads, 188 B/cycle/SM stores,
-// a store followed by a load of the same columns is ordered without a wait.
-__device__ __forceinline__ void tm_ld8(uint32_t taddr, float (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=f"(r[0]), "=f"(r[1]), "=f"(r[2]), "=f"(r[3]), "=f"(r[4]), "=f"(r[5]), "=f"(r[6]), "=f"(r[7])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tm_st8(uint32_t taddr, const float (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "f"(r[0]), "f"(r[1]),
-                 "f"(r[2]), "f"(r[3]), "f"(r[4]), "f"(r[5]), "f"(r[6]), "f"(r[7])
-                 : "memory");
-}
-// the loaded registers may be read after this (the operands tie their uses behind the wait)
-__device__ __forceinline__ void tm_wait_ld(float (&r)[8]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+f"(r[0]), "+f"(r[1]), "+f"(r[2]), "+f"(r[3]), "+f"(r[4]), "+f"(r[5]), "+f"(r[6]), "+f"(r[7])
-                 :
-                 : "memory");
-}
-__device__ __forceinline__ void tm_wait_ld2(float (&r)[8], float (&t)[8]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+f"(r[0]), "+f"(r[1]), "+f"(r[2]), "+f"(r[3]), "+f"(r[4]), "+f"(r[5]), "+f"(r[6]), "+f"(r[7]),
-                   "+f"(t[0]), "+f"(t[1]), "+f"(t[2]), "+f"(t[3]), "+f"(t[4]), "+f"(t[5]), "+f"(t[6]), "+f"(t[7])
-                 :
-                 : "memory");
-}
-__device__ __forceinline__ void tm_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-constexpr int kTmemColsPerWarp = 128;   // columns between the rings of the warps that share a lane quarter (L <= 104)
-
 // body length for a chip length: the smallest L >= CL + 1 with L % 8 == 0 and L / 8 odd
 constexpr int fast_body_len(int CL) {
     int L = ((CL + 1 + 7) / 8) * 8;
@@ -188,17 +123,14 @@ struct FastGeom {
     static constexpr int kWarpBytes = kStages * kStageBytes;
     static constexpr int kFullWords = L / 32;           // whole output words per body
     static constexpr int kTailBits = L % 32;
-    // the three non-sequential adds of two neighbouring steps as packed FADD2 (one issue slot for two
-    // IEEE adds); rings longer than 88 run out of registers with the pair constraints and stay scalar
-    static constexpr bool kPacked = (L <= 88);
     static_assert(L % 8 == 0 && (kRowUnits & 1) == 1 && L >= CL && kPad >= 0 && kPad < L, "bad body length");
-    static_assert(CL % 2 == 0, "the packed-pair rings need an even chip length");
+    static_assert(CL % 2 == 0, "the two samples of a word take neighbouring ring slots: needs an even chip length");
 };
 
 // smem map (byte offsets inside the dynamic segment, computed at run time):
 //   [bars: 2 x 8 B per warp][pad][staging of the first warps ...][LUT at the next 64 KiB boundary]
 //   [staging of the remaining warps ...]
-// VAR: tuning variants kept for the record (bit 0 = HYBRID magnitude, bit 1 = 3-stage staging ring)
+// VAR: tuning variants kept for the record (bit 0 = HYBRID magnitude, bit 1 = 3-stage staging ring, bit 2 = tight ring)
 template <int CL, int WARPS, int VAR = 0>
 __global__ void __launch_bounds__(WARPS * 32, 1)
 demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __restrict__ iq,
@@ -206,15 +138,8 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
                   const float* __restrict__ lut_g, uint32_t* __restrict__ plane_out, long long nblocks, int BS,
                   unsigned long long* __restrict__ tile_counter, long long dyn_tiles) {
     constexpr bool HYBRID = (VAR & 1) != 0;
-    constexpr bool TMEMA = (VAR & 8) != 0;   // the chip-sum ring lives in Tensor Memory
-    // Packed f32x2 adds (FADD2) or scalar ones (VAR bit 6).  Measured on B200 (tools/pipe_probe.cu): FADD2 holds the dispatch
-    // port for 2 cycles and does not overlap with an ALU-pipe instruction (PRMT + FADD2 = 3.9 cycles), a scalar FADD is hidden
-    // completely behind one (PRMT + FADD = 2.4 cycles): the packed form saves issue slots but costs dispatch cycles.
-    constexpr bool kPk = FastGeom<CL>::kPacked && (VAR & 64) == 0;
-    constexpr int CT = (TMEMA && (VAR & 32)) ? 5 : 0;   // ... and so do the first CT groups of 8 slots of the running-sum ring
     using G = FastGeom<CL, (VAR & 2) ? 3 : 2, (VAR & 4) != 0>;
     constexpr int L = G::L;
-    static_assert(!TMEMA || ((L - CL) % 8 == 0 && L + 8 * CT <= kTmemColsPerWarp && WARPS <= 16 && CT < L / 8), "TMEM ring: groups of 8 slots must not wrap");
     extern __shared__ __align__(128) uint8_t fast_smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t sbase = smem_u32(fast_smem);
@@ -244,22 +169,7 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
         for (int s = 0; s < G::kStages; s++) mbar_init(bar0 + s * 8, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    uint32_t tring = 0;   // TMEM address of this warp's ring: lane quarter (warp % 4), columns of sharer (warp / 4)
-    if constexpr (TMEMA) {
-        // all 512 columns of this SM (one CTA per SM; a CTA of the next launch waits here until we free them)
-        if (warp == 0) {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sbase + 1008), "r"(512) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    }
     __syncthreads();
-    if constexpr (TMEMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t tbase;
-        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tbase) : "r"(sbase + 1008) : "memory");
-        tring = tbase + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)((warp >> 2) * kTmemColsPerWarp);
-    }
 
     const int wpb = BS >> 5;                         // words per block
     const int nbody = (2 * L + BS - 1 + L - 1) / L;  // bodies covering steps 0 .. 2L+BS-2
@@ -315,21 +225,9 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
         // exception: block 0 takes its lead-in from the history buffer, so that tile uses one 1D bulk
         // copy per lane instead (its own instantiation of the tile code: the hot loop carries neither
         // that path nor the lead-in special cases).
-        float cr[L], ar[TMEMA ? 2 : L];  // rings; (even, odd) neighbours are used as packed pairs
+        float cr[L], ar[L];  // rings of the running sums and the chip sums
 #pragma unroll
-        for (int j = 0; j < L; j++) cr[j] = 0.0f;
-#pragma unroll
-        for (int j = 0; j < (TMEMA ? 2 : L); j++) ar[j] = 0.0f;
-        float ao[8], co[8];   // TMEMA: the chip sums / running sums born CL steps before the current group of 8 steps
-#pragma unroll
-        for (int j = 0; j < 8; j++) { ao[j] = 0.0f; co[j] = 0.0f; }
-        if constexpr (TMEMA) {
-            float z[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
-#pragma unroll
-            for (int j = 0; j < L + 8 * CT; j += 8) tm_st8(tring + j, z);
-            tm_ld8(tring + (L - CL) % L, ao);
-            if ((L - CL) / 8 < CT) tm_ld8(tring + L + (L - CL) % L, co);
-        }
+        for (int j = 0; j < L; j++) { cr[j] = 0.0f; ar[j] = 0.0f; }
         uint32_t acc = 0;   // pending output bits (low nacc bits), still as SIGN bits (inverted at store)
         int nacc = 0;       // warp-uniform
         int wi = 0;
@@ -396,104 +294,11 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
                 const uint32_t lo_a = (PHASE == 0) ? lo_zero : lo_b;  // the first kPad steps of body 0
                 const float rh_a = (lo_a == lo_zero) ? 0.0f : kRhi, rl_a = (lo_a == lo_zero) ? 0.0f : kRlo;
                 const float rh_b = (lo_b == lo_zero) ? 0.0f : kRhi, rl_b = (lo_b == lo_zero) ? 0.0f : kRlo;
+                (void)rh_a; (void)rl_a; (void)rh_b; (void)rl_b;
                 const uint32_t src = row + st * G::kStageBytes;
                 uint32_t w = 0;
                 float c = cr[L - 1];  // the running sum = the last slot of the ring
 
-                if constexpr (TMEMA) {
-                    // Group of 8 steps: (1) magnitudes and the running sum -- registers only; (2) wait for the group's
-                    // old values (asked for one group earlier): chip sums a = c - c[CL ago], filter f = a[CL ago] - a, sign
-                    // bits; (3) the new values go to their ring slots, the next group's old ones are asked for.
-                    // The chip-sum ring is entirely in Tensor Memory, the running-sum ring with its first CT groups.
-                    constexpr int NG = L / 8, DG = (L - CL) / 8;   // groups per body; a value is read NG - DG groups after its birth
-#pragma unroll
-                    for (int g = 0; g < NG; g++) {
-                        const uint4 v = lds128(src + g * 16);
-                        const uint32_t xs[4] = {v.x, v.y, v.z, v.w};
-                        if (g == L / 16) {
-                            const int nst = (st + 1 == G::kStages) ? 0 : st + 1;
-                            ready = mbar_test(bar0 + nst * 8, (phases >> nst) & 1u);
-                        }
-                        const int go = (g + DG) % NG;          // the group whose slots hold the values born CL steps ago
-                        const bool c_rd_t = go < CT;           // ... in Tensor Memory (buffer co) or in registers
-                        const bool c_wr_t = g < CT;
-                        float cs[8];
-#pragma unroll
-                        for (int q = 0; q < 4; q++) {
-                            const int j = g * 8 + q * 2;
-                            const uint32_t lo = (j < G::kPad) ? lo_a : lo_b;
-                            const float li0 = lds_f32(__byte_perm(xs[q], lo, 0x7604));
-                            const float li1 = lds_f32(__byte_perm(xs[q], lo, 0x7624));
-                            float m0, m1;
-                            // computed Q magnitude (see HYBRID below) for all (VAR bit 0) or every other (VAR bit 4) word:
-                            // trades one shared-memory wavefront per sample for one issue slot
-                            const bool hyb = HYBRID || ((VAR & 16) != 0 && (q & 1) == 0);
-                            if (hyb && (!kPk || (VAR & 128) != 0)) {   // VAR bit 7: scalar hybrid arithmetic (overlaps with the ALU pipe) next to packed ring adds
-                                const float rh = (j < G::kPad) ? rh_a : rh_b, rl = (j < G::kPad) ? rl_a : rl_b;
-                                const float mq0 = __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7614));  // 32768 + Q
-                                const float mq1 = __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7634));
-                                const float nq0 = __fsub_rn(32895.5f, mq0), nq1 = __fsub_rn(32895.5f, mq1);  // 127.5 - Q, exact
-                                const float xq0 = __fmaf_rn(nq0, rh, __fmul_rn(nq0, rl));                    // fl((127.5-Q)/127.5)
-                                const float xq1 = __fmaf_rn(nq1, rh, __fmul_rn(nq1, rl));
-                                m0 = __fadd_rn(li0, __fmul_rn(xq0, xq0));                                    // decode.go:213,222
-                                m1 = __fadd_rn(li1, __fmul_rn(xq1, xq1));
-                            } else if (hyb) {
-                                const float rh = (j < G::kPad) ? rh_a : rh_b, rl = (j < G::kPad) ? rl_a : rl_b;
-                                const uint64_t mq = pack2(__uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7614)),   // 32768 + Q
-                                                          __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7634)));
-                                const uint64_t nq = sub2(pack2(32895.5f, 32895.5f), mq);                              // 127.5 - Q, exact
-                                const uint64_t xq = fma2(nq, pack2(rh, rh), mul2(nq, pack2(rl, rl)));                 // fl((127.5-Q)/127.5)
-                                unpack2(add2(pack2(li0, li1), mul2(xq, xq)), m0, m1);                                 // decode.go:213,222
-                            } else if constexpr (kPk) {
-                                const float lq0 = lds_f32(__byte_perm(xs[q], lo, 0x7614));
-                                const float lq1 = lds_f32(__byte_perm(xs[q], lo, 0x7634));
-                                unpack2(add2(pack2(li0, li1), pack2(lq0, lq1)), m0, m1);  // decode.go:222
-                            } else {
-                                const float lq0 = lds_f32(__byte_perm(xs[q], lo, 0x7614));
-                                const float lq1 = lds_f32(__byte_perm(xs[q], lo, 0x7634));
-                                m0 = __fadd_rn(li0, lq0);
-                                m1 = __fadd_rn(li1, lq1);
-                            }
-                            cs[2 * q] = __fadd_rn(c, m0);                                 // csum[k+1], decode.go:234
-                            c = __fadd_rn(cs[2 * q], m1);
-                            cs[2 * q + 1] = c;
-                        }
-                        tm_wait_ld2(ao, co);
-                        float a[8];
-#pragma unroll
-                        for (int q = 0; q < 4; q++) {
-                            const int j = g * 8 + q * 2;
-                            const int jo = (j + L - CL) % L;
-                            const float o0 = c_rd_t ? co[2 * q] : cr[jo], o1 = c_rd_t ? co[2 * q + 1] : cr[jo + 1];
-                            float f0, f1;
-                            if constexpr (kPk) {
-                                const uint64_t a2 = sub2(pack2(cs[2 * q], cs[2 * q + 1]), pack2(o0, o1));   // csum[k+1] - csum[k+1-CL]
-                                unpack2(sub2(pack2(ao[2 * q], ao[2 * q + 1]), a2), f0, f1);                   // decode.go:242
-                                unpack2(a2, a[2 * q], a[2 * q + 1]);
-                            } else {
-                                a[2 * q] = __fsub_rn(cs[2 * q], o0);
-                                a[2 * q + 1] = __fsub_rn(cs[2 * q + 1], o1);
-                                f0 = __fsub_rn(ao[2 * q], a[2 * q]);
-                                f1 = __fsub_rn(ao[2 * q + 1], a[2 * q + 1]);
-                            }
-                            if (!c_wr_t) {
-                                cr[j] = cs[2 * q];
-                                cr[j + 1] = cs[2 * q + 1];
-                            }
-                            w = __funnelshift_l(__float_as_uint(f0), w, 1);           // sign bits in
-                            w = __funnelshift_l(__float_as_uint(f1), w, 1);
-                            if (((j + 1) & 31) == 31 && PHASE == 2) {
-                                put(__funnelshift_r(w, acc, nacc));
-                                acc = w;
-                            }
-                        }
-                        tm_st8(tring + g * 8, a);
-                        if (c_wr_t) tm_st8(tring + L + g * 8, cs);
-                        const int gn = (g + 1) % NG, gon = (gn + DG) % NG;
-                        tm_ld8(tring + gon * 8, ao);
-                        if (gon < CT) tm_ld8(tring + L + gon * 8, co);
-                    }
-                } else {
 #pragma unroll
                 for (int g = 0; g < L / 8; g++) {
                     const uint4 v = lds128(src + g * 16);
@@ -504,61 +309,35 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
                     }
 #pragma unroll
                     for (int q = 0; q < 4; q++) {
-                        // two samples (I0 Q0 I1 Q1) per 32-bit word.  kPacked: the three non-sequential adds of the
-                        // pair go through FADD2 (add.f32x2: two independent IEEE fp32 adds, one issue slot); only
-                        // the running sum stays scalar.  CL, L and kPad are even, so pairs never straddle.  The
-                        // rings stay scalar arrays (packed at the point of use): 64-bit ring slots make ptxas
-                        // rotate the pairs and pay it back with ~1.5 MOVs per step at the loop edge.
+                        // two samples (I0 Q0 I1 Q1) per 32-bit word.  CL, L and kPad are even, so the two samples of
+                        // a word never straddle the end of the ring.
                         const int j = g * 8 + q * 2;
                         const int jo = (j + L - CL) % L;  // the slots written CL steps ago
                         const uint32_t lo = (j < G::kPad) ? lo_a : lo_b;
-                        const float rh = (j < G::kPad) ? rh_a : rh_b, rl = (j < G::kPad) ? rl_a : rl_b;
-                        (void)rh; (void)rl;
                         // {byte0: lane*4 (or the zero column), byte1: I or Q, bytes 2-3: LUT base >> 16}
                         const float li0 = lds_f32(__byte_perm(xs[q], lo, 0x7604));
                         const float li1 = lds_f32(__byte_perm(xs[q], lo, 0x7624));
-                        float m0, m1, f0, f1;
-                        if constexpr (HYBRID && kPk) {
-                            // the four roundings of the computed Q magnitude, two samples per instruction
-                            const uint64_t mq = pack2(__uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7614)),   // 32768 + Q
-                                                      __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7634)));
-                            const uint64_t nq = sub2(pack2(32895.5f, 32895.5f), mq);                              // 127.5 - Q, exact
-                            const uint64_t xq = fma2(nq, pack2(rh, rh), mul2(nq, pack2(rl, rl)));                 // fl((127.5-Q)/127.5)
-                            unpack2(add2(pack2(li0, li1), mul2(xq, xq)), m0, m1);                                 // decode.go:213,222
+                        float lq0, lq1;
+                        if constexpr (HYBRID) {
+                            const float rh = (j < G::kPad) ? rh_a : rh_b, rl = (j < G::kPad) ? rl_a : rl_b;
+                            const float mq0 = __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7614));  // 32768 + Q
+                            const float mq1 = __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7634));
+                            const float nq0 = __fsub_rn(32895.5f, mq0), nq1 = __fsub_rn(32895.5f, mq1);  // 127.5 - Q, exact
+                            const float xq0 = __fmaf_rn(nq0, rh, __fmul_rn(nq0, rl));                    // fl((127.5-Q)/127.5)
+                            const float xq1 = __fmaf_rn(nq1, rh, __fmul_rn(nq1, rl));
+                            lq0 = __fmul_rn(xq0, xq0);
+                            lq1 = __fmul_rn(xq1, xq1);
                         } else {
-                            float lq0, lq1;
-                            if constexpr (HYBRID) {
-                                const float mq0 = __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7614));  // 32768 + Q
-                                const float mq1 = __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7634));
-                                const float nq0 = __fsub_rn(32895.5f, mq0), nq1 = __fsub_rn(32895.5f, mq1);  // 127.5 - Q, exact
-                                const float xq0 = __fmaf_rn(nq0, rh, __fmul_rn(nq0, rl));                    // fl((127.5-Q)/127.5)
-                                const float xq1 = __fmaf_rn(nq1, rh, __fmul_rn(nq1, rl));
-                                lq0 = __fmul_rn(xq0, xq0);
-                                lq1 = __fmul_rn(xq1, xq1);
-                            } else {
-                                lq0 = lds_f32(__byte_perm(xs[q], lo, 0x7614));
-                                lq1 = lds_f32(__byte_perm(xs[q], lo, 0x7634));
-                            }
-                            if constexpr (kPk) {
-                                unpack2(add2(pack2(li0, li1), pack2(lq0, lq1)), m0, m1);  // decode.go:222
-                            } else {
-                                m0 = __fadd_rn(li0, lq0);
-                                m1 = __fadd_rn(li1, lq1);
-                            }
+                            lq0 = lds_f32(__byte_perm(xs[q], lo, 0x7614));
+                            lq1 = lds_f32(__byte_perm(xs[q], lo, 0x7634));
                         }
+                        const float m0 = __fadd_rn(li0, lq0), m1 = __fadd_rn(li1, lq1);   // decode.go:222
                         const float c0 = __fadd_rn(c, m0);                            // csum[k+1], decode.go:234
                         c = __fadd_rn(c0, m1);
-                        if constexpr (kPk) {
-                            const uint64_t a = sub2(pack2(c0, c), pack2(cr[jo], cr[jo + 1]));  // csum[k+1] - csum[k+1-CL]
-                            unpack2(sub2(pack2(ar[jo], ar[jo + 1]), a), f0, f1);               // decode.go:242
-                            unpack2(a, ar[j], ar[j + 1]);
-                        } else {
-                            const float a0 = __fsub_rn(c0, cr[jo]), a1 = __fsub_rn(c, cr[jo + 1]);
-                            f0 = __fsub_rn(ar[jo], a0);
-                            f1 = __fsub_rn(ar[jo + 1], a1);
-                            ar[j] = a0;
-                            ar[j + 1] = a1;
-                        }
+                        const float a0 = __fsub_rn(c0, cr[jo]), a1 = __fsub_rn(c, cr[jo + 1]);   // csum[k+1] - csum[k+1-CL]
+                        const float f0 = __fsub_rn(ar[jo], a0), f1 = __fsub_rn(ar[jo + 1], a1);  // decode.go:242
+                        ar[j] = a0;
+                        ar[j + 1] = a1;
                         cr[j] = c0;  // slots j, j+1 died L-CL steps ago
                         cr[j + 1] = c;
                         w = __funnelshift_l(__float_as_uint(f0), w, 1);           // sign bits in
@@ -569,7 +348,6 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
                             acc = w;
                         }
                     }
-                }
                 }
                 // every lane has read its row of this stage into registers: refill it with body t+kStages
                 __syncwarp();
@@ -602,20 +380,9 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
         };
         if (tile == 0) run_tile(std::true_type{});
         else run_tile(std::false_type{});
-        if constexpr (TMEMA) tm_wait_ld2(ao, co);   // the look-ahead of the last group is never used
         __syncwarp();
         npref = npref_next;
         tile = next_tile;
-    }
-    if constexpr (TMEMA) {
-        tm_wait_st();
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        if (warp == 0) {
-            uint32_t tbase;
-            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tbase) : "r"(sbase + 1008) : "memory");
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tbase), "r"(512) : "memory");
-        }
     }
 }
 
@@ -654,13 +421,13 @@ inline int current_device() {
 inline int sm_count_of(int dev) {
     static std::atomic<int> cache[64];
     if (dev < 0 || dev >= 64) {
-        int n = 148;
+        int n = 132;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
         return n;
     }
     int n = cache[dev].load(std::memory_order_relaxed);
     if (n == 0) {
-        n = 148;
+        n = 132;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
         cache[dev].store(n, std::memory_order_relaxed);
     }
@@ -717,8 +484,8 @@ inline long long fast_dynamic_tiles(long long ntiles, long long grid, int W) {
     if (full < 1 || rest == 0 || rest > 4 * grid) return ntiles;
     return full * cap;
 }
-// Rounds of SMs x W tiles a call takes, in units of an 8-warp round (measured on B200: a 7-warp round takes 0.94 of
-// an 8-warp one; a last round with at most one tile per scheduler ~0.62).
+// Rounds of SMs x W tiles a call takes, in units of an 8-warp round.  Model: a 7-warp round costs 0.94 of an 8-warp
+// one, and a last round with at most one tile per scheduler 0.62 of one.
 inline double fast_round_cost(long long ntiles, long long sms, int W) {
     const long long cap = sms * W, full = ntiles / cap, rest = ntiles - full * cap;
     const double unit = W == 8 ? 1.0 : 0.94;
@@ -762,7 +529,7 @@ int launch_demod_fast_cw(const uint8_t* iq, const uint8_t* hist, int hist_sample
     const cuuint64_t gstride[1] = {(cuuint64_t)(2 * BS)};
     const cuuint32_t box[2] = {(cuuint32_t)G::kRowBytes, 32u};
     const cuuint32_t estr[2] = {1u, 1u};
-    // L2 promotion: how much the L2 fetches from DRAM around a box row (ERTGPU_TMA_L2PROMO = 0 none, 1 64 B, 2 128 B, 3 256 B; measured at 8 GiB scm: 0.722 / 0.749 / 0.761 of the HBM roofline for 64 / 128 / 256 B)
+    // L2 promotion: how much the L2 fetches from DRAM around a box row (ERTGPU_TMA_L2PROMO = 0 none, 1 64 B, 2 128 B, 3 256 B)
     static const CUtensorMapL2promotion promo = [] {
         const char* e = getenv("ERTGPU_TMA_L2PROMO");
         const int v = e ? atoi(e) : 3;
@@ -803,9 +570,8 @@ inline int launch_demod_fast(int variant, int warps, const uint8_t* iq, const ui
                              int* var_out = nullptr) {
 #define ERT_FAST_ARGS iq, hist, hist_samples, hist_valid, lut, plane_out, nblocks, BS, tile_counter, st, w_out, var_out
     // Work tiles are handed out in rounds of (SMs x resident warps).  With two warps per scheduler the SM's
-    // rate still grows almost linearly with the warp count (measured round time, 7 : 8 warps = 0.93 : 1), so
-    // when 7 warps need no more rounds than 8 (e.g. 4096 tiles of a 1 GiB scm call: 3.95 vs 3.46 rounds, both
-    // end in the 4th) the fuller last round of 7 wins; long calls keep 8.
+    // rate still grows almost linearly with the warp count, so when 7 warps need no more rounds than 8 the
+    // fuller last round of 7 wins (fast_round_cost); long calls keep 8.
     bool seven = false;
     if (warps == 0) {
         const int sms = sm_count_of(current_device());
@@ -824,15 +590,8 @@ inline int launch_demod_fast(int variant, int warps, const uint8_t* iq, const ui
         const int w = warps % 100, var = warps / 100;
 #define ERT_FAST_TUNE(W_, V_) if (w == W_ && var == V_) return launch_demod_fast_cw<72, W_, V_>(ERT_FAST_ARGS);
         ERT_FAST_TUNE(7, 0) ERT_FAST_TUNE(8, 0) ERT_FAST_TUNE(8, 1) ERT_FAST_TUNE(8, 2) ERT_FAST_TUNE(8, 4)
-        // Tensor-Memory rings (bit 3), + half of the Q magnitudes computed (bit 4), + part of the running-sum ring (bit 5),
-        // scalar adds (bit 6)
-        ERT_FAST_TUNE(12, 8) ERT_FAST_TUNE(12, 24) ERT_FAST_TUNE(10, 24) ERT_FAST_TUNE(14, 40) ERT_FAST_TUNE(8, 64) ERT_FAST_TUNE(12, 72)
 #undef ERT_FAST_TUNE
         return (int)cudaErrorInvalidValue;   // a knob without an instantiation must not silently run the default
-    }
-    if (variant == 72 && warps == 0) {
-        const char* e = getenv("ERTGPU_FAST_TMEM");   // read per launch: 0 restores the register-ring kernel
-        if (!(e && atoi(e) == 0)) return launch_demod_fast_cw<72, 12, 24>(ERT_FAST_ARGS);
     }
     switch (variant) {
         ERT_FAST_CASE(32) ERT_FAST_CASE(40) ERT_FAST_CASE(48) ERT_FAST_CASE(56) ERT_FAST_CASE(64)

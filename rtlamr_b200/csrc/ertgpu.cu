@@ -1,5 +1,5 @@
 // ertgpu.cu -- C ABI of libertgpu.so (see include/ertgpu.h) and the host-side pipeline that
-// drives the sm_100a kernels.  One handle mirrors one reference protocol.Decoder
+// drives the sm_90a kernels.  One handle mirrors one reference protocol.Decoder
 // (protocol/decode.go:45-63).
 //
 // Device data layout (all per handle):
@@ -33,7 +33,6 @@
 #include "demod_generic.cuh"
 #include "ert_common.cuh"
 #include "search.cuh"
-#include "r900_tmem.cuh"
 #include "synth.cuh"
 
 using namespace ert;
@@ -88,9 +87,9 @@ struct ertgpu_handle {
     int demod_variant = 0;      // 0 generic, else specialised chip length
     int demod_warps = 0;        // 0 default; tuning override (env ERTGPU_FAST_WARPS)
     bool search_legacy = false; // env ERTGPU_SEARCH_LEGACY: the per-bit-load Search kernel (kept for chip lengths like 78 and as a cross-check)
-    int sm_count = 148;
+    int sm_count = 132;
     bool use_pdl = true;      // env ERTGPU_PDL=0: ordinary launches for Search and Slice
-    int r900_chain_mode = 0;  // env ERTGPU_R900_CHAIN: (default) producer/consumer warps through shared memory; "tmem" = Tensor Memory between the stages; "smem" = one warp, serial lane 0; "shfl" = one warp, shuffled sums
+    int r900_chain_mode = 0;  // env ERTGPU_R900_CHAIN: (default) producer/consumer warps through shared memory; "smem" = one warp, serial lane 0; "shfl" = one warp, shuffled sums
 
     // state of the last enqueued pipeline (for fetch and taps)
     bool pending = false;       // a pipeline is enqueued and not yet synchronised
@@ -360,7 +359,7 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
         } else if (make_search_params(c, p0, nwords, &sp)) {
             const size_t smem = 0;
             long long tiles = (nwords + kSearchTile - 1) / kSearchTile;
-            unsigned grid = (unsigned)std::min<long long>(tiles, 148 * 4);
+            unsigned grid = (unsigned)std::min<long long>(tiles, (long long)h->sm_count * 4);
             if (grid < 1) grid = 1;
             const int mode = search_mode(c, p0);
 #define ERT_SEARCH(N, M) CUDA_TRY(h, launch_dep(pdl, search_kernel<N, M>, dim3(grid), dim3(kSearchThreads), smem, st, (const uint32_t*)plane, sp, h->d_hits, h->d_words, h->cand_cap, h->d_counters))
@@ -375,7 +374,7 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
 #undef ERT_SEARCH
         } else {
             const int nthr = 256;
-            long long blocks = std::min<long long>((nwords + nthr - 1) / nthr, 148 * 16);
+            long long blocks = std::min<long long>((nwords + nthr - 1) / nthr, (long long)h->sm_count * 16);
             if (blocks < 1) blocks = 1;
             CUDA_TRY(h, launch_dep(pdl, search_generic_kernel, dim3((unsigned)blocks), dim3(nthr), 0, st, (const uint32_t*)plane, p0, nwords, c,
                                    h->d_hits, h->d_words, h->cand_cap, h->d_counters));
@@ -390,35 +389,30 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
     if (h->has_r900) {
         CUDA_TRY(h, cudaMemsetAsync(h->d_block_slot, 0xFF, (size_t)nblocks * sizeof(int), st));
         CUDA_TRY(h, cudaMemsetAsync(h->d_slot_count, 0, sizeof(unsigned int), st));
-        r900_mark_kernel<<<148, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->d_slot_block,
+        r900_mark_kernel<<<(unsigned)h->sm_count, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->d_slot_block,
                                               h->r900_slots, h->d_slot_count);
         CUDA_TRY(h, cudaGetLastError());
         // the two-warp pipeline loads 8 samples (16 bytes) at a time: chain starts and the call's bytes must be 16-byte aligned
         const bool vec_ok = (reinterpret_cast<uintptr_t>(d_iq) & 15u) == 0 && (reinterpret_cast<uintptr_t>(hist) & 15u) == 0 &&
                             c.BUF % 8 == 0 && c.BS % 8 == 0 && c.hist_samples % 8 == 0;
         if (h->r900_chain_mode == 2) {
-            r900_chain_kernel<true><<<148 * 16, kR900ChainWarps * 32, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c,
+            r900_chain_kernel<true><<<(unsigned)h->sm_count * 16, kR900ChainWarps * 32, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c,
                                                                        h->d_slot_block, h->r900_slots, h->d_slot_count,
                                                                        h->r900_span, h->d_r900_scratch);
         } else if (h->r900_chain_mode == 1 || !vec_ok) {
-            r900_chain_kernel<false><<<148 * 16, kR900ChainWarps * 32, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c,
+            r900_chain_kernel<false><<<(unsigned)h->sm_count * 16, kR900ChainWarps * 32, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c,
                                                                        h->d_slot_block, h->r900_slots, h->d_slot_count,
                                                                        h->r900_span, h->d_r900_scratch);
-        } else if (h->r900_chain_mode == 3) {   // Tensor Memory between the stages (r900_tmem.cuh): exact, measured no faster (212 vs 203 us)
-            static OncePerDevice t3_once;
-            if (t3_once.first(current_device())) CUDA_TRY(h, cudaFuncSetAttribute(r900_chain3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kT3SmemBytes));
-            r900_chain3_kernel<<<(unsigned)h->sm_count * 2, kT3Warps * 32, kT3SmemBytes, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, c, h->d_slot_block,
-                                                        h->r900_slots, h->d_slot_count, h->r900_span, h->d_r900_scratch);
         } else {   // default: producer warps + one consumer warp per 16 chains, hand-offs through shared memory
             r900_chain2_kernel<<<(unsigned)h->sm_count * 2, (kChainProducers + 1) * 32, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, c, h->d_slot_block,
                                                         h->r900_slots, h->d_slot_count, h->r900_span, h->d_r900_scratch);
         }
         CUDA_TRY(h, cudaGetLastError());
-        r900_digits_kernel<<<148 * 16, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->r900_span,
+        r900_digits_kernel<<<(unsigned)h->sm_count * 16, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->r900_span,
                                                     h->d_r900_scratch, h->d_digits);
         CUDA_TRY(h, cudaGetLastError());
         // blocks that found no scratch slot: exact per-candidate replay
-        r900_replay_kernel<<<148, 64, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c, h->d_hits,
+        r900_replay_kernel<<<(unsigned)h->sm_count, 64, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c, h->d_hits,
                                                h->cand_cap, h->d_counters, h->d_block_slot, h->d_digits, h->d_slot_count, h->r900_slots);
         CUDA_TRY(h, cudaGetLastError());
         h->launches += 4;
@@ -721,7 +715,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     CUDA_TRY(h, cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(h, cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail(h, ERTGPU_ECUDA, "libertgpu is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail(h, ERTGPU_ECUDA, "libertgpu is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
 
     if (max_blocks_per_call <= 0) max_blocks_per_call = std::max<int64_t>(1, (64ll << 20) / c.block_size2);
     if (max_candidates <= 0) max_candidates = 1 << 18;
@@ -785,9 +779,9 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     if (const char* e = getenv("ERTGPU_FAST_WARPS")) h->demod_warps = atoi(e);   // 100 * VAR + W, see launch_demod_fast
     if (const char* e = getenv("ERTGPU_SEARCH_LEGACY")) h->search_legacy = atoi(e) != 0;
     if (const char* e = getenv("ERTGPU_PDL")) h->use_pdl = atoi(e) != 0;
-    if (const char* e = getenv("ERTGPU_R900_CHAIN")) h->r900_chain_mode = strcmp(e, "shfl") == 0 ? 2 : (strcmp(e, "smem") == 0 ? 1 : (strcmp(e, "tmem") == 0 ? 3 : 0));
+    if (const char* e = getenv("ERTGPU_R900_CHAIN")) h->r900_chain_mode = strcmp(e, "shfl") == 0 ? 2 : (strcmp(e, "smem") == 0 ? 1 : 0);
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->device);
-    if (h->sm_count < 1) h->sm_count = 148;
+    if (h->sm_count < 1) h->sm_count = 132;
     h->cur_plane = h->cur_hist = 0;
     h->hist_valid = 0;
     h->block_counter = 0;
@@ -1143,7 +1137,7 @@ int ertgpu_synth_fill(int32_t device, void* d_out, int64_t first_sample, int64_t
         return ERTGPU_ECUDA;
     }
     long long groups = (nsamples + 7) / 8;
-    long long blocks = std::min<long long>((groups + 255) / 256, 148 * 32);
+    long long blocks = std::min<long long>((groups + 255) / 256, (long long)sm_count_of(current_device()) * 32);
     if (blocks < 1) blocks = 1;
     synth_kernel<<<(unsigned)blocks, 256, 0, st>>>(static_cast<uint8_t*>(d_out), first_sample, nsamples, seed, d_pk, n);
     cudaError_t e = cudaGetLastError();

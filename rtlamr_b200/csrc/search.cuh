@@ -787,17 +787,14 @@ __device__ __forceinline__ float lut_of_magic(float mag) {
     return __fmul_rn(x, x);
 }
 
-// Why this shape.  A chain is ~24 700 DEPENDENT float32 adds: 4.2 cycles each (measured), 55 us of pure latency, and the
-// kernel's time is one chain's time as long as every chain of the call is resident.  What the chain really pays on top
-// (measured, B200): every shared- or global-memory instruction that sits in the in-order instruction stream of the warp
-// that runs the adds costs it 5-12 cycles -- nothing of it hides behind the add latency.  So the consumer warp does the
-// minimum: one LDS.128 and one STG.128 per four adds, sixteen chains side by side (one SIMT instruction advances all of
-// them; the whole-vector stores go straight to the padded scratch rows, no second ring), and everything else lives in the
-// producer warps: asynchronous 16-byte copies (in-order completion, any depth), magnitudes COMPUTED instead of looked up
-// (the table lookups of 16 chains would take the shared-memory bandwidth the hand-offs need).  Round-2 history at 4 GiB /
-// ~2400 chains: 451 us (4 chains per CTA, scalar 2-byte loads, lookups, second ring) -> 293 (16-byte loads) -> 192 (two
-// producers) -> 203 (this kernel; 131 us of it remain with the adds and the stores switched off: hand-off and issue
-// overhead of the lone consumer warp).
+// Why this shape.  A chain is ~24 700 DEPENDENT float32 adds, and the kernel's time is one chain's time as long as every
+// chain of the call is resident.  What the chain pays on top is every shared- or global-memory instruction that sits in
+// the in-order instruction stream of the warp that runs the adds -- little of it hides behind the add latency.  So the
+// consumer warp does the minimum: one LDS.128 and one STG.128 per four adds, sixteen chains side by side (one SIMT
+// instruction advances all of them; the whole-vector stores go straight to the padded scratch rows, no second ring), and
+// everything else lives in the producer warps: asynchronous 16-byte copies (in-order completion, any depth), magnitudes
+// COMPUTED instead of looked up (the table lookups of 16 chains would take the shared-memory bandwidth the hand-offs
+// need), mbarrier rings between the two sides.
 __global__ void __launch_bounds__((kChainProducers + 1) * 32)
 r900_chain2_kernel(const uint8_t* __restrict__ iq, const uint8_t* __restrict__ hist, int hist_samples, int hist_valid,
                    DevCfg cfg, const int* __restrict__ slot_block, int slot_cap,

@@ -11,14 +11,14 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
 
 
 def _usable_gpu() -> bool:
-    """One probe per session: is there a CUDA device of compute capability 10.x (libertgpu is sm_100a only)?"""
+    """One probe per session: is there a CUDA device of compute capability 9.0 (libertgpu is sm_90a only)?"""
     try:
         import torch
-        return torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 10
+        return torch.cuda.is_available() and torch.cuda.get_device_capability(0) == (9, 0)
     except Exception:
         return False
 
@@ -27,7 +27,7 @@ def pytest_collection_modifyitems(config, items):
     """CPU-only machines: every test marked `gpu` is skipped (not failed, not an error at collection) -- the
     product has no CPU fallback to run them on."""
     if any("gpu" in item.keywords for item in items) and not _usable_gpu():
-        skip = pytest.mark.skip(reason="no sm_100 CUDA device: GPU parity tests need a B200 (run with -m gpu there)")
+        skip = pytest.mark.skip(reason="no sm_90 CUDA device: GPU parity tests need an H100 (run with -m gpu there)")
         for item in items:
             if "gpu" in item.keywords:
                 item.add_marker(skip)

@@ -42,12 +42,7 @@ if len(sys.argv) == 3 and sys.argv[1] == "--synthetic-inputs":
 if __name__ != "__main__":
     raise ImportError("make_golden is a script; import SYNTH_CASES / synth_input via tests/test_go_golden.py's loader")
 
-src = "/root/reference/assets/sample.bin"
-dst = os.path.join(here, "sample_cl78.bin")
-if os.path.exists(src) and not os.path.exists(dst):
-    import shutil
-    shutil.copyfile(src, dst)
-iq = np.fromfile(dst, dtype=np.uint8)
+iq = np.fromfile(os.path.join(here, "sample_cl78.bin"), dtype=np.uint8)
 out = {}
 for name, mode in (("exact", oracle.SEARCH_EXACT), ("go_faithful", oracle.SEARCH_GO)):
     o = oracle.Oracle("scm", 78, mode)

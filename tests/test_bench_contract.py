@@ -1,4 +1,4 @@
-"""bench.py's JSON contract, checked on CPU through the reference arm (the GPU arm needs a B200)."""
+"""bench.py's JSON contract, checked on CPU through the reference arm (the GPU arm needs an H100)."""
 import json
 import os
 import subprocess
@@ -60,3 +60,31 @@ def test_non_zero_ranks_of_the_reference_arm_do_no_work(built):
     out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--gpus", "2"],
                          capture_output=True, text=True, timeout=60, env=env)
     assert out.returncode == 0 and out.stdout.strip() == ""
+
+
+def test_dump_outputs_writes_float_arrays_within_the_limit(tmp_path, monkeypatch):
+    """--dump-outputs: one float64 / float32 .npy per candidate field; above the size limit a seeded sample of whole
+    records in stream order, the same one every run."""
+    import numpy as np
+
+    import bench
+    from rtlamr_b200 import capi
+    got = np.zeros(1000, dtype=capi.CAND_DTYPE)
+    got["block"] = np.arange(1000)
+    got["bytes"][:, 0] = np.arange(1000) % 256
+    bench.dump_outputs(str(tmp_path / "a"), "scm1g", got)
+    blk = np.load(tmp_path / "a" / "scm1g_block.npy")
+    assert blk.dtype == np.float64 and np.array_equal(blk, np.arange(1000))
+    b = np.load(tmp_path / "a" / "scm1g_bytes.npy")
+    assert b.dtype == np.float32 and b.shape == (1000, capi.MAX_PACKET_BYTES) and np.array_equal(b[:, 0], np.arange(1000) % 256)
+    assert sorted(os.listdir(tmp_path / "a")) == sorted(f"scm1g_{f}.npy" for f in
+                                                          ("block", "idx", "preamble_id", "check_mask", "flags", "bytes", "r900_digits"))
+    monkeypatch.setattr(bench, "DUMP_LIMIT_BYTES", 100 * 1000)
+    for d in ("b", "c"):
+        bench.dump_outputs(str(tmp_path / d), "scm1g", got)
+    bench.dump_outputs(str(tmp_path / "d"), "scm1g", got, 50 * 1000)
+    assert sum(os.path.getsize(tmp_path / "d" / f) for f in os.listdir(tmp_path / "d")) <= 50 * 1000
+    total = sum(os.path.getsize(tmp_path / "b" / f) for f in os.listdir(tmp_path / "b"))
+    blk_b, blk_c = np.load(tmp_path / "b" / "scm1g_block.npy"), np.load(tmp_path / "c" / "scm1g_block.npy")
+    assert 0 < len(blk_b) < 1000 and np.all(np.diff(blk_b) > 0) and np.array_equal(blk_b, blk_c)
+    assert total <= 100 * 1000

@@ -2,7 +2,7 @@
 // Every warp walks work tiles of 32 rows (row pitch = PITCH bytes) in boxes of [32 rows][BOXB bytes] with S boxes in
 // flight, exactly like demod_fast_kernel, but does nothing with the data.  MODE 1 streams the same bytes as contiguous
 // 1-D bulk copies (the friendliest pattern) for comparison.
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tma_probe tma_probe.cu -lcuda
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tma_probe tma_probe.cu -lcuda
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdio>
@@ -79,7 +79,7 @@ int main(int argc, char** argv) {
     void* fp = nullptr; cudaDriverEntryPointQueryResult q;
     cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &q);
     EncodeTiledFn enc = (EncodeTiledFn)fp;
-    int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     cudaFuncSetAttribute(probe<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaFuncSetAttribute(probe<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     struct Cfg { int mode, boxb, stages, warps, promo; };
