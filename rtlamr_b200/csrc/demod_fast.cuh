@@ -35,7 +35,6 @@
 #include <cuda.h>
 
 #include <atomic>
-#include <cstdlib>
 #include <type_traits>
 
 #include "ert_common.cuh"
@@ -109,17 +108,14 @@ constexpr int fast_body_len(int CL) {
     return L;
 }
 
-// the tight ring: L = CL (every slot is read, then overwritten, in the same step) when CL / 8 is odd
-constexpr bool fast_tight_ok(int CL) { return CL % 8 == 0 && ((CL / 8) & 1) == 1; }
-
-template <int CL, int STAGES = 2, bool TIGHT = false>
+template <int CL>
 struct FastGeom {
-    static constexpr int L = TIGHT ? CL : fast_body_len(CL);
+    static constexpr int L = fast_body_len(CL);
     static constexpr int kPad = 2 * L - 2 * CL;        // zero-magnitude steps in front of the lead-in
     static constexpr int kRowBytes = 2 * L;            // one body's IQ bytes per chain
     static constexpr int kRowUnits = kRowBytes / 16;   // odd: conflict-free LDS.128
     static constexpr int kStageBytes = 32 * kRowBytes;
-    static constexpr int kStages = STAGES;              // bodies in flight per warp (3 measured no faster than 2: the refill is not what the warps wait for)
+    static constexpr int kStages = 2;                   // bodies in flight per warp (3 measured no faster than 2: the refill is not what the warps wait for)
     static constexpr int kWarpBytes = kStages * kStageBytes;
     static constexpr int kFullWords = L / 32;           // whole output words per body
     static constexpr int kTailBits = L % 32;
@@ -130,15 +126,13 @@ struct FastGeom {
 // smem map (byte offsets inside the dynamic segment, computed at run time):
 //   [bars: 2 x 8 B per warp][pad][staging of the first warps ...][LUT at the next 64 KiB boundary]
 //   [staging of the remaining warps ...]
-// VAR: tuning variants kept for the record (bit 0 = HYBRID magnitude, bit 1 = 3-stage staging ring, bit 2 = tight ring)
-template <int CL, int WARPS, int VAR = 0>
+template <int CL, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, 1)
 demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __restrict__ iq,
                   const uint8_t* __restrict__ hist, int hist_samples, int hist_valid,
                   const float* __restrict__ lut_g, uint32_t* __restrict__ plane_out, long long nblocks, int BS,
                   unsigned long long* __restrict__ tile_counter, long long dyn_tiles) {
-    constexpr bool HYBRID = (VAR & 1) != 0;
-    using G = FastGeom<CL, (VAR & 2) ? 3 : 2, (VAR & 4) != 0>;
+    using G = FastGeom<CL>;
     constexpr int L = G::L;
     extern __shared__ __align__(128) uint8_t fast_smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -285,16 +279,8 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
                 // its first probe) is only paid when the refill really is late
                 if (!ready) mbar_wait(bar0 + st * 8, (phases >> st) & 1u);
                 phases ^= 1u << st;
-                // HYBRID: the Q component is computed instead of looked up: x = (127.5 - q) / 127.5 rounded to
-                // nearest is exactly fma(n, rhi, n * rlo) for all 256 byte values (verified exhaustively with
-                // exact arithmetic, tests/test_oracle.py), then squared -- the two roundings of decode.go:212-213.
-                // Zero-magnitude steps multiply by 0 instead.
-                const float kRhi = __uint_as_float(1006665857u), kRlo = __uint_as_float(2952724223u);
                 const uint32_t lo_b = (PHASE == 2) ? lo_main : lo_lead;
                 const uint32_t lo_a = (PHASE == 0) ? lo_zero : lo_b;  // the first kPad steps of body 0
-                const float rh_a = (lo_a == lo_zero) ? 0.0f : kRhi, rl_a = (lo_a == lo_zero) ? 0.0f : kRlo;
-                const float rh_b = (lo_b == lo_zero) ? 0.0f : kRhi, rl_b = (lo_b == lo_zero) ? 0.0f : kRlo;
-                (void)rh_a; (void)rl_a; (void)rh_b; (void)rl_b;
                 const uint32_t src = row + st * G::kStageBytes;
                 uint32_t w = 0;
                 float c = cr[L - 1];  // the running sum = the last slot of the ring
@@ -317,20 +303,8 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
                         // {byte0: lane*4 (or the zero column), byte1: I or Q, bytes 2-3: LUT base >> 16}
                         const float li0 = lds_f32(__byte_perm(xs[q], lo, 0x7604));
                         const float li1 = lds_f32(__byte_perm(xs[q], lo, 0x7624));
-                        float lq0, lq1;
-                        if constexpr (HYBRID) {
-                            const float rh = (j < G::kPad) ? rh_a : rh_b, rl = (j < G::kPad) ? rl_a : rl_b;
-                            const float mq0 = __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7614));  // 32768 + Q
-                            const float mq1 = __uint_as_float(__byte_perm(xs[q], 0x47000000u, 0x7634));
-                            const float nq0 = __fsub_rn(32895.5f, mq0), nq1 = __fsub_rn(32895.5f, mq1);  // 127.5 - Q, exact
-                            const float xq0 = __fmaf_rn(nq0, rh, __fmul_rn(nq0, rl));                    // fl((127.5-Q)/127.5)
-                            const float xq1 = __fmaf_rn(nq1, rh, __fmul_rn(nq1, rl));
-                            lq0 = __fmul_rn(xq0, xq0);
-                            lq1 = __fmul_rn(xq1, xq1);
-                        } else {
-                            lq0 = lds_f32(__byte_perm(xs[q], lo, 0x7614));
-                            lq1 = lds_f32(__byte_perm(xs[q], lo, 0x7634));
-                        }
+                        const float lq0 = lds_f32(__byte_perm(xs[q], lo, 0x7614));
+                        const float lq1 = lds_f32(__byte_perm(xs[q], lo, 0x7634));
                         const float m0 = __fadd_rn(li0, lq0), m1 = __fadd_rn(li1, lq1);   // decode.go:222
                         const float c0 = __fadd_rn(c, m0);                            // csum[k+1], decode.go:234
                         c = __fadd_rn(c0, m1);
@@ -475,11 +449,10 @@ inline int fast_smem_bytes(int W, uint32_t sbase) {
 }
 
 // Tiles handed out dynamically; the rest (a last round that fills at most one warp per scheduler) is pre-assigned
-// inside the kernel.  ERTGPU_FAST_TAIL=0 keeps everything dynamic (tuning / cross-check).
+// inside the kernel.
 inline long long fast_dynamic_tiles(long long ntiles, long long grid, int W) {
-    static const bool enabled = [] { const char* e = getenv("ERTGPU_FAST_TAIL"); return !(e && atoi(e) == 0); }();
     const long long cap = grid * W;
-    if (!enabled || W < 4 || cap <= 0) return ntiles;
+    if (W < 4 || cap <= 0) return ntiles;
     const long long full = ntiles / cap, rest = ntiles - full * cap;
     if (full < 1 || rest == 0 || rest > 4 * grid) return ntiles;
     return full * cap;
@@ -494,14 +467,13 @@ inline double fast_round_cost(long long ntiles, long long sms, int W) {
     return full * unit + last;
 }
 
-template <int CL, int W, int VAR = 0>
+template <int CL, int W>
 int launch_demod_fast_cw(const uint8_t* iq, const uint8_t* hist, int hist_samples, int hist_valid,
                          const float* lut, uint32_t* plane_out, long long nblocks, int BS,
-                         unsigned long long* tile_counter, cudaStream_t st, int* w_out, int* var_out) {
+                         unsigned long long* tile_counter, cudaStream_t st, int* w_out) {
     if (w_out) *w_out = W;
-    if (var_out) *var_out = VAR;
-    using G = FastGeom<CL, (VAR & 2) ? 3 : 2, (VAR & 4) != 0>;
-    auto kern = demod_fast_kernel<CL, W, VAR>;
+    using G = FastGeom<CL>;
+    auto kern = demod_fast_kernel<CL, W>;
     const int smem = fast_smem_bytes<G>(W, dynamic_smem_base());
     if (smem > 227 * 1024) return (int)cudaErrorInvalidValue;
     const int dev = current_device();
@@ -520,7 +492,7 @@ int launch_demod_fast_cw(const uint8_t* iq, const uint8_t* hist, int hist_sample
     // staging buffer reuse it.  Invariant: the key is everything the encoded map contains -- a buffer that was freed and
     // re-allocated at the same address with the same number of blocks and block size gives a byte-identical descriptor (a
     // tensor map holds addresses and extents, no handle to the allocation), so a stale hit cannot exist; the cache is per
-    // thread and per template instantiation (the box is part of the type), and the L2 promotion knob is read once per process.
+    // thread and per template instantiation (the box is part of the type).
     struct MapKey { const void* iq; long long nblocks; int BS; };
     static thread_local MapKey last_key = {nullptr, 0, 0};
     static thread_local CUtensorMap map;
@@ -529,15 +501,9 @@ int launch_demod_fast_cw(const uint8_t* iq, const uint8_t* hist, int hist_sample
     const cuuint64_t gstride[1] = {(cuuint64_t)(2 * BS)};
     const cuuint32_t box[2] = {(cuuint32_t)G::kRowBytes, 32u};
     const cuuint32_t estr[2] = {1u, 1u};
-    // L2 promotion: how much the L2 fetches from DRAM around a box row (ERTGPU_TMA_L2PROMO = 0 none, 1 64 B, 2 128 B, 3 256 B)
-    static const CUtensorMapL2promotion promo = [] {
-        const char* e = getenv("ERTGPU_TMA_L2PROMO");
-        const int v = e ? atoi(e) : 3;
-        return v == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : v == 1 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B
-             : v == 3 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
-    }();
+    // L2 promotion: the L2 fetches 256 B from DRAM around a box row
     CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(iq), gdim, gstride, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, promo,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return (int)cudaErrorInvalidValue;
     last_key = {iq, nblocks, BS};
@@ -563,36 +529,22 @@ inline int demod_fast_variant(int CL, int BS) {
     }
 }
 
-// warps == 0 picks the default resident-warp count for the chip length
-inline int launch_demod_fast(int variant, int warps, const uint8_t* iq, const uint8_t* hist, int hist_samples,
+inline int launch_demod_fast(int variant, const uint8_t* iq, const uint8_t* hist, int hist_samples,
                              int hist_valid, const float* lut, uint32_t* plane_out, long long nblocks,
-                             int BS, unsigned long long* tile_counter, cudaStream_t st, int* w_out = nullptr,
-                             int* var_out = nullptr) {
-#define ERT_FAST_ARGS iq, hist, hist_samples, hist_valid, lut, plane_out, nblocks, BS, tile_counter, st, w_out, var_out
+                             int BS, unsigned long long* tile_counter, cudaStream_t st, int* w_out = nullptr) {
+#define ERT_FAST_ARGS iq, hist, hist_samples, hist_valid, lut, plane_out, nblocks, BS, tile_counter, st, w_out
     // Work tiles are handed out in rounds of (SMs x resident warps).  With two warps per scheduler the SM's
     // rate still grows almost linearly with the warp count, so when 7 warps need no more rounds than 8 the
     // fuller last round of 7 wins (fast_round_cost); long calls keep 8.
-    bool seven = false;
-    if (warps == 0) {
-        const int sms = sm_count_of(current_device());
-        const long long T = (nblocks + 31) / 32;
-        seven = fast_round_cost(T, sms, 7) < fast_round_cost(T, sms, 8);
-    }
+    const int sms = sm_count_of(current_device());
+    const long long T = (nblocks + 31) / 32;
+    const bool seven = fast_round_cost(T, sms, 7) < fast_round_cost(T, sms, 8);
 #define ERT_FAST_CASE(N)                                                                         \
     case N:                                                                                      \
         if constexpr (fast_warps<N>() == 8) {                                                    \
-            if (seven || warps == 7) return launch_demod_fast_cw<N, 7>(ERT_FAST_ARGS);           \
+            if (seven) return launch_demod_fast_cw<N, 7>(ERT_FAST_ARGS);                         \
         }                                                                                        \
         return launch_demod_fast_cw<N, fast_warps<N>()>(ERT_FAST_ARGS);
-    // tuning knobs for the headline chip length: ERTGPU_FAST_WARPS = 100 * VAR + W  (W resident warps;
-    // VAR bit 0 = hybrid magnitude, bit 1 = 3-stage staging ring, bit 2 = tight ring L = CL)
-    if (variant == 72 && warps >= 4) {
-        const int w = warps % 100, var = warps / 100;
-#define ERT_FAST_TUNE(W_, V_) if (w == W_ && var == V_) return launch_demod_fast_cw<72, W_, V_>(ERT_FAST_ARGS);
-        ERT_FAST_TUNE(7, 0) ERT_FAST_TUNE(8, 0) ERT_FAST_TUNE(8, 1) ERT_FAST_TUNE(8, 2) ERT_FAST_TUNE(8, 4)
-#undef ERT_FAST_TUNE
-        return (int)cudaErrorInvalidValue;   // a knob without an instantiation must not silently run the default
-    }
     switch (variant) {
         ERT_FAST_CASE(32) ERT_FAST_CASE(40) ERT_FAST_CASE(48) ERT_FAST_CASE(56) ERT_FAST_CASE(64)
         ERT_FAST_CASE(72) ERT_FAST_CASE(78) ERT_FAST_CASE(80) ERT_FAST_CASE(88) ERT_FAST_CASE(96)

@@ -40,23 +40,6 @@ __device__ __forceinline__ float mag_at(const uint8_t* __restrict__ iq, const ui
     return __fadd_rn(lut[iq16 & 0xFFu], lut[iq16 >> 8]);
 }
 
-// The same in two halves, for loops that fetch ahead: raw_at only loads (0x10000 = "before the start of the
-// stream"), mag_of does the table lookups.  Looking up right after the load would make an in-order warp
-// wait for the load it meant to overlap.
-__device__ __forceinline__ uint32_t raw_at(const uint8_t* __restrict__ iq, const uint8_t* __restrict__ hist,
-                                           int hist_samples, int hist_valid, long long j) {
-    // branch-free: selects + one predicated load (divergent branches cost more than the load they skip)
-    const bool in_call = j >= 0;
-    const bool ok = in_call || (-j <= (long long)hist_valid);
-    const uint8_t* p = in_call ? iq + 2 * j : hist + 2 * ((long long)hist_samples + j);
-    uint32_t v = 0x10000u;
-    if (ok) v = *reinterpret_cast<const uint16_t*>(p);
-    return v;
-}
-__device__ __forceinline__ float mag_of(uint32_t raw, const float* __restrict__ lut) {
-    return (raw & 0x10000u) ? 0.0f : __fadd_rn(lut[raw & 0xFFu], lut[(raw >> 8) & 0xFFu]);
-}
-
 // grid: ceil(nblocks / blockDim.x) CTAs; dynamic smem: (256 + 2*CL*blockDim.x) floats
 __global__ void demod_generic_kernel(const uint8_t* __restrict__ iq, const uint8_t* __restrict__ hist,
                                      int hist_samples, int hist_valid, const float* __restrict__ lut_g,

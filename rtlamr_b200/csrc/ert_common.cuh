@@ -19,11 +19,6 @@ struct DevProto {
     int32_t crc_from, crc_to;
     uint16_t crc_init, crc_residue;
     int32_t table;  // index into the CRC table array
-    // position tables for the warp-parallel CRC (see extract_kernel): contribution of byte value v at
-    // position p of a message of n bytes with zero init, [n][256] uint16 at pos_base; pos_k = CRC(init, n zero bytes)
-    int32_t pos_base, pos_n;
-    int32_t pos2_base, pos2_n;  // second message of the IDM screen (6 bytes)
-    uint16_t pos_k, pos2_k;
 };
 
 struct DevCfg {

@@ -53,7 +53,6 @@ struct ertgpu_handle {
 
     float* d_lut = nullptr;
     uint16_t* d_crc = nullptr;
-    uint16_t* d_crc_pos = nullptr;  // per-position CRC tables of every screen
     uint32_t* d_plane[2] = {nullptr, nullptr};
     size_t plane_words = 0;
     int cur_plane = 0;
@@ -74,6 +73,7 @@ struct ertgpu_handle {
     unsigned int* d_slot_count = nullptr;
     float* d_r900_scratch = nullptr;  // [slot][r900_span] running sums
     int r900_slots = 0, r900_span = 0;
+    bool r900_vec = false;            // PKL % 8 == 0: r900 chains start on 8-sample (16-byte) boundaries
     ertgpu_candidate* d_out = nullptr;
     unsigned long long cand_cap = 0;
     unsigned long long* d_counters = nullptr;  // kCntHits, kCntOut, kCntValid, kCntTile (demod work tiles), kCntWords
@@ -85,11 +85,7 @@ struct ertgpu_handle {
     int64_t block_counter = 0;  // number of reference Decode calls consumed so far
     bool has_r900 = false;
     int demod_variant = 0;      // 0 generic, else specialised chip length
-    int demod_warps = 0;        // 0 default; tuning override (env ERTGPU_FAST_WARPS)
-    bool search_legacy = false; // env ERTGPU_SEARCH_LEGACY: the per-bit-load Search kernel (kept for chip lengths like 78 and as a cross-check)
     int sm_count = 132;
-    bool use_pdl = true;      // env ERTGPU_PDL=0: ordinary launches for Search and Slice
-    int r900_chain_mode = 0;  // env ERTGPU_R900_CHAIN: (default) producer/consumer warps through shared memory; "smem" = one warp, serial lane 0; "shfl" = one warp, shuffled sums
 
     // state of the last enqueued pipeline (for fetch and taps)
     bool pending = false;       // a pipeline is enqueued and not yet synchronised
@@ -199,7 +195,6 @@ void free_device(ertgpu_handle* h) {
     for (auto& set : h->ev_pool) for (int k = 0; k < 5; k++) evfree(set[k]);
     dfree(h->d_lut);
     dfree(h->d_crc);
-    dfree(h->d_crc_pos);
     dfree(h->d_hits);
     dfree(h->d_words);
     dfree(h->d_digits);
@@ -271,7 +266,7 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
     }
 
     const bool tm = h->stage_timing;
-    const bool pdl = h->use_pdl && !tm;   // events recorded between the kernels would sit between primary and dependent
+    const bool pdl = !tm;   // events recorded between the kernels would sit between primary and dependent
     if (tm) {
         if (h->stage_unread == ertgpu_handle::kStageSets) fold_stage_times(h);  // every earlier pipeline has been waited for
         h->ev_stage = h->ev_pool[h->stage_next];
@@ -282,11 +277,11 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
     // 1. magnitude + matched filter + quantize + pack
     char kname[160];
     if (h->demod_variant != 0) {
-        int w_used = 0, var_used = 0;
-        int rc = launch_demod_fast(h->demod_variant, h->demod_warps, d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut,
-                                   plane + c.hist_words, nblocks, c.BS, h->d_counters + kCntTile, st, &w_used, &var_used);
+        int w_used = 0;
+        int rc = launch_demod_fast(h->demod_variant, d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut,
+                                   plane + c.hist_words, nblocks, c.BS, h->d_counters + kCntTile, st, &w_used);
         if (rc != 0) return fail(h, ERTGPU_ECUDA, "demod_fast launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-        snprintf(kname, sizeof(kname), "demod_fast_kernel<%d,%d,%d>", h->demod_variant, w_used, var_used);
+        snprintf(kname, sizeof(kname), "demod_fast_kernel<%d,%d>", h->demod_variant, w_used);
         h->kernels = kname;
     } else {
         h->kernels = "demod_generic_kernel";
@@ -307,7 +302,7 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
     {
         SearchParams sp;
         SlideParams sl;
-        if (!h->search_legacy && make_slide_params(c, p0, nwords, &sl)) {
+        if (make_slide_params(c, p0, nwords, &sl)) {
             const int smem = 2 * sl.load_words * 4 + 16;
             const long long tiles = (nwords + sl.tile_words - 1) / sl.tile_words;
             int per_sm = (227 * 1024) / (smem + 1024);
@@ -325,6 +320,8 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
     } while (0)
 #define ERT_SLIDE(N, ...)                                                                    \
     do {                                                                                     \
+        snprintf(kname, sizeof(kname), ";search_slide_kernel<%d,%s%s%s>", N, half ? "true" : "false", \
+                 sizeof(#__VA_ARGS__) > 1 ? "," : "", #__VA_ARGS__);                         \
         if (half) ERT_SLIDE_K((search_slide_kernel<N, true, ##__VA_ARGS__>));                \
         else ERT_SLIDE_K((search_slide_kernel<N, false, ##__VA_ARGS__>));                    \
     } while (0)
@@ -362,6 +359,7 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
             unsigned grid = (unsigned)std::min<long long>(tiles, (long long)h->sm_count * 4);
             if (grid < 1) grid = 1;
             const int mode = search_mode(c, p0);
+            snprintf(kname, sizeof(kname), ";search_kernel<%d,%d>", c.npre, mode);
 #define ERT_SEARCH(N, M) CUDA_TRY(h, launch_dep(pdl, search_kernel<N, M>, dim3(grid), dim3(kSearchThreads), smem, st, (const uint32_t*)plane, sp, h->d_hits, h->d_words, h->cand_cap, h->d_counters))
 #define ERT_SEARCH_N(N) do { if (mode == 1) ERT_SEARCH(N, 1); else if (mode == 2) ERT_SEARCH(N, 2); else ERT_SEARCH(N, 0); } while (0)
             switch (c.npre) {
@@ -376,11 +374,13 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
             const int nthr = 256;
             long long blocks = std::min<long long>((nwords + nthr - 1) / nthr, (long long)h->sm_count * 16);
             if (blocks < 1) blocks = 1;
+            snprintf(kname, sizeof(kname), ";search_generic_kernel");
             CUDA_TRY(h, launch_dep(pdl, search_generic_kernel, dim3((unsigned)blocks), dim3(nthr), 0, st, (const uint32_t*)plane, p0, nwords, c,
                                    h->d_hits, h->d_words, h->cand_cap, h->d_counters));
         }
         CUDA_TRY(h, cudaGetLastError());
         h->launches++;
+        h->kernels += kname;
     }
 
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[2], st));
@@ -389,33 +389,29 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
     if (h->has_r900) {
         CUDA_TRY(h, cudaMemsetAsync(h->d_block_slot, 0xFF, (size_t)nblocks * sizeof(int), st));
         CUDA_TRY(h, cudaMemsetAsync(h->d_slot_count, 0, sizeof(unsigned int), st));
+        // the chain kernel loads 8 samples (16 bytes) at a time from chain starts (b + 1) * BS - BUF: without that
+        // alignment no block gets a scratch slot and every r900 hit takes the exact per-candidate replay
+        const int slots = h->r900_vec ? h->r900_slots : 0;
         r900_mark_kernel<<<(unsigned)h->sm_count, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->d_slot_block,
-                                              h->r900_slots, h->d_slot_count);
+                                              slots, h->d_slot_count);
         CUDA_TRY(h, cudaGetLastError());
-        // the two-warp pipeline loads 8 samples (16 bytes) at a time: chain starts and the call's bytes must be 16-byte aligned
-        const bool vec_ok = (reinterpret_cast<uintptr_t>(d_iq) & 15u) == 0 && (reinterpret_cast<uintptr_t>(hist) & 15u) == 0 &&
-                            c.BUF % 8 == 0 && c.BS % 8 == 0 && c.hist_samples % 8 == 0;
-        if (h->r900_chain_mode == 2) {
-            r900_chain_kernel<true><<<(unsigned)h->sm_count * 16, kR900ChainWarps * 32, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c,
-                                                                       h->d_slot_block, h->r900_slots, h->d_slot_count,
-                                                                       h->r900_span, h->d_r900_scratch);
-        } else if (h->r900_chain_mode == 1 || !vec_ok) {
-            r900_chain_kernel<false><<<(unsigned)h->sm_count * 16, kR900ChainWarps * 32, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c,
-                                                                       h->d_slot_block, h->r900_slots, h->d_slot_count,
-                                                                       h->r900_span, h->d_r900_scratch);
-        } else {   // default: producer warps + one consumer warp per 16 chains, hand-offs through shared memory
+        if (h->r900_vec) {   // producer warps + one consumer warp per 16 chains, hand-offs through shared memory
             r900_chain2_kernel<<<(unsigned)h->sm_count * 2, (kChainProducers + 1) * 32, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, c, h->d_slot_block,
-                                                        h->r900_slots, h->d_slot_count, h->r900_span, h->d_r900_scratch);
+                                                        slots, h->d_slot_count, h->r900_span, h->d_r900_scratch);
+            CUDA_TRY(h, cudaGetLastError());
+            r900_digits_kernel<<<(unsigned)h->sm_count * 16, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->r900_span,
+                                                        h->d_r900_scratch, h->d_digits);
+            CUDA_TRY(h, cudaGetLastError());
+            h->launches += 2;
+            h->kernels += ";r900_chain2_kernel";
+        } else {
+            h->kernels += ";r900_replay_kernel";
         }
-        CUDA_TRY(h, cudaGetLastError());
-        r900_digits_kernel<<<(unsigned)h->sm_count * 16, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->r900_span,
-                                                    h->d_r900_scratch, h->d_digits);
-        CUDA_TRY(h, cudaGetLastError());
         // blocks that found no scratch slot: exact per-candidate replay
         r900_replay_kernel<<<(unsigned)h->sm_count, 64, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c, h->d_hits,
-                                               h->cand_cap, h->d_counters, h->d_block_slot, h->d_digits, h->d_slot_count, h->r900_slots);
+                                               h->cand_cap, h->d_counters, h->d_block_slot, h->d_digits, h->d_slot_count, slots);
         CUDA_TRY(h, cudaGetLastError());
-        h->launches += 4;
+        h->launches += 2;
         digits = h->d_digits;
     }
 
@@ -428,16 +424,19 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
         ca.nsamples = nblocks * c.BS;
         const unsigned grid = (unsigned)h->sm_count * 4;
         const bool dep = pdl && !h->has_r900;   // the r900 kernels between Search and Slice are ordinary launches
+        constexpr int kFullK = (ERTGPU_MAX_PACKET_BYTES * 8 + 31) / 32;
         if (c.PK <= 128)
             CUDA_TRY(h, launch_dep(dep, extract_words_kernel<4>, dim3(grid), dim3(kExtractWarps * 32), 0, st, (const uint32_t*)plane, p0, c,
                                    (const HitWord*)h->d_words, h->cand_cap, (const uint16_t*)h->d_crc, h->gf, digits, (long long)h->block_counter,
                                    flags, h->d_out, h->cand_cap, h->d_counters, ca));
         else
-            CUDA_TRY(h, launch_dep(dep, extract_words_kernel<(ERTGPU_MAX_PACKET_BYTES * 8 + 31) / 32>, dim3(grid), dim3(kExtractWarps * 32), 0,
+            CUDA_TRY(h, launch_dep(dep, extract_words_kernel<kFullK>, dim3(grid), dim3(kExtractWarps * 32), 0,
                                    st, (const uint32_t*)plane, p0, c, (const HitWord*)h->d_words, h->cand_cap, (const uint16_t*)h->d_crc, h->gf,
                                    digits, (long long)h->block_counter, flags, h->d_out, h->cand_cap, h->d_counters, ca));
         CUDA_TRY(h, cudaGetLastError());
         h->launches++;
+        snprintf(kname, sizeof(kname), ";extract_words_kernel<%d>", c.PK <= 128 ? 4 : kFullK);
+        h->kernels += kname;
     }
 
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[3], st));
@@ -653,7 +652,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     d.hist_samples = d.PKL;
     d.packet_bytes = c.packet_bytes;
     d.nproto = (int32_t)h->protos.size();
-    std::vector<uint16_t> tables, pos_tables;
+    std::vector<uint16_t> tables;
     h->has_r900 = false;
     for (int i = 0; i < d.nproto; i++) {
         const ertgpu_protocol& p = h->protos[i];
@@ -679,28 +678,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
         dp.table = i;
         tables.resize((size_t)(i + 1) * 256);
         make_crc_table(p.crc_poly, tables.data() + (size_t)i * 256);
-        {
-            const uint16_t* tb = tables.data() + (size_t)i * 256;
-            auto add_pos = [&](int n, int32_t* base, int32_t* cnt, uint16_t* k) {
-                *base = (int32_t)(pos_tables.size() / 256);
-                *cnt = n;
-                for (int pp = 0; pp < n; pp++)
-                    for (int v = 0; v < 256; v++) {
-                        uint16_t crc = tb[v];                       // byte v processed with a zero register
-                        for (int z = 0; z < n - 1 - pp; z++) crc = (uint16_t)((crc << 8) ^ tb[crc >> 8]);
-                        pos_tables.push_back(crc);
-                    }
-                uint16_t crc = p.crc_init;                          // CRC(init, n zero bytes)
-                for (int z = 0; z < n; z++) crc = (uint16_t)((crc << 8) ^ tb[crc >> 8]);
-                *k = crc;
-            };
-            if (p.check_kind == ERTGPU_CHECK_CRC16) add_pos(p.crc_to - p.crc_from, &dp.pos_base, &dp.pos_n, &dp.pos_k);
-            if (p.check_kind == ERTGPU_CHECK_IDM) {
-                dp.crc_from = 4;
-                add_pos(88, &dp.pos_base, &dp.pos_n, &dp.pos_k);
-                add_pos(6, &dp.pos2_base, &dp.pos2_n, &dp.pos2_k);
-            }
-        }
+        if (p.check_kind == ERTGPU_CHECK_IDM) dp.crc_from = 4;   // the IDM screen's first CRC starts at byte 4 whatever crc_from says (idm.go:77-87)
         if (p.check_kind == ERTGPU_CHECK_R900) {
             d.pre_has_r900[found] = 1;
             h->has_r900 = true;
@@ -738,9 +716,6 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     CUDA_TRY(h, cudaMemcpy(h->d_lut, h->h_lut, 256 * sizeof(float), cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMalloc(&h->d_crc, tables.size() * sizeof(uint16_t)));
     CUDA_TRY(h, cudaMemcpy(h->d_crc, tables.data(), tables.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMalloc(&h->d_crc_pos, std::max<size_t>(pos_tables.size(), 256) * sizeof(uint16_t)));
-    if (!pos_tables.empty())
-        CUDA_TRY(h, cudaMemcpy(h->d_crc_pos, pos_tables.data(), pos_tables.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
 
     h->plane_words = (size_t)d.hist_words + (size_t)max_blocks_per_call * d.words_per_block + kSearchTile + kSearchMaxHalo + kSlideMaxLoad + 8;
     for (int k = 0; k < 2; k++) {
@@ -756,6 +731,9 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
         CUDA_TRY(h, cudaMalloc(&h->d_digits, h->cand_cap * ERTGPU_R900_DIGITS));
         h->r900_span = d.BS + d.PL - d.SL + 4 * ERTGPU_R900_DIGITS * d.CL + 1;
         if (h->r900_span > d.BUF + 1) h->r900_span = d.BUF + 1;
+        // BS is a power of two >= 32 and the call's bytes are 16-byte aligned: chain starts (b + 1) * BS - BUF are
+        // multiples of 8 samples when PKL is (BUF = PKL + BS, the history holds PKL samples)
+        h->r900_vec = d.PKL % 8 == 0;
         // scratch slots: one per block that holds an r900 hit.  Sized for one packet per 16 blocks
         // (at least 64 slots), at most 1 GiB; blocks beyond that use the per-candidate replay.
         {
@@ -776,10 +754,6 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     CUDA_TRY(h, cudaMalloc(&h->d_tap, h->tap_floats * sizeof(float)));
 
     h->demod_variant = demod_fast_variant(d.CL, d.BS);
-    if (const char* e = getenv("ERTGPU_FAST_WARPS")) h->demod_warps = atoi(e);   // 100 * VAR + W, see launch_demod_fast
-    if (const char* e = getenv("ERTGPU_SEARCH_LEGACY")) h->search_legacy = atoi(e) != 0;
-    if (const char* e = getenv("ERTGPU_PDL")) h->use_pdl = atoi(e) != 0;
-    if (const char* e = getenv("ERTGPU_R900_CHAIN")) h->r900_chain_mode = strcmp(e, "shfl") == 0 ? 2 : (strcmp(e, "smem") == 0 ? 1 : 0);
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->device);
     if (h->sm_count < 1) h->sm_count = 132;
     h->cur_plane = h->cur_hist = 0;

@@ -25,7 +25,7 @@ namespace ert {
 // ---- Search, per-bit-load form -------------------------------------------------------------
 //
 // (The kernel for geometries the sliding-window kernel further down does not cover -- SL % 16 != 0 such as
-// chip length 78, preambles shorter than 16 bits -- and the cross-check of that kernel, ERTGPU_SEARCH_LEGACY=1.)
+// chip length 78, SL outside [64, 192], preambles shorter than 16 bits.)
 // A CTA stages a tile of the bit-plane (kSearchTile words of start positions + the halo the last
 // preamble bit reaches) in shared memory; a thread then tests 32 consecutive start positions at a
 // time.  For preamble bit k every start of the word looks at the SAME relative window: word offset
@@ -607,9 +607,9 @@ extract_words_kernel(const uint32_t* __restrict__ plane, long long p0, const __g
 // reads 42 digits at payload + k*4*CL, payload = Idx + PL - SL (r900.go:187-193).  All candidates of
 // one block therefore share one chain, and only its first r900_span = BS + PL - SL + 168*CL + 1 running
 // sums can ever be read.  Three small kernels: (1) give every block that has an r900 hit a scratch
-// slot, (2) one WARP per slot rebuilds the chain -- lanes fetch 32 magnitudes in parallel, lane 0 adds
-// them in the reference's order -- (3) one thread per (hit, digit) evaluates the three 4-chip
-// correlators.  Blocks beyond the scratch capacity fall back to r900_replay_kernel.
+// slot, (2) r900_chain2_kernel rebuilds the chain of every slot, (3) one thread per (hit, digit)
+// evaluates the three 4-chip correlators.  Blocks beyond the scratch capacity, and every block of a
+// geometry whose chain starts are not multiples of 8 samples, fall back to r900_replay_kernel.
 
 // Scratch row of a slot: csum[i] sits at row[i] with row = base + slot * pitch + 3, so that csum[1], csum[5], ... are 16-byte
 // aligned (the chain kernel stores four running sums per instruction; csum[0] = 0 is never produced by an add).
@@ -640,90 +640,11 @@ __global__ void r900_mark_kernel(DevCfg cfg, const RawHit* __restrict__ hits, un
     }
 }
 
-constexpr int kR900ChainWarps = 4;
-
-// SHFL: the 32 magnitudes of a group stay in the lanes' registers and every lane runs the same left-to-right
-// sum over shuffled values, keeping the prefix that belongs to it -- no shared-memory round trip, no divergent
-// single-lane section, no warp barriers (same additions in the same order: identical sums).
-template <bool SHFL>
-__global__ void __launch_bounds__(kR900ChainWarps * 32)
-r900_chain_kernel(const uint8_t* __restrict__ iq, const uint8_t* __restrict__ hist, int hist_samples, int hist_valid,
-                  const float* __restrict__ lut_g, DevCfg cfg, const int* __restrict__ slot_block, int slot_cap,
-                  const unsigned int* __restrict__ slot_count, int span, float* __restrict__ scratch) {
-    __shared__ float lut[256];
-    __shared__ __align__(16) float mbuf[kR900ChainWarps][32];
-    for (int i = threadIdx.x; i < 256; i += blockDim.x) lut[i] = lut_g[i];
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned int nslots = *slot_count;
-    if (nslots > (unsigned)slot_cap) nslots = (unsigned)slot_cap;
-    for (unsigned int slot = blockIdx.x * kR900ChainWarps + warp; slot < nslots; slot += gridDim.x * kR900ChainWarps) {
-        const long long b = slot_block[slot];
-        const long long first = (b + 1) * cfg.BS - cfg.BUF;  // sample of the parser's signal[0]
-        float* out = r900_row(scratch, slot, span);   // out[i] = csum[i], i in [0, span)
-        float s = 0.0f;
-        if (lane == 0) out[0] = 0.0f;
-        // raw IQ is fetched kR900Ahead groups ahead of the sequential adds (global-load latency).  Two things keep
-        // the loads really in flight for an in-order warp: the table lookups wait until the group is consumed,
-        // and the registers rotate by unrolling (a register move out of a pending load would wait for it).
-        constexpr int kR900Ahead = 8;
-        uint32_t rq[kR900Ahead];
-#pragma unroll
-        for (int a = 0; a < kR900Ahead; a++)
-            rq[a] = (a * 32 + 1 < span) ? raw_at(iq, hist, hist_samples, hist_valid, first + a * 32 + lane) : 0x10000u;
-        for (int base0 = 0; base0 + 1 < span; base0 += 32 * kR900Ahead) {
-#pragma unroll
-            for (int a = 0; a < kR900Ahead; a++) {
-                const int base = base0 + a * 32;
-                if (base + 1 >= span) break;  // warp-uniform
-                const float mine_m = mag_of(rq[a], lut);
-                rq[a] = (base + kR900Ahead * 32 + 1 < span)
-                            ? raw_at(iq, hist, hist_samples, hist_valid, first + base + kR900Ahead * 32 + lane)
-                            : 0x10000u;
-                if constexpr (SHFL) {
-                    float acc = s, keep = 0.0f;
-#pragma unroll
-                    for (int k = 0; k < 32; k++) {          // strictly left to right, r900.go:97-99
-                        acc = __fadd_rn(acc, __shfl_sync(0xFFFFFFFFu, mine_m, k));
-                        keep = (lane == k) ? acc : keep;
-                    }
-                    s = acc;
-                    if (base + lane + 1 < span) out[base + lane + 1] = keep;
-                    continue;
-                }
-                mbuf[warp][lane] = mine_m;
-                __syncwarp();
-                if (lane == 0) {
-                    // 32 magnitudes into registers with vector loads, 32 dependent adds, vector stores back
-                    float4 v[8];
-                    float4* mv = reinterpret_cast<float4*>(&mbuf[warp][0]);
-#pragma unroll
-                    for (int k = 0; k < 8; k++) v[k] = mv[k];
-                    float acc = s;
-#pragma unroll
-                    for (int k = 0; k < 8; k++) {          // strictly left to right, r900.go:97-99
-                        acc = __fadd_rn(acc, v[k].x); v[k].x = acc;
-                        acc = __fadd_rn(acc, v[k].y); v[k].y = acc;
-                        acc = __fadd_rn(acc, v[k].z); v[k].z = acc;
-                        acc = __fadd_rn(acc, v[k].w); v[k].w = acc;
-                    }
-#pragma unroll
-                    for (int k = 0; k < 8; k++) mv[k] = v[k];
-                    s = acc;
-                }
-                __syncwarp();
-                if (base + lane + 1 < span) out[base + lane + 1] = mbuf[warp][lane];
-                __syncwarp();
-            }
-        }
-    }
-}
-
-// ---- the same chain, software-pipelined over two warps ---------------------------------------
+// ---- the chain, software-pipelined over producer and consumer warps ----------------------------
 //
 // A chain is span-1 (about 24 700) DEPENDENT float32 adds: its latency, not its work, is what the r900 path
 // pays (all chains of a call run concurrently).  One warp cannot both feed and run the serial section without
-// the feeding instructions sitting inside the dependent chain's issue stream (~10 cycles per add above).  Here a
+// the feeding instructions sitting inside the dependent chain's issue stream (~10 cycles per add).  Here a
 // CTA is two warps and kChainsPerCta chains:
 //  * the PRODUCER warp fetches IQ bytes kChainAhead units ahead, looks the magnitudes up and hands units of
 //    kChainUnit samples per chain through a shared-memory ring; afterwards it streams the finished running sums

@@ -10,12 +10,11 @@
 template <int CL>
 void row(bool first) {
     using G = ert::FastGeom<CL>;
-    using G3 = ert::FastGeom<CL, 3>;
     const int W = ert::fast_warps<CL>();
     printf("%s{\"CL\":%d,\"L\":%d,\"pad\":%d,\"row_bytes\":%d,\"stages\":%d,\"warps\":%d,\"tail_bits\":%d,"
-           "\"smem\":%d,\"smem7\":%d,\"smem3\":%d,\"variant\":%d}",
+           "\"smem\":%d,\"smem7\":%d,\"variant\":%d}",
            first ? "" : ",", CL, G::L, G::kPad, G::kRowBytes, G::kStages, W, G::kTailBits,
-           ert::fast_smem_bytes<G>(W, 1024), ert::fast_smem_bytes<G>(W == 8 ? 7 : W, 1024), ert::fast_smem_bytes<G3>(W, 1024),
+           ert::fast_smem_bytes<G>(W, 1024), ert::fast_smem_bytes<G>(W == 8 ? 7 : W, 1024),
            ert::demod_fast_variant(CL, 4096));
 }
 

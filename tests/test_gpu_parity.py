@@ -106,17 +106,14 @@ def test_synthetic_candidates_match_oracle(built, mt, cl, variant):
     h.close()
 
 
-def test_hybrid_magnitude_variant_is_bit_exact(built, monkeypatch, sample_iq):
-    """demod_fast<72, 8, HYBRID>: Q magnitude computed with two float constants instead of the LUT."""
-    monkeypatch.setenv("ERTGPU_FAST_WARPS", "108")
-    _variant_is_bit_exact(sample_iq)
-
-
-@pytest.mark.parametrize("knob", ["7", "8", "208", "408"])
-def test_demod_tuning_variants_are_bit_exact(built, monkeypatch, sample_iq, knob):
-    """Every variant of the headline kernel gives the same bits: resident warps, staging depth, ring length."""
-    monkeypatch.setenv("ERTGPU_FAST_WARPS", knob)
-    _variant_is_bit_exact(sample_iq)
+@pytest.mark.parametrize("knob", ["7", "8"])
+def test_demod_tuning_variants_are_bit_exact(built, sample_iq, knob):
+    """The headline kernel gives the same bits with 7 and with 8 resident warps.  The call size picks the count
+    (fast_round_cost): a call of a few work tiles runs 7 warps, one of exactly 8 x SMs tiles (one full round of
+    8 warps, where 7 would need a second round) runs 8."""
+    import torch
+    ntiles = None if knob == "7" else 8 * torch.cuda.get_device_properties(0).multi_processor_count
+    _variant_is_bit_exact(sample_iq, f"demod_fast_kernel<72,{knob}>", ntiles)
 
 
 def test_register_ring_default_is_bit_exact(built, sample_iq):
@@ -124,7 +121,10 @@ def test_register_ring_default_is_bit_exact(built, sample_iq):
     _variant_is_bit_exact(sample_iq)
 
 
-def _variant_is_bit_exact(sample_iq):
+def _variant_is_bit_exact(sample_iq, kernel=None, ntiles=None):
+    """Synthetic, sample and uniform-random bytes against the oracle.  ntiles: tile each source to that many demod
+    work tiles (32 blocks each) and decode it in one device-resident call; kernel: the demod instance that must run."""
+    import torch
     mt, cl = "scm", 72
     for src in ("synthetic", "sample", "extremes"):
         if src == "synthetic":
@@ -133,50 +133,91 @@ def _variant_is_bit_exact(sample_iq):
             iq = sample_iq
         else:
             iq = np.random.default_rng(3).integers(0, 256, 1 << 21, dtype=np.uint8)   # every byte value, uniformly
-        o, cands, msgs = oracle_run(mt, cl, iq, oracle.SEARCH_EXACT)
-        h = capi.new_decoder(mt, cl)
-        iqb = whole_blocks(iq, h.cfg.block_size2)
-        got = h.decode(iqb)
+        if ntiles is None:
+            h = capi.new_decoder(mt, cl)
+            iqb = whole_blocks(iq, h.cfg.block_size2)
+            got = h.decode(iqb)
+        else:
+            h = capi.new_decoder(mt, cl, max_blocks_per_call=32 * ntiles, max_candidates=1 << 20)
+            src_b = whole_blocks(iq, h.cfg.block_size2)
+            reps = -(-32 * ntiles * h.cfg.block_size2 // src_b.size)
+            iqb = np.tile(src_b, reps)[: 32 * ntiles * h.cfg.block_size2]
+            d = torch.from_numpy(iqb).cuda()
+            h.decode_device_async(d.data_ptr(), d.numel(), 0, torch.cuda.current_stream().cuda_stream)
+            got = h.fetch(1 << 20)
+        o, cands, msgs = oracle_run(mt, cl, iqb, oracle.SEARCH_EXACT)
         compare_candidates(h, got, o, cands)
         last = iqb.size // h.cfg.block_size2 - 1
         assert np.array_equal(h.tap(capi.TAP_QUANTIZED, last), o.quantized())
+        if kernel is not None:
+            assert h.demod_kernel_name() == kernel, (src, h.last_kernels())
         h.close()
 
 
-@pytest.mark.parametrize("mt,cl", [("scm", 72), ("scm,scm+,idm", 72), ("r900", 72), ("scm", 64)])
-def test_legacy_search_kernel_agrees(built, monkeypatch, mt, cl):
-    """ERTGPU_SEARCH_LEGACY=1: the per-bit-load Search kernel finds the same candidates as the sliding-window one
-    (both are compared with the oracle's list)."""
+# Search instance each geometry reaches by default (prefix of the second entry of last_kernels()): the sliding-window
+# kernel for the stock geometries; search_kernel<NPRE, MODE> where it does not fit (SL % 16 != 0, SL outside
+# [64, 192]); search_generic_kernel where the halo of search_kernel is too large
+SEARCH_KERNEL = {("scm", 72): "search_slide_kernel<1,true,0xF953u",    # SL 144: odd bits half a word in
+                 ("scm,scm+,idm", 72): "search_slide_kernel<3,true,0xF953u",
+                 ("r900", 72): "search_slide_kernel<1,true,0x0000u",
+                 ("scm", 64): "search_slide_kernel<1,false,0xF953u",   # SL 128
+                 ("scm", 78): "search_kernel<1,0>",         # SL 156: SL % 16 != 0, SL % 32 == 28
+                 ("scm", 16): "search_kernel<1,1>",         # SL 32 < 64, first start word aligned
+                 ("scm", 24): "search_kernel<1,2>",         # SL 48 < 64, SL % 32 == 16
+                 ("idm", 100): "search_generic_kernel"}     # SL 200: a 32-bit preamble's halo of 195 words is too large
+
+
+@pytest.mark.parametrize("mt,cl", list(SEARCH_KERNEL))
+def test_legacy_search_kernel_agrees(built, mt, cl):
+    """Every Search kernel finds the oracle's candidates on a geometry that reaches it by default."""
     iq, _, _ = synth_stream(mt, cl, 1 << 21, spacing=1 << 18)
     o, cands, msgs = oracle_run(mt, cl, iq)
     assert len(cands) > 0
-    for legacy in ("1", "0"):
-        monkeypatch.setenv("ERTGPU_SEARCH_LEGACY", legacy)
-        h = capi.new_decoder(mt, cl)
-        got = h.decode(whole_blocks(iq, h.cfg.block_size2))
-        compare_candidates(h, got, o, cands)
-        h.close()
+    h = capi.new_decoder(mt, cl)
+    got = h.decode(whole_blocks(iq, h.cfg.block_size2))
+    assert h.last_kernels().split(";")[1].startswith(SEARCH_KERNEL[(mt, cl)]), h.last_kernels()
+    compare_candidates(h, got, o, cands)
+    h.close()
 
 
 @pytest.mark.parametrize("mt,cl", [("r900", 72), ("scm,scm+,idm,r900", 72), ("r900bcd", 32)])
-def test_r900_chain_shuffle_form_agrees(built, monkeypatch, mt, cl):
-    """ERTGPU_R900_CHAIN=shfl: the r900 running sum with the serial adds done over shuffled registers (every
-    lane the same left-to-right sum) returns records identical to the shared-memory form -- digits, syndrome
-    verdicts and all -- and the candidate list of the oracle; the shared-memory form's digits are compared with
-    the oracle's quantized buffer in test_r900_digits_and_tap."""
+def test_r900_chain_shuffle_form_agrees(built, mt, cl):
+    """The r900 running sums of the producer / consumer chain kernel give the oracle's candidate list with digits that
+    pass the syndrome screen; its digits are compared with the oracle's quantized buffer in test_r900_digits_and_tap."""
     iq, _, _ = synth_stream(mt, cl, 1 << 21, spacing=1 << 18)
     o, cands, msgs = oracle_run(mt, cl, iq)
-    out = {}
-    for form in ("shfl", "smem", "pipe"):     # pipe = the default producer / consumer chain
-        monkeypatch.setenv("ERTGPU_R900_CHAIN", form)
-        h = capi.new_decoder(mt, cl)
-        got = h.decode(whole_blocks(iq, h.cfg.block_size2))
-        compare_candidates(h, got, o, cands)
-        out[form] = np.sort(got, order=["block", "idx", "preamble_id"])
-        h.close()
-    assert (out["shfl"]["flags"] & capi.CAND_HAS_R900).any()
-    assert out["shfl"].tobytes() == out["smem"].tobytes() == out["pipe"].tobytes()
-    assert (out["shfl"]["check_mask"] != 0).any()
+    h = capi.new_decoder(mt, cl)
+    got = h.decode(whole_blocks(iq, h.cfg.block_size2))
+    assert "r900_chain2_kernel" in h.last_kernels().split(";"), h.last_kernels()
+    compare_candidates(h, got, o, cands)
+    assert (got["flags"] & capi.CAND_HAS_R900).any()
+    assert (got["check_mask"] != 0).any()
+    h.close()
+
+
+def test_r900_replay_when_packet_length_is_not_a_multiple_of_8(built):
+    """r900 with 118 packet symbols at chip length 73 (PacketLength 17 228 samples): the chain starts are not 16-byte
+    aligned, so every block takes the exact per-candidate replay.  Its digits are the r900 parser's quantized buffer."""
+    mt, cl = "r900", 73
+    p = capi.stock_protocol(mt, cl)
+    p.packet_symbols = 118
+    h = capi.Handle()
+    h.register(p)
+    h.allocate()
+    assert h.cfg.packet_length % 8 != 0
+    iq, _, _ = synth_stream(mt, cl, 1 << 21, spacing=1 << 18)
+    got = h.decode(whole_blocks(iq, h.cfg.block_size2))
+    kernels = h.last_kernels().split(";")
+    assert "r900_replay_kernel" in kernels and "r900_chain2_kernel" not in kernels, kernels
+    assert len(got) > 0
+    taps = {}
+    for r in got:
+        assert r["flags"] & capi.CAND_HAS_R900
+        b = int(r["block"])
+        q = taps[b] if b in taps else taps.setdefault(b, h.tap(capi.TAP_R900_QUANTIZED, b))
+        payload = int(r["idx"]) + h.cfg.preamble_length - h.cfg.symbol_length
+        assert list(r["r900_digits"]) == [int(q[payload + k * 4 * cl]) for k in range(42)]
+    h.close()
 
 
 def test_r900_digits_and_tap(built):

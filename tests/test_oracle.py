@@ -154,7 +154,7 @@ def test_gf32_syndrome_of_encoded_r900_is_zero():
 
 
 def test_two_constant_reciprocal_reproduces_the_lut_division_exactly():
-    """demod_fast's HYBRID variant computes x = fl((127.5 - v) / 127.5) as fma(n, rhi, fl(n * rlo)).
+    """r900_chain2_kernel computes x = fl((127.5 - v) / 127.5) as fma(n, rhi, fl(n * rlo)).
     Exhaustive proof over the 256 byte values with exact rational arithmetic (a true single-rounding fma)."""
     from fractions import Fraction
 

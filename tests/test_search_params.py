@@ -111,9 +111,9 @@ def test_demod_fast_geometry(demod_geom):
         assert r["warps"] in (8, 12, 16) and r["stages"] == 2
         # registers are handed out per scheduler: 2 x L ring values + working set must fit the warp count
         assert 2 * L + 40 <= {8: 255, 12: 168, 16: 128}[r["warps"]]
-        for key in ("smem", "smem7", "smem3"):
+        for key in ("smem", "smem7"):
             assert r[key] <= 227 * 1024, (cl, key, r[key])
-        assert r["smem7"] <= r["smem"] <= r["smem3"]
+        assert r["smem7"] <= r["smem"]
     by = {r["CL"]: r for r in demod_geom}
     assert by[72]["L"] == 88 and by[72]["pad"] == 32 and by[72]["smem"] == 65536 + 65536 + 3 * 2 * 32 * 176 - 1024
 
