@@ -129,13 +129,17 @@ def _parse_filtered(self, cands, filterid: str = "", filtertype: str = "", uniqu
     return _messages(out, min(n, cap)), int(dup.value), int(flt.value)
 
 
+FORMATS = {"plain": 0, "csv": 1, "json": 2, "xml": 3}
+
+
 def _encode(self, cands, fmt: str = "plain", unix_seconds: int = 0, nanos: int = 0, offset: int = 0, length: int = 0,
             sample_file_is_devnull: bool = True) -> str:
-    """erthost_encode: every parsed message through the plain or csv encoder (flags.go:140-151) as one string of lines."""
+    """erthost_encode: every parsed message through the plain, csv, json or xml encoder (flags.go:140-170) as one string
+    of lines."""
     cands = np.ascontiguousarray(cands)
     cap = 1 << 22
     buf = C.create_string_buffer(cap)
-    n = self._L.erthost_encode(self._h, cands.ctypes.data, len(cands), 1 if fmt == "csv" else 0, unix_seconds, nanos, offset, length,
+    n = self._L.erthost_encode(self._h, cands.ctypes.data, len(cands), FORMATS[fmt], unix_seconds, nanos, offset, length,
                                1 if sample_file_is_devnull else 0, buf, cap)
     if n < 0 or n >= cap:
         raise RuntimeError("erthost_encode failed" if n < 0 else "encode buffer too small")

@@ -174,9 +174,10 @@ long long erthost_parse_filtered(erthost* h, const ertgpu_candidate* cands, long
     }
 }
 
-// The encoders (flags.go:140-151) on every message of erthost_parse: format 0 = plain (PlainEncoder, flags.go:261-272),
-// 1 = csv (csv/csv.go:27-38); the LogMessage fields (parse.go:103-109) are the caller's.  Returns the number of bytes the
-// lines need (they are written when they fit `cap`), or -1.
+// The encoders (flags.go:140-170) on every message of erthost_parse: format 0 = plain (PlainEncoder, flags.go:261-272),
+// 1 = csv (csv/csv.go:27-38), 2 = json (encoding/json), 3 = xml (encoding/xml + NewLineEncoder); the LogMessage fields
+// (parse.go:103-109) are the caller's.  Returns the number of bytes the lines need (they are written when they fit `cap`),
+// or -1.
 long long erthost_encode(erthost* h, const ertgpu_candidate* cands, long long n, int format, long long unix_seconds, int nanos,
                          long long offset, int length, int sample_file_is_devnull, char* buf, long long cap) {
     try {
@@ -190,7 +191,12 @@ long long erthost_encode(erthost* h, const ertgpu_candidate* cands, long long n,
             lm.Offset = offset;
             lm.Length = length;
             lm.Message = m.get();
-            all += format == 1 ? receiver::CsvLine(lm.Record()) : receiver::PlainLine(lm, sample_file_is_devnull != 0) + "\n";
+            switch (format) {
+            case 1: all += receiver::CsvLine(lm.Record()); break;
+            case 2: all += receiver::JsonLine(lm); break;
+            case 3: all += receiver::XmlLine(lm); break;
+            default: all += receiver::PlainLine(lm, sample_file_is_devnull != 0) + "\n";
+            }
         }
         if ((long long)all.size() < cap && buf) memcpy(buf, all.c_str(), all.size() + 1);
         return (long long)all.size();

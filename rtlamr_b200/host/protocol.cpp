@@ -35,6 +35,12 @@ std::string hexbytes(const uint8_t* p, size_t n) {  // fmt "%02X" applied to a [
 std::string u(uint64_t v) { return std::to_string(v); }
 std::string hex0x(uint64_t v) { return sprintf_str("0x%llx", (unsigned long long)v); }  // "0x"+FormatUint(v,16)
 
+using protocol::Field;
+Field fu(const char* name, uint64_t v, const char* attr = nullptr) { return Field{name, attr, Field::UINT, v, {}, {}}; }
+Field fattr(const char* name, uint64_t v) { return fu(name, v, name); }  // `xml:",attr"`
+Field fbytes(const char* name, const uint8_t* p, size_t n) { return Field{name, nullptr, Field::BYTES, 0, {p, p + n}, {}}; }
+Field fu16s(const char* name, const uint16_t* p, size_t n) { return Field{name, nullptr, Field::UINT16S, 0, {}, {p, p + n}}; }
+
 }  // namespace
 
 // ======================================================================= crc
@@ -157,6 +163,10 @@ struct SCM : Message {  // scm/scm.go:94-101
     std::vector<std::string> Record() const override {  // scm.go:145-154
         return {u(ID), u(Type), hex0x(TamperPhy), hex0x(TamperEnc), u(Consumption), hex0x(ChecksumVal)};
     }
+    std::vector<Field> Fields() const override {  // scm.go:94-101
+        return {fattr("ID", ID), fattr("Type", Type), fattr("TamperPhy", TamperPhy), fattr("TamperEnc", TamperEnc),
+                fattr("Consumption", Consumption), fu("ChecksumVal", ChecksumVal, "Checksum")};
+    }
 };
 
 struct SCMPlus : Message {  // scmplus/scmplus.go:94-102
@@ -174,6 +184,13 @@ struct SCMPlus : Message {  // scmplus/scmplus.go:94-102
     }
     std::vector<std::string> Record() const override {  // scmplus.go:141-151
         return {hex0x(FrameSync), hex0x(ProtocolID), hex0x(EndpointType), u(EndpointID), u(Consumption), hex0x(Tamper), hex0x(PacketCRC)};
+    }
+    // scmplus.go:94-102.  PacketCRC's tag `xml:"Checksum,attr",json:"Checksum"` has a comma where StructTag.Get wants a
+    // space: the xml key parses, the json key does not, so JSON keeps the Go name.
+    std::vector<Field> Fields() const override {
+        return {fattr("FrameSync", FrameSync), fattr("ProtocolID", ProtocolID), fattr("EndpointType", EndpointType),
+                fattr("EndpointID", EndpointID), fattr("Consumption", Consumption), fattr("Tamper", Tamper),
+                fu("PacketCRC", PacketCRC, "Checksum")};
     }
 };
 
@@ -221,6 +238,16 @@ struct IDM : Message {  // idm/idm.go:101-119
         r.push_back(sprintf_str("0x%04X", PacketCRC));
         return r;
     }
+    std::vector<Field> Fields() const override {  // idm.go:101-119, no tags
+        return {fu("Preamble", Preamble), fu("PacketTypeID", PacketTypeID), fu("PacketLength", PacketLength),
+                fu("HammingCode", HammingCode), fu("ApplicationVersion", ApplicationVersion), fu("ERTType", ERTType),
+                fu("ERTSerialNumber", ERTSerialNumber), fu("ConsumptionIntervalCount", ConsumptionIntervalCount),
+                fu("ModuleProgrammingState", ModuleProgrammingState), fbytes("TamperCounters", TamperCounters.data(), 6),
+                fu("AsynchronousCounters", AsynchronousCounters), fbytes("PowerOutageFlags", PowerOutageFlags.data(), 6),
+                fu("LastConsumptionCount", LastConsumptionCount),
+                fu16s("DifferentialConsumptionIntervals", DifferentialConsumptionIntervals.data(), 47),
+                fu("TransmitTimeOffset", TransmitTimeOffset), fu("SerialNumberCRC", SerialNumberCRC), fu("PacketCRC", PacketCRC)};
+    }
 };
 
 struct NetIDM : Message {  // netidm/netidm.go:112-129
@@ -256,6 +283,15 @@ struct NetIDM : Message {  // netidm/netidm.go:112-129
         r.push_back(sprintf_str("0x%04X", PacketCRC));
         return r;
     }
+    std::vector<Field> Fields() const override {  // netidm.go:112-129, no tags
+        return {fu("Preamble", Preamble), fu("ProtocolID", ProtocolID), fu("PacketLength", PacketLength),
+                fu("HammingCode", HammingCode), fu("ApplicationVersion", ApplicationVersion), fu("ERTType", ERTType),
+                fu("ERTSerialNumber", ERTSerialNumber), fu("ConsumptionIntervalCount", ConsumptionIntervalCount),
+                fu("ProgrammingState", ProgrammingState), fu("LastGeneration", LastGeneration), fu("LastConsumption", LastConsumption),
+                fu("LastConsumptionNet", LastConsumptionNet),
+                fu16s("DifferentialConsumptionIntervals", DifferentialConsumptionIntervals.data(), 27),
+                fu("TransmitTimeOffset", TransmitTimeOffset), fu("SerialNumberCRC", SerialNumberCRC), fu("PacketCRC", PacketCRC)};
+    }
 };
 
 struct R900 : Message {  // r900/r900.go:248-258
@@ -275,6 +311,11 @@ struct R900 : Message {  // r900/r900.go:248-258
     }
     std::vector<std::string> Record() const override {  // r900.go:291-302
         return {u(ID), u(Unkn1), u(NoUse), u(BackFlow), u(Consumption), u(Unkn3), u(Leak), u(LeakNow)};
+    }
+    // r900.go:248-258; `checksum` is unexported.  R900BCD embeds r900.R900 (r900bcd.go:39-41), so its fields are these.
+    std::vector<Field> Fields() const override {
+        return {fattr("ID", ID), fattr("Unkn1", Unkn1), fattr("NoUse", NoUse), fattr("BackFlow", BackFlow),
+                fattr("Consumption", Consumption), fattr("Unkn3", Unkn3), fattr("Leak", Leak), fattr("LeakNow", LeakNow)};
     }
 };
 

@@ -82,6 +82,17 @@ struct Data {
 };
 Data NewData(const uint8_t* data, size_t n);  // parse.go:61-69
 
+// One exported field of a message struct as encoding/json and encoding/xml see it through reflection.
+struct Field {
+    enum Kind { UINT, BYTES, UINT16S };  // uintN, []byte, [N]uint16
+    const char* Name;                    // Go field name; also the JSON key, since no message carries a json tag Go can parse
+    const char* XmlAttr;                 // attribute name of an `xml:"..,attr"` tag; nullptr for an untagged field (child element)
+    Kind kind;
+    uint64_t Uint = 0;
+    std::vector<uint8_t> Bytes;
+    std::vector<uint16_t> Uint16s;
+};
+
 // parse.go:78-84 (csv.Recorder folded in)
 struct Message {
     virtual ~Message() = default;
@@ -91,6 +102,7 @@ struct Message {
     virtual std::vector<uint8_t> Checksum() const = 0;
     virtual std::string String() const = 0;
     virtual std::vector<std::string> Record() const = 0;
+    virtual std::vector<Field> Fields() const = 0;  // exported fields in Go declaration order (embedded structs flattened)
     int64_t Block = 0;  // bookkeeping for the parity tests (not in the reference)
     int Idx = 0;
 };

@@ -1,6 +1,9 @@
 // receiver.cpp -- see receiver.hpp.
 #include "receiver.hpp"
 
+#include <algorithm>
+#include <cctype>
+#include <cerrno>
 #include <chrono>
 #include <cstring>
 #include <sstream>
@@ -45,45 +48,137 @@ void Receiver::Filter(std::vector<protocol::MessagePtr>& msgs, bool block_dedup,
 
 void BlockDedup::Filter(std::vector<protocol::MessagePtr>& msgs, bool block_dedup,
                         const std::function<void(const protocol::Message&)>& emit, Stats& st, FilterChain* fc) {
+    size_t i = 0;
+    while (i < msgs.size()) {
+        size_t j = i;
+        while (j < msgs.size() && msgs[j]->Block == msgs[i]->Block) j++;
+        FilterBlock(msgs.data() + i, j - i, block_dedup, [&](const protocol::Message& m) { emit(m); return true; }, st, fc);
+        i = j;
+    }
+}
+
+bool BlockDedup::FilterBlock(protocol::MessagePtr* msgs, size_t n, bool block_dedup,
+                             const std::function<bool(const protocol::Message&)>& emit, Stats& st, FilterChain* fc) {
     // main.go:221-224,244-260,292: `next` collects the digests of the current block, a message whose digest
     // was seen in the previous block is skipped, and the maps swap after every block -- including blocks
     // without messages, which is why a gap in the block numbers empties `prev`.
-    size_t i = 0;
-    while (i < msgs.size()) {
-        const int64_t b = msgs[i]->Block;
-        if (b != prev_block_ + 1) prev_.clear();
-        std::set<Digest> next;
-        for (; i < msgs.size() && msgs[i]->Block == b; i++) {
-            if (fc && !fc->Match(*msgs[i])) {   // main.go:236-239: rejected before the digest is recorded
-                st.filtered++;
-                continue;
-            }
-            Digest dg = NewDigest(*msgs[i]);
-            next.insert(dg);
-            if (block_dedup && prev_.count(dg)) {
-                st.duplicates++;
-                continue;
-            }
-            st.messages++;
-            emit(*msgs[i]);
+    if (!n) return true;
+    const int64_t b = msgs[0]->Block;
+    if (b != prev_block_ + 1) prev_.clear();
+    std::set<Digest> next;
+    bool go_on = true;
+    for (size_t i = 0; i < n && go_on; i++) {
+        if (fc && !fc->Match(*msgs[i])) {   // main.go:236-239: rejected before the digest is recorded
+            st.filtered++;
+            continue;
         }
-        prev_.swap(next);
-        prev_block_ = b;
+        Digest dg = NewDigest(*msgs[i]);
+        next.insert(dg);
+        if (block_dedup && prev_.count(dg)) {
+            st.duplicates++;
+            continue;
+        }
+        st.messages++;
+        go_on = emit(*msgs[i]);
     }
+    prev_.swap(next);
+    prev_block_ = b;
+    return go_on;
+}
+
+int64_t ParseDuration(const std::string& str) {   // time.ParseDuration
+    const auto bad = [&] { return std::invalid_argument("time: invalid duration \"" + str + "\""); };
+    std::string s = str;
+    bool neg = false;
+    if (!s.empty() && (s[0] == '-' || s[0] == '+')) {
+        neg = s[0] == '-';
+        s = s.substr(1);
+    }
+    if (s == "0") return 0;
+    if (s.empty()) throw bad();
+    static const std::pair<const char*, double> units[] = {{"ns", 1}, {"us", 1e3}, {"\xC2\xB5s", 1e3}, {"\xCE\xBCs", 1e3},
+                                                           {"ms", 1e6}, {"s", 1e9}, {"m", 60e9}, {"h", 3600e9}};
+    double total = 0;
+    size_t i = 0;
+    while (i < s.size()) {
+        const size_t num0 = i;
+        while (i < s.size() && isdigit((unsigned char)s[i])) i++;
+        const size_t int_digits = i - num0;
+        size_t frac_digits = 0;
+        if (i < s.size() && s[i] == '.') {
+            i++;
+            const size_t f0 = i;
+            while (i < s.size() && isdigit((unsigned char)s[i])) i++;
+            frac_digits = i - f0;
+        }
+        if (!int_digits && !frac_digits) throw bad();
+        const double v = std::stod("0" + s.substr(num0, i - num0));
+        const size_t u0 = i;
+        while (i < s.size() && s[i] != '.' && !isdigit((unsigned char)s[i])) i++;
+        const std::string unit = s.substr(u0, i - u0);
+        double scale = 0;
+        for (const auto& un : units)
+            if (unit == un.first) scale = un.second;
+        if (!scale) throw std::invalid_argument(unit.empty() ? "time: missing unit in duration \"" + str + "\""
+                                                             : "time: unknown unit \"" + unit + "\" in duration \"" + str + "\"");
+        total += v * scale;
+    }
+    if (total > 9.223372036854775807e18) throw bad();
+    return neg ? -(int64_t)total : (int64_t)total;
 }
 
 void Receiver::Reset() {
     d_.Reset();
     dedup_.Reset();
+    stream_blocks_ = 0;
+    history_.clear();
 }
 
-Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&)>& emit) {
+// Append block `block`'s sampleBuf to the sample file: blocks [block - sample_blocks_ + 1, block] of the stream,
+// clipped at its start.  Blocks from call_first on are in `call`, the earlier ones at the end of history_.
+void Receiver::DumpSampleBuf(const uint8_t* call, int64_t call_first, int64_t block) {
+    const size_t bs2 = (size_t)d_.Cfg.BlockSize2;
+    const int64_t first = std::max<int64_t>(0, block - sample_blocks_ + 1);
+    const int64_t hist_first = call_first - (int64_t)(history_.size() / bs2);
+    if (first < hist_first) throw std::logic_error("sample history lost a block");
+    size_t wrote = 0, want = (size_t)(block + 1 - first) * bs2;
+    if (first < call_first) {
+        const size_t from = (size_t)(first - hist_first) * bs2;
+        wrote += fwrite(history_.data() + from, 1, history_.size() - from, sample_file_);
+    }
+    const int64_t in_call = std::max(first, call_first);
+    wrote += fwrite(call + (size_t)(in_call - call_first) * bs2, 1, (size_t)(block + 1 - in_call) * bs2, sample_file_);
+    if (wrote != want) throw std::runtime_error(std::string("writing the sample file: ") + strerror(errno));
+    sample_offset_ += (int64_t)wrote;
+}
+
+// After a call: keep the stream's last (sample_blocks_ - 1) blocks, the part of a later block's sampleBuf that the
+// next call's buffer does not hold.
+void Receiver::KeepHistory(const uint8_t* call, size_t nblocks) {
+    const size_t bs2 = (size_t)d_.Cfg.BlockSize2;
+    const size_t keep = (size_t)(sample_blocks_ - 1) * bs2, n = nblocks * bs2;
+    if (n >= keep) {
+        history_.assign(call + n - keep, call + n);
+        return;
+    }
+    history_.insert(history_.end(), call, call + n);
+    if (history_.size() > keep) history_.erase(history_.begin(), history_.end() - (ptrdiff_t)keep);
+}
+
+Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&, int64_t, int)>& emit) {
     Stats st;
     const size_t bs2 = (size_t)d_.Cfg.BlockSize2;
+    // main.go:225-230: sampleBuf grows by one block per block until it holds more than BufferLength<<1 bytes
+    sample_blocks_ = 2 * (int64_t)d_.Cfg.BufferLength / (int64_t)bs2 + 1;
+    FilterChain* fc = fc_.empty() ? nullptr : &fc_;
     const auto t0 = std::chrono::steady_clock::now();
     int k = 0;
     size_t carry = 0;  // bytes of a partial block kept at the front of the next buffer
     for (;;) {
+        if (std::chrono::steady_clock::now() >= deadline_) {
+            st.stopped = true;
+            break;
+        }
         size_t have = carry;
         while (have < buf_bytes_) {
             const size_t n = fread(buf_[k] + have, 1, buf_bytes_ - have, in);
@@ -93,9 +188,31 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
         const size_t whole = have / bs2 * bs2;
         if (whole) {
             auto msgs = d_.Decode(buf_[k], whole);
-            st.blocks += (int64_t)(whole / bs2);
+            const int64_t call_first = stream_blocks_, nblocks = (int64_t)(whole / bs2);
+            st.blocks += nblocks;
             st.bytes += (int64_t)whole;
-            Filter(msgs, block_dedup, emit, st);
+            stream_blocks_ += nblocks;
+            for (size_t i = 0; i < msgs.size() && !st.stopped;) {
+                size_t j = i;
+                const int64_t b = msgs[i]->Block;
+                while (j < msgs.size() && msgs[j]->Block == b) j++;
+                const int64_t offset = sample_file_ ? sample_offset_ : 0;
+                const int length = sample_file_ ? (int)(std::min(b + 1, sample_blocks_) * (int64_t)bs2) : 0;
+                bool found = false;
+                dedup_.FilterBlock(msgs.data() + i, j - i, block_dedup, [&](const protocol::Message& m) {
+                    emit(m, offset, length);
+                    found = true;
+                    if (!single_) return true;
+                    if (!single_ids_ || single_ids_->empty()) return false;   // main.go:271-276
+                    single_ids_->erase(m.MeterID());
+                    return true;
+                }, st, fc);
+                if (found && sample_file_) DumpSampleBuf(buf_[k], call_first, b);   // main.go:279-284
+                if (found && single_ && (!single_ids_ || single_ids_->empty())) st.stopped = true;   // main.go:285-287
+                i = j;
+            }
+            if (st.stopped) break;
+            if (sample_file_) KeepHistory(buf_[k], (size_t)nblocks);
         }
         carry = have - whole;
         if (carry) memcpy(buf_[k ^ 1], buf_[k] + whole, carry);

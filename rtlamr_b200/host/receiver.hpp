@@ -4,10 +4,12 @@
 //   * the block reader (main.go:156-205) -- here it reads K*BlockSize2 bytes per iteration from a file or
 //     stdin into pinned host buffers (ertgpu_host_alloc) instead of one block from a TCP socket;
 //   * the decode loop (main.go:207-294) -- Decode, then the prev/next digest maps that drop a message
-//     already reported for the previous block (main.go:244-260,292).
+//     already reported for the previous block (main.go:244-260,292), the -samplefile dump of the last blocks
+//     (main.go:225-230,279-284), -single (main.go:269-287) and -duration (main.go:350-353).
 // Whole blocks only: a trailing partial block is never decoded (main.go:166-186).
 #pragma once
 
+#include <chrono>
 #include <cstdio>
 #include <functional>
 #include <set>
@@ -27,7 +29,11 @@ Digest NewDigest(const protocol::Message& m);
 struct Stats {
     int64_t blocks = 0, bytes = 0, messages = 0, duplicates = 0, filtered = 0;
     double seconds = 0;
+    bool stopped = false;  // -single or -duration ended the run: nothing after it is read
 };
+
+// Go duration syntax (time.ParseDuration: "500ms", "1h5m10s", "-1.5h", "0") in nanoseconds; throws invalid_argument.
+int64_t ParseDuration(const std::string& s);
 
 // The receive loop's prev/next digest maps (main.go:221-224,244-260,292) on their own: a message whose digest was
 // reported for the previous block is dropped; a gap in the block numbers empties the memory.
@@ -37,6 +43,10 @@ public:
     // receive loop's filter chain (main.go:236-239): a message it rejects is skipped BEFORE its digest is recorded.
     void Filter(std::vector<protocol::MessagePtr>& msgs, bool block_dedup,
                 const std::function<void(const protocol::Message&)>& emit, Stats& st, FilterChain* fc = nullptr);
+    // The same for the n messages of ONE block.  `emit` returns false to drop the rest of the block (-single's `break`,
+    // main.go:275-277); FilterBlock then returns false too.
+    bool FilterBlock(protocol::MessagePtr* msgs, size_t n, bool block_dedup,
+                     const std::function<bool(const protocol::Message&)>& emit, Stats& st, FilterChain* fc = nullptr);
     void Reset() {
         prev_.clear();
         prev_block_ = -2;
@@ -56,11 +66,27 @@ public:
     protocol::Decoder& decoder() { return d_; }
     FilterChain& filters() { return fc_; }   // -filterid / -filtertype / -unique (flags.go:147-170)
 
-    // Run over a FILE* until EOF.  `emit` is called once per reported message (after the cross-block dedup when block_dedup).
-    Stats Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&)>& emit);
+    // -samplefile (main.go:225-230,279-284): after every block with at least one reported message, the receive loop's
+    // sampleBuf -- the last blocks of the stream, one dropped from the front before a block is appended once it holds
+    // more than BufferLength<<1 bytes -- is appended to `f`.  Every message of that block carries Offset = the file's
+    // size before the dump and Length = sampleBuf's size.  The file is shared by all streams of a batch.
+    void SetSampleFile(FILE* f) { sample_file_ = f; }
+    // -single (main.go:269-287).  ids == nullptr (no -filterid): stop after the first reported message.  Otherwise each
+    // reported meter ID is erased from `ids` -- the set the chain's MeterIDFilter reads -- and the run stops at the end of
+    // the block that empties it.
+    void SetSingle(UintMap* ids) {
+        single_ = true;
+        single_ids_ = ids;
+    }
+    // -duration: checked before every read, so a call already read is decoded and reported in full.
+    void SetDeadline(std::chrono::steady_clock::time_point t) { deadline_ = t; }
+
+    // Run over a FILE* until EOF, -single or the deadline.  `emit` is called once per reported message (after the
+    // cross-block dedup when block_dedup) with its LogMessage Offset and Length (0 without a sample file).
+    Stats Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&, int64_t, int)>& emit);
 
     // Start a new, independent stream (the next file of a batch): zeroed Decoder history (decode.go:144-145),
-    // block numbers restart at 0, empty dedup set.
+    // block numbers restart at 0, empty dedup set, empty sampleBuf.
     void Reset();
 
     // The dedup step on one Decode result (messages grouped by ascending Block), exposed for tests.
@@ -74,6 +100,18 @@ private:
     size_t buf_bytes_ = 0;
     BlockDedup dedup_;
     FilterChain fc_;
+
+    FILE* sample_file_ = nullptr;
+    int64_t sample_offset_ = 0;       // bytes written to sample_file_
+    int64_t sample_blocks_ = 0;       // how many blocks sampleBuf holds once full
+    int64_t stream_blocks_ = 0;       // blocks decoded since Reset
+    std::vector<uint8_t> history_;    // the stream's last (sample_blocks_ - 1) blocks before the current call
+    bool single_ = false;
+    UintMap* single_ids_ = nullptr;
+    std::chrono::steady_clock::time_point deadline_ = std::chrono::steady_clock::time_point::max();
+
+    void DumpSampleBuf(const uint8_t* call, int64_t call_first, int64_t block);
+    void KeepHistory(const uint8_t* call, size_t nblocks);
 };
 
 }  // namespace receiver
