@@ -224,13 +224,30 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
         for (int j = 0; j < L; j++) { cr[j] = 0.0f; ar[j] = 0.0f; }
         uint32_t acc = 0;   // pending output bits (low nacc bits), still as SIGN bits (inverted at store)
         int nacc = 0;       // warp-uniform
+        uint32_t ow0 = 0, ow1 = 0, ow2 = 0;  // the last words of the current 16-byte output group
+        uint4 pend = make_uint4(0, 0, 0, 0); // the group that fills the first half of the current 32-byte sector
+        // Each lane writes its own row, so every store of the warp touches 32 lines.  The 16-byte groups go out a
+        // whole 32-byte sector at a time (two stores back to back): with lone 16-byte stores (half sectors) the 1 GiB
+        // scm demod took 9 % longer on H100.  The rows may start in the middle of a sector (r900's plane history is
+        // 16 mod 32 bytes), so which groups share a sector is read from the plane's base address (ph = 4: group 0
+        // is a second half).  A row of BS/32 words is a whole number of sectors for every block size >= 256; with a
+        // row of 4 mod 8 words the odd rows would pair across sectors, slower but storing the same words.  A group
+        // is stored iff its last word is < wlimit.
         int wi = 0;
         const int wlimit = live ? wpb : 0;   // words this lane may store
-        uint32_t ow0 = 0, ow1 = 0, ow2 = 0;  // the last words of the current 16-byte output group
         uint4* const out4 = reinterpret_cast<uint4*>(plane_out + b * wpb);
-        // one 16-byte store per 4 words: 4x fewer L1 wavefronts than word stores (each lane hits its own line)
+        auto ph = [&]() { return (int)((uint32_t)reinterpret_cast<uintptr_t>(plane_out) >> 2) & 4; };   // warp-uniform
         auto put = [&](uint32_t o) {
-            if ((wi & 3) == 3 && wi < wlimit) out4[wi >> 2] = make_uint4(~ow0, ~ow1, ~ow2, ~o);
+            if ((wi & 3) == 3) {
+                const uint4 q = make_uint4(~ow0, ~ow1, ~ow2, ~o);
+                if ((wi ^ ph()) & 4) {   // second half: the sector is complete
+                    // (unsigned): no first half in front of group 0
+                    if ((unsigned)(wi - 4) < (unsigned)wlimit) out4[(wi >> 2) - 1] = pend;
+                    if (wi < wlimit) out4[wi >> 2] = q;
+                } else {
+                    pend = q;
+                }
+            }
             ow0 = ow1; ow1 = ow2; ow2 = o;
             wi++;
         };
@@ -354,6 +371,10 @@ demod_fast_kernel(const __grid_constant__ CUtensorMap iq_map, const uint8_t* __r
         };
         if (tile == 0) run_tile(std::true_type{});
         else run_tile(std::false_type{});
+        {   // the last whole group, if it is a first half still waiting for the rest of its sector
+            const int g = (wi >> 2) - 1;
+            if (g >= 0 && !(((4 * g) ^ ph()) & 4) && 4 * g + 3 < wlimit) out4[g] = pend;
+        }
         __syncwarp();
         npref = npref_next;
         tile = next_tile;
