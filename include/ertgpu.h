@@ -110,8 +110,20 @@ typedef struct {
 #define ERTGPU_TAP_QUANTIZED 2 /* uint8[BUF]       Decoder.Quantized after block b (decode.go:145,166,243) */
 #define ERTGPU_TAP_PACKED 3    /* uint8[(BS+PL+7)>>3] Decoder.packed after block b (decode.go:159,259-265) */
 #define ERTGPU_TAP_R900_QUANTIZED 4 /* uint8[BUF]  r900 Parser.quantized after block b (r900/r900.go:82-150) */
+#define ERTGPU_TAP_RESAMPLED 5 /* uint8[BlockSize2] the resampled IQ bytes of block b as the decoder read them (handles with an input rate) */
 
 typedef struct ertgpu_handle ertgpu_handle;
+
+/* The input-rate resampler of a handle (ertgpu_set_input_rate; include/ertgpu_resample.h has the
+ * arithmetic).  Output rate R_out = DataRate * ChipLength; R_out / R_in = L / M reduced. */
+typedef struct {
+    int64_t rate_in, rate_out;
+    int64_t L, M;
+    int32_t T;  /* taps per output sample                      */
+    int32_t P;  /* table sub-phases per input sample            */
+    int32_t S;  /* DC gain of every coefficient set is 2^S      */
+    int32_t F;  /* bits of the sub-phase interpolation weight   */
+} ertgpu_resampler_info;
 
 /* ---- lifecycle -------------------------------------------------------- */
 
@@ -139,9 +151,30 @@ int ertgpu_allocate(ertgpu_handle *h, int32_t device, int64_t max_blocks_per_cal
 /* Decoder.Cfg (decode.go:46), valid after ertgpu_allocate. */
 int ertgpu_get_config(const ertgpu_handle *h, ertgpu_decoder_config *cfg);
 
-/* Forget the stream history (Signal tail, Quantized history, block counter):
- * the next decode behaves like the first Decode of a fresh Decoder. */
+/* Forget the stream history (Signal tail, Quantized history, block counter, and the
+ * resampler's input history and partial block): the next decode behaves like the first
+ * Decode of a fresh Decoder. */
 int ertgpu_reset(ertgpu_handle *h);
+
+/* Declare the sample rate of the IQ the handle will be fed (Hz), between the last
+ * ertgpu_register_protocol and ertgpu_allocate.  The decoder keeps its own rate
+ * R_out = DataRate * ChipLength (and its geometry, blocks, Idx and taps); when hz != R_out the
+ * input is converted to R_out by an exact integer resampler on the GPU, and Block / Idx refer to
+ * the resampled stream.  hz == R_out (or never calling this) changes nothing.  R_out / hz must
+ * lie in [1/4, 4], otherwise ERTGPU_EINVAL.  With resampling, ertgpu_decode and
+ * ertgpu_decode_device_async take any whole number of IQ samples (nbytes even, else
+ * ERTGPU_ESIZE): the handle carries the input history, the outputs still waiting for look-ahead
+ * and the partial output block across calls and decodes every whole block it has.
+ * ertgpu_decode_sharded rejects such handles (ERTGPU_EINVAL).  A call that completes no whole block
+ * runs only resample_kernel; ertgpu_last_kernels then keeps the list of the last call that ran the
+ * decoder (demod first, resample_kernel last). */
+int ertgpu_set_input_rate(ertgpu_handle *h, int64_t hz);
+
+/* The resampler of a handle with an input rate: *info, and the (P+1)*T int16 prototype table
+ * when table != NULL and cap (entries) is large enough; *n_out = number of table entries.
+ * ERTGPU_EINVAL when the handle does not resample. */
+int ertgpu_get_resampler(const ertgpu_handle *h, ertgpu_resampler_info *info, int16_t *table,
+                         size_t cap, size_t *n_out);
 
 void ertgpu_destroy(ertgpu_handle *h);
 

@@ -1,0 +1,153 @@
+/*
+ * ertgpu_resample.h -- the prototype lowpass of the input-rate resampler, as one header shared by
+ * libertgpu.so (rtlamr_b200/csrc/resample.cuh) and by the CPU restatement the tests check it
+ * against, so both use the same integer table.  Not part of the reference API: rtlamr decodes only
+ * at DataRate * ChipLength samples per second (protocol/decode.go:132-133).
+ *
+ * Resampling R_in -> R_out = L/M * R_in (L/M reduced, 1/4 <= L/M <= 4).  Output n sits at input
+ * time n*M/L: k_n = floor(n*M/L), phase phi_n = n*M mod L.  It reads the T input samples
+ * k_n - T/2 + 1 ... k_n + T/2 (samples before the stream start count as s = 0).
+ *
+ * The table holds the windowed-sinc prototype h(d) (d in input samples, h(-d) = h(d)) at P
+ * sub-phases per input sample:  table[p*T + t] = round(2^S * h(t - T/2 + 1 - p/P)) for p = 0..P
+ * (row P is the extra row for interpolation).  Every row sums to exactly 2^S, and
+ * table[p][t] == table[P-p][T-1-t].  The design is a Kaiser window (70 dB) on a sinc cut off at
+ * half of min(R_in, R_out), with the transition band 0.40 ... 0.60 * min(R_in, R_out).
+ *
+ * Per output, with q = floor(phi_n * P * 2^F / L), p = q >> F, w = q & (2^F - 1):
+ *   c_t = table[p][t] + (((table[p+1][t] - table[p][t]) * w + 2^(F-1)) >> F)
+ *   c_{T/2-1+(p >= P/2)} += 2^S - sum_t c_t        (the tap nearest the output time; DC gain exactly 2^S)
+ *   acc = sum_t c_t * s_t,   s = 2u - 255
+ *   u_out = clamp((acc + 2^(S+8)) >> (S+1), 0, 255)
+ * so a constant input u comes out as exactly u.  All of that is integer arithmetic; only the table
+ * design below uses floating point, once, on the host.
+ */
+#ifndef ERTGPU_RESAMPLE_H
+#define ERTGPU_RESAMPLE_H
+
+#include <stdint.h>
+
+#include "ertgpu.h"
+
+#define ERTRS_P 256      /* sub-phases per input sample                   */
+#define ERTRS_S 14       /* DC gain 2^S (peak tap <= 2^S fits int16)      */
+#define ERTRS_F 16       /* bits of the interpolation weight              */
+#define ERTRS_MAX_T 128  /* taps per output                               */
+#define ERTRS_ATTEN_DB 70.0
+
+static inline int64_t ertrs_gcd(int64_t a, int64_t b) {
+    while (b) {
+        int64_t t = a % b;
+        a = b;
+        b = t;
+    }
+    return a;
+}
+
+/* sin(pi*x) from IEEE adds and multiplies only (no libm), so every build computes the same table */
+static inline double ertrs_sinpi(double x) {
+    double n = (double)(int64_t)(x >= 0 ? x + 0.5 : x - 0.5); /* nearest integer */
+    double r = x - n;                                           /* |r| <= 0.5 */
+    const double pr = 3.14159265358979323846 * r, p2 = pr * pr;
+    double term = pr, sum = pr;
+    for (int k = 1; k < 14; k++) {
+        term *= -p2 / (double)((2 * k) * (2 * k + 1));
+        sum += term;
+    }
+    return ((int64_t)n & 1) ? -sum : sum;
+}
+
+/* modified Bessel function I0 by its power series */
+static inline double ertrs_i0(double x) {
+    double term = 1.0, sum = 1.0;
+    const double q = x * x / 4.0;
+    for (int k = 1; k < 200; k++) {
+        term *= q / ((double)k * (double)k);
+        sum += term;
+        if (term < sum * 1e-18) break;
+    }
+    return sum;
+}
+
+/* Fill *info for R_in -> R_out.  Returns 0, or -1 when a rate is not positive or the ratio is outside
+ * [1/4, 4]. */
+static inline int ertrs_plan(int64_t rate_in, int64_t rate_out, ertgpu_resampler_info* info) {
+    if (rate_in <= 0 || rate_out <= 0) return -1;
+    if (rate_out * 4 < rate_in || rate_out > rate_in * 4) return -1;
+    const int64_t g = ertrs_gcd(rate_out, rate_in);
+    info->rate_in = rate_in;
+    info->rate_out = rate_out;
+    info->L = rate_out / g;
+    info->M = rate_in / g;
+    /* cut-off scale: min(R_in, R_out) in cycles per input sample */
+    const double nu = rate_out < rate_in ? (double)rate_out / (double)rate_in : 1.0;
+    const double width = 0.2 * nu; /* 0.40 ... 0.60 * nu */
+    const double n = (ERTRS_ATTEN_DB - 7.95) / (14.36 * width);
+    int32_t T = 2 * (int32_t)((n + 1.999999) / 2.0);
+    if (T < 8) T = 8;
+    if (T > ERTRS_MAX_T) T = ERTRS_MAX_T;
+    info->T = T;
+    info->P = ERTRS_P;
+    info->S = ERTRS_S;
+    info->F = ERTRS_F;
+    return 0;
+}
+
+/* h(d) * 2^S for the plan's window */
+static inline double ertrs_proto(const ertgpu_resampler_info* info, double d) {
+    const double nu = info->rate_out < info->rate_in ? (double)info->rate_out / (double)info->rate_in : 1.0;
+    const double half = 0.5 * (double)info->T;
+    if (d <= -half || d >= half) return 0.0;
+    const double beta = 0.1102 * (ERTRS_ATTEN_DB - 8.7);
+    const double z = d / half;
+    const double w = ertrs_i0(beta * __builtin_sqrt(1.0 - z * z)) / ertrs_i0(beta);
+    const double fc = 0.5 * nu; /* cut-off, cycles per input sample */
+    const double x = 2.0 * fc * d;
+    const double sinc = x == 0.0 ? 1.0 : ertrs_sinpi(x) / (3.14159265358979323846 * x);
+    return (double)(1 << info->S) * 2.0 * fc * sinc * w;
+}
+
+/* Build the (P+1) x T table.  Returns 0, or -1 if a tap or an interpolation step does not fit
+ * (never for plans ertrs_plan makes). */
+static inline int ertrs_build_table(const ertgpu_resampler_info* info, int16_t* table) {
+    const int32_t T = info->T, P = info->P;
+    const int32_t one = 1 << info->S;
+    for (int32_t p = 0; p <= P / 2; p++) {
+        int16_t* row = table + (int64_t)p * T;
+        int64_t sum = 0;
+        if (p < P / 2) {
+            for (int32_t t = 0; t < T; t++) {
+                const double v = ertrs_proto(info, (double)(t - T / 2 + 1) - (double)p / (double)P);
+                const double r = v >= 0 ? (double)(int64_t)(v + 0.5) : -(double)(int64_t)(-v + 0.5);
+                if (r > 32767.0 || r < -32768.0) return -1;
+                row[t] = (int16_t)r;
+                sum += row[t];
+            }
+            const int64_t c = row[T / 2 - 1] + (one - sum);
+            if (c > 32767 || c < -32768) return -1;
+            row[T / 2 - 1] = (int16_t)c;
+        } else { /* the half-sample row mirrors itself: build one half, mirror, split the residual */
+            for (int32_t t = 0; t < T / 2; t++) {
+                const double v = ertrs_proto(info, (double)(t - T / 2 + 1) - 0.5);
+                const double r = v >= 0 ? (double)(int64_t)(v + 0.5) : -(double)(int64_t)(-v + 0.5);
+                if (r > 32767.0 || r < -32768.0) return -1;
+                row[t] = row[T - 1 - t] = (int16_t)r;
+                sum += 2 * (int64_t)row[t];
+            }
+            const int64_t c = row[T / 2 - 1] + (one - sum) / 2; /* sum is even */
+            if (c > 32767 || c < -32768) return -1;
+            row[T / 2 - 1] = row[T / 2] = (int16_t)c;
+        }
+    }
+    for (int32_t p = P / 2 + 1; p <= P; p++)
+        for (int32_t t = 0; t < T; t++) table[(int64_t)p * T + t] = table[(int64_t)(P - p) * T + (T - 1 - t)];
+    /* h0 * 2^F + 2^(F-1) + (h1 - h0) * w must fit int32 */
+    for (int32_t p = 0; p < P; p++)
+        for (int32_t t = 0; t < T; t++) {
+            const int32_t d = (int32_t)table[(int64_t)(p + 1) * T + t] - (int32_t)table[(int64_t)p * T + t];
+            if (d >= (1 << (30 - info->F)) || d <= -(1 << (30 - info->F))) return -1;
+        }
+    return 0;
+}
+
+#endif

@@ -19,7 +19,7 @@ MAX_PROTOCOLS, MAX_PREAMBLE, MAX_PACKET_BYTES, R900_DIGITS = 8, 32, 92, 42
 CHECK_NONE, CHECK_CRC16, CHECK_IDM, CHECK_R900 = 0, 1, 2, 3
 DECODE_ONLY_VALID = 1
 CAND_HAS_R900 = 1
-TAP_SIGNAL, TAP_CSUM, TAP_QUANTIZED, TAP_PACKED, TAP_R900_QUANTIZED = range(5)
+TAP_SIGNAL, TAP_CSUM, TAP_QUANTIZED, TAP_PACKED, TAP_R900_QUANTIZED, TAP_RESAMPLED = range(6)
 
 
 class Protocol(C.Structure):
@@ -44,6 +44,11 @@ class Candidate(C.Structure):
                 ("check_mask", C.c_uint32), ("flags", C.c_uint32),
                 ("bytes", C.c_uint8 * MAX_PACKET_BYTES), ("r900_digits", C.c_uint8 * R900_DIGITS),
                 ("pad", C.c_uint8 * 2)]
+
+
+class ResamplerInfo(C.Structure):
+    _fields_ = [("rate_in", C.c_int64), ("rate_out", C.c_int64), ("L", C.c_int64), ("M", C.c_int64),
+                ("T", C.c_int32), ("P", C.c_int32), ("S", C.c_int32), ("F", C.c_int32)]
 
 
 class Shard(C.Structure):
@@ -71,6 +76,7 @@ EXPORTS = [
     "ertgpu_last_stage_ms", "ertgpu_stage_ms_mean", "ertgpu_tap", "ertgpu_set_demod_variant",
     "ertgpu_host_alloc", "ertgpu_host_free", "ertgpu_synth_fill",
     "ertgpu_bind_host_thread", "ertgpu_last_kernels", "ertgpu_plan_shards", "ertgpu_decode_sharded",
+    "ertgpu_set_input_rate", "ertgpu_get_resampler",
 ]
 
 _lib = None
@@ -123,6 +129,8 @@ def lib() -> C.CDLL:
     L.ertgpu_last_kernels.argtypes = [vp]
     L.ertgpu_plan_shards.argtypes = [i64, i32, i32, i32, C.POINTER(Shard)]
     L.ertgpu_decode_sharded.argtypes = [C.POINTER(vp), i32, vp, sz, u32, vp, sz, C.POINTER(sz)]
+    L.ertgpu_set_input_rate.argtypes = [vp, i64]
+    L.ertgpu_get_resampler.argtypes = [vp, C.POINTER(ResamplerInfo), vp, sz, C.POINTER(sz)]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the library does not export it
     _lib = L
@@ -163,6 +171,18 @@ class Handle:
 
     def register(self, proto: Protocol):
         self._check(self._L.ertgpu_register_protocol(self._h, C.byref(proto)))
+
+    def set_input_rate(self, hz: int):
+        """ertgpu_set_input_rate: the IQ fed to this handle is sampled at `hz` (between register and allocate)."""
+        self._check(self._L.ertgpu_set_input_rate(self._h, int(hz)))
+
+    def resampler(self):
+        """ertgpu_get_resampler: (info dict, int16 table of (P+1)*T entries)."""
+        info, n = ResamplerInfo(), C.c_size_t(0)
+        self._check(self._L.ertgpu_get_resampler(self._h, C.byref(info), None, 0, C.byref(n)))
+        table = np.zeros(n.value, dtype=np.int16)
+        self._check(self._L.ertgpu_get_resampler(self._h, C.byref(info), table.ctypes.data, table.size, C.byref(n)))
+        return {k: getattr(info, k) for k, _ in ResamplerInfo._fields_}, table
 
     def allocate(self, device: int = 0, max_blocks_per_call: int = 0, max_candidates: int = 0):
         self._check(self._L.ertgpu_allocate(self._h, device, max_blocks_per_call, max_candidates))
@@ -253,14 +273,16 @@ class Handle:
 
 
 def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per_call: int = 0,
-                max_candidates: int = 0) -> Handle:
+                max_candidates: int = 0, input_rate: int = 0) -> Handle:
     """NewDecoder + RegisterProtocol(NewParser(name, chip_length)) for each name + Allocate
-    (reference main.go:64-86)."""
+    (reference main.go:64-86).  input_rate > 0: the IQ is sampled at that rate (ertgpu_set_input_rate)."""
     if isinstance(msgtypes, str):
         msgtypes = [m.strip() for m in msgtypes.split(",") if m.strip()]
     h = Handle()
     for m in msgtypes:
         h.register(stock_protocol(m, chip_length))
+    if input_rate:
+        h.set_input_rate(input_rate)
     h.allocate(device, max_blocks_per_call, max_candidates)
     return h
 

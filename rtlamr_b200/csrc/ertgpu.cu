@@ -32,6 +32,7 @@
 #include "demod_fast.cuh"
 #include "demod_generic.cuh"
 #include "ert_common.cuh"
+#include "resample.cuh"
 #include "search.cuh"
 #include "synth.cuh"
 
@@ -114,6 +115,28 @@ struct ertgpu_handle {
     double stage_sum[4] = {0, 0, 0, 0};  // accumulated since ertgpu_set_stage_timing(1)
     int64_t stage_n = 0;
     std::vector<ertgpu_candidate> results;
+
+    // input-rate resampler (ertgpu_set_input_rate); on only when the input rate differs from the decoder's
+    int64_t rate_in = 0;
+    bool rs_on = false;
+    ertgpu_resampler_info rs{};
+    std::vector<int16_t> rs_table;
+    int32_t* d_rs_A = nullptr;       // the table as the kernel reads it (rs_pack_table)
+    uint32_t* d_rs_D = nullptr;
+    uint8_t* d_rs_hist[2] = {nullptr, nullptr};  // input samples the next outputs still read
+    int rs_cur_hist = 0;
+    uint8_t* d_rs_out[2] = {nullptr, nullptr};   // [partial block | new outputs]; the demod reads whole blocks of it
+    int rs_cur_out = 0;
+    size_t rs_out_bytes = 0;
+    size_t rs_smem = 0;
+    int rs_grid = 0;
+    int64_t rs_in_total = 0;    // input samples received since the stream start
+    int64_t rs_out_next = 0;    // first output not yet computed
+    int64_t rs_hist_first = 0;  // first input sample held in d_rs_hist[rs_cur_hist]
+    int64_t rs_hist_n = 0;
+    int64_t rs_pend = 0;        // outputs at the front of d_rs_out[rs_cur_out] that wait for a whole block
+    bool rs_inflight = false;   // a resample_kernel launch without a pipeline behind it has not been waited for
+    cudaStream_t rs_stream = nullptr;
 };
 
 namespace {
@@ -205,6 +228,13 @@ void free_device(ertgpu_handle* h) {
     dfree(h->d_out);
     dfree(h->d_counters);
     dfree(h->d_tap);
+    dfree(h->d_rs_A);
+    dfree(h->d_rs_D);
+    for (int k = 0; k < 2; k++) {
+        dfree(h->d_rs_hist[k]);
+        dfree(h->d_rs_out[k]);
+    }
+    h->rs_out_bytes = 0;
     if (h->h_counters) cudaFreeHost(h->h_counters);
     h->h_counters = nullptr;
     if (h->stream) cudaStreamDestroy(h->stream);
@@ -247,9 +277,12 @@ cudaError_t launch_dep(bool pdl, K kern, dim3 grid, dim3 block, size_t smem, cud
     return cudaLaunchKernelEx(&cfg, kern, args...);
 }
 
-// Enqueue the whole per-call pipeline for `nblocks` blocks whose IQ bytes are at d_iq.
+int launch_resample(ertgpu_handle* h, const RsArgs& a, cudaStream_t st);
+
+// Enqueue the whole per-call pipeline for `nblocks` blocks whose IQ bytes are at d_iq.  With rs, the resampler step
+// that writes those bytes runs first (its time counts as demod time).
 int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uint32_t flags,
-                     cudaStream_t st) {
+                     cudaStream_t st, const RsArgs* rs = nullptr) {
     const DevCfg& c = h->dcfg;
     uint32_t* plane = h->d_plane[h->cur_plane];
     uint32_t* plane_next = h->d_plane[h->cur_plane ^ 1];
@@ -274,6 +307,10 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
         h->stage_unread++;
     }
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[0], st));
+    if (rs) {
+        int rc = launch_resample(h, *rs, st);
+        if (rc) return rc;
+    }
     // 1. magnitude + matched filter + quantize + pack
     char kname[160];
     if (h->demod_variant != 0) {
@@ -438,6 +475,7 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
         snprintf(kname, sizeof(kname), ";extract_words_kernel<%d>", c.PK <= 128 ? 4 : kFullK);
         h->kernels += kname;
     }
+    if (rs) h->kernels += ";resample_kernel";
 
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[3], st));
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[4], st));
@@ -469,6 +507,10 @@ bool cand_less(const ertgpu_candidate& a, const ertgpu_candidate& b) {
 
 // Wait for the pending pipeline and read its counters (candidates stay on the device).
 int collect_sync(ertgpu_handle* h) {
+    if (h->rs_inflight) {  // it read the caller's input and wrote the resampler state the next call reads
+        CUDA_TRY(h, cudaStreamSynchronize(h->rs_stream));
+        h->rs_inflight = false;
+    }
     if (!h->pending) return ERTGPU_OK;
     CUDA_TRY(h, cudaStreamSynchronize(h->pending_stream));
     h->pending = false;
@@ -511,6 +553,195 @@ int deliver(ertgpu_handle* h, ertgpu_candidate* out, size_t cap, size_t* n_out) 
     if (h->results.size() > cap) return fail(h, ERTGPU_ECAPACITY, "output array holds %zu candidates, %zu needed", cap, h->results.size());
     if (!h->results.empty() && out) memcpy(out, h->results.data(), h->results.size() * sizeof(ertgpu_candidate));
     return ERTGPU_OK;
+}
+
+// Device staging buffers of `bytes` each (kept when large enough) and, for pageable input, the pinned staging
+// buffers and the copy threads.
+int prepare_staging(ertgpu_handle* h, size_t bytes, const void* iq, bool* pageable) {
+    if (h->stage_bytes < bytes) {
+        for (int k = 0; k < 2; k++) {
+            cudaFree(h->d_stage[k]);
+            h->d_stage[k] = nullptr;
+        }
+        h->stage_bytes = 0;
+        for (int k = 0; k < 2; k++) CUDA_TRY(h, cudaMalloc(&h->d_stage[k], bytes));
+        h->stage_bytes = bytes;
+    }
+    // Pinned (or registered / managed) input goes to the device directly.  Ordinary pageable memory -- a Go slice,
+    // main.go:166's block buffer -- would make every cudaMemcpyAsync a synchronous driver-staged copy: it is staged
+    // through two pinned buffers of the handle instead, filled by a few host threads while the previous chunk's
+    // transfer is in flight.
+    {
+        cudaPointerAttributes at{};
+        if (cudaPointerGetAttributes(&at, iq) == cudaSuccess) *pageable = at.type == cudaMemoryTypeUnregistered;
+        else cudaGetLastError();
+    }
+    if (*pageable && h->h_stage_bytes < h->stage_bytes) {
+        for (int k = 0; k < 2; k++) {
+            if (h->h_stage[k]) cudaFreeHost(h->h_stage[k]);
+            h->h_stage[k] = nullptr;
+        }
+        h->h_stage_bytes = 0;
+        for (int k = 0; k < 2; k++) CUDA_TRY(h, cudaHostAlloc(&h->h_stage[k], h->stage_bytes, cudaHostAllocDefault));
+        h->h_stage_bytes = h->stage_bytes;
+    }
+    if (*pageable) {
+        int copy_threads = (int)std::min(8u, std::max(1u, std::thread::hardware_concurrency() / 4));  // ~6 GB/s per memcpy stream; 8 fill a PCIe 5 x16 link
+        if (const char* e = getenv("ERTGPU_STAGE_THREADS")) copy_threads = std::min(64, std::max(1, atoi(e)));
+        if (!h->copy_pool || h->copy_pool->size() != copy_threads) h->copy_pool.reset(new CopyPool(copy_threads - 1));
+    }
+    return ERTGPU_OK;
+}
+
+// ---- input-rate resampler (include/ertgpu_resample.h) ----
+
+int launch_resample(ertgpu_handle* h, const RsArgs& a, cudaStream_t st) {
+    if (a.count <= 0 && a.carry_n <= 0) return ERTGPU_OK;
+    const long long tiles = (a.count + kRsTile - 1) / kRsTile;
+    const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(tiles, h->rs_grid));
+    resample_kernel<<<grid, kRsThreads, h->rs_smem, st>>>(h->d_rs_A, h->d_rs_D, a);
+    CUDA_TRY(h, cudaGetLastError());
+    h->launches++;
+    return ERTGPU_OK;
+}
+
+// Number of outputs whose window lies inside the first x input samples (k_n + T/2 <= x - 1).
+int64_t rs_out_end(const ertgpu_handle* h, int64_t x) {
+    const int64_t a = x - h->rs.T / 2;
+    if (a <= 0) return 0;
+    return (int64_t)(((__int128)a * h->rs.L + h->rs.M - 1) / h->rs.M);
+}
+
+int64_t rs_k(const ertgpu_handle* h, int64_t n) { return (int64_t)((__int128)n * h->rs.M / h->rs.L); }
+
+// Most input samples the next step may take so that it completes at most max_blocks decoder blocks.
+int64_t rs_max_input(const ertgpu_handle* h) {
+    const int64_t cap_out = (h->max_blocks + 1) * (int64_t)h->cfg.block_size - 1 - h->rs_pend;
+    return h->rs.T / 2 + rs_k(h, h->rs_out_next + cap_out) - h->rs_in_total;
+}
+
+// One step over c new input samples at d_in (device): every output whose window is complete.  *nblocks = whole
+// decoder blocks the step completes.  Nothing of the handle changes until rs_commit.
+void rs_plan_step(const ertgpu_handle* h, const uint8_t* d_in, int64_t c, RsArgs* a, int64_t* nblocks) {
+    const int64_t BS = h->cfg.block_size, L = h->rs.L, M = h->rs.M, T = h->rs.T;
+    const int64_t in_new = h->rs_in_total + c;
+    const int64_t ne = rs_out_end(h, in_new);
+    const int64_t cnt = ne - h->rs_out_next;
+    *nblocks = (h->rs_pend + cnt) / BS;
+    memset(a, 0, sizeof(*a));
+    a->hist = h->d_rs_hist[h->rs_cur_hist];
+    a->cur = d_in;
+    a->hist_first = h->rs_hist_first;
+    a->hist_n = h->rs_hist_n;
+    a->cur_n = c;
+    a->n0 = h->rs_out_next;
+    a->count = cnt;
+    a->split = *nblocks > 0 ? *nblocks * BS - h->rs_pend : LLONG_MAX;
+    a->base_n = (h->rs_out_next / L) * L;
+    a->base_k = (h->rs_out_next / L) * M;
+    a->out = h->d_rs_out[h->rs_cur_out] + 2 * h->rs_pend;
+    a->out2 = h->d_rs_out[h->rs_cur_out ^ 1];
+    const int64_t first = std::min(in_new, std::max<int64_t>(0, rs_k(h, ne) - T / 2 + 1));
+    a->carry_dst = h->d_rs_hist[h->rs_cur_hist ^ 1];
+    a->carry_first = first;
+    a->carry_n = in_new - first;
+    a->L = L;
+    a->M = M;
+    a->T = (int)T;
+    const int64_t Q = (int64_t)ERTRS_P << ERTRS_F, step = kRsThreads * M;
+    a->step_k = step / L;
+    a->step_phi = step % L;
+    a->step_q = (int64_t)(((__int128)a->step_phi * Q) / L);
+    a->step_r = (int64_t)(((__int128)a->step_phi * Q) % L);
+}
+
+void rs_commit(ertgpu_handle* h, const RsArgs& a, int64_t nblocks) {
+    h->rs_in_total += a.cur_n;
+    h->rs_out_next += a.count;
+    h->rs_hist_first = a.carry_first;
+    h->rs_hist_n = a.carry_n;
+    h->rs_cur_hist ^= 1;
+    const int64_t total = h->rs_pend + a.count;
+    if (nblocks > 0) {
+        h->rs_cur_out ^= 1;  // the outputs past the last whole block are already at the front of the other buffer
+        h->rs_pend = total - nblocks * (int64_t)h->cfg.block_size;
+    } else {
+        h->rs_pend = total;
+    }
+}
+
+// Enqueue one planned step: the resampler, then the decoder pipeline over the whole blocks it completed.
+int rs_run(ertgpu_handle* h, const RsArgs& a, int64_t nblocks, uint32_t flags, cudaStream_t st) {
+    int rc;
+    if (nblocks > 0) {
+        rc = enqueue_pipeline(h, h->d_rs_out[h->rs_cur_out], nblocks, flags, st, &a);
+    } else {  // no pipeline to wait for: collect_sync waits for this launch instead
+        h->launches = 0;
+        rc = launch_resample(h, a, st);
+        if (rc == ERTGPU_OK && h->launches) {
+            h->rs_inflight = true;
+            h->rs_stream = st;
+            if (h->kernels.empty()) h->kernels = "resample_kernel";  // otherwise the last pipeline's list stays
+        }
+    }
+    if (rc) return rc;
+    rs_commit(h, a, nblocks);
+    return ERTGPU_OK;
+}
+
+void rs_reset_stream(ertgpu_handle* h) {
+    h->rs_in_total = h->rs_out_next = h->rs_hist_first = h->rs_hist_n = h->rs_pend = 0;
+}
+
+// ertgpu_decode for a handle with an input rate: chunks of at most the staging size and of at most max_blocks
+// completed blocks; the H2D copy of chunk i+1 overlaps the kernels of chunk i as in the native path.
+int decode_resampled(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t flags, ertgpu_candidate* out,
+                     size_t cap, size_t* n_out) {
+    const int64_t total = (int64_t)(nbytes / 2);
+    if (total == 0) return deliver(h, out, cap, n_out);
+    int64_t chunk_mib = 32;
+    if (const char* e = getenv("ERTGPU_CHUNK_MIB")) chunk_mib = std::max(1, atoi(e));  // tuning knob
+    const int64_t chunk = std::min<int64_t>((chunk_mib << 20) / 2,
+                                            4 * (h->max_blocks + 1) * (int64_t)h->cfg.block_size + h->rs.T + 8);
+    bool pageable = true;
+    {
+        int rc = prepare_staging(h, (size_t)chunk * 2, iq, &pageable);
+        if (rc) return rc;
+    }
+    int64_t done = 0, launches = 0;
+    std::string kernels;
+    for (int64_t i = 0; done < total; i++) {
+        const int k = (int)(i & 1);
+        const int64_t c = std::min(std::min(chunk, total - done), rs_max_input(h));
+        if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // the kernels that read d_stage[k] (and its H2D) are done
+        const uint8_t* src = iq + (size_t)done * 2;
+        if (pageable) {
+            h->copy_pool->copy(h->h_stage[k], src, (size_t)c * 2);
+            src = h->h_stage[k];
+        }
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * 2, cudaMemcpyHostToDevice, h->copy_stream));
+        CUDA_TRY(h, cudaEventRecord(h->ev_h2d[k], h->copy_stream));
+        if (i >= 1) {
+            int rc = collect(h);
+            if (rc) return rc;
+        }
+        CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[k], 0));
+        RsArgs a;
+        int64_t nb = 0;
+        rs_plan_step(h, h->d_stage[k], c, &a, &nb);
+        int rc = rs_run(h, a, nb, flags, h->stream);
+        if (rc) return rc;
+        if (nb > 0) kernels = h->kernels;
+        launches += h->launches;
+        CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
+        done += c;
+    }
+    int rc = collect(h);  // also waits for a last step that completed no block (ertgpu_decode is synchronous)
+    if (rc) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));  // a step that launched nothing still copied from iq
+    h->launches = launches;
+    if (!kernels.empty()) h->kernels = kernels;
+    return deliver(h, out, cap, n_out);
 }
 
 void begin_call(ertgpu_handle* h) {
@@ -586,6 +817,7 @@ int ertgpu_stock_protocol(const char* msgtype, int32_t chip_length, ertgpu_proto
 int ertgpu_register_protocol(ertgpu_handle* h, const ertgpu_protocol* p) {
     if (!h || !p) return ERTGPU_EINVAL;
     if (h->allocated) return fail(h, ERTGPU_EINVAL, "register_protocol after allocate");
+    if (h->rate_in) return fail(h, ERTGPU_EINVAL, "register_protocol after set_input_rate");
     if (h->protos.size() >= ERTGPU_MAX_PROTOCOLS) return fail(h, ERTGPU_EINVAL, "too many protocols");
     const size_t n = strnlen(p->preamble, sizeof(p->preamble));
     if (n == 0 || n > ERTGPU_MAX_PREAMBLE) return fail(h, ERTGPU_EINVAL, "bad preamble length %zu", n);
@@ -756,6 +988,35 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     h->demod_variant = demod_fast_variant(d.CL, d.BS);
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->device);
     if (h->sm_count < 1) h->sm_count = 132;
+
+    if (h->rs_on) {
+        const ertgpu_resampler_info& r = h->rs;
+        std::vector<int32_t> A((size_t)r.P * r.T);
+        std::vector<uint32_t> D((size_t)r.P * (r.T / 2));
+        rs_pack_table(h->rs_table.data(), r.P, r.T, A.data(), D.data());
+        CUDA_TRY(h, cudaMalloc(&h->d_rs_A, A.size() * sizeof(int32_t)));
+        CUDA_TRY(h, cudaMemcpy(h->d_rs_A, A.data(), A.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+        CUDA_TRY(h, cudaMalloc(&h->d_rs_D, D.size() * sizeof(uint32_t)));
+        CUDA_TRY(h, cudaMemcpy(h->d_rs_D, D.data(), D.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        for (int k = 0; k < 2; k++) {
+            CUDA_TRY(h, cudaMalloc(&h->d_rs_hist[k], (size_t)r.T * 2 + 16));
+            // a step completes at most max_blocks blocks: less than (max_blocks + 1) * BS outputs are buffered
+            h->rs_out_bytes = (size_t)(max_blocks_per_call + 1) * c.block_size2 + 64;
+            CUDA_TRY(h, cudaMalloc(&h->d_rs_out[k], h->rs_out_bytes));
+        }
+        h->rs_smem = rs_smem_bytes(r.T, r.L, r.M);
+        {   // a property of the kernel, not of the handle: every handle on the device gets the largest any table needs
+            static OncePerDevice once;
+            if (once.first(h->device))
+                CUDA_TRY(h, cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        }
+        if (h->rs_smem > 227 * 1024) return fail(h, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", h->rs_smem);
+        int per_sm = 0;
+        CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel, kRsThreads, h->rs_smem));
+        h->rs_grid = std::max(1, per_sm) * h->sm_count;
+        h->rs_cur_hist = h->rs_cur_out = 0;
+        rs_reset_stream(h);
+    }
     h->cur_plane = h->cur_hist = 0;
     h->hist_valid = 0;
     h->block_counter = 0;
@@ -772,6 +1033,10 @@ int ertgpu_get_config(const ertgpu_handle* h, ertgpu_decoder_config* cfg) {
 int ertgpu_reset(ertgpu_handle* h) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
+    if (h->rs_inflight) {
+        CUDA_TRY(h, cudaStreamSynchronize(h->rs_stream));
+        h->rs_inflight = false;
+    }
     if (h->pending) {
         CUDA_TRY(h, cudaStreamSynchronize(h->pending_stream));
         h->pending = false;
@@ -781,7 +1046,38 @@ int ertgpu_reset(ertgpu_handle* h) {
     h->fresh = true;
     h->hist_valid = 0;
     h->block_counter = 0;
+    rs_reset_stream(h);
     begin_call(h);
+    return ERTGPU_OK;
+}
+
+int ertgpu_set_input_rate(ertgpu_handle* h, int64_t hz) {
+    if (!h) return ERTGPU_EINVAL;
+    if (h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_rate after allocate");
+    if (h->protos.empty()) return fail(h, ERTGPU_EINVAL, "set_input_rate before register_protocol");
+    const int64_t rate_out = (int64_t)h->cfg.data_rate * h->cfg.chip_length;
+    ertgpu_resampler_info info{};
+    if (ertrs_plan(hz, rate_out, &info) != 0)
+        return fail(h, ERTGPU_EINVAL, "input rate %lld Hz: the decoder rate %lld Hz must be within 1/4 ... 4 times it",
+                    (long long)hz, (long long)rate_out);
+    std::vector<int16_t> table;
+    if (hz != rate_out) {
+        table.resize((size_t)(info.P + 1) * info.T);
+        if (ertrs_build_table(&info, table.data()) != 0) return fail(h, ERTGPU_EINVAL, "resampler table does not fit int16");
+    }
+    h->rate_in = hz;
+    h->rs_on = hz != rate_out;
+    h->rs = info;
+    h->rs_table.swap(table);
+    return ERTGPU_OK;
+}
+
+int ertgpu_get_resampler(const ertgpu_handle* h, ertgpu_resampler_info* info, int16_t* table, size_t cap,
+                         size_t* n_out) {
+    if (!h || !h->rs_on) return ERTGPU_EINVAL;
+    if (info) *info = h->rs;
+    if (n_out) *n_out = h->rs_table.size();
+    if (table && cap >= h->rs_table.size()) memcpy(table, h->rs_table.data(), h->rs_table.size() * sizeof(int16_t));
     return ERTGPU_OK;
 }
 
@@ -795,15 +1091,33 @@ int ertgpu_set_demod_variant(ertgpu_handle* h, int32_t variant) {
 }
 
 int ertgpu_decode_device_async(ertgpu_handle* h, const void* d_iq, size_t nbytes, uint32_t flags, void* stream) {
+    if (h && h->rs_on && nbytes % 2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of IQ samples", nbytes);
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     if (!d_iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
+    if (h->rs_on) {
+        if ((reinterpret_cast<uintptr_t>(d_iq) & 1) != 0) return fail(h, ERTGPU_EINVAL, "device input must be 2-byte aligned");
+        RsArgs a;
+        int64_t nb = 0;
+        rs_plan_step(h, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / 2), &a, &nb);
+        if (nb > h->max_blocks)
+            return fail(h, ERTGPU_ESIZE, "%zu input bytes complete %lld blocks, more than max_blocks_per_call %lld", nbytes,
+                        (long long)nb, (long long)h->max_blocks);
+        CUDA_TRY(h, cudaSetDevice(h->device));
+        if (h->pending || h->rs_inflight) {
+            int rc = collect(h);
+            if (rc) return rc;
+        }
+        begin_call(h);
+        if (nbytes == 0) return ERTGPU_OK;
+        return rs_run(h, a, nb, flags, stream ? (cudaStream_t)stream : h->stream);
+    }
     if ((reinterpret_cast<uintptr_t>(d_iq) & 15) != 0) return fail(h, ERTGPU_EINVAL, "device input must be 16-byte aligned");
     const size_t bs2 = (size_t)h->cfg.block_size2;
     if (nbytes % bs2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize2 %zu", nbytes, bs2);
     const int64_t nblocks = (int64_t)(nbytes / bs2);
     if (nblocks > h->max_blocks) return fail(h, ERTGPU_ESIZE, "%lld blocks exceed max_blocks_per_call %lld", (long long)nblocks, (long long)h->max_blocks);
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending) {
+    if (h->pending || h->rs_inflight) {
         int rc = collect(h);
         if (rc) return rc;
     }
@@ -822,12 +1136,22 @@ int ertgpu_fetch(ertgpu_handle* h, ertgpu_candidate* out, size_t cap, size_t* n_
 
 int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t flags, ertgpu_candidate* out,
                   size_t cap, size_t* n_out) {
+    if (h && h->rs_on && nbytes % 2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of IQ samples", nbytes);
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     if (!iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
+    if (h->rs_on) {
+        CUDA_TRY(h, cudaSetDevice(h->device));
+        if (h->pending || h->rs_inflight) {
+            int rc = collect(h);
+            if (rc) return rc;
+        }
+        begin_call(h);
+        return decode_resampled(h, iq, nbytes, flags, out, cap, n_out);
+    }
     const size_t bs2 = (size_t)h->cfg.block_size2;
     if (nbytes % bs2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize2 %zu", nbytes, bs2);
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending) {
+    if (h->pending || h->rs_inflight) {
         int rc = collect(h);
         if (rc) return rc;
     }
@@ -839,38 +1163,10 @@ int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t f
     int64_t chunk_mib = 32;
     if (const char* e = getenv("ERTGPU_CHUNK_MIB")) chunk_mib = std::max(1, atoi(e));  // tuning knob
     const int64_t chunk_blocks = std::min<int64_t>(h->max_blocks, std::max<int64_t>(1, (chunk_mib << 20) / (int64_t)bs2));
-    if (h->stage_bytes < (size_t)chunk_blocks * bs2) {
-        for (int k = 0; k < 2; k++) {
-            cudaFree(h->d_stage[k]);
-            h->d_stage[k] = nullptr;
-        }
-        h->stage_bytes = 0;
-        for (int k = 0; k < 2; k++) CUDA_TRY(h, cudaMalloc(&h->d_stage[k], (size_t)chunk_blocks * bs2));
-        h->stage_bytes = (size_t)chunk_blocks * bs2;
-    }
-    // Pinned (or registered / managed) input goes to the device directly.  Ordinary pageable memory -- a Go slice,
-    // main.go:166's block buffer -- would make every cudaMemcpyAsync a synchronous driver-staged copy: it is staged
-    // through two pinned buffers of the handle instead, filled by a few host threads while the previous chunk's
-    // transfer is in flight.
     bool pageable = true;
     {
-        cudaPointerAttributes at{};
-        if (cudaPointerGetAttributes(&at, iq) == cudaSuccess) pageable = at.type == cudaMemoryTypeUnregistered;
-        else cudaGetLastError();
-    }
-    if (pageable && h->h_stage_bytes < h->stage_bytes) {
-        for (int k = 0; k < 2; k++) {
-            if (h->h_stage[k]) cudaFreeHost(h->h_stage[k]);
-            h->h_stage[k] = nullptr;
-        }
-        h->h_stage_bytes = 0;
-        for (int k = 0; k < 2; k++) CUDA_TRY(h, cudaHostAlloc(&h->h_stage[k], h->stage_bytes, cudaHostAllocDefault));
-        h->h_stage_bytes = h->stage_bytes;
-    }
-    if (pageable) {
-        int copy_threads = (int)std::min(8u, std::max(1u, std::thread::hardware_concurrency() / 4));  // ~6 GB/s per memcpy stream; 8 fill a PCIe 5 x16 link
-        if (const char* e = getenv("ERTGPU_STAGE_THREADS")) copy_threads = std::min(64, std::max(1, atoi(e)));
-        if (!h->copy_pool || h->copy_pool->size() != copy_threads) h->copy_pool.reset(new CopyPool(copy_threads - 1));
+        int rc = prepare_staging(h, (size_t)chunk_blocks * bs2, iq, &pageable);
+        if (rc) return rc;
     }
     int64_t done = 0, launches = 0;
     for (int64_t i = 0; done < nblocks; i++) {
@@ -904,7 +1200,7 @@ int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t f
 
 int ertgpu_last_counts(ertgpu_handle* h, int64_t* n_candidates, int64_t* n_valid) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
-    if (h->pending) {
+    if (h->pending || h->rs_inflight) {
         CUDA_TRY(h, cudaSetDevice(h->device));
         int rc = collect_sync(h);  // counters only; ertgpu_fetch copies the candidates if wanted
         if (rc) return rc;
@@ -919,7 +1215,7 @@ int64_t ertgpu_last_launches(const ertgpu_handle* h) { return h ? h->launches : 
 int ertgpu_tap(ertgpu_handle* h, int32_t which, int64_t block, void* dst, size_t cap, size_t* n_out) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending) {
+    if (h->pending || h->rs_inflight) {
         int rc = collect(h);
         if (rc) return rc;
     }
@@ -972,6 +1268,11 @@ int ertgpu_tap(ertgpu_handle* h, int32_t which, int64_t block, void* dst, size_t
         bytes.resize((size_t)c.BUF);
         CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), qd, bytes.size(), cudaMemcpyDeviceToHost, h->stream));
         CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    } else if (which == ERTGPU_TAP_RESAMPLED) {
+        if (!h->rs_on) return fail(h, ERTGPU_EINVAL, "the handle does not resample");
+        bytes.resize((size_t)c.BS * 2);
+        CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), h->last_iq + (size_t)b * c.BS * 2, bytes.size(), cudaMemcpyDeviceToHost, h->stream));
+        CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     } else {
         return fail(h, ERTGPU_EINVAL, "unknown tap %d", which);
     }
@@ -983,7 +1284,7 @@ int ertgpu_tap(ertgpu_handle* h, int32_t which, int64_t block, void* dst, size_t
 int ertgpu_set_stage_timing(ertgpu_handle* h, int32_t enable) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending) {
+    if (h->pending || h->rs_inflight) {
         int rc = collect_sync(h);
         if (rc) return rc;
     }
@@ -999,7 +1300,7 @@ int ertgpu_set_stage_timing(ertgpu_handle* h, int32_t enable) {
 int ertgpu_last_stage_ms(ertgpu_handle* h, float* ms4) {
     if (!h || !h->allocated || !ms4) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending) {
+    if (h->pending || h->rs_inflight) {
         int rc = collect_sync(h);
         if (rc) return rc;
     }
@@ -1011,7 +1312,7 @@ int ertgpu_last_stage_ms(ertgpu_handle* h, float* ms4) {
 int ertgpu_stage_ms_mean(ertgpu_handle* h, float* ms4, int64_t* n_pipelines) {
     if (!h || !h->allocated || !ms4) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending) {
+    if (h->pending || h->rs_inflight) {
         int rc = collect_sync(h);
         if (rc) return rc;
     }

@@ -39,6 +39,10 @@ int ertgpu_decode_sharded(ertgpu_handle* const* handles, int32_t nhandles, const
     if (!handles || nhandles < 1 || (!iq && nbytes)) return ERTGPU_EINVAL;
     for (int32_t r = 0; r < nhandles; r++)
         if (!handles[r]) return ERTGPU_EINVAL;
+    for (int32_t r = 0; r < nhandles; r++) {  // shards are cut at decoder blocks of the input: no resampling handles
+        ertgpu_resampler_info ri;
+        if (ertgpu_get_resampler(handles[r], &ri, nullptr, 0, nullptr) == ERTGPU_OK) return ERTGPU_EINVAL;
+    }
     ertgpu_decoder_config c0;
     int rc = ertgpu_get_config(handles[0], &c0);
     if (rc) return rc;

@@ -41,6 +41,9 @@ def lib():
         L = C.CDLL(LIB_PATH)
         L.erthost_new.restype = C.c_void_p
         L.erthost_new.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_char_p, C.c_int]
+        L.erthost_new_rate.restype = C.c_void_p
+        L.erthost_new_rate.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_char_p,
+                                       C.c_int]
         L.erthost_free.argtypes = [C.c_void_p]
         L.erthost_error.restype = C.c_char_p
         L.erthost_error.argtypes = [C.c_void_p]
@@ -156,10 +159,17 @@ class Receiver:
     CFG = ("DataRate", "BlockSize", "BlockSize2", "ChipLength", "SymbolLength", "SampleRate", "PreambleSymbols",
            "PacketSymbols", "PreambleLength", "PacketLength", "BufferLength", "CenterFreq")
 
-    def __init__(self, msgtypes: str, chip_length: int = 72, device: int = 0, max_blocks: int = 0, max_cands: int = 0):
+    def __init__(self, msgtypes: str, chip_length: int = 72, device: int = 0, max_blocks: int = 0, max_cands: int = 0,
+                 input_rate: int = 0):
+        """input_rate > 0: the IQ given to decode() is sampled at that rate (erthost_new_rate); any rate other than
+        DataRate * ChipLength is resampled on the GPU and decode() then takes any even number of bytes."""
         self._L = lib()
         err = C.create_string_buffer(512)
-        self._h = self._L.erthost_new(msgtypes.encode(), chip_length, device, max_blocks, max_cands, err, 512)
+        if input_rate:
+            self._h = self._L.erthost_new_rate(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate,
+                                               err, 512)
+        else:
+            self._h = self._L.erthost_new(msgtypes.encode(), chip_length, device, max_blocks, max_cands, err, 512)
         if not self._h:
             raise RuntimeError(err.value.decode())
         v = (C.c_int32 * 12)()

@@ -3,7 +3,10 @@
 // in rtlamr's plain format without the time fields (protocol/parse.go:119-121 StringNoOffset).
 //   ertgpu_decode_file [-msgtype=scm,idm|all] [-symbollength=72] [-blockdedup=true] [-blocks=4096] [-device=0]
 //                      [-filterid=1,2] [-filtertype=4,5] [-unique=true] [-format=plain|csv|json|xml]
-//                      [-samplefile=PATH] [-single] [-duration=1h5m10s] FILE|- [FILE ...]
+//                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ] FILE|- [FILE ...]
+// -samplerate is rtlamr's (rtltcp's) flag name; here it names the capture's sample rate.  The default,
+// 32768 * -symbollength, decodes the bytes as they are; any other rate within 1/4 ... 4 times it is resampled
+// exactly on the GPU first, and Block / Idx then count resampled samples.  It cannot be combined with -samplefile.
 // -filterid / -filtertype / -unique, -format, -samplefile, -single and -duration are rtlamr's flags of the same names
 // (flags.go:37-58,69-70,140-170; the filter chain runs before the cross-block dedup, main.go:236-260).  With -format=csv a
 // line is LogMessage.Record() (parse.go:123-129: time, offset, length, then the message's own record) through Go's
@@ -29,7 +32,7 @@ int main(int argc, char** argv) {
     std::string msgtype = "scm";
     std::vector<std::string> files;
     int chip = 72, device = 0;
-    long long blocks = 4096;
+    long long blocks = 4096, samplerate = 0;
     bool block_dedup = true, quiet = false, unique = false, single = false;
     std::string filterid, filtertype, format = "plain", samplefile, duration;
     for (int i = 1; i < argc; i++) {
@@ -37,6 +40,7 @@ int main(int argc, char** argv) {
         if (a.rfind("-msgtype=", 0) == 0) msgtype = a.substr(9);
         else if (a.rfind("-symbollength=", 0) == 0) chip = atoi(a.c_str() + 14);
         else if (a.rfind("-device=", 0) == 0) device = atoi(a.c_str() + 8);
+        else if (a.rfind("-samplerate=", 0) == 0) samplerate = atoll(a.c_str() + 12);
         else if (a.rfind("-blocks=", 0) == 0) blocks = atoll(a.c_str() + 8);
         else if (a.rfind("-blockdedup=", 0) == 0) block_dedup = a.substr(12) != "false";
         else if (a.rfind("-filterid=", 0) == 0) filterid = a.substr(10);
@@ -54,7 +58,7 @@ int main(int argc, char** argv) {
     if (files.empty()) {
         fprintf(stderr, "usage: %s [-msgtype=scm,scm+,idm,netidm,r900,r900bcd|all] [-symbollength=N] [-blockdedup=true|false] "
                         "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
-                        "[-samplefile=PATH] [-single] [-duration=D] [-quiet] FILE|- [FILE ...]\n", argv[0]);
+                        "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-quiet] FILE|- [FILE ...]\n", argv[0]);
         return 2;
     }
     const bool csv = format == "csv", json = format == "json", xml = format == "xml";
@@ -63,6 +67,13 @@ int main(int argc, char** argv) {
         if (!duration.empty()) limit_ns = receiver::ParseDuration(duration);
     } catch (const std::exception& e) {
         fprintf(stderr, "invalid value \"%s\" for flag -duration: %s\n", duration.c_str(), e.what());
+        return 2;
+    }
+    // -samplerate names the capture's rate; the default DataRate*ChipLength (32768 * -symbollength) resamples nothing
+    const bool resampling = samplerate != 0 && samplerate != 32768LL * chip;
+    if (resampling && !samplefile.empty() && samplefile != "/dev/null") {
+        fprintf(stderr, "-samplefile cannot be combined with -samplerate=%lld (the capture is not at 32768 * -symbollength = %lld Hz)\n",
+                samplerate, 32768LL * chip);
         return 2;
     }
     FILE* sample = nullptr;   // os.DevNull, the default, is never opened (flags.go:136-141)
@@ -74,7 +85,7 @@ int main(int argc, char** argv) {
         }
     }
     try {
-        receiver::Receiver rcvr(msgtype, chip, device, blocks);
+        receiver::Receiver rcvr(msgtype, chip, device, blocks, resampling ? samplerate : 0);
         fputs(rcvr.decoder().Log().c_str(), stderr);
         if (sample) rcvr.SetSampleFile(sample);
         if (limit_ns) rcvr.SetDeadline(start + std::chrono::nanoseconds(limit_ns));

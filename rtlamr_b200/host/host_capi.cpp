@@ -27,9 +27,19 @@ struct erthost {
     std::string err;
 };
 
+erthost* erthost_new_rate(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
+                          long long input_rate, char* errbuf, int errcap);
+
 // main.go:59-86: NewDecoder; for each -msgtype NewParser + RegisterProtocol; Allocate
 erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
                      char* errbuf, int errcap) {
+    return erthost_new_rate(msgtypes_csv, chip_length, device, max_blocks, max_cands, 0, errbuf, errcap);
+}
+
+// The same for IQ sampled at input_rate Hz (0: the decoder's own DataRate * ChipLength); erthost_decode then takes
+// any whole number of IQ samples.
+erthost* erthost_new_rate(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
+                          long long input_rate, char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;   // released only on success: a throwing NewParser / Allocate must not leak the handle
     try {
         protocol::RegisterStockParsers();
@@ -40,6 +50,7 @@ erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long
             if (name.empty()) continue;
             h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
         }
+        if (input_rate > 0) h->d.SetInputRate(input_rate);
         h->d.Allocate(device, max_blocks, max_cands);
         return h.release();
     } catch (const std::exception& e) {

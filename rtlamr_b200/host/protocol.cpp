@@ -595,11 +595,32 @@ void Decoder::Allocate(int device, int64_t maxBlocksPerCall, int64_t maxCandidat
 void Decoder::Reset() {
     int rc = ertgpu_reset(h_);
     if (rc != ERTGPU_OK) raise(h_, rc, "Reset");
+    input_samples_ = 0;
+}
+
+void Decoder::SetInputRate(int64_t hz) {
+    if (allocated_) throw std::logic_error("SetInputRate after Allocate");
+    int rc = ertgpu_set_input_rate(h_, hz);
+    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
+    if (rc != ERTGPU_OK) raise(h_, rc, "SetInputRate");
+    resampling_ = ertgpu_get_resampler(h_, &rs_, nullptr, 0, nullptr) == ERTGPU_OK;
+}
+
+int64_t Decoder::BlocksDecoded() const {
+    if (!allocated_ || Cfg.BlockSize <= 0) return 0;
+    if (!resampling_) return input_samples_ / Cfg.BlockSize;
+    // outputs whose filter window lies inside the input so far (include/ertgpu_resample.h)
+    const int64_t a = input_samples_ - rs_.T / 2;
+    if (a <= 0) return 0;
+    const int64_t outputs = (int64_t)(((__int128)a * rs_.L + rs_.M - 1) / rs_.M);
+    return outputs / Cfg.BlockSize;
 }
 
 std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
     if (!allocated_) throw std::logic_error("Decode before Allocate");
-    if (len % (size_t)Cfg.BlockSize2) throw std::length_error("input is not a whole number of BlockSize2-byte blocks");
+    if (resampling_ ? (len % 2) != 0 : (len % (size_t)Cfg.BlockSize2) != 0)
+        throw std::length_error(resampling_ ? "input is not a whole number of IQ samples"
+                                            : "input is not a whole number of BlockSize2-byte blocks");
     size_t n = 0;
     if (cands_.size() < 1024) cands_.resize(1024);
     int rc = ertgpu_decode(h_, input, len, ERTGPU_DECODE_ONLY_VALID, cands_.data(), cands_.size(), &n);
@@ -608,6 +629,7 @@ std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
         rc = ertgpu_fetch(h_, cands_.data(), cands_.size(), &n);
     }
     if (rc != ERTGPU_OK) raise(h_, rc, "Decode");
+    input_samples_ += (int64_t)(len / 2);
 
     std::vector<MessagePtr> out;
     Dispatch(cands_.data(), n, out);

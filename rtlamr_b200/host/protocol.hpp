@@ -137,10 +137,18 @@ public:
     Decoder& operator=(const Decoder&) = delete;
 
     void RegisterProtocol(ParserPtr p);  // decode.go:100-128
+    // The IQ fed to Decode is sampled at hz (not part of the reference, which decodes at DataRate*ChipLength
+    // only): between RegisterProtocol and Allocate; hz != DataRate*ChipLength resamples on the GPU
+    // (ertgpu_set_input_rate).  Throws std::invalid_argument for a rate outside [1/4, 4] x the decoder's.
+    void SetInputRate(int64_t hz);
+    bool Resampling() const { return resampling_; }
     void Allocate(int device = 0, int64_t maxBlocksPerCall = 0, int64_t maxCandidates = 0);  // decode.go:131-160
     // decode.go:163-197 for N = len/BlockSize2 consecutive blocks; throws std::length_error when len is
-    // not a multiple of BlockSize2 (the reference panics with a slice-bounds error, decode.go:222)
+    // not a multiple of BlockSize2 (the reference panics with a slice-bounds error, decode.go:222).  With an
+    // input rate, len is any whole number of IQ samples (even) and the blocks are those of the resampled stream.
     std::vector<MessagePtr> Decode(const uint8_t* input, size_t len);
+    // Whole blocks decoded since Allocate / Reset (resampled blocks with an input rate).
+    int64_t BlocksDecoded() const;
     // The second half of Decode (decode.go:177-187 + parse.go): candidates sorted by (block, preamble, idx) are
     // regrouped into per-block, per-preamble []Data and handed to the parsers filed under that preamble.  Needs
     // RegisterProtocol only (no device), so the parsers can be exercised on candidates from any source.
@@ -156,6 +164,9 @@ private:
     std::vector<std::vector<size_t>> by_pre_;   // parser indices per preamble (decode.go:124)
     std::vector<ertgpu_candidate> cands_;
     bool allocated_ = false;
+    bool resampling_ = false;
+    ertgpu_resampler_info rs_{};
+    int64_t input_samples_ = 0;  // since Allocate / Reset
 };
 
 void RegisterStockParsers();  // the effect of the reference's blank imports (main.go:37-44)

@@ -13,7 +13,7 @@ namespace receiver {
 
 Digest NewDigest(const protocol::Message& m) { return Digest(m.MsgType(), m.MeterType(), m.MeterID(), m.Checksum()); }
 
-Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall) {
+Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, int64_t sampleRate) {
     protocol::RegisterStockParsers();
     std::string list = msgtypes == "all" ? "scm,scm+,idm,r900" : msgtypes;  // main.go:67-73
     std::stringstream ss(list);
@@ -22,6 +22,7 @@ Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int6
         if (!name.empty()) d_.RegisterProtocol(protocol::NewParser(name, chipLength));  // main.go:77-82
     if (blocksPerCall <= 0) blocksPerCall = 4096;
     blocks_per_call_ = blocksPerCall;
+    if (sampleRate > 0) d_.SetInputRate(sampleRate);
     d_.Allocate(device, blocksPerCall, 0);  // main.go:86
     buf_bytes_ = (size_t)blocksPerCall * (size_t)d_.Cfg.BlockSize2;
     for (int k = 0; k < 2; k++) {
@@ -172,8 +173,10 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
     sample_blocks_ = 2 * (int64_t)d_.Cfg.BufferLength / (int64_t)bs2 + 1;
     FilterChain* fc = fc_.empty() ? nullptr : &fc_;
     const auto t0 = std::chrono::steady_clock::now();
+    const bool rs = d_.Resampling();   // the decoder takes any whole number of IQ samples and keeps the rest itself
+    if (rs && sample_file_) throw std::logic_error("-samplefile with a resampling input rate");
     int k = 0;
-    size_t carry = 0;  // bytes of a partial block kept at the front of the next buffer
+    size_t carry = 0;  // bytes of a partial block (a partial IQ sample when resampling) kept for the next buffer
     for (;;) {
         if (std::chrono::steady_clock::now() >= deadline_) {
             st.stopped = true;
@@ -185,12 +188,13 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
             if (n == 0) break;
             have += n;
         }
-        const size_t whole = have / bs2 * bs2;
+        const size_t whole = rs ? have / 2 * 2 : have / bs2 * bs2;
         if (whole) {
             auto msgs = d_.Decode(buf_[k], whole);
-            const int64_t call_first = stream_blocks_, nblocks = (int64_t)(whole / bs2);
+            const int64_t call_first = stream_blocks_;
+            const int64_t nblocks = rs ? d_.BlocksDecoded() - stream_blocks_ : (int64_t)(whole / bs2);
             st.blocks += nblocks;
-            st.bytes += (int64_t)whole;
+            st.bytes += (int64_t)whole;   // input bytes: two per input sample
             stream_blocks_ += nblocks;
             for (size_t i = 0; i < msgs.size() && !st.stopped;) {
                 size_t j = i;

@@ -60,7 +60,9 @@ private:
 class Receiver {
 public:
     // msgtypes: comma list as for -msgtype ("all" = scm,scm+,idm,r900, main.go:67-73)
-    Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall);
+    // sampleRate > 0: the capture's sample rate in Hz; a rate other than DataRate*ChipLength is resampled on the GPU
+    // (protocol::Decoder::SetInputRate) and blocks, dedup and filters then work on the resampled stream.
+    Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, int64_t sampleRate = 0);
     ~Receiver();
 
     protocol::Decoder& decoder() { return d_; }
