@@ -89,8 +89,9 @@ struct ertgpu_handle {
     int sm_count = 132;
 
     // state of the last enqueued pipeline (for fetch and taps)
-    bool pending = false;       // a pipeline is enqueued and not yet synchronised
-    bool uncopied = false;      // ... synchronised, candidates still only on the device
+    bool pending = false;       // work is enqueued on pending_stream and not yet synchronised
+    bool pending_counts = false;  // ... and it copies counters back (a resample_kernel launch alone does not)
+    bool uncopied = false;      // a pipeline is synchronised, its candidates still only on the device
     unsigned long long uncopied_n = 0;
     bool fresh = true;          // next pipeline must see zeroed history (start of stream / after reset)
     cudaStream_t pending_stream = nullptr;
@@ -135,8 +136,6 @@ struct ertgpu_handle {
     int64_t rs_hist_first = 0;  // first input sample held in d_rs_hist[rs_cur_hist]
     int64_t rs_hist_n = 0;
     int64_t rs_pend = 0;        // outputs at the front of d_rs_out[rs_cur_out] that wait for a whole block
-    bool rs_inflight = false;   // a resample_kernel launch without a pipeline behind it has not been waited for
-    cudaStream_t rs_stream = nullptr;
 };
 
 namespace {
@@ -277,6 +276,47 @@ cudaError_t launch_dep(bool pdl, K kern, dim3 grid, dim3 block, size_t smem, cud
     return cudaLaunchKernelEx(&cfg, kern, args...);
 }
 
+// Search by the sliding-window kernel; PAT...: the preambles' first 16 bits as compile-time constants (none: read
+// from sl).  Appends the instantiation to h->kernels, the constants spelt as in the source ("0xF953u, 0x16A3u").
+template <int NPRE, uint32_t... PAT>
+int launch_slide(ertgpu_handle* h, const uint32_t* plane, const SlideParams& sl, bool pdl, cudaStream_t st) {
+    const bool half = (h->dcfg.SL % 32) == 16;
+    const auto kern = half ? search_slide_kernel<NPRE, true, PAT...> : search_slide_kernel<NPRE, false, PAT...>;
+    static OncePerDevice once[2];
+    if (once[half].first(h->device))
+        CUDA_TRY(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (2 * kSlideMaxLoad + 4)));
+    const int smem = 2 * sl.load_words * 4 + 16;
+    const long long tiles = (sl.nwords + sl.tile_words - 1) / sl.tile_words;
+    int per_sm = (227 * 1024) / (smem + 1024);
+    if (per_sm > 2048 / kSlideThreads) per_sm = 2048 / kSlideThreads;
+    unsigned grid = (unsigned)std::min<long long>(tiles, (long long)h->sm_count * per_sm);
+    if (grid < 1) grid = 1;
+    CUDA_TRY(h, launch_dep(pdl, kern, dim3(grid), dim3(kSlideThreads), (size_t)smem, st, plane, sl, h->d_hits, h->d_words,
+                           h->cand_cap, h->d_counters));
+    h->kernels += ";search_slide_kernel<" + std::to_string(NPRE) + (half ? ",true" : ",false");
+    const uint32_t pat[] = {PAT..., kSlideRuntimePat};
+    for (int i = 0; pat[i] != kSlideRuntimePat; i++) {
+        char s[16];
+        snprintf(s, sizeof(s), "%s0x%04Xu", i ? ", " : ",", pat[i]);
+        h->kernels += s;
+    }
+    h->kernels += ">";
+    return ERTGPU_OK;
+}
+
+// Search by the per-bit-load kernel; mode = search_mode().
+template <int NPRE>
+int launch_search(ertgpu_handle* h, const uint32_t* plane, const SearchParams& sp, int mode, bool pdl, cudaStream_t st) {
+    const auto kern = mode == 1 ? search_kernel<NPRE, 1> : mode == 2 ? search_kernel<NPRE, 2> : search_kernel<NPRE, 0>;
+    const long long tiles = (sp.nwords + kSearchTile - 1) / kSearchTile;
+    unsigned grid = (unsigned)std::min<long long>(tiles, (long long)h->sm_count * 4);
+    if (grid < 1) grid = 1;
+    CUDA_TRY(h, launch_dep(pdl, kern, dim3(grid), dim3(kSearchThreads), 0, st, plane, sp, h->d_hits, h->d_words,
+                           h->cand_cap, h->d_counters));
+    h->kernels += ";search_kernel<" + std::to_string(NPRE) + "," + std::to_string(mode) + ">";
+    return ERTGPU_OK;
+}
+
 int launch_resample(ertgpu_handle* h, const RsArgs& a, cudaStream_t st);
 
 // Enqueue the whole per-call pipeline for `nblocks` blocks whose IQ bytes are at d_iq.  With rs, the resampler step
@@ -312,14 +352,12 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
         if (rc) return rc;
     }
     // 1. magnitude + matched filter + quantize + pack
-    char kname[160];
     if (h->demod_variant != 0) {
         int w_used = 0;
         int rc = launch_demod_fast(h->demod_variant, d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut,
                                    plane + c.hist_words, nblocks, c.BS, h->d_counters + kCntTile, st, &w_used);
         if (rc != 0) return fail(h, ERTGPU_ECUDA, "demod_fast launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-        snprintf(kname, sizeof(kname), "demod_fast_kernel<%d,%d>", h->demod_variant, w_used);
-        h->kernels = kname;
+        h->kernels = "demod_fast_kernel<" + std::to_string(h->demod_variant) + "," + std::to_string(w_used) + ">";
     } else {
         h->kernels = "demod_generic_kernel";
         int nthr = 128;
@@ -339,85 +377,53 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
     {
         SearchParams sp;
         SlideParams sl;
+        int rc = ERTGPU_OK;
         if (make_slide_params(c, p0, nwords, &sl)) {
-            const int smem = 2 * sl.load_words * 4 + 16;
-            const long long tiles = (nwords + sl.tile_words - 1) / sl.tile_words;
-            int per_sm = (227 * 1024) / (smem + 1024);
-            if (per_sm > 2048 / kSlideThreads) per_sm = 2048 / kSlideThreads;
-            unsigned grid = (unsigned)std::min<long long>(tiles, (long long)h->sm_count * per_sm);
-            if (grid < 1) grid = 1;
-            const bool half = (c.SL % 32) == 16;
-#define ERT_SLIDE_K(K)                                                                                           \
-    do {                                                                                                         \
-        static OncePerDevice once;                                                                               \
-        if (once.first(h->device))                                                                               \
-            CUDA_TRY(h, cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (2 * kSlideMaxLoad + 4))); \
-        CUDA_TRY(h, launch_dep(pdl, K, dim3(grid), dim3(kSlideThreads), (size_t)smem, st, (const uint32_t*)plane, sl, h->d_hits, h->d_words, \
-                               h->cand_cap, h->d_counters));                                                     \
-    } while (0)
-#define ERT_SLIDE(N, ...)                                                                    \
-    do {                                                                                     \
-        snprintf(kname, sizeof(kname), ";search_slide_kernel<%d,%s%s%s>", N, half ? "true" : "false", \
-                 sizeof(#__VA_ARGS__) > 1 ? "," : "", #__VA_ARGS__);                         \
-        if (half) ERT_SLIDE_K((search_slide_kernel<N, true, ##__VA_ARGS__>));                \
-        else ERT_SLIDE_K((search_slide_kernel<N, false, ##__VA_ARGS__>));                    \
-    } while (0)
             if (c.npre == 1) {
                 // single preamble: the stock protocols' first 16 bits are compile-time constants
                 // (scm 0xF953, scm+ 0x16A3, idm/netidm 0x5555, r900 0x0000), anything else runs the generic probe
                 switch (slide_pattern(c, 0)) {
-                    case 0xF953u: ERT_SLIDE(1, 0xF953u); break;
-                    case 0x16A3u: ERT_SLIDE(1, 0x16A3u); break;
-                    case 0x5555u: ERT_SLIDE(1, 0x5555u); break;
-                    case 0x0000u: ERT_SLIDE(1, 0x0000u); break;
-                    default: ERT_SLIDE(1); break;
+                    case 0xF953u: rc = launch_slide<1, 0xF953u>(h, plane, sl, pdl, st); break;
+                    case 0x16A3u: rc = launch_slide<1, 0x16A3u>(h, plane, sl, pdl, st); break;
+                    case 0x5555u: rc = launch_slide<1, 0x5555u>(h, plane, sl, pdl, st); break;
+                    case 0x0000u: rc = launch_slide<1, 0x0000u>(h, plane, sl, pdl, st); break;
+                    default: rc = launch_slide<1>(h, plane, sl, pdl, st); break;
                 }
             } else if (c.npre == 2) {
-                ERT_SLIDE(2);
+                rc = launch_slide<2>(h, plane, sl, pdl, st);
             } else if (c.npre == 3) {
                 // scm, scm+, idm (or netidm) registered in that order: BASELINE.json configs[2]
                 if (slide_pattern(c, 0) == 0xF953u && slide_pattern(c, 1) == 0x16A3u && slide_pattern(c, 2) == 0x5555u)
-                    ERT_SLIDE(3, 0xF953u, 0x16A3u, 0x5555u);
+                    rc = launch_slide<3, 0xF953u, 0x16A3u, 0x5555u>(h, plane, sl, pdl, st);
                 else
-                    ERT_SLIDE(3);
+                    rc = launch_slide<3>(h, plane, sl, pdl, st);
             } else {
                 // "-msgtype=all" = scm, scm+, idm, r900 (main.go:67-73)
                 if (c.npre == 4 && slide_pattern(c, 0) == 0xF953u && slide_pattern(c, 1) == 0x16A3u &&
                     slide_pattern(c, 2) == 0x5555u && slide_pattern(c, 3) == 0x0000u)
-                    ERT_SLIDE(4, 0xF953u, 0x16A3u, 0x5555u, 0x0000u);
+                    rc = launch_slide<4, 0xF953u, 0x16A3u, 0x5555u, 0x0000u>(h, plane, sl, pdl, st);
                 else
-                    ERT_SLIDE(4);
+                    rc = launch_slide<4>(h, plane, sl, pdl, st);
             }
-#undef ERT_SLIDE
-#undef ERT_SLIDE_K
         } else if (make_search_params(c, p0, nwords, &sp)) {
-            const size_t smem = 0;
-            long long tiles = (nwords + kSearchTile - 1) / kSearchTile;
-            unsigned grid = (unsigned)std::min<long long>(tiles, (long long)h->sm_count * 4);
-            if (grid < 1) grid = 1;
             const int mode = search_mode(c, p0);
-            snprintf(kname, sizeof(kname), ";search_kernel<%d,%d>", c.npre, mode);
-#define ERT_SEARCH(N, M) CUDA_TRY(h, launch_dep(pdl, search_kernel<N, M>, dim3(grid), dim3(kSearchThreads), smem, st, (const uint32_t*)plane, sp, h->d_hits, h->d_words, h->cand_cap, h->d_counters))
-#define ERT_SEARCH_N(N) do { if (mode == 1) ERT_SEARCH(N, 1); else if (mode == 2) ERT_SEARCH(N, 2); else ERT_SEARCH(N, 0); } while (0)
             switch (c.npre) {
-                case 1: ERT_SEARCH_N(1); break;
-                case 2: ERT_SEARCH_N(2); break;
-                case 3: ERT_SEARCH_N(3); break;
-                default: ERT_SEARCH_N(4); break;
+                case 1: rc = launch_search<1>(h, plane, sp, mode, pdl, st); break;
+                case 2: rc = launch_search<2>(h, plane, sp, mode, pdl, st); break;
+                case 3: rc = launch_search<3>(h, plane, sp, mode, pdl, st); break;
+                default: rc = launch_search<4>(h, plane, sp, mode, pdl, st); break;
             }
-#undef ERT_SEARCH_N
-#undef ERT_SEARCH
         } else {
             const int nthr = 256;
             long long blocks = std::min<long long>((nwords + nthr - 1) / nthr, (long long)h->sm_count * 16);
             if (blocks < 1) blocks = 1;
-            snprintf(kname, sizeof(kname), ";search_generic_kernel");
             CUDA_TRY(h, launch_dep(pdl, search_generic_kernel, dim3((unsigned)blocks), dim3(nthr), 0, st, (const uint32_t*)plane, p0, nwords, c,
                                    h->d_hits, h->d_words, h->cand_cap, h->d_counters));
+            h->kernels += ";search_generic_kernel";
         }
+        if (rc) return rc;
         CUDA_TRY(h, cudaGetLastError());
         h->launches++;
-        h->kernels += kname;
     }
 
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[2], st));
@@ -462,18 +468,14 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
         const unsigned grid = (unsigned)h->sm_count * 4;
         const bool dep = pdl && !h->has_r900;   // the r900 kernels between Search and Slice are ordinary launches
         constexpr int kFullK = (ERTGPU_MAX_PACKET_BYTES * 8 + 31) / 32;
-        if (c.PK <= 128)
-            CUDA_TRY(h, launch_dep(dep, extract_words_kernel<4>, dim3(grid), dim3(kExtractWarps * 32), 0, st, (const uint32_t*)plane, p0, c,
-                                   (const HitWord*)h->d_words, h->cand_cap, (const uint16_t*)h->d_crc, h->gf, digits, (long long)h->block_counter,
-                                   flags, h->d_out, h->cand_cap, h->d_counters, ca));
-        else
-            CUDA_TRY(h, launch_dep(dep, extract_words_kernel<kFullK>, dim3(grid), dim3(kExtractWarps * 32), 0,
-                                   st, (const uint32_t*)plane, p0, c, (const HitWord*)h->d_words, h->cand_cap, (const uint16_t*)h->d_crc, h->gf,
-                                   digits, (long long)h->block_counter, flags, h->d_out, h->cand_cap, h->d_counters, ca));
+        const bool short_packets = c.PK <= 128;
+        const auto kern = short_packets ? extract_words_kernel<4> : extract_words_kernel<kFullK>;
+        CUDA_TRY(h, launch_dep(dep, kern, dim3(grid), dim3(kExtractWarps * 32), 0, st, (const uint32_t*)plane, p0, c,
+                               (const HitWord*)h->d_words, h->cand_cap, (const uint16_t*)h->d_crc, h->gf, digits, (long long)h->block_counter,
+                               flags, h->d_out, h->cand_cap, h->d_counters, ca));
         CUDA_TRY(h, cudaGetLastError());
         h->launches++;
-        snprintf(kname, sizeof(kname), ";extract_words_kernel<%d>", c.PK <= 128 ? 4 : kFullK);
-        h->kernels += kname;
+        h->kernels += ";extract_words_kernel<" + std::to_string(short_packets ? 4 : kFullK) + ">";
     }
     if (rs) h->kernels += ";resample_kernel";
 
@@ -488,7 +490,7 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
     h->last_plane = plane;
     h->last_first_block = h->block_counter;
     h->last_nblocks = nblocks;
-    h->pending = true;
+    h->pending = h->pending_counts = true;
     h->pending_stream = st;
 
     h->cur_plane ^= 1;
@@ -505,15 +507,13 @@ bool cand_less(const ertgpu_candidate& a, const ertgpu_candidate& b) {
     return a.idx < b.idx;
 }
 
-// Wait for the pending pipeline and read its counters (candidates stay on the device).
+// Wait for the pending work and read the counters of its pipeline (candidates stay on the device).  A resample_kernel
+// launch alone is waited for too: it read the caller's input and wrote the resampler state the next call reads.
 int collect_sync(ertgpu_handle* h) {
-    if (h->rs_inflight) {  // it read the caller's input and wrote the resampler state the next call reads
-        CUDA_TRY(h, cudaStreamSynchronize(h->rs_stream));
-        h->rs_inflight = false;
-    }
     if (!h->pending) return ERTGPU_OK;
     CUDA_TRY(h, cudaStreamSynchronize(h->pending_stream));
     h->pending = false;
+    if (!h->pending_counts) return ERTGPU_OK;
     const unsigned long long nh = h->h_counters[0], no = h->h_counters[1], nv = h->h_counters[2];
     h->total_hits += (int64_t)nh;
     h->total_valid += (int64_t)nv;
@@ -670,78 +670,42 @@ void rs_commit(ertgpu_handle* h, const RsArgs& a, int64_t nblocks) {
     }
 }
 
-// Enqueue one planned step: the resampler, then the decoder pipeline over the whole blocks it completed.
-int rs_run(ertgpu_handle* h, const RsArgs& a, int64_t nblocks, uint32_t flags, cudaStream_t st) {
-    int rc;
-    if (nblocks > 0) {
-        rc = enqueue_pipeline(h, h->d_rs_out[h->rs_cur_out], nblocks, flags, st, &a);
-    } else {  // no pipeline to wait for: collect_sync waits for this launch instead
-        h->launches = 0;
-        rc = launch_resample(h, a, st);
-        if (rc == ERTGPU_OK && h->launches) {
-            h->rs_inflight = true;
-            h->rs_stream = st;
-            if (h->kernels.empty()) h->kernels = "resample_kernel";  // otherwise the last pipeline's list stays
-        }
-    }
-    if (rc) return rc;
-    rs_commit(h, a, nblocks);
-    return ERTGPU_OK;
-}
-
 void rs_reset_stream(ertgpu_handle* h) {
     h->rs_in_total = h->rs_out_next = h->rs_hist_first = h->rs_hist_n = h->rs_pend = 0;
 }
 
-// ertgpu_decode for a handle with an input rate: chunks of at most the staging size and of at most max_blocks
-// completed blocks; the H2D copy of chunk i+1 overlaps the kernels of chunk i as in the native path.
-int decode_resampled(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t flags, ertgpu_candidate* out,
-                     size_t cap, size_t* n_out) {
-    const int64_t total = (int64_t)(nbytes / 2);
-    if (total == 0) return deliver(h, out, cap, n_out);
-    int64_t chunk_mib = 32;
-    if (const char* e = getenv("ERTGPU_CHUNK_MIB")) chunk_mib = std::max(1, atoi(e));  // tuning knob
-    const int64_t chunk = std::min<int64_t>((chunk_mib << 20) / 2,
-                                            4 * (h->max_blocks + 1) * (int64_t)h->cfg.block_size + h->rs.T + 8);
-    bool pageable = true;
-    {
-        int rc = prepare_staging(h, (size_t)chunk * 2, iq, &pageable);
-        if (rc) return rc;
-    }
-    int64_t done = 0, launches = 0;
-    std::string kernels;
-    for (int64_t i = 0; done < total; i++) {
-        const int k = (int)(i & 1);
-        const int64_t c = std::min(std::min(chunk, total - done), rs_max_input(h));
-        if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // the kernels that read d_stage[k] (and its H2D) are done
-        const uint8_t* src = iq + (size_t)done * 2;
-        if (pageable) {
-            h->copy_pool->copy(h->h_stage[k], src, (size_t)c * 2);
-            src = h->h_stage[k];
+// Whole decoder blocks that the next n input samples complete.
+int64_t step_blocks(const ertgpu_handle* h, int64_t n) {
+    if (!h->rs_on) return n / h->cfg.block_size;
+    RsArgs a;
+    int64_t nb = 0;
+    rs_plan_step(h, nullptr, n, &a, &nb);
+    return nb;
+}
+
+// Enqueue the work for the next n input samples, at d_in on the device, on st: the pipeline over the whole blocks
+// they complete, behind the resampler step that produces those blocks when the handle resamples.
+int enqueue_step(ertgpu_handle* h, const uint8_t* d_in, int64_t n, uint32_t flags, cudaStream_t st) {
+    if (!h->rs_on) return enqueue_pipeline(h, d_in, n / h->cfg.block_size, flags, st);
+    RsArgs a;
+    int64_t nb = 0;
+    rs_plan_step(h, d_in, n, &a, &nb);
+    int rc;
+    if (nb > 0) {
+        rc = enqueue_pipeline(h, h->d_rs_out[h->rs_cur_out], nb, flags, st, &a);
+    } else {  // no pipeline: the launch alone is pending, with no counters to read
+        h->launches = 0;
+        rc = launch_resample(h, a, st);
+        if (rc == ERTGPU_OK && h->launches) {
+            h->pending = true;
+            h->pending_counts = false;
+            h->pending_stream = st;
+            if (h->kernels.empty()) h->kernels = "resample_kernel";  // otherwise the last pipeline's list stays
         }
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * 2, cudaMemcpyHostToDevice, h->copy_stream));
-        CUDA_TRY(h, cudaEventRecord(h->ev_h2d[k], h->copy_stream));
-        if (i >= 1) {
-            int rc = collect(h);
-            if (rc) return rc;
-        }
-        CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[k], 0));
-        RsArgs a;
-        int64_t nb = 0;
-        rs_plan_step(h, h->d_stage[k], c, &a, &nb);
-        int rc = rs_run(h, a, nb, flags, h->stream);
-        if (rc) return rc;
-        if (nb > 0) kernels = h->kernels;
-        launches += h->launches;
-        CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
-        done += c;
     }
-    int rc = collect(h);  // also waits for a last step that completed no block (ertgpu_decode is synchronous)
     if (rc) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));  // a step that launched nothing still copied from iq
-    h->launches = launches;
-    if (!kernels.empty()) h->kernels = kernels;
-    return deliver(h, out, cap, n_out);
+    rs_commit(h, a, nb);
+    return ERTGPU_OK;
 }
 
 void begin_call(ertgpu_handle* h) {
@@ -750,6 +714,34 @@ void begin_call(ertgpu_handle* h) {
     h->overflow = false;
     h->need = 0;
     h->total_hits = h->total_valid = 0;
+}
+
+// The start of both decode calls.  The input is checked before anything is collected, so that a rejected call leaves
+// the stream as it was: a resampling handle takes whole IQ samples (2-byte aligned on the device), a native one whole
+// blocks (16-byte aligned on the device), and a device call completes at most max_blocks_per_call blocks.  Then the
+// previous call's work is collected and this call's results start empty.
+int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
+    if (h && h->rs_on && nbytes % 2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of IQ samples", nbytes);
+    if (!h || !h->allocated) return ERTGPU_EINVAL;
+    if (!iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
+    const int align = h->rs_on ? 2 : 16;
+    if (device && (reinterpret_cast<uintptr_t>(iq) & (align - 1)) != 0)
+        return fail(h, ERTGPU_EINVAL, "device input must be %d-byte aligned", align);
+    const size_t bs2 = (size_t)h->cfg.block_size2;
+    if (!h->rs_on && nbytes % bs2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize2 %zu", nbytes, bs2);
+    if (device) {
+        const int64_t nb = step_blocks(h, (int64_t)(nbytes / 2));
+        if (nb > h->max_blocks)
+            return fail(h, ERTGPU_ESIZE, "%zu input bytes complete %lld blocks, more than max_blocks_per_call %lld", nbytes,
+                        (long long)nb, (long long)h->max_blocks);
+    }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    if (h->pending) {
+        int rc = collect(h);
+        if (rc) return rc;
+    }
+    begin_call(h);
+    return ERTGPU_OK;
 }
 
 }  // namespace
@@ -1033,14 +1025,8 @@ int ertgpu_get_config(const ertgpu_handle* h, ertgpu_decoder_config* cfg) {
 int ertgpu_reset(ertgpu_handle* h) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->rs_inflight) {
-        CUDA_TRY(h, cudaStreamSynchronize(h->rs_stream));
-        h->rs_inflight = false;
-    }
-    if (h->pending) {
-        CUDA_TRY(h, cudaStreamSynchronize(h->pending_stream));
-        h->pending = false;
-    }
+    int rc = collect_sync(h);
+    if (rc) return rc;
     h->uncopied = false;
     // the history in front of the next call is zeroed on that call's stream (enqueue_pipeline)
     h->fresh = true;
@@ -1091,39 +1077,10 @@ int ertgpu_set_demod_variant(ertgpu_handle* h, int32_t variant) {
 }
 
 int ertgpu_decode_device_async(ertgpu_handle* h, const void* d_iq, size_t nbytes, uint32_t flags, void* stream) {
-    if (h && h->rs_on && nbytes % 2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of IQ samples", nbytes);
-    if (!h || !h->allocated) return ERTGPU_EINVAL;
-    if (!d_iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
-    if (h->rs_on) {
-        if ((reinterpret_cast<uintptr_t>(d_iq) & 1) != 0) return fail(h, ERTGPU_EINVAL, "device input must be 2-byte aligned");
-        RsArgs a;
-        int64_t nb = 0;
-        rs_plan_step(h, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / 2), &a, &nb);
-        if (nb > h->max_blocks)
-            return fail(h, ERTGPU_ESIZE, "%zu input bytes complete %lld blocks, more than max_blocks_per_call %lld", nbytes,
-                        (long long)nb, (long long)h->max_blocks);
-        CUDA_TRY(h, cudaSetDevice(h->device));
-        if (h->pending || h->rs_inflight) {
-            int rc = collect(h);
-            if (rc) return rc;
-        }
-        begin_call(h);
-        if (nbytes == 0) return ERTGPU_OK;
-        return rs_run(h, a, nb, flags, stream ? (cudaStream_t)stream : h->stream);
-    }
-    if ((reinterpret_cast<uintptr_t>(d_iq) & 15) != 0) return fail(h, ERTGPU_EINVAL, "device input must be 16-byte aligned");
-    const size_t bs2 = (size_t)h->cfg.block_size2;
-    if (nbytes % bs2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize2 %zu", nbytes, bs2);
-    const int64_t nblocks = (int64_t)(nbytes / bs2);
-    if (nblocks > h->max_blocks) return fail(h, ERTGPU_ESIZE, "%lld blocks exceed max_blocks_per_call %lld", (long long)nblocks, (long long)h->max_blocks);
-    CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending || h->rs_inflight) {
-        int rc = collect(h);
-        if (rc) return rc;
-    }
-    begin_call(h);
-    if (nblocks == 0) return ERTGPU_OK;
-    return enqueue_pipeline(h, static_cast<const uint8_t*>(d_iq), nblocks, flags, stream ? (cudaStream_t)stream : h->stream);
+    const int rc = begin_decode(h, d_iq, nbytes, true);
+    if (rc || nbytes == 0) return rc;
+    return enqueue_step(h, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / 2), flags,
+                        stream ? (cudaStream_t)stream : h->stream);
 }
 
 int ertgpu_fetch(ertgpu_handle* h, ertgpu_candidate* out, size_t cap, size_t* n_out) {
@@ -1136,71 +1093,53 @@ int ertgpu_fetch(ertgpu_handle* h, ertgpu_candidate* out, size_t cap, size_t* n_
 
 int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t flags, ertgpu_candidate* out,
                   size_t cap, size_t* n_out) {
-    if (h && h->rs_on && nbytes % 2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of IQ samples", nbytes);
-    if (!h || !h->allocated) return ERTGPU_EINVAL;
-    if (!iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
-    if (h->rs_on) {
-        CUDA_TRY(h, cudaSetDevice(h->device));
-        if (h->pending || h->rs_inflight) {
-            int rc = collect(h);
-            if (rc) return rc;
-        }
-        begin_call(h);
-        return decode_resampled(h, iq, nbytes, flags, out, cap, n_out);
-    }
-    const size_t bs2 = (size_t)h->cfg.block_size2;
-    if (nbytes % bs2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize2 %zu", nbytes, bs2);
-    CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending || h->rs_inflight) {
-        int rc = collect(h);
-        if (rc) return rc;
-    }
-    begin_call(h);
-    const int64_t nblocks = (int64_t)(nbytes / bs2);
-    if (nblocks == 0) return deliver(h, out, cap, n_out);
+    int rc = begin_decode(h, iq, nbytes, false);
+    if (rc) return rc;
+    const int64_t total = (int64_t)(nbytes / 2), BS = h->cfg.block_size;
+    if (total == 0) return deliver(h, out, cap, n_out);
 
-    // staging chunks (allocated on first use): H2D of chunk i+1 overlaps the kernels of chunk i
-    int64_t chunk_mib = 32;
-    if (const char* e = getenv("ERTGPU_CHUNK_MIB")) chunk_mib = std::max(1, atoi(e));  // tuning knob
-    const int64_t chunk_blocks = std::min<int64_t>(h->max_blocks, std::max<int64_t>(1, (chunk_mib << 20) / (int64_t)bs2));
+    // Staging chunks (allocated on first use): the H2D copy of chunk i+1 overlaps the kernels of chunk i.  32 MiB of
+    // whole blocks natively; a resampling chunk also covers the filter's look-ahead, and the step that takes it
+    // completes at most max_blocks blocks (rs_max_input).
+    const int64_t chunk = h->rs_on ? std::min<int64_t>(16 << 20, 4 * (h->max_blocks + 1) * BS + h->rs.T + 8)
+                                   : BS * std::min<int64_t>(h->max_blocks, std::max<int64_t>(1, (32 << 20) / h->cfg.block_size2));
     bool pageable = true;
-    {
-        int rc = prepare_staging(h, (size_t)chunk_blocks * bs2, iq, &pageable);
-        if (rc) return rc;
-    }
+    rc = prepare_staging(h, (size_t)chunk * 2, iq, &pageable);
+    if (rc) return rc;
     int64_t done = 0, launches = 0;
-    for (int64_t i = 0; done < nblocks; i++) {
+    for (int64_t i = 0; done < total; i++) {
         const int k = (int)(i & 1);
-        const int64_t nb = std::min(chunk_blocks, nblocks - done);
+        int64_t c = std::min(chunk, total - done);
+        if (h->rs_on) c = std::min(c, rs_max_input(h));
         if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // the kernels that read d_stage[k] (and its H2D) are done
-        const uint8_t* src = iq + (size_t)done * bs2;
-        const size_t nbytes_chunk = (size_t)nb * bs2;
+        const uint8_t* src = iq + (size_t)done * 2;
         if (pageable) {
-            h->copy_pool->copy(h->h_stage[k], src, nbytes_chunk);
+            h->copy_pool->copy(h->h_stage[k], src, (size_t)c * 2);
             src = h->h_stage[k];
         }
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, nbytes_chunk, cudaMemcpyHostToDevice, h->copy_stream));
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * 2, cudaMemcpyHostToDevice, h->copy_stream));
         CUDA_TRY(h, cudaEventRecord(h->ev_h2d[k], h->copy_stream));
         if (i >= 1) {
-            int rc = collect(h);
+            rc = collect(h);
             if (rc) return rc;
         }
         CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[k], 0));
-        int rc = enqueue_pipeline(h, h->d_stage[k], nb, flags, h->stream);
+        rc = enqueue_step(h, h->d_stage[k], c, flags, h->stream);
         if (rc) return rc;
         launches += h->launches;
         CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
-        done += nb;
+        done += c;
     }
-    int rc = collect(h);
+    rc = collect(h);  // also waits for a last step that completed no block (ertgpu_decode is synchronous)
     if (rc) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));  // a step that launched nothing still copied from iq
     h->launches = launches;
     return deliver(h, out, cap, n_out);
 }
 
 int ertgpu_last_counts(ertgpu_handle* h, int64_t* n_candidates, int64_t* n_valid) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
-    if (h->pending || h->rs_inflight) {
+    if (h->pending) {
         CUDA_TRY(h, cudaSetDevice(h->device));
         int rc = collect_sync(h);  // counters only; ertgpu_fetch copies the candidates if wanted
         if (rc) return rc;
@@ -1215,7 +1154,7 @@ int64_t ertgpu_last_launches(const ertgpu_handle* h) { return h ? h->launches : 
 int ertgpu_tap(ertgpu_handle* h, int32_t which, int64_t block, void* dst, size_t cap, size_t* n_out) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending || h->rs_inflight) {
+    if (h->pending) {
         int rc = collect(h);
         if (rc) return rc;
     }
@@ -1284,10 +1223,8 @@ int ertgpu_tap(ertgpu_handle* h, int32_t which, int64_t block, void* dst, size_t
 int ertgpu_set_stage_timing(ertgpu_handle* h, int32_t enable) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending || h->rs_inflight) {
-        int rc = collect_sync(h);
-        if (rc) return rc;
-    }
+    const int rc = collect_sync(h);
+    if (rc) return rc;
     h->stage_timing = enable != 0;
     if (enable) {
         for (int k = 0; k < 4; k++) h->stage_sum[k] = 0;
@@ -1300,10 +1237,8 @@ int ertgpu_set_stage_timing(ertgpu_handle* h, int32_t enable) {
 int ertgpu_last_stage_ms(ertgpu_handle* h, float* ms4) {
     if (!h || !h->allocated || !ms4) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending || h->rs_inflight) {
-        int rc = collect_sync(h);
-        if (rc) return rc;
-    }
+    const int rc = collect_sync(h);
+    if (rc) return rc;
     if (!h->stage_valid) return fail(h, ERTGPU_EINVAL, "stage timing was not enabled for the last decode");
     for (int k = 0; k < 4; k++) CUDA_TRY(h, cudaEventElapsedTime(&ms4[k], h->ev_stage[k], h->ev_stage[k + 1]));
     return ERTGPU_OK;
@@ -1312,10 +1247,8 @@ int ertgpu_last_stage_ms(ertgpu_handle* h, float* ms4) {
 int ertgpu_stage_ms_mean(ertgpu_handle* h, float* ms4, int64_t* n_pipelines) {
     if (!h || !h->allocated || !ms4) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending || h->rs_inflight) {
-        int rc = collect_sync(h);
-        if (rc) return rc;
-    }
+    const int rc = collect_sync(h);
+    if (rc) return rc;
     fold_stage_times(h);
     for (int k = 0; k < 4; k++) ms4[k] = h->stage_n ? (float)(h->stage_sum[k] / (double)h->stage_n) : 0.0f;
     if (n_pipelines) *n_pipelines = h->stage_n;

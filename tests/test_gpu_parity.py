@@ -154,13 +154,16 @@ def _variant_is_bit_exact(sample_iq, kernel=None, ntiles=None):
         h.close()
 
 
-# Search instance each geometry reaches by default (prefix of the second entry of last_kernels()): the sliding-window
-# kernel for the stock geometries; search_kernel<NPRE, MODE> where it does not fit (SL % 16 != 0, SL outside
-# [64, 192]); search_generic_kernel where the halo of search_kernel is too large
-SEARCH_KERNEL = {("scm", 72): "search_slide_kernel<1,true,0xF953u",    # SL 144: odd bits half a word in
-                 ("scm,scm+,idm", 72): "search_slide_kernel<3,true,0xF953u",
-                 ("r900", 72): "search_slide_kernel<1,true,0x0000u",
-                 ("scm", 64): "search_slide_kernel<1,false,0xF953u",   # SL 128
+# Search instance each geometry reaches by default (the second entry of last_kernels()): the sliding-window kernel for
+# the stock geometries, with the stock preamble sets' patterns as compile-time constants; search_kernel<NPRE, MODE>
+# where it does not fit (SL % 16 != 0, SL outside [64, 192]); search_generic_kernel where the halo of search_kernel
+# is too large
+SEARCH_KERNEL = {("scm", 72): "search_slide_kernel<1,true,0xF953u>",    # SL 144: odd bits half a word in
+                 ("scm,scm+,idm", 72): "search_slide_kernel<3,true,0xF953u, 0x16A3u, 0x5555u>",
+                 ("scm,scm+,idm,r900", 72): "search_slide_kernel<4,true,0xF953u, 0x16A3u, 0x5555u, 0x0000u>",
+                 ("scm,scm+", 72): "search_slide_kernel<2,true>",        # no stock set: patterns read at run time
+                 ("r900", 72): "search_slide_kernel<1,true,0x0000u>",
+                 ("scm", 64): "search_slide_kernel<1,false,0xF953u>",   # SL 128
                  ("scm", 78): "search_kernel<1,0>",         # SL 156: SL % 16 != 0, SL % 32 == 28
                  ("scm", 16): "search_kernel<1,1>",         # SL 32 < 64, first start word aligned
                  ("scm", 24): "search_kernel<1,2>",         # SL 48 < 64, SL % 32 == 16
@@ -175,7 +178,7 @@ def test_legacy_search_kernel_agrees(built, mt, cl):
     assert len(cands) > 0
     h = capi.new_decoder(mt, cl)
     got = h.decode(whole_blocks(iq, h.cfg.block_size2))
-    assert h.last_kernels().split(";")[1].startswith(SEARCH_KERNEL[(mt, cl)]), h.last_kernels()
+    assert h.last_kernels().split(";")[1] == SEARCH_KERNEL[(mt, cl)], h.last_kernels()
     compare_candidates(h, got, o, cands)
     h.close()
 
