@@ -110,7 +110,13 @@ typedef struct {
 #define ERTGPU_TAP_QUANTIZED 2 /* uint8[BUF]       Decoder.Quantized after block b (decode.go:145,166,243) */
 #define ERTGPU_TAP_PACKED 3    /* uint8[(BS+PL+7)>>3] Decoder.packed after block b (decode.go:159,259-265) */
 #define ERTGPU_TAP_R900_QUANTIZED 4 /* uint8[BUF]  r900 Parser.quantized after block b (r900/r900.go:82-150) */
-#define ERTGPU_TAP_RESAMPLED 5 /* uint8[BlockSize2] the resampled IQ bytes of block b as the decoder read them (handles with an input rate) */
+#define ERTGPU_TAP_RESAMPLED 5 /* uint8[BlockSize2] the uint8 IQ bytes of block b as the decoder read them (handles that resample or convert their input) */
+
+/* input sample formats (ertgpu_set_input_format) */
+#define ERTGPU_FORMAT_CU8 0  /* interleaved uint8 I,Q (rtl_sdr, rtl_tcp): 2 bytes per sample, decoded as they are */
+#define ERTGPU_FORMAT_CS8 1  /* interleaved int8 I,Q (hackrf_transfer): 2 bytes per sample        */
+#define ERTGPU_FORMAT_CS16 2 /* interleaved little-endian int16 I,Q: 4 bytes per sample              */
+#define ERTGPU_FORMAT_CF32 3 /* interleaved little-endian float32 I,Q: 8 bytes per sample            */
 
 typedef struct ertgpu_handle ertgpu_handle;
 
@@ -169,6 +175,23 @@ int ertgpu_reset(ertgpu_handle *h);
  * runs only resample_kernel; ertgpu_last_kernels then keeps the list of the last call that ran the
  * decoder (demod first, resample_kernel last). */
 int ertgpu_set_input_rate(ertgpu_handle *h, int64_t hz);
+
+/* Declare the sample format of the IQ the handle will be fed (ERTGPU_FORMAT_*), before
+ * ertgpu_allocate (its order relative to ertgpu_set_input_rate is free).  Each component x is
+ * converted on the GPU to the byte the decoder reads,
+ *     u = (isnan(p) ? 0 : clamp(rint(p), -128, 127)) + 128,   p = fl32(x * scale)
+ * (one float32 multiply, both roundings to nearest even).  scale == 0 selects the format's
+ * default: 1 for cs8, 2^-8 for cs16, 2^7 for cf32, which map full scale to full scale.
+ * ERTGPU_FORMAT_CU8 (or never calling this) changes nothing; it takes no scale.  ERTGPU_EINVAL
+ * for an unknown format, a negative or non-finite scale, cu8 with a scale other than 0, or a
+ * call after ertgpu_allocate.  With s bytes per IQ sample, a handle that resamples takes any
+ * nbytes that is a multiple of s (device input s-byte aligned); one at the decoder's own rate
+ * takes a multiple of BlockSize * s (device input 16-byte aligned); otherwise ERTGPU_ESIZE /
+ * ERTGPU_EINVAL as for uint8 input.  ertgpu_decode_sharded rejects converting handles. */
+int ertgpu_set_input_format(ertgpu_handle *h, int32_t format, float scale);
+
+/* The format and the scale in effect (the default filled in). */
+int ertgpu_get_input_format(const ertgpu_handle *h, int32_t *format, float *scale);
 
 /* The resampler of a handle with an input rate: *info, and the (P+1)*T int16 prototype table
  * when table != NULL and cap (entries) is large enough; *n_out = number of table entries.

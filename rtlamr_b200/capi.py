@@ -20,6 +20,8 @@ CHECK_NONE, CHECK_CRC16, CHECK_IDM, CHECK_R900 = 0, 1, 2, 3
 DECODE_ONLY_VALID = 1
 CAND_HAS_R900 = 1
 TAP_SIGNAL, TAP_CSUM, TAP_QUANTIZED, TAP_PACKED, TAP_R900_QUANTIZED, TAP_RESAMPLED = range(6)
+FORMAT_CU8, FORMAT_CS8, FORMAT_CS16, FORMAT_CF32 = range(4)
+FORMAT_BYTES = {FORMAT_CU8: 2, FORMAT_CS8: 2, FORMAT_CS16: 4, FORMAT_CF32: 8}  # bytes per IQ sample
 
 
 class Protocol(C.Structure):
@@ -76,7 +78,7 @@ EXPORTS = [
     "ertgpu_last_stage_ms", "ertgpu_stage_ms_mean", "ertgpu_tap", "ertgpu_set_demod_variant",
     "ertgpu_host_alloc", "ertgpu_host_free", "ertgpu_synth_fill",
     "ertgpu_bind_host_thread", "ertgpu_last_kernels", "ertgpu_plan_shards", "ertgpu_decode_sharded",
-    "ertgpu_set_input_rate", "ertgpu_get_resampler",
+    "ertgpu_set_input_rate", "ertgpu_get_resampler", "ertgpu_set_input_format", "ertgpu_get_input_format",
 ]
 
 _lib = None
@@ -131,6 +133,8 @@ def lib() -> C.CDLL:
     L.ertgpu_decode_sharded.argtypes = [C.POINTER(vp), i32, vp, sz, u32, vp, sz, C.POINTER(sz)]
     L.ertgpu_set_input_rate.argtypes = [vp, i64]
     L.ertgpu_get_resampler.argtypes = [vp, C.POINTER(ResamplerInfo), vp, sz, C.POINTER(sz)]
+    L.ertgpu_set_input_format.argtypes = [vp, i32, C.c_float]
+    L.ertgpu_get_input_format.argtypes = [vp, C.POINTER(i32), C.POINTER(C.c_float)]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the library does not export it
     _lib = L
@@ -175,6 +179,17 @@ class Handle:
     def set_input_rate(self, hz: int):
         """ertgpu_set_input_rate: the IQ fed to this handle is sampled at `hz` (between register and allocate)."""
         self._check(self._L.ertgpu_set_input_rate(self._h, int(hz)))
+
+    def set_input_format(self, fmt: int, scale: float = 0.0):
+        """ertgpu_set_input_format: the IQ fed to this handle is in format FORMAT_* with gain `scale` (0: the format's
+        default), before allocate."""
+        self._check(self._L.ertgpu_set_input_format(self._h, int(fmt), float(scale)))
+
+    def input_format(self):
+        """ertgpu_get_input_format: (format, scale in effect)."""
+        f, g = C.c_int32(0), C.c_float(0)
+        self._check(self._L.ertgpu_get_input_format(self._h, C.byref(f), C.byref(g)))
+        return f.value, g.value
 
     def resampler(self):
         """ertgpu_get_resampler: (info dict, int16 table of (P+1)*T entries)."""
@@ -273,9 +288,11 @@ class Handle:
 
 
 def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per_call: int = 0,
-                max_candidates: int = 0, input_rate: int = 0) -> Handle:
+                max_candidates: int = 0, input_rate: int = 0, input_format: int = FORMAT_CU8,
+                input_scale: float = 0.0) -> Handle:
     """NewDecoder + RegisterProtocol(NewParser(name, chip_length)) for each name + Allocate
-    (reference main.go:64-86).  input_rate > 0: the IQ is sampled at that rate (ertgpu_set_input_rate)."""
+    (reference main.go:64-86).  input_rate > 0: the IQ is sampled at that rate (ertgpu_set_input_rate);
+    input_format / input_scale: its sample format and gain (ertgpu_set_input_format, not called for plain cu8)."""
     if isinstance(msgtypes, str):
         msgtypes = [m.strip() for m in msgtypes.split(",") if m.strip()]
     h = Handle()
@@ -283,6 +300,8 @@ def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per
         h.register(stock_protocol(m, chip_length))
     if input_rate:
         h.set_input_rate(input_rate)
+    if input_format != FORMAT_CU8 or input_scale:
+        h.set_input_format(input_format, input_scale)
     h.allocate(device, max_blocks_per_call, max_candidates)
     return h
 

@@ -3,7 +3,8 @@
 // (protocol/decode.go:45-63).
 //
 // Device data layout (all per handle):
-//   iq      : the call's interleaved uint8 I,Q bytes (caller's device buffer or a staging chunk)
+//   iq      : the call's interleaved uint8 I,Q bytes (caller's device buffer or a staging chunk; the resampler's or
+//             the format conversion's output buffer when the handle has an input rate or format)
 //   hist[2] : last PKL samples of the previous call (ping-pong) -- replaces the Signal tail
 //             (decode.go:165) and the r900 parser's private signal history (r900.go:169)
 //   plane[2]: packed quantizer output, 1 bit per sample, MSB first, laid out as
@@ -16,6 +17,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -28,6 +30,7 @@
 #include <thread>
 #include <vector>
 
+#include "convert.cuh"
 #include "copy_pool.hpp"
 #include "demod_fast.cuh"
 #include "demod_generic.cuh"
@@ -136,6 +139,12 @@ struct ertgpu_handle {
     int64_t rs_hist_first = 0;  // first input sample held in d_rs_hist[rs_cur_hist]
     int64_t rs_hist_n = 0;
     int64_t rs_pend = 0;        // outputs at the front of d_rs_out[rs_cur_out] that wait for a whole block
+
+    // input format (ertgpu_set_input_format); ERTGPU_FORMAT_CU8 converts nothing
+    int32_t fmt = ERTGPU_FORMAT_CU8;
+    float fmt_scale = 0.0f;
+    int sample_bytes = 2;
+    uint8_t* d_cvt = nullptr;   // native rate, other formats: the converted uint8 IQ of the call's blocks
 };
 
 namespace {
@@ -229,6 +238,7 @@ void free_device(ertgpu_handle* h) {
     dfree(h->d_tap);
     dfree(h->d_rs_A);
     dfree(h->d_rs_D);
+    dfree(h->d_cvt);
     for (int k = 0; k < 2; k++) {
         dfree(h->d_rs_hist[k]);
         dfree(h->d_rs_out[k]);
@@ -318,11 +328,22 @@ int launch_search(ertgpu_handle* h, const uint32_t* plane, const SearchParams& s
 }
 
 int launch_resample(ertgpu_handle* h, const RsArgs& a, cudaStream_t st);
+int launch_convert(ertgpu_handle* h, const uint8_t* in, uint8_t* out, int64_t nsamples, cudaStream_t st);
+
+// "cs16" for the kernel labels of ertgpu_last_kernels
+const char* fmt_name(int f) {
+    return f == ERTGPU_FORMAT_CS8 ? "cs8" : f == ERTGPU_FORMAT_CS16 ? "cs16" : f == ERTGPU_FORMAT_CF32 ? "cf32" : "cu8";
+}
+
+std::string resample_label(const ertgpu_handle* h) {
+    return h->fmt == ERTGPU_FORMAT_CU8 ? "resample_kernel" : std::string("resample_kernel<") + fmt_name(h->fmt) + ">";
+}
 
 // Enqueue the whole per-call pipeline for `nblocks` blocks whose IQ bytes are at d_iq.  With rs, the resampler step
-// that writes those bytes runs first (its time counts as demod time).
+// that writes those bytes runs first; with cvt_in, the format conversion of the call's input at cvt_in into d_iq (either
+// one's time counts as demod time).
 int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uint32_t flags,
-                     cudaStream_t st, const RsArgs* rs = nullptr) {
+                     cudaStream_t st, const RsArgs* rs = nullptr, const uint8_t* cvt_in = nullptr) {
     const DevCfg& c = h->dcfg;
     uint32_t* plane = h->d_plane[h->cur_plane];
     uint32_t* plane_next = h->d_plane[h->cur_plane ^ 1];
@@ -349,6 +370,9 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[0], st));
     if (rs) {
         int rc = launch_resample(h, *rs, st);
+        if (rc) return rc;
+    } else if (cvt_in) {
+        int rc = launch_convert(h, cvt_in, const_cast<uint8_t*>(d_iq), nblocks * c.BS, st);
         if (rc) return rc;
     }
     // 1. magnitude + matched filter + quantize + pack
@@ -477,7 +501,8 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
         h->launches++;
         h->kernels += ";extract_words_kernel<" + std::to_string(short_packets ? 4 : kFullK) + ">";
     }
-    if (rs) h->kernels += ";resample_kernel";
+    if (rs) h->kernels += ";" + resample_label(h);
+    else if (cvt_in) h->kernels += std::string(";convert_kernel<") + fmt_name(h->fmt) + ">";
 
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[3], st));
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[4], st));
@@ -595,11 +620,36 @@ int prepare_staging(ertgpu_handle* h, size_t bytes, const void* iq, bool* pageab
 
 // ---- input-rate resampler (include/ertgpu_resample.h) ----
 
+// The resample_kernel instance of an input format.
+decltype(&resample_kernel<ERTGPU_FORMAT_CU8>) resample_kernel_of(int f) {
+    switch (f) {
+        case ERTGPU_FORMAT_CS8: return resample_kernel<ERTGPU_FORMAT_CS8>;
+        case ERTGPU_FORMAT_CS16: return resample_kernel<ERTGPU_FORMAT_CS16>;
+        case ERTGPU_FORMAT_CF32: return resample_kernel<ERTGPU_FORMAT_CF32>;
+        default: return resample_kernel<ERTGPU_FORMAT_CU8>;
+    }
+}
+
 int launch_resample(ertgpu_handle* h, const RsArgs& a, cudaStream_t st) {
     if (a.count <= 0 && a.carry_n <= 0) return ERTGPU_OK;
     const long long tiles = (a.count + kRsTile - 1) / kRsTile;
     const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(tiles, h->rs_grid));
-    resample_kernel<<<grid, kRsThreads, h->rs_smem, st>>>(h->d_rs_A, h->d_rs_D, a);
+    resample_kernel_of(h->fmt)<<<grid, kRsThreads, h->rs_smem, st>>>(h->d_rs_A, h->d_rs_D, a);
+    CUDA_TRY(h, cudaGetLastError());
+    h->launches++;
+    return ERTGPU_OK;
+}
+
+// Native-rate conversion of nsamples (a multiple of 8) IQ samples of the handle's format at `in` into uint8 IQ at out.
+int launch_convert(ertgpu_handle* h, const uint8_t* in, uint8_t* out, int64_t nsamples, cudaStream_t st) {
+    const long long groups = nsamples / 8;
+    const unsigned grid = (unsigned)std::max<long long>(
+        1, std::min<long long>((groups + kCvtThreads - 1) / kCvtThreads, (long long)h->sm_count * 8));
+    switch (h->fmt) {
+        case ERTGPU_FORMAT_CS8: convert_kernel<ERTGPU_FORMAT_CS8><<<grid, kCvtThreads, 0, st>>>(in, out, groups, h->fmt_scale); break;
+        case ERTGPU_FORMAT_CS16: convert_kernel<ERTGPU_FORMAT_CS16><<<grid, kCvtThreads, 0, st>>>(in, out, groups, h->fmt_scale); break;
+        default: convert_kernel<ERTGPU_FORMAT_CF32><<<grid, kCvtThreads, 0, st>>>(in, out, groups, h->fmt_scale); break;
+    }
     CUDA_TRY(h, cudaGetLastError());
     h->launches++;
     return ERTGPU_OK;
@@ -648,6 +698,7 @@ void rs_plan_step(const ertgpu_handle* h, const uint8_t* d_in, int64_t c, RsArgs
     a->L = L;
     a->M = M;
     a->T = (int)T;
+    a->scale = h->fmt_scale;
     const int64_t Q = (int64_t)ERTRS_P << ERTRS_F, step = kRsThreads * M;
     a->step_k = step / L;
     a->step_phi = step % L;
@@ -684,8 +735,10 @@ int64_t step_blocks(const ertgpu_handle* h, int64_t n) {
 }
 
 // Enqueue the work for the next n input samples, at d_in on the device, on st: the pipeline over the whole blocks
-// they complete, behind the resampler step that produces those blocks when the handle resamples.
+// they complete, behind the resampler step that produces those blocks when the handle resamples, or behind the
+// conversion of the input format at the decoder's own rate.
 int enqueue_step(ertgpu_handle* h, const uint8_t* d_in, int64_t n, uint32_t flags, cudaStream_t st) {
+    if (!h->rs_on && h->d_cvt) return enqueue_pipeline(h, h->d_cvt, n / h->cfg.block_size, flags, st, nullptr, d_in);
     if (!h->rs_on) return enqueue_pipeline(h, d_in, n / h->cfg.block_size, flags, st);
     RsArgs a;
     int64_t nb = 0;
@@ -700,7 +753,7 @@ int enqueue_step(ertgpu_handle* h, const uint8_t* d_in, int64_t n, uint32_t flag
             h->pending = true;
             h->pending_counts = false;
             h->pending_stream = st;
-            if (h->kernels.empty()) h->kernels = "resample_kernel";  // otherwise the last pipeline's list stays
+            if (h->kernels.empty()) h->kernels = resample_label(h);  // otherwise the last pipeline's list stays
         }
     }
     if (rc) return rc;
@@ -717,20 +770,26 @@ void begin_call(ertgpu_handle* h) {
 }
 
 // The start of both decode calls.  The input is checked before anything is collected, so that a rejected call leaves
-// the stream as it was: a resampling handle takes whole IQ samples (2-byte aligned on the device), a native one whole
-// blocks (16-byte aligned on the device), and a device call completes at most max_blocks_per_call blocks.  Then the
-// previous call's work is collected and this call's results start empty.
+// the stream as it was: with s bytes per IQ sample, a resampling handle takes whole IQ samples (s-byte aligned on the
+// device), a native one whole blocks of BlockSize * s bytes (16-byte aligned on the device), and a device call
+// completes at most max_blocks_per_call blocks.  Then the previous call's work is collected and this call's results
+// start empty.
 int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
-    if (h && h->rs_on && nbytes % 2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of IQ samples", nbytes);
+    if (h && h->rs_on && nbytes % h->sample_bytes)
+        return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of %d-byte IQ samples", nbytes, h->sample_bytes);
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     if (!iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
-    const int align = h->rs_on ? 2 : 16;
+    const int align = h->rs_on ? h->sample_bytes : 16;
     if (device && (reinterpret_cast<uintptr_t>(iq) & (align - 1)) != 0)
         return fail(h, ERTGPU_EINVAL, "device input must be %d-byte aligned", align);
     const size_t bs2 = (size_t)h->cfg.block_size2;
-    if (!h->rs_on && nbytes % bs2) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize2 %zu", nbytes, bs2);
+    if (!h->rs_on && h->fmt == ERTGPU_FORMAT_CU8 && nbytes % bs2)
+        return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize2 %zu", nbytes, bs2);
+    const size_t bsf = (size_t)h->cfg.block_size * h->sample_bytes;
+    if (!h->rs_on && nbytes % bsf)
+        return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize * %d = %zu", nbytes, h->sample_bytes, bsf);
     if (device) {
-        const int64_t nb = step_blocks(h, (int64_t)(nbytes / 2));
+        const int64_t nb = step_blocks(h, (int64_t)(nbytes / h->sample_bytes));
         if (nb > h->max_blocks)
             return fail(h, ERTGPU_ESIZE, "%zu input bytes complete %lld blocks, more than max_blocks_per_call %lld", nbytes,
                         (long long)nb, (long long)h->max_blocks);
@@ -1000,14 +1059,17 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
         {   // a property of the kernel, not of the handle: every handle on the device gets the largest any table needs
             static OncePerDevice once;
             if (once.first(h->device))
-                CUDA_TRY(h, cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF32; f++)
+                    CUDA_TRY(h, cudaFuncSetAttribute(resample_kernel_of(f), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         }
         if (h->rs_smem > 227 * 1024) return fail(h, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", h->rs_smem);
         int per_sm = 0;
-        CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel, kRsThreads, h->rs_smem));
+        CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel_of(h->fmt), kRsThreads, h->rs_smem));
         h->rs_grid = std::max(1, per_sm) * h->sm_count;
         h->rs_cur_hist = h->rs_cur_out = 0;
         rs_reset_stream(h);
+    } else if (h->fmt != ERTGPU_FORMAT_CU8) {
+        CUDA_TRY(h, cudaMalloc(&h->d_cvt, (size_t)max_blocks_per_call * c.block_size2));   // 256-byte aligned
     }
     h->cur_plane = h->cur_hist = 0;
     h->hist_valid = 0;
@@ -1058,6 +1120,27 @@ int ertgpu_set_input_rate(ertgpu_handle* h, int64_t hz) {
     return ERTGPU_OK;
 }
 
+int ertgpu_set_input_format(ertgpu_handle* h, int32_t format, float scale) {
+    if (!h) return ERTGPU_EINVAL;
+    if (h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_format after allocate");
+    if (format < ERTGPU_FORMAT_CU8 || format > ERTGPU_FORMAT_CF32) return fail(h, ERTGPU_EINVAL, "unknown input format %d", format);
+    if (!std::isfinite(scale) || scale < 0.0f) return fail(h, ERTGPU_EINVAL, "input scale %g is not a finite value >= 0", (double)scale);
+    if (format == ERTGPU_FORMAT_CU8 && scale != 0.0f) return fail(h, ERTGPU_EINVAL, "cu8 input is not scaled (scale %g)", (double)scale);
+    if (scale == 0.0f)
+        scale = format == ERTGPU_FORMAT_CS8 ? 1.0f : format == ERTGPU_FORMAT_CS16 ? 1.0f / 256.0f : format == ERTGPU_FORMAT_CF32 ? 128.0f : 0.0f;
+    h->fmt = format;
+    h->fmt_scale = scale;
+    h->sample_bytes = fmt_sample_bytes(format);
+    return ERTGPU_OK;
+}
+
+int ertgpu_get_input_format(const ertgpu_handle* h, int32_t* format, float* scale) {
+    if (!h) return ERTGPU_EINVAL;
+    if (format) *format = h->fmt;
+    if (scale) *scale = h->fmt_scale;
+    return ERTGPU_OK;
+}
+
 int ertgpu_get_resampler(const ertgpu_handle* h, ertgpu_resampler_info* info, int16_t* table, size_t cap,
                          size_t* n_out) {
     if (!h || !h->rs_on) return ERTGPU_EINVAL;
@@ -1079,7 +1162,7 @@ int ertgpu_set_demod_variant(ertgpu_handle* h, int32_t variant) {
 int ertgpu_decode_device_async(ertgpu_handle* h, const void* d_iq, size_t nbytes, uint32_t flags, void* stream) {
     const int rc = begin_decode(h, d_iq, nbytes, true);
     if (rc || nbytes == 0) return rc;
-    return enqueue_step(h, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / 2), flags,
+    return enqueue_step(h, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / h->sample_bytes), flags,
                         stream ? (cudaStream_t)stream : h->stream);
 }
 
@@ -1095,16 +1178,17 @@ int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t f
                   size_t cap, size_t* n_out) {
     int rc = begin_decode(h, iq, nbytes, false);
     if (rc) return rc;
-    const int64_t total = (int64_t)(nbytes / 2), BS = h->cfg.block_size;
+    const size_t s = (size_t)h->sample_bytes;
+    const int64_t total = (int64_t)(nbytes / s), BS = h->cfg.block_size;
     if (total == 0) return deliver(h, out, cap, n_out);
 
-    // Staging chunks (allocated on first use): the H2D copy of chunk i+1 overlaps the kernels of chunk i.  32 MiB of
-    // whole blocks natively; a resampling chunk also covers the filter's look-ahead, and the step that takes it
+    // Staging chunks (allocated on first use) of s bytes per sample: the H2D copy of chunk i+1 overlaps the kernels of
+    // chunk i.  32 MiB of whole decoder blocks natively; a resampling chunk also covers the filter's look-ahead, and the step that takes it
     // completes at most max_blocks blocks (rs_max_input).
     const int64_t chunk = h->rs_on ? std::min<int64_t>(16 << 20, 4 * (h->max_blocks + 1) * BS + h->rs.T + 8)
                                    : BS * std::min<int64_t>(h->max_blocks, std::max<int64_t>(1, (32 << 20) / h->cfg.block_size2));
     bool pageable = true;
-    rc = prepare_staging(h, (size_t)chunk * 2, iq, &pageable);
+    rc = prepare_staging(h, (size_t)chunk * s, iq, &pageable);
     if (rc) return rc;
     int64_t done = 0, launches = 0;
     for (int64_t i = 0; done < total; i++) {
@@ -1112,12 +1196,12 @@ int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t f
         int64_t c = std::min(chunk, total - done);
         if (h->rs_on) c = std::min(c, rs_max_input(h));
         if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // the kernels that read d_stage[k] (and its H2D) are done
-        const uint8_t* src = iq + (size_t)done * 2;
+        const uint8_t* src = iq + (size_t)done * s;
         if (pageable) {
-            h->copy_pool->copy(h->h_stage[k], src, (size_t)c * 2);
+            h->copy_pool->copy(h->h_stage[k], src, (size_t)c * s);
             src = h->h_stage[k];
         }
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * 2, cudaMemcpyHostToDevice, h->copy_stream));
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * s, cudaMemcpyHostToDevice, h->copy_stream));
         CUDA_TRY(h, cudaEventRecord(h->ev_h2d[k], h->copy_stream));
         if (i >= 1) {
             rc = collect(h);
@@ -1208,7 +1292,7 @@ int ertgpu_tap(ertgpu_handle* h, int32_t which, int64_t block, void* dst, size_t
         CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), qd, bytes.size(), cudaMemcpyDeviceToHost, h->stream));
         CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     } else if (which == ERTGPU_TAP_RESAMPLED) {
-        if (!h->rs_on) return fail(h, ERTGPU_EINVAL, "the handle does not resample");
+        if (!h->rs_on && h->fmt == ERTGPU_FORMAT_CU8) return fail(h, ERTGPU_EINVAL, "the handle neither resamples nor converts its input");
         bytes.resize((size_t)c.BS * 2);
         CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), h->last_iq + (size_t)b * c.BS * 2, bytes.size(), cudaMemcpyDeviceToHost, h->stream));
         CUDA_TRY(h, cudaStreamSynchronize(h->stream));

@@ -1,12 +1,13 @@
-// Input-rate resampler: uint8 IQ at R_in -> uint8 IQ at R_out = DataRate * ChipLength, in front of the demod.
+// Input-rate resampler: IQ at R_in -> uint8 IQ at R_out = DataRate * ChipLength, in front of the demod.
 // The arithmetic is include/ertgpu_resample.h's, all of it integer, so the bytes do not depend on the order
-// in which anything is summed.
+// in which anything is summed.  Input of another format (convert.cuh) is converted to uint8 as it is staged.
 #pragma once
 
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/ertgpu_resample.h"
+#include "convert.cuh"
 
 namespace ert {
 
@@ -15,7 +16,7 @@ constexpr int kRsPerThread = 8;
 constexpr long long kRsTile = (long long)kRsThreads * kRsPerThread;  // outputs per tile
 
 struct RsArgs {
-    // input samples [hist_first, hist_first + hist_n) are in hist, the next cur_n ones in cur
+    // input samples [hist_first, hist_first + hist_n) are in hist (uint8), the next cur_n ones in cur (the handle's format)
     const uint8_t* hist;
     const uint8_t* cur;
     long long hist_first, hist_n, cur_n;
@@ -32,6 +33,7 @@ struct RsArgs {
     // stepping kRsThreads outputs: phase + step_phi (wrapping at L), k + step_k, q + step_q remainder step_r
     long long step_k, step_phi, step_q, step_r;
     int T;
+    float scale;  // g of the input format (not read for uint8 input)
 };
 
 // The table as the kernel reads it: A[p][t] = h0 * 2^F + 2^(F-1) (int32), D[p][m] = the int16 pair
@@ -46,17 +48,25 @@ inline void rs_pack_table(const int16_t* table, int P, int T, int32_t* A, uint32
         }
 }
 
+// Input sample g as uint8 IQ: from the history as it is, from cur converted from format F.
+template <int F>
 __device__ __forceinline__ uchar2 rs_input(const RsArgs& a, long long g) {  // g >= 0
     const long long e = a.hist_first + a.hist_n;
-    const uint8_t* src = g < e ? a.hist + 2 * (g - a.hist_first) : a.cur + 2 * (g - e);
-    return *reinterpret_cast<const uchar2*>(src);
+    if constexpr (F == ERTGPU_FORMAT_CU8) {
+        const uint8_t* src = g < e ? a.hist + 2 * (g - a.hist_first) : a.cur + 2 * (g - e);
+        return *reinterpret_cast<const uchar2*>(src);
+    } else {
+        if (g < e) return *reinterpret_cast<const uchar2*>(a.hist + 2 * (g - a.hist_first));
+        return fmt_sample<F>(a.cur, g - e, a.scale);
+    }
 }
 
 // Persistent grid over tiles of kRsTile outputs.  Each CTA keeps the table in shared memory and stages the input
 // span of a tile as words X[j] = int8 bytes (v_I[j], v_I[j+1], v_Q[j], v_Q[j+1]), v = u - 128, so that one dp2a
 // per component applies two taps: with s = 2v + 1 and sum_t c_t = 2^S, acc = 2 * sum_t c_t * v_t + 2^S.  Thread t
 // computes outputs t, t + 256, ... of the tile.  Outputs whose window reaches before the stream start (s = 0 there)
-// take a per-tap path.
+// take a per-tap path.  F: the input format; the history and the carried samples are uint8 after conversion.
+template <int F>
 __global__ void __launch_bounds__(kRsThreads) resample_kernel(const int32_t* __restrict__ g_A,
                                                               const uint32_t* __restrict__ g_D, RsArgs a) {
     extern __shared__ __align__(16) int32_t rs_smem[];
@@ -68,7 +78,7 @@ __global__ void __launch_bounds__(kRsThreads) resample_kernel(const int32_t* __r
     for (int i = threadIdx.x; i < ERTRS_P * T2; i += blockDim.x) tabD[i] = g_D[i];
     if (blockIdx.x == 0)
         for (long long i = threadIdx.x; i < a.carry_n; i += blockDim.x)
-            *reinterpret_cast<uchar2*>(a.carry_dst + 2 * i) = rs_input(a, a.carry_first + i);  // carry_first >= 0
+            *reinterpret_cast<uchar2*>(a.carry_dst + 2 * i) = rs_input<F>(a, a.carry_first + i);  // carry_first >= 0
     const long long Q = (long long)ERTRS_P << ERTRS_F;
     const long long ntiles = (a.count + kRsTile - 1) / kRsTile;
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -80,8 +90,8 @@ __global__ void __launch_bounds__(kRsThreads) resample_kernel(const int32_t* __r
         __syncthreads();  // the previous tile's span is no longer read (and the table is in place)
         for (int i = threadIdx.x; i < nspan; i += blockDim.x) {
             const long long g = j_lo + i;
-            const uchar2 u0 = g >= 0 ? rs_input(a, g) : make_uchar2(128, 128);
-            const uchar2 u1 = (i + 1 < nspan && g + 1 >= 0) ? rs_input(a, g + 1) : make_uchar2(128, 128);
+            const uchar2 u0 = g >= 0 ? rs_input<F>(a, g) : make_uchar2(128, 128);
+            const uchar2 u1 = (i + 1 < nspan && g + 1 >= 0) ? rs_input<F>(a, g + 1) : make_uchar2(128, 128);
             X[i] = ((uint32_t)u0.x | ((uint32_t)u1.x << 8) | ((uint32_t)u0.y << 16) | ((uint32_t)u1.y << 24)) ^ 0x80808080u;
         }
         __syncthreads();

@@ -39,9 +39,11 @@ int ertgpu_decode_sharded(ertgpu_handle* const* handles, int32_t nhandles, const
     if (!handles || nhandles < 1 || (!iq && nbytes)) return ERTGPU_EINVAL;
     for (int32_t r = 0; r < nhandles; r++)
         if (!handles[r]) return ERTGPU_EINVAL;
-    for (int32_t r = 0; r < nhandles; r++) {  // shards are cut at decoder blocks of the input: no resampling handles
+    for (int32_t r = 0; r < nhandles; r++) {  // shards are cut at decoder blocks of uint8 input: no resampling or converting handles
         ertgpu_resampler_info ri;
         if (ertgpu_get_resampler(handles[r], &ri, nullptr, 0, nullptr) == ERTGPU_OK) return ERTGPU_EINVAL;
+        int32_t fmt = ERTGPU_FORMAT_CU8;
+        if (ertgpu_get_input_format(handles[r], &fmt, nullptr) != ERTGPU_OK || fmt != ERTGPU_FORMAT_CU8) return ERTGPU_EINVAL;
     }
     ertgpu_decoder_config c0;
     int rc = ertgpu_get_config(handles[0], &c0);

@@ -44,6 +44,11 @@ def lib():
         L.erthost_new_rate.restype = C.c_void_p
         L.erthost_new_rate.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_char_p,
                                        C.c_int]
+        L.erthost_new_format.restype = C.c_void_p
+        L.erthost_new_format.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_int,
+                                         C.c_float, C.c_char_p, C.c_int]
+        L.erthost_wav_probe.argtypes = [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
+                                        C.POINTER(C.c_longlong), C.c_char_p, C.c_int]
         L.erthost_free.argtypes = [C.c_void_p]
         L.erthost_error.restype = C.c_char_p
         L.erthost_error.argtypes = [C.c_void_p]
@@ -153,6 +158,17 @@ Parsers.parse_filtered = _parse_filtered
 Parsers.encode = _encode
 
 
+def wav_probe(path) -> dict:
+    """erthost_wav_probe: the header of a baseband WAV file (format = capi.FORMAT_*, rate in Hz, data offset and size
+    in bytes, size -1 = to the end of the file).  Raises ValueError naming the field that cannot be decoded."""
+    L = lib()
+    fmt, rate, off, size = C.c_int(0), C.c_longlong(0), C.c_longlong(0), C.c_longlong(0)
+    err = C.create_string_buffer(512)
+    if L.erthost_wav_probe(os.fsencode(path), C.byref(fmt), C.byref(rate), C.byref(off), C.byref(size), err, 512) != 0:
+        raise ValueError(err.value.decode())
+    return {"format": fmt.value, "rate": rate.value, "data_offset": off.value, "data_size": size.value}
+
+
 class Receiver:
     """NewDecoder + RegisterProtocol(NewParser(..)) + Allocate, then Decode (main.go:59-86,235)."""
 
@@ -160,12 +176,16 @@ class Receiver:
            "PacketSymbols", "PreambleLength", "PacketLength", "BufferLength", "CenterFreq")
 
     def __init__(self, msgtypes: str, chip_length: int = 72, device: int = 0, max_blocks: int = 0, max_cands: int = 0,
-                 input_rate: int = 0):
+                 input_rate: int = 0, input_format: int = 0, input_scale: float = 0.0):
         """input_rate > 0: the IQ given to decode() is sampled at that rate (erthost_new_rate); any rate other than
-        DataRate * ChipLength is resampled on the GPU and decode() then takes any even number of bytes."""
+        DataRate * ChipLength is resampled on the GPU and decode() then takes any whole number of IQ samples.
+        input_format / input_scale: the IQ's sample format (capi.FORMAT_*) and gain (erthost_new_format)."""
         self._L = lib()
         err = C.create_string_buffer(512)
-        if input_rate:
+        if input_format or input_scale:
+            self._h = self._L.erthost_new_format(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate,
+                                                 input_format, input_scale, err, 512)
+        elif input_rate:
             self._h = self._L.erthost_new_rate(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate,
                                                err, 512)
         else:

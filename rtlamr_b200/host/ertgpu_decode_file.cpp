@@ -1,12 +1,20 @@
-// ertgpu_decode_file -- decode a raw uint8 IQ capture (rtl_sdr / rtlamr -samplefile format) or stdin
-// through the C++ mirror of rtlamr's receive loop (receiver.hpp) on the GPU and print one line per message
-// in rtlamr's plain format without the time fields (protocol/parse.go:119-121 StringNoOffset).
+// ertgpu_decode_file -- decode an IQ capture (raw uint8 IQ as rtl_sdr and rtlamr -samplefile write it, raw int8,
+// int16 or float32 IQ, or a baseband WAV recording) or stdin through the C++ mirror of rtlamr's receive loop
+// (receiver.hpp) on the GPU and print one line per message in rtlamr's plain format without the time fields
+// (protocol/parse.go:119-121 StringNoOffset).
 //   ertgpu_decode_file [-msgtype=scm,idm|all] [-symbollength=72] [-blockdedup=true] [-blocks=4096] [-device=0]
 //                      [-filterid=1,2] [-filtertype=4,5] [-unique=true] [-format=plain|csv|json|xml]
-//                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ] FILE|- [FILE ...]
+//                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ]
+//                      [-sampleformat=cu8|cs8|cs16|cf32|wav] [-samplescale=G] FILE|- [FILE ...]
 // -samplerate is rtlamr's (rtltcp's) flag name; here it names the capture's sample rate.  The default,
 // 32768 * -symbollength, decodes the bytes as they are; any other rate within 1/4 ... 4 times it is resampled
-// exactly on the GPU first, and Block / Idx then count resampled samples.  It cannot be combined with -samplefile.
+// exactly on the GPU first, and Block / Idx then count resampled samples.
+// -sampleformat names the capture's samples: cu8 (the default: uint8, rtl_sdr), cs8 (int8, hackrf_transfer), cs16
+// (little-endian int16: airspy_rx, rx_sdr, SoapySDR), cf32 (little-endian float32: GNU Radio, gqrx) or wav (SDR#,
+// SDR++, SDRuno, HDSDR: each file's header gives the format and the rate; wav.hpp).  Other formats are converted to
+// uint8 on the GPU, u = clamp(rint(x * G), -128, 127) + 128; -samplescale=G is that gain (default 1 for cs8, 2^-8 for
+// cs16, 2^7 for cf32: full scale to full scale; a 12-bit Airspy wants 0.0625).  A WAV file is never detected by its
+// content or name.  -samplefile takes only uint8 input at 32768 * -symbollength (an 8-bit WAV at that rate is uint8).
 // -filterid / -filtertype / -unique, -format, -samplefile, -single and -duration are rtlamr's flags of the same names
 // (flags.go:37-58,69-70,140-170; the filter chain runs before the cross-block dedup, main.go:236-260).  With -format=csv a
 // line is LogMessage.Record() (parse.go:123-129: time, offset, length, then the message's own record) through Go's
@@ -19,6 +27,7 @@
 // each starts from zeroed history with block numbers from 0, exactly as if it were decoded alone.  They share the
 // sample file, whose offsets keep growing from one file to the next.
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <ctime>
@@ -26,6 +35,7 @@
 #include <vector>
 
 #include "receiver.hpp"
+#include "wav.hpp"
 
 int main(int argc, char** argv) {
     const auto start = std::chrono::steady_clock::now();   // main.go:350-353: the time limit covers the whole run
@@ -34,13 +44,19 @@ int main(int argc, char** argv) {
     int chip = 72, device = 0;
     long long blocks = 4096, samplerate = 0;
     bool block_dedup = true, quiet = false, unique = false, single = false;
-    std::string filterid, filtertype, format = "plain", samplefile, duration;
+    std::string filterid, filtertype, format = "plain", samplefile, duration, sampleformat = "cu8", samplescale;
+    bool have_scale = false;
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
         if (a.rfind("-msgtype=", 0) == 0) msgtype = a.substr(9);
         else if (a.rfind("-symbollength=", 0) == 0) chip = atoi(a.c_str() + 14);
         else if (a.rfind("-device=", 0) == 0) device = atoi(a.c_str() + 8);
         else if (a.rfind("-samplerate=", 0) == 0) samplerate = atoll(a.c_str() + 12);
+        else if (a.rfind("-sampleformat=", 0) == 0) sampleformat = a.substr(14);
+        else if (a.rfind("-samplescale=", 0) == 0) {
+            samplescale = a.substr(13);
+            have_scale = true;
+        }
         else if (a.rfind("-blocks=", 0) == 0) blocks = atoll(a.c_str() + 8);
         else if (a.rfind("-blockdedup=", 0) == 0) block_dedup = a.substr(12) != "false";
         else if (a.rfind("-filterid=", 0) == 0) filterid = a.substr(10);
@@ -58,7 +74,8 @@ int main(int argc, char** argv) {
     if (files.empty()) {
         fprintf(stderr, "usage: %s [-msgtype=scm,scm+,idm,netidm,r900,r900bcd|all] [-symbollength=N] [-blockdedup=true|false] "
                         "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
-                        "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-quiet] FILE|- [FILE ...]\n", argv[0]);
+                        "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|wav] [-samplescale=G] "
+                        "[-quiet] FILE|- [FILE ...]\n", argv[0]);
         return 2;
     }
     const bool csv = format == "csv", json = format == "json", xml = format == "xml";
@@ -69,11 +86,65 @@ int main(int argc, char** argv) {
         fprintf(stderr, "invalid value \"%s\" for flag -duration: %s\n", duration.c_str(), e.what());
         return 2;
     }
+    const bool wav_in = sampleformat == "wav";
+    int32_t fmt = ERTGPU_FORMAT_CU8;
+    if (sampleformat == "cs8") fmt = ERTGPU_FORMAT_CS8;
+    else if (sampleformat == "cs16") fmt = ERTGPU_FORMAT_CS16;
+    else if (sampleformat == "cf32") fmt = ERTGPU_FORMAT_CF32;
+    else if (sampleformat != "cu8" && !wav_in) {
+        fprintf(stderr, "invalid value \"%s\" for flag -sampleformat: cu8, cs8, cs16, cf32 or wav\n", sampleformat.c_str());
+        return 2;
+    }
+    float scale = 0.0f;
+    if (have_scale) {
+        char* end = nullptr;
+        scale = strtof(samplescale.c_str(), &end);
+        if (samplescale.empty() || *end || !std::isfinite(scale) || scale <= 0.0f) {
+            fprintf(stderr, "invalid value \"%s\" for flag -samplescale: a finite gain > 0\n", samplescale.c_str());
+            return 2;
+        }
+    }
+    // wav: every file's header, before anything else (stdin's is consumed here, the files' are read again below)
+    std::vector<wav::Header> wav_hdr(files.size());
+    if (wav_in) {
+        for (size_t fi = 0; fi < files.size(); fi++) {
+            FILE* in = files[fi] == "-" ? stdin : fopen(files[fi].c_str(), "rb");
+            if (!in) {
+                perror(files[fi].c_str());
+                return 1;
+            }
+            try {
+                wav_hdr[fi] = wav::ReadHeader(in);
+            } catch (const std::exception& e) {
+                fprintf(stderr, "%s: %s\n", files[fi].c_str(), e.what());
+                if (in != stdin) fclose(in);
+                return 1;
+            }
+            if (in != stdin) fclose(in);
+            if (wav_hdr[fi].rate != wav_hdr[0].rate || wav_hdr[fi].format != wav_hdr[0].format) {
+                fprintf(stderr, "%s: %lld Hz, format %d, but %s: %lld Hz, format %d: the files of a batch share one decoder\n",
+                        files[0].c_str(), (long long)wav_hdr[0].rate, wav_hdr[0].format, files[fi].c_str(),
+                        (long long)wav_hdr[fi].rate, wav_hdr[fi].format);
+                return 2;
+            }
+        }
+        if (samplerate != 0 && samplerate != wav_hdr[0].rate) {
+            fprintf(stderr, "-samplerate=%lld disagrees with the WAV header's %lld Hz\n", samplerate, (long long)wav_hdr[0].rate);
+            return 2;
+        }
+        samplerate = wav_hdr[0].rate;
+        fmt = wav_hdr[0].format;
+    }
+    if (have_scale && fmt == ERTGPU_FORMAT_CU8) {
+        fprintf(stderr, "-samplescale does not apply to uint8 (cu8) input\n");
+        return 2;
+    }
     // -samplerate names the capture's rate; the default DataRate*ChipLength (32768 * -symbollength) resamples nothing
     const bool resampling = samplerate != 0 && samplerate != 32768LL * chip;
-    if (resampling && !samplefile.empty() && samplefile != "/dev/null") {
-        fprintf(stderr, "-samplefile cannot be combined with -samplerate=%lld (the capture is not at 32768 * -symbollength = %lld Hz)\n",
-                samplerate, 32768LL * chip);
+    if ((resampling || fmt != ERTGPU_FORMAT_CU8) && !samplefile.empty() && samplefile != "/dev/null") {
+        fprintf(stderr, "-samplefile needs uint8 (cu8) input at 32768 * -symbollength = %lld Hz; this input is %s at %lld Hz\n",
+                32768LL * chip, fmt == ERTGPU_FORMAT_CU8 ? "cu8" : fmt == ERTGPU_FORMAT_CS8 ? "cs8" : fmt == ERTGPU_FORMAT_CS16 ? "cs16" : "cf32",
+                samplerate ? samplerate : 32768LL * chip);
         return 2;
     }
     FILE* sample = nullptr;   // os.DevNull, the default, is never opened (flags.go:136-141)
@@ -85,7 +156,7 @@ int main(int argc, char** argv) {
         }
     }
     try {
-        receiver::Receiver rcvr(msgtype, chip, device, blocks, resampling ? samplerate : 0);
+        receiver::Receiver rcvr(msgtype, chip, device, blocks, resampling ? samplerate : 0, fmt, scale);
         fputs(rcvr.decoder().Log().c_str(), stderr);
         if (sample) rcvr.SetSampleFile(sample);
         if (limit_ns) rcvr.SetDeadline(start + std::chrono::nanoseconds(limit_ns));
@@ -111,6 +182,7 @@ int main(int argc, char** argv) {
                 return 1;
             }
             if (fi) rcvr.Reset();
+            if (wav_in && in != stdin) wav_hdr[fi] = wav::ReadHeader(in);   // the same header as above: to the samples
             auto st = rcvr.Run(in, block_dedup, [&](const protocol::Message& m, int64_t offset, int length) {
                 if (quiet) return;
                 if (csv || json || xml) {
@@ -126,12 +198,12 @@ int main(int argc, char** argv) {
                 } else {
                     printf("{Block:%lld Idx:%d %s:%s}\n", (long long)m.Block, m.Idx, m.MsgType().c_str(), m.String().c_str());
                 }
-            });
+            }, wav_in ? wav_hdr[fi].data_size : -1);
             if (in != stdin) fclose(in);
             fprintf(stderr, "%s%s%lld messages (%lld duplicates dropped) from %lld blocks, %.1f MB in %.3f s = %.1f Msamples/s\n",
                     files.size() > 1 ? file.c_str() : "", files.size() > 1 ? ": " : "", (long long)st.messages,
                     (long long)st.duplicates, (long long)st.blocks, st.bytes / 1e6, st.seconds,
-                    st.bytes / 2e6 / (st.seconds > 0 ? st.seconds : 1));
+                    st.samples / 1e6 / (st.seconds > 0 ? st.seconds : 1));
             if (st.stopped) break;
         }
     } catch (const std::exception& e) {

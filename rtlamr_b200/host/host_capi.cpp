@@ -1,5 +1,6 @@
 // host_capi.cpp -- a small C surface over the C++ protocol mirror so that the Python parity tests
 // (and a CLI) can drive Decoder/Parser exactly like rtlamr's main.go does (main.go:59-86,235).
+#include <cerrno>
 #include <cstdio>
 #include <cstring>
 #include <memory>
@@ -7,6 +8,7 @@
 
 #include "protocol.hpp"
 #include "receiver.hpp"
+#include "wav.hpp"
 
 extern "C" {
 
@@ -27,19 +29,28 @@ struct erthost {
     std::string err;
 };
 
-erthost* erthost_new_rate(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
-                          long long input_rate, char* errbuf, int errcap);
+erthost* erthost_new_format(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
+                            long long input_rate, int format, float scale, char* errbuf, int errcap);
 
 // main.go:59-86: NewDecoder; for each -msgtype NewParser + RegisterProtocol; Allocate
 erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
                      char* errbuf, int errcap) {
-    return erthost_new_rate(msgtypes_csv, chip_length, device, max_blocks, max_cands, 0, errbuf, errcap);
+    return erthost_new_format(msgtypes_csv, chip_length, device, max_blocks, max_cands, 0, ERTGPU_FORMAT_CU8, 0.0f, errbuf,
+                              errcap);
 }
 
 // The same for IQ sampled at input_rate Hz (0: the decoder's own DataRate * ChipLength); erthost_decode then takes
 // any whole number of IQ samples.
 erthost* erthost_new_rate(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
                           long long input_rate, char* errbuf, int errcap) {
+    return erthost_new_format(msgtypes_csv, chip_length, device, max_blocks, max_cands, input_rate, ERTGPU_FORMAT_CU8, 0.0f,
+                              errbuf, errcap);
+}
+
+// The same for IQ in sample format `format` (ERTGPU_FORMAT_*) with gain `scale` (0: the format's default);
+// erthost_decode then counts the format's bytes per sample.
+erthost* erthost_new_format(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
+                            long long input_rate, int format, float scale, char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;   // released only on success: a throwing NewParser / Allocate must not leak the handle
     try {
         protocol::RegisterStockParsers();
@@ -51,6 +62,7 @@ erthost* erthost_new_rate(const char* msgtypes_csv, int chip_length, int device,
             h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
         }
         if (input_rate > 0) h->d.SetInputRate(input_rate);
+        if (format != ERTGPU_FORMAT_CU8 || scale != 0.0f) h->d.SetInputFormat(format, scale);
         h->d.Allocate(device, max_blocks, max_cands);
         return h.release();
     } catch (const std::exception& e) {
@@ -253,6 +265,30 @@ static long long fill_msgs(const std::vector<protocol::MessagePtr>& msgs, erthos
             n++;
         }
         return n;
+    }
+}
+
+// The header of the WAV file at `path` (wav.hpp), nothing else: *format = ERTGPU_FORMAT_*, *rate in Hz, *data_offset and
+// *data_size in bytes (-1: to the end of the file).  Returns 0, or -1 with the message in errbuf.
+int erthost_wav_probe(const char* path, int* format, long long* rate, long long* data_offset, long long* data_size,
+                      char* errbuf, int errcap) {
+    FILE* f = fopen(path, "rb");
+    if (!f) {
+        if (errbuf && errcap > 0) snprintf(errbuf, (size_t)errcap, "%s: %s", path, strerror(errno));
+        return -1;
+    }
+    try {
+        const wav::Header w = wav::ReadHeader(f);
+        fclose(f);
+        *format = w.format;
+        *rate = w.rate;
+        *data_offset = w.data_offset;
+        *data_size = w.data_size;
+        return 0;
+    } catch (const std::exception& e) {
+        fclose(f);
+        if (errbuf && errcap > 0) snprintf(errbuf, (size_t)errcap, "%s", e.what());
+        return -1;
     }
 }
 

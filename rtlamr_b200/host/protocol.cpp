@@ -606,6 +606,14 @@ void Decoder::SetInputRate(int64_t hz) {
     resampling_ = ertgpu_get_resampler(h_, &rs_, nullptr, 0, nullptr) == ERTGPU_OK;
 }
 
+void Decoder::SetInputFormat(int32_t format, float scale) {
+    if (allocated_) throw std::logic_error("SetInputFormat after Allocate");
+    int rc = ertgpu_set_input_format(h_, format, scale);
+    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
+    if (rc != ERTGPU_OK) raise(h_, rc, "SetInputFormat");
+    sample_bytes_ = format == ERTGPU_FORMAT_CS16 ? 4 : format == ERTGPU_FORMAT_CF32 ? 8 : 2;
+}
+
 int64_t Decoder::BlocksDecoded() const {
     if (!allocated_ || Cfg.BlockSize <= 0) return 0;
     if (!resampling_) return input_samples_ / Cfg.BlockSize;
@@ -618,9 +626,11 @@ int64_t Decoder::BlocksDecoded() const {
 
 std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
     if (!allocated_) throw std::logic_error("Decode before Allocate");
-    if (resampling_ ? (len % 2) != 0 : (len % (size_t)Cfg.BlockSize2) != 0)
+    const size_t s = (size_t)sample_bytes_;
+    if (resampling_ ? (len % s) != 0 : (len % ((size_t)Cfg.BlockSize * s)) != 0)
         throw std::length_error(resampling_ ? "input is not a whole number of IQ samples"
-                                            : "input is not a whole number of BlockSize2-byte blocks");
+                                            : s == 2 ? "input is not a whole number of BlockSize2-byte blocks"
+                                                     : "input is not a whole number of blocks");
     size_t n = 0;
     if (cands_.size() < 1024) cands_.resize(1024);
     int rc = ertgpu_decode(h_, input, len, ERTGPU_DECODE_ONLY_VALID, cands_.data(), cands_.size(), &n);
@@ -629,7 +639,7 @@ std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
         rc = ertgpu_fetch(h_, cands_.data(), cands_.size(), &n);
     }
     if (rc != ERTGPU_OK) raise(h_, rc, "Decode");
-    input_samples_ += (int64_t)(len / 2);
+    input_samples_ += (int64_t)(len / s);
 
     std::vector<MessagePtr> out;
     Dispatch(cands_.data(), n, out);

@@ -142,10 +142,16 @@ public:
     // (ertgpu_set_input_rate).  Throws std::invalid_argument for a rate outside [1/4, 4] x the decoder's.
     void SetInputRate(int64_t hz);
     bool Resampling() const { return resampling_; }
+    // The IQ fed to Decode is in format ERTGPU_FORMAT_* (not part of the reference, which takes uint8 IQ only): before
+    // Allocate; each component is converted on the GPU to the decoder's byte with gain `scale` (0: the format's
+    // default; ertgpu_set_input_format).  Throws std::invalid_argument for an unknown format or a bad scale.
+    void SetInputFormat(int32_t format, float scale = 0.0f);
+    int BytesPerSample() const { return sample_bytes_; }
     void Allocate(int device = 0, int64_t maxBlocksPerCall = 0, int64_t maxCandidates = 0);  // decode.go:131-160
     // decode.go:163-197 for N = len/BlockSize2 consecutive blocks; throws std::length_error when len is
     // not a multiple of BlockSize2 (the reference panics with a slice-bounds error, decode.go:222).  With an
-    // input rate, len is any whole number of IQ samples (even) and the blocks are those of the resampled stream.
+    // input rate, len is any whole number of IQ samples and the blocks are those of the resampled stream.  With an
+    // input format of s bytes per sample, len counts s bytes per sample (BlockSize * s per block).
     std::vector<MessagePtr> Decode(const uint8_t* input, size_t len);
     // Whole blocks decoded since Allocate / Reset (resampled blocks with an input rate).
     int64_t BlocksDecoded() const;
@@ -167,6 +173,7 @@ private:
     bool resampling_ = false;
     ertgpu_resampler_info rs_{};
     int64_t input_samples_ = 0;  // since Allocate / Reset
+    int sample_bytes_ = 2;       // bytes per input IQ sample
 };
 
 void RegisterStockParsers();  // the effect of the reference's blank imports (main.go:37-44)

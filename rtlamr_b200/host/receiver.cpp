@@ -5,6 +5,7 @@
 #include <cctype>
 #include <cerrno>
 #include <chrono>
+#include <cstdint>
 #include <cstring>
 #include <sstream>
 #include <stdexcept>
@@ -13,7 +14,8 @@ namespace receiver {
 
 Digest NewDigest(const protocol::Message& m) { return Digest(m.MsgType(), m.MeterType(), m.MeterID(), m.Checksum()); }
 
-Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, int64_t sampleRate) {
+Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, int64_t sampleRate,
+                   int32_t format, float scale) {
     protocol::RegisterStockParsers();
     std::string list = msgtypes == "all" ? "scm,scm+,idm,r900" : msgtypes;  // main.go:67-73
     std::stringstream ss(list);
@@ -23,8 +25,9 @@ Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int6
     if (blocksPerCall <= 0) blocksPerCall = 4096;
     blocks_per_call_ = blocksPerCall;
     if (sampleRate > 0) d_.SetInputRate(sampleRate);
+    if (format != ERTGPU_FORMAT_CU8) d_.SetInputFormat(format, scale);
     d_.Allocate(device, blocksPerCall, 0);  // main.go:86
-    buf_bytes_ = (size_t)blocksPerCall * (size_t)d_.Cfg.BlockSize2;
+    buf_bytes_ = (size_t)blocksPerCall * (size_t)d_.Cfg.BlockSize * (size_t)d_.BytesPerSample();
     for (int k = 0; k < 2; k++) {
         void* p = nullptr;
         if (ertgpu_host_alloc(&p, buf_bytes_) != ERTGPU_OK) {
@@ -166,9 +169,13 @@ void Receiver::KeepHistory(const uint8_t* call, size_t nblocks) {
     if (history_.size() > keep) history_.erase(history_.begin(), history_.end() - (ptrdiff_t)keep);
 }
 
-Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&, int64_t, int)>& emit) {
+Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&, int64_t, int)>& emit,
+                    int64_t max_bytes) {
     Stats st;
     const size_t bs2 = (size_t)d_.Cfg.BlockSize2;
+    const size_t s = (size_t)d_.BytesPerSample(), bsf = (size_t)d_.Cfg.BlockSize * s;   // bytes per input sample, per block
+    if (s != 2 && sample_file_) throw std::logic_error("-samplefile with converted input");
+    uint64_t left = max_bytes < 0 ? UINT64_MAX : (uint64_t)max_bytes;
     // main.go:225-230: sampleBuf grows by one block per block until it holds more than BufferLength<<1 bytes
     sample_blocks_ = 2 * (int64_t)d_.Cfg.BufferLength / (int64_t)bs2 + 1;
     FilterChain* fc = fc_.empty() ? nullptr : &fc_;
@@ -177,24 +184,28 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
     if (rs && sample_file_) throw std::logic_error("-samplefile with a resampling input rate");
     int k = 0;
     size_t carry = 0;  // bytes of a partial block (a partial IQ sample when resampling) kept for the next buffer
+    bool eof = false;
     for (;;) {
         if (std::chrono::steady_clock::now() >= deadline_) {
             st.stopped = true;
             break;
         }
         size_t have = carry;
-        while (have < buf_bytes_) {
-            const size_t n = fread(buf_[k] + have, 1, buf_bytes_ - have, in);
+        while (have < buf_bytes_ && left) {
+            const size_t n = fread(buf_[k] + have, 1, (size_t)std::min<uint64_t>(buf_bytes_ - have, left), in);
             if (n == 0) break;
             have += n;
+            left -= n;
         }
-        const size_t whole = rs ? have / 2 * 2 : have / bs2 * bs2;
+        eof = have < buf_bytes_;
+        const size_t whole = rs ? have / s * s : have / bsf * bsf;
         if (whole) {
             auto msgs = d_.Decode(buf_[k], whole);
             const int64_t call_first = stream_blocks_;
-            const int64_t nblocks = rs ? d_.BlocksDecoded() - stream_blocks_ : (int64_t)(whole / bs2);
+            const int64_t nblocks = rs ? d_.BlocksDecoded() - stream_blocks_ : (int64_t)(whole / bsf);
             st.blocks += nblocks;
-            st.bytes += (int64_t)whole;   // input bytes: two per input sample
+            st.bytes += (int64_t)whole;   // input bytes: s per input sample
+            st.samples += (int64_t)(whole / s);
             stream_blocks_ += nblocks;
             for (size_t i = 0; i < msgs.size() && !st.stopped;) {
                 size_t j = i;
@@ -221,7 +232,7 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
         carry = have - whole;
         if (carry) memcpy(buf_[k ^ 1], buf_[k] + whole, carry);
         k ^= 1;
-        if (have < buf_bytes_) break;  // EOF: the trailing partial block is dropped like main.go does
+        if (eof) break;  // EOF: the trailing partial block is dropped like main.go does
     }
     st.seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     return st;

@@ -6,7 +6,8 @@
 //   * the decode loop (main.go:207-294) -- Decode, then the prev/next digest maps that drop a message
 //     already reported for the previous block (main.go:244-260,292), the -samplefile dump of the last blocks
 //     (main.go:225-230,279-284), -single (main.go:269-287) and -duration (main.go:350-353).
-// Whole blocks only: a trailing partial block is never decoded (main.go:166-186).
+// Whole blocks only: a trailing partial block is never decoded (main.go:166-186).  Input of another sample format
+// (cs8, cs16, cf32) is read in whole samples of its own size and converted on the GPU.
 #pragma once
 
 #include <chrono>
@@ -27,7 +28,7 @@ using Digest = std::tuple<std::string, uint8_t, uint32_t, std::vector<uint8_t>>;
 Digest NewDigest(const protocol::Message& m);
 
 struct Stats {
-    int64_t blocks = 0, bytes = 0, messages = 0, duplicates = 0, filtered = 0;
+    int64_t blocks = 0, bytes = 0, samples = 0, messages = 0, duplicates = 0, filtered = 0;   // bytes, samples: input
     double seconds = 0;
     bool stopped = false;  // -single or -duration ended the run: nothing after it is read
 };
@@ -62,7 +63,9 @@ public:
     // msgtypes: comma list as for -msgtype ("all" = scm,scm+,idm,r900, main.go:67-73)
     // sampleRate > 0: the capture's sample rate in Hz; a rate other than DataRate*ChipLength is resampled on the GPU
     // (protocol::Decoder::SetInputRate) and blocks, dedup and filters then work on the resampled stream.
-    Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, int64_t sampleRate = 0);
+    // format / scale: the input's sample format (ERTGPU_FORMAT_*) and gain (protocol::Decoder::SetInputFormat).
+    Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, int64_t sampleRate = 0,
+             int32_t format = ERTGPU_FORMAT_CU8, float scale = 0.0f);
     ~Receiver();
 
     protocol::Decoder& decoder() { return d_; }
@@ -84,8 +87,10 @@ public:
     void SetDeadline(std::chrono::steady_clock::time_point t) { deadline_ = t; }
 
     // Run over a FILE* until EOF, -single or the deadline.  `emit` is called once per reported message (after the
-    // cross-block dedup when block_dedup) with its LogMessage Offset and Length (0 without a sample file).
-    Stats Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&, int64_t, int)>& emit);
+    // cross-block dedup when block_dedup) with its LogMessage Offset and Length (0 without a sample file).  max_bytes >= 0
+    // stops reading after that many bytes (the data chunk of a WAV file).
+    Stats Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&, int64_t, int)>& emit,
+              int64_t max_bytes = -1);
 
     // Start a new, independent stream (the next file of a batch): zeroed Decoder history (decode.go:144-145),
     // block numbers restart at 0, empty dedup set, empty sampleBuf.
