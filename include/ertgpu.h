@@ -131,6 +131,15 @@ typedef struct {
     int32_t F;  /* bits of the sub-phase interpolation weight   */
 } ertgpu_resampler_info;
 
+/* The tuning of a handle (ertgpu_set_input_tuning; include/ertgpu_resample.h has the arithmetic). */
+typedef struct {
+    int64_t capture_center_hz; /* the frequency at the centre of the capture                    */
+    int64_t center_hz;         /* the channel decoded (the decoder's CenterFreq when given as 0) */
+    int64_t offset_hz;         /* center_hz - capture_center_hz                                  */
+    uint32_t nco_step;         /* W = round(offset * 2^32 / R_in) mod 2^32                        */
+    int32_t nco_bits;          /* bits of the mixer's phase index (2^nco_bits table entries)     */
+} ertgpu_tuning_info;
+
 /* ---- lifecycle -------------------------------------------------------- */
 
 /* protocol.NewDecoder (decode.go:65-71).  No CUDA work yet. */
@@ -167,7 +176,7 @@ int ertgpu_reset(ertgpu_handle *h);
  * R_out = DataRate * ChipLength (and its geometry, blocks, Idx and taps); when hz != R_out the
  * input is converted to R_out by an exact integer resampler on the GPU, and Block / Idx refer to
  * the resampled stream.  hz == R_out (or never calling this) changes nothing.  R_out / hz must
- * lie in [1/4, 4], otherwise ERTGPU_EINVAL.  With resampling, ertgpu_decode and
+ * lie in [1/4, 4] ([1/10, 4] on a handle tuned by ertgpu_set_input_tuning), otherwise ERTGPU_EINVAL.  With resampling, ertgpu_decode and
  * ertgpu_decode_device_async take any whole number of IQ samples (nbytes even, else
  * ERTGPU_ESIZE): the handle carries the input history, the outputs still waiting for look-ahead
  * and the partial output block across calls and decodes every whole block it has.
@@ -175,6 +184,23 @@ int ertgpu_reset(ertgpu_handle *h);
  * runs only resample_kernel; ertgpu_last_kernels then keeps the list of the last call that ran the
  * decoder (demod first, resample_kernel last). */
 int ertgpu_set_input_rate(ertgpu_handle *h, int64_t hz);
+
+/* Decode the channel at center_hz of a capture recorded centred at capture_center_hz (both Hz;
+ * center_hz == 0 selects the decoder's CenterFreq, what rtlamr tunes to by default).  Call it after
+ * the last ertgpu_register_protocol and before ertgpu_set_input_rate and ertgpu_allocate; otherwise,
+ * or for capture_center_hz <= 0 or center_hz < 0, ERTGPU_EINVAL (and ertgpu_register_protocol after
+ * it is ERTGPU_EINVAL too).  The resampler then multiplies each input sample by
+ * e^(-j 2 pi (center_hz - capture_center_hz) g / R_in) before its lowpass, which is the channel filter,
+ * all in integers (include/ertgpu_resample.h).  A tuned handle takes R_out / R_in in [1/10, 4], and
+ * the channel must lie inside the capture: |offset| + 0.4 * min(R_in, R_out) <= 0.5 * R_in, checked by
+ * ertgpu_set_input_rate, or by ertgpu_allocate when the input is at the decoder's own rate.  An offset
+ * of 0 decodes exactly like an untuned handle.  ertgpu_reset restarts the mixer's phase;
+ * ERTGPU_TAP_RESAMPLED returns the mixed and filtered bytes; ertgpu_decode_sharded rejects tuned
+ * handles.  Several channels of one capture are several handles fed the same bytes. */
+int ertgpu_set_input_tuning(ertgpu_handle *h, int64_t capture_center_hz, int64_t center_hz);
+
+/* The tuning of a handle; ERTGPU_EINVAL when ertgpu_set_input_tuning was not called. */
+int ertgpu_get_tuning(const ertgpu_handle *h, ertgpu_tuning_info *info);
 
 /* Declare the sample format of the IQ the handle will be fed (ERTGPU_FORMAT_*), before
  * ertgpu_allocate (its order relative to ertgpu_set_input_rate is free).  Each component x is

@@ -32,8 +32,11 @@
 #define ERTRS_P 256      /* sub-phases per input sample                   */
 #define ERTRS_S 14       /* DC gain 2^S (peak tap <= 2^S fits int16)      */
 #define ERTRS_F 16       /* bits of the interpolation weight              */
-#define ERTRS_MAX_T 128  /* taps per output                               */
+#define ERTRS_MAX_T 224  /* taps per output (untuned plans stay <= 88)    */
 #define ERTRS_ATTEN_DB 70.0
+#define ERTRS_NCO_BITS 12 /* log2 of the entries of the mixer table E     */
+#define ERTRS_NCO_N (1 << ERTRS_NCO_BITS)
+#define ERTRS_E_S 14      /* |E[k]| ~ 2^E_S                                */
 
 static inline int64_t ertrs_gcd(int64_t a, int64_t b) {
     while (b) {
@@ -69,11 +72,8 @@ static inline double ertrs_i0(double x) {
     return sum;
 }
 
-/* Fill *info for R_in -> R_out.  Returns 0, or -1 when a rate is not positive or the ratio is outside
- * [1/4, 4]. */
-static inline int ertrs_plan(int64_t rate_in, int64_t rate_out, ertgpu_resampler_info* info) {
-    if (rate_in <= 0 || rate_out <= 0) return -1;
-    if (rate_out * 4 < rate_in || rate_out > rate_in * 4) return -1;
+/* Fill *info for R_in -> R_out at P = ERTRS_P (rates positive, checked by the caller). */
+static inline void ertrs_fill_plan(int64_t rate_in, int64_t rate_out, ertgpu_resampler_info* info) {
     const int64_t g = ertrs_gcd(rate_out, rate_in);
     info->rate_in = rate_in;
     info->rate_out = rate_out;
@@ -90,7 +90,71 @@ static inline int ertrs_plan(int64_t rate_in, int64_t rate_out, ertgpu_resampler
     info->P = ERTRS_P;
     info->S = ERTRS_S;
     info->F = ERTRS_F;
+}
+
+/* Fill *info for R_in -> R_out.  Returns 0, or -1 when a rate is not positive or the ratio is outside
+ * [1/4, 4]. */
+static inline int ertrs_plan(int64_t rate_in, int64_t rate_out, ertgpu_resampler_info* info) {
+    if (rate_in <= 0 || rate_out <= 0) return -1;
+    if (rate_out * 4 < rate_in || rate_out > rate_in * 4) return -1;
+    ertrs_fill_plan(rate_in, rate_out, info);
     return 0;
+}
+
+/*
+ * Tuned input (ertgpu_set_input_tuning): the channel at offset D = center - capture_center Hz from the
+ * capture's centre is mixed to 0 Hz as the resampler stages its input, so the same lowpass is the channel
+ * filter.  All integer:
+ *   W   = round(D * 2^32 / R_in) (half away from zero) mod 2^32        (ertrs_nco_step)
+ *   k_g = ((uint32)g * W + 2^19) >> 20,  g = input index since the stream start
+ *   E[k] = (round(2^14 cos 2 pi k/4096), round(2^14 sin 2 pi k/4096))  (ertrs_nco_table)
+ *   s'_I = (s_I C + s_Q S + 2^13) >> 14,  s'_Q = (s_Q C - s_I S + 2^13) >> 14  (floor; ertrs_mix)
+ * i.e. s * e^(-j 2 pi D g / R_in), and the outputs are the untuned formula with s' for s.  |s'| <= 361.
+ */
+
+/* The plan of a tuned handle: R_out / R_in in [1/10, 4] and the channel inside the capture,
+ * |D| + 0.4 * min(R_in, R_out) <= 0.5 * R_in.  T as ertrs_plan (at most ERTRS_MAX_T); P = 256 for T <= 96,
+ * 128 for T <= 160 and 64 above, so that the table, one tile's input span and E fit one CTA's shared
+ * memory.  Inside [1/4, 4] every plan is ertrs_plan's (T <= 88).  Returns 0 or -1. */
+static inline int ertrs_plan_tuned(int64_t rate_in, int64_t rate_out, int64_t offset_hz, ertgpu_resampler_info* info) {
+    if (rate_in <= 0 || rate_out <= 0) return -1;
+    if (rate_out * 10 < rate_in || rate_out > rate_in * 4) return -1;
+    const int64_t lo = rate_out < rate_in ? rate_out : rate_in;
+    const int64_t ad = offset_hz < 0 ? -offset_hz : offset_hz;
+    if (ad > rate_in || 10 * ad + 4 * lo > 5 * rate_in) return -1;
+    ertrs_fill_plan(rate_in, rate_out, info);
+    info->P = info->T <= 96 ? 256 : info->T <= 160 ? 128 : 64;
+    return 0;
+}
+
+/* W = round(D * 2^32 / R_in), rounded half away from zero, modulo 2^32 (|D| <= R_in) */
+static inline uint32_t ertrs_nco_step(int64_t offset_hz, int64_t rate_in) {
+    const int64_t ad = offset_hz < 0 ? -offset_hz : offset_hz;
+    const int64_t w = (int64_t)((((__int128)ad << 33) + rate_in) / ((__int128)2 * rate_in));
+    return (uint32_t)(offset_hz < 0 ? -w : w);
+}
+
+/* E[k] = C | S << 16 (int16 each), k = 0 .. ERTRS_NCO_N - 1; sin and cos from ertrs_sinpi, no libm */
+static inline void ertrs_nco_table(uint32_t* E) {
+    for (int32_t k = 0; k < ERTRS_NCO_N; k++) {
+        const double c = (double)(1 << ERTRS_E_S) * ertrs_sinpi((double)(k + ERTRS_NCO_N / 4) / (double)(ERTRS_NCO_N / 2));
+        const double s = (double)(1 << ERTRS_E_S) * ertrs_sinpi((double)k / (double)(ERTRS_NCO_N / 2));
+        const int32_t ci = (int32_t)(c >= 0 ? (int64_t)(c + 0.5) : -(int64_t)(-c + 0.5));
+        const int32_t si = (int32_t)(s >= 0 ? (int64_t)(s + 0.5) : -(int64_t)(-s + 0.5));
+        E[k] = ((uint32_t)ci & 0xffffu) | ((uint32_t)si << 16);
+    }
+}
+
+/* phase index of input sample g */
+static inline uint32_t ertrs_nco_index(int64_t g, uint32_t W) {
+    return ((uint32_t)g * W + (1u << (31 - ERTRS_NCO_BITS))) >> (32 - ERTRS_NCO_BITS);
+}
+
+/* s' = s * conj(E[k]) for s = (si, sq) */
+static inline void ertrs_mix(int32_t si, int32_t sq, uint32_t e, int32_t* oi, int32_t* oq) {
+    const int32_t c = (int32_t)(int16_t)(e & 0xffffu), s = (int32_t)(int16_t)(e >> 16);
+    *oi = (si * c + sq * s + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
+    *oq = (sq * c - si * s + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
 }
 
 /* h(d) * 2^S for the plan's window */

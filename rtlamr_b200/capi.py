@@ -53,6 +53,11 @@ class ResamplerInfo(C.Structure):
                 ("T", C.c_int32), ("P", C.c_int32), ("S", C.c_int32), ("F", C.c_int32)]
 
 
+class TuningInfo(C.Structure):
+    _fields_ = [("capture_center_hz", C.c_int64), ("center_hz", C.c_int64), ("offset_hz", C.c_int64),
+                ("nco_step", C.c_uint32), ("nco_bits", C.c_int32)]
+
+
 class Shard(C.Structure):
     _fields_ = [("first_block", C.c_int64), ("last_block", C.c_int64), ("first_fed_block", C.c_int64)]
 
@@ -79,6 +84,7 @@ EXPORTS = [
     "ertgpu_host_alloc", "ertgpu_host_free", "ertgpu_synth_fill",
     "ertgpu_bind_host_thread", "ertgpu_last_kernels", "ertgpu_plan_shards", "ertgpu_decode_sharded",
     "ertgpu_set_input_rate", "ertgpu_get_resampler", "ertgpu_set_input_format", "ertgpu_get_input_format",
+    "ertgpu_set_input_tuning", "ertgpu_get_tuning",
 ]
 
 _lib = None
@@ -135,6 +141,8 @@ def lib() -> C.CDLL:
     L.ertgpu_get_resampler.argtypes = [vp, C.POINTER(ResamplerInfo), vp, sz, C.POINTER(sz)]
     L.ertgpu_set_input_format.argtypes = [vp, i32, C.c_float]
     L.ertgpu_get_input_format.argtypes = [vp, C.POINTER(i32), C.POINTER(C.c_float)]
+    L.ertgpu_set_input_tuning.argtypes = [vp, i64, i64]
+    L.ertgpu_get_tuning.argtypes = [vp, C.POINTER(TuningInfo)]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the library does not export it
     _lib = L
@@ -179,6 +187,17 @@ class Handle:
     def set_input_rate(self, hz: int):
         """ertgpu_set_input_rate: the IQ fed to this handle is sampled at `hz` (between register and allocate)."""
         self._check(self._L.ertgpu_set_input_rate(self._h, int(hz)))
+
+    def set_input_tuning(self, capture_hz: int, center_hz: int = 0):
+        """ertgpu_set_input_tuning: the IQ was recorded centred at capture_hz; decode the channel at center_hz (0: the
+        decoder's CenterFreq).  After the protocols, before the rate and allocate."""
+        self._check(self._L.ertgpu_set_input_tuning(self._h, int(capture_hz), int(center_hz)))
+
+    def tuning(self):
+        """ertgpu_get_tuning as a dict."""
+        info = TuningInfo()
+        self._check(self._L.ertgpu_get_tuning(self._h, C.byref(info)))
+        return {k: getattr(info, k) for k, _ in TuningInfo._fields_}
 
     def set_input_format(self, fmt: int, scale: float = 0.0):
         """ertgpu_set_input_format: the IQ fed to this handle is in format FORMAT_* with gain `scale` (0: the format's
@@ -289,15 +308,19 @@ class Handle:
 
 def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per_call: int = 0,
                 max_candidates: int = 0, input_rate: int = 0, input_format: int = FORMAT_CU8,
-                input_scale: float = 0.0) -> Handle:
+                input_scale: float = 0.0, capture_freq: int = 0, center_freq: int = 0) -> Handle:
     """NewDecoder + RegisterProtocol(NewParser(name, chip_length)) for each name + Allocate
     (reference main.go:64-86).  input_rate > 0: the IQ is sampled at that rate (ertgpu_set_input_rate);
-    input_format / input_scale: its sample format and gain (ertgpu_set_input_format, not called for plain cu8)."""
+    input_format / input_scale: its sample format and gain (ertgpu_set_input_format, not called for plain cu8);
+    capture_freq > 0: the IQ was recorded centred there, and the channel at center_freq (0: the protocols'
+    CenterFreq) is decoded (ertgpu_set_input_tuning, before the rate)."""
     if isinstance(msgtypes, str):
         msgtypes = [m.strip() for m in msgtypes.split(",") if m.strip()]
     h = Handle()
     for m in msgtypes:
         h.register(stock_protocol(m, chip_length))
+    if capture_freq or center_freq:
+        h.set_input_tuning(capture_freq, center_freq)
     if input_rate:
         h.set_input_rate(input_rate)
     if input_format != FORMAT_CU8 or input_scale:

@@ -140,6 +140,13 @@ struct ertgpu_handle {
     int64_t rs_hist_n = 0;
     int64_t rs_pend = 0;        // outputs at the front of d_rs_out[rs_cur_out] that wait for a whole block
 
+    // tuned input (ertgpu_set_input_tuning): the channel at center_hz of a capture centred at capture_hz
+    bool tuned = false;
+    int64_t capture_hz = 0, center_hz = 0;
+    uint32_t nco_step = 0;      // W at the input rate in effect
+    bool rs_mix = false;        // the resampler runs its tuned instance (W != 0 or P != ERTRS_P)
+    uint32_t* d_rs_E = nullptr; // the mixer table (ertrs_nco_table)
+
     // input format (ertgpu_set_input_format); ERTGPU_FORMAT_CU8 converts nothing
     int32_t fmt = ERTGPU_FORMAT_CU8;
     float fmt_scale = 0.0f;
@@ -238,6 +245,7 @@ void free_device(ertgpu_handle* h) {
     dfree(h->d_tap);
     dfree(h->d_rs_A);
     dfree(h->d_rs_D);
+    dfree(h->d_rs_E);
     dfree(h->d_cvt);
     for (int k = 0; k < 2; k++) {
         dfree(h->d_rs_hist[k]);
@@ -336,6 +344,7 @@ const char* fmt_name(int f) {
 }
 
 std::string resample_label(const ertgpu_handle* h) {
+    if (h->rs_mix) return std::string("resample_kernel<") + fmt_name(h->fmt) + ",tuned>";
     return h->fmt == ERTGPU_FORMAT_CU8 ? "resample_kernel" : std::string("resample_kernel<") + fmt_name(h->fmt) + ">";
 }
 
@@ -620,13 +629,13 @@ int prepare_staging(ertgpu_handle* h, size_t bytes, const void* iq, bool* pageab
 
 // ---- input-rate resampler (include/ertgpu_resample.h) ----
 
-// The resample_kernel instance of an input format.
-decltype(&resample_kernel<ERTGPU_FORMAT_CU8>) resample_kernel_of(int f) {
+// The resample_kernel instance of an input format, untuned or tuned.
+decltype(&resample_kernel<ERTGPU_FORMAT_CU8, false>) resample_kernel_of(int f, bool tuned) {
     switch (f) {
-        case ERTGPU_FORMAT_CS8: return resample_kernel<ERTGPU_FORMAT_CS8>;
-        case ERTGPU_FORMAT_CS16: return resample_kernel<ERTGPU_FORMAT_CS16>;
-        case ERTGPU_FORMAT_CF32: return resample_kernel<ERTGPU_FORMAT_CF32>;
-        default: return resample_kernel<ERTGPU_FORMAT_CU8>;
+        case ERTGPU_FORMAT_CS8: return tuned ? resample_kernel<ERTGPU_FORMAT_CS8, true> : resample_kernel<ERTGPU_FORMAT_CS8, false>;
+        case ERTGPU_FORMAT_CS16: return tuned ? resample_kernel<ERTGPU_FORMAT_CS16, true> : resample_kernel<ERTGPU_FORMAT_CS16, false>;
+        case ERTGPU_FORMAT_CF32: return tuned ? resample_kernel<ERTGPU_FORMAT_CF32, true> : resample_kernel<ERTGPU_FORMAT_CF32, false>;
+        default: return tuned ? resample_kernel<ERTGPU_FORMAT_CU8, true> : resample_kernel<ERTGPU_FORMAT_CU8, false>;
     }
 }
 
@@ -634,7 +643,7 @@ int launch_resample(ertgpu_handle* h, const RsArgs& a, cudaStream_t st) {
     if (a.count <= 0 && a.carry_n <= 0) return ERTGPU_OK;
     const long long tiles = (a.count + kRsTile - 1) / kRsTile;
     const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(tiles, h->rs_grid));
-    resample_kernel_of(h->fmt)<<<grid, kRsThreads, h->rs_smem, st>>>(h->d_rs_A, h->d_rs_D, a);
+    resample_kernel_of(h->fmt, h->rs_mix)<<<grid, kRsThreads, h->rs_smem, st>>>(h->d_rs_A, h->d_rs_D, a);
     CUDA_TRY(h, cudaGetLastError());
     h->launches++;
     return ERTGPU_OK;
@@ -699,7 +708,10 @@ void rs_plan_step(const ertgpu_handle* h, const uint8_t* d_in, int64_t c, RsArgs
     a->M = M;
     a->T = (int)T;
     a->scale = h->fmt_scale;
-    const int64_t Q = (int64_t)ERTRS_P << ERTRS_F, step = kRsThreads * M;
+    a->E = h->d_rs_E;
+    a->W = h->nco_step;
+    a->P = h->rs.P;
+    const int64_t Q = (int64_t)h->rs.P << ERTRS_F, step = kRsThreads * M;
     a->step_k = step / L;
     a->step_phi = step % L;
     a->step_q = (int64_t)(((__int128)a->step_phi * Q) / L);
@@ -869,6 +881,7 @@ int ertgpu_register_protocol(ertgpu_handle* h, const ertgpu_protocol* p) {
     if (!h || !p) return ERTGPU_EINVAL;
     if (h->allocated) return fail(h, ERTGPU_EINVAL, "register_protocol after allocate");
     if (h->rate_in) return fail(h, ERTGPU_EINVAL, "register_protocol after set_input_rate");
+    if (h->tuned) return fail(h, ERTGPU_EINVAL, "register_protocol after set_input_tuning");
     if (h->protos.size() >= ERTGPU_MAX_PROTOCOLS) return fail(h, ERTGPU_EINVAL, "too many protocols");
     const size_t n = strnlen(p->preamble, sizeof(p->preamble));
     if (n == 0 || n > ERTGPU_MAX_PREAMBLE) return fail(h, ERTGPU_EINVAL, "bad preamble length %zu", n);
@@ -910,8 +923,14 @@ int ertgpu_allocate(ertgpu_handle* h, int32_t device, int64_t max_blocks_per_cal
     return rc;
 }
 
+static int configure_rate(ertgpu_handle* h, int64_t hz);
+
 static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_per_call, int64_t max_candidates) {
     if (h->protos.empty()) return fail(h, ERTGPU_EINVAL, "no protocol registered");
+    if (h->tuned && !h->rate_in) {  // a tuned handle at the decoder's own rate: the channel must lie inside it
+        const int rc = configure_rate(h, (int64_t)h->cfg.data_rate * h->cfg.chip_length);
+        if (rc) return rc;
+    }
 
     // decode.go:131-141
     ertgpu_decoder_config& c = h->cfg;
@@ -1049,22 +1068,29 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
         CUDA_TRY(h, cudaMemcpy(h->d_rs_A, A.data(), A.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
         CUDA_TRY(h, cudaMalloc(&h->d_rs_D, D.size() * sizeof(uint32_t)));
         CUDA_TRY(h, cudaMemcpy(h->d_rs_D, D.data(), D.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        if (h->rs_mix) {
+            std::vector<uint32_t> E(ERTRS_NCO_N);
+            ertrs_nco_table(E.data());
+            CUDA_TRY(h, cudaMalloc(&h->d_rs_E, E.size() * sizeof(uint32_t)));
+            CUDA_TRY(h, cudaMemcpy(h->d_rs_E, E.data(), E.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        }
         for (int k = 0; k < 2; k++) {
             CUDA_TRY(h, cudaMalloc(&h->d_rs_hist[k], (size_t)r.T * 2 + 16));
             // a step completes at most max_blocks blocks: less than (max_blocks + 1) * BS outputs are buffered
             h->rs_out_bytes = (size_t)(max_blocks_per_call + 1) * c.block_size2 + 64;
             CUDA_TRY(h, cudaMalloc(&h->d_rs_out[k], h->rs_out_bytes));
         }
-        h->rs_smem = rs_smem_bytes(r.T, r.L, r.M);
+        h->rs_smem = rs_smem_bytes(r.P, r.T, r.L, r.M, h->rs_mix);
         {   // a property of the kernel, not of the handle: every handle on the device gets the largest any table needs
             static OncePerDevice once;
             if (once.first(h->device))
                 for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF32; f++)
-                    CUDA_TRY(h, cudaFuncSetAttribute(resample_kernel_of(f), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+                    for (int tuned = 0; tuned < 2; tuned++)
+                        CUDA_TRY(h, cudaFuncSetAttribute(resample_kernel_of(f, tuned), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         }
         if (h->rs_smem > 227 * 1024) return fail(h, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", h->rs_smem);
         int per_sm = 0;
-        CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel_of(h->fmt), kRsThreads, h->rs_smem));
+        CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel_of(h->fmt, h->rs_mix), kRsThreads, h->rs_smem));
         h->rs_grid = std::max(1, per_sm) * h->sm_count;
         h->rs_cur_hist = h->rs_cur_out = 0;
         rs_reset_stream(h);
@@ -1099,24 +1125,74 @@ int ertgpu_reset(ertgpu_handle* h) {
     return ERTGPU_OK;
 }
 
+// The resampler for input at hz: ertrs_plan, or ertrs_plan_tuned and the NCO step on a tuned handle.  It runs when
+// the rates differ or a tuned handle mixes; the tuned instance when it mixes or its plan has P != ERTRS_P.
+static int configure_rate(ertgpu_handle* h, int64_t hz) {
+    const int64_t rate_out = (int64_t)h->cfg.data_rate * h->cfg.chip_length;
+    ertgpu_resampler_info info{};
+    uint32_t w = 0;
+    if (h->tuned) {
+        const int64_t off = h->center_hz - h->capture_hz;
+        if (ertrs_plan_tuned(hz, rate_out, off, &info) != 0)
+            return fail(h, ERTGPU_EINVAL,
+                        "input rate %lld Hz, channel offset %lld Hz: the decoder rate %lld Hz must be within 1/10 ... 4 "
+                        "times the input rate, and |offset| + 0.4 * min(rates) at most half the input rate",
+                        (long long)hz, (long long)off, (long long)rate_out);
+        w = ertrs_nco_step(off, hz);
+    } else if (ertrs_plan(hz, rate_out, &info) != 0) {
+        return fail(h, ERTGPU_EINVAL, "input rate %lld Hz: the decoder rate %lld Hz must be within 1/4 ... 4 times it",
+                    (long long)hz, (long long)rate_out);
+    }
+    const bool on = hz != rate_out || w != 0;
+    std::vector<int16_t> table;
+    if (on) {
+        table.resize((size_t)(info.P + 1) * info.T);
+        if (ertrs_build_table(&info, table.data()) != 0) return fail(h, ERTGPU_EINVAL, "resampler table does not fit int16");
+    }
+    h->rs_on = on;
+    h->rs_mix = on && (w != 0 || info.P != ERTRS_P);
+    h->nco_step = w;
+    h->rs = info;
+    h->rs_table.swap(table);
+    return ERTGPU_OK;
+}
+
 int ertgpu_set_input_rate(ertgpu_handle* h, int64_t hz) {
     if (!h) return ERTGPU_EINVAL;
     if (h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_rate after allocate");
     if (h->protos.empty()) return fail(h, ERTGPU_EINVAL, "set_input_rate before register_protocol");
-    const int64_t rate_out = (int64_t)h->cfg.data_rate * h->cfg.chip_length;
-    ertgpu_resampler_info info{};
-    if (ertrs_plan(hz, rate_out, &info) != 0)
-        return fail(h, ERTGPU_EINVAL, "input rate %lld Hz: the decoder rate %lld Hz must be within 1/4 ... 4 times it",
-                    (long long)hz, (long long)rate_out);
-    std::vector<int16_t> table;
-    if (hz != rate_out) {
-        table.resize((size_t)(info.P + 1) * info.T);
-        if (ertrs_build_table(&info, table.data()) != 0) return fail(h, ERTGPU_EINVAL, "resampler table does not fit int16");
-    }
+    const int rc = configure_rate(h, hz);
+    if (rc) return rc;
     h->rate_in = hz;
-    h->rs_on = hz != rate_out;
-    h->rs = info;
-    h->rs_table.swap(table);
+    return ERTGPU_OK;
+}
+
+int ertgpu_set_input_tuning(ertgpu_handle* h, int64_t capture_center_hz, int64_t center_hz) {
+    if (!h) return ERTGPU_EINVAL;
+    if (h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_tuning after allocate");
+    if (h->protos.empty()) return fail(h, ERTGPU_EINVAL, "set_input_tuning before register_protocol");
+    if (h->rate_in) return fail(h, ERTGPU_EINVAL, "set_input_tuning after set_input_rate");
+    if (capture_center_hz <= 0 || center_hz < 0)
+        return fail(h, ERTGPU_EINVAL, "capture centre %lld Hz must be > 0 and channel %lld Hz >= 0",
+                    (long long)capture_center_hz, (long long)center_hz);
+    h->tuned = true;
+    h->capture_hz = capture_center_hz;
+    h->center_hz = center_hz ? center_hz : (int64_t)h->cfg.center_freq;  // decode.go:105: the last CenterFreq
+    return ERTGPU_OK;
+}
+
+int ertgpu_get_tuning(const ertgpu_handle* h, ertgpu_tuning_info* info) {
+    if (!h || !h->tuned) return ERTGPU_EINVAL;
+    if (info) {
+        const int64_t rate = h->rate_in ? h->rate_in : (int64_t)h->cfg.data_rate * h->cfg.chip_length;
+        info->capture_center_hz = h->capture_hz;
+        info->center_hz = h->center_hz;
+        info->offset_hz = h->center_hz - h->capture_hz;
+        // W at the input rate in effect (the decoder's own until set_input_rate)
+        const int64_t ad = info->offset_hz < 0 ? -info->offset_hz : info->offset_hz;
+        info->nco_step = ad <= rate ? ertrs_nco_step(info->offset_hz, rate) : 0;
+        info->nco_bits = ERTRS_NCO_BITS;
+    }
     return ERTGPU_OK;
 }
 
@@ -1184,8 +1260,10 @@ int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t f
 
     // Staging chunks (allocated on first use) of s bytes per sample: the H2D copy of chunk i+1 overlaps the kernels of
     // chunk i.  32 MiB of whole decoder blocks natively; a resampling chunk also covers the filter's look-ahead, and the step that takes it
-    // completes at most max_blocks blocks (rs_max_input).
-    const int64_t chunk = h->rs_on ? std::min<int64_t>(16 << 20, 4 * (h->max_blocks + 1) * BS + h->rs.T + 8)
+    // completes at most max_blocks blocks (rs_max_input).  Decimating by more than 4 (tuned handles, up to 10) the
+    // chunk grows with M / L, so that it still reaches max_blocks blocks.
+    const int64_t ratio = h->rs_on ? std::max<int64_t>(4, (h->rs.M + h->rs.L - 1) / h->rs.L) : 4;
+    const int64_t chunk = h->rs_on ? std::min<int64_t>(16 << 20, ratio * (h->max_blocks + 1) * BS + h->rs.T + 8)
                                    : BS * std::min<int64_t>(h->max_blocks, std::max<int64_t>(1, (32 << 20) / h->cfg.block_size2));
     bool pageable = true;
     rc = prepare_staging(h, (size_t)chunk * s, iq, &pageable);

@@ -34,6 +34,10 @@ struct RsArgs {
     long long step_k, step_phi, step_q, step_r;
     int T;
     float scale;  // g of the input format (not read for uint8 input)
+    // tuned instances only: the mixer table E (ertrs_nco_table), the NCO step W and the table's sub-phases P
+    const uint32_t* E;
+    uint32_t W;
+    int P;
 };
 
 // The table as the kernel reads it: A[p][t] = h0 * 2^F + 2^(F-1) (int32), D[p][m] = the int16 pair
@@ -61,15 +65,114 @@ __device__ __forceinline__ uchar2 rs_input(const RsArgs& a, long long g) {  // g
     }
 }
 
+// The tuned resampler (ertrs_plan_tuned): as below, but every staged sample is mixed by E[k_g] first, so X[j] holds
+// the int16 pair (s'_I[j], s'_Q[j]) with s' = 0 before the stream start, and the taps are plain multiply-adds (dp2a
+// takes only 8-bit samples).  One path serves every output.  P is the plan's (a.P).
+template <int F>
+__device__ __forceinline__ void resample_tuned(const int32_t* __restrict__ g_A, const uint32_t* __restrict__ g_D,
+                                               const RsArgs& a, int32_t* smem) {
+    const int T = a.T, T2 = a.T / 2, P = a.P;
+    int32_t* tabA = smem;
+    uint32_t* tabD = reinterpret_cast<uint32_t*>(smem + P * T);
+    uint32_t* tabE = tabD + P * T2;
+    uint32_t* X = tabE + ERTRS_NCO_N;
+    for (int i = threadIdx.x; i < P * T; i += kRsThreads) tabA[i] = g_A[i];
+    for (int i = threadIdx.x; i < P * T2; i += kRsThreads) tabD[i] = g_D[i];
+    for (int i = threadIdx.x; i < ERTRS_NCO_N; i += kRsThreads) tabE[i] = a.E[i];
+    if (blockIdx.x == 0)
+        for (long long i = threadIdx.x; i < a.carry_n; i += kRsThreads)
+            *reinterpret_cast<uchar2*>(a.carry_dst + 2 * i) = rs_input<F>(a, a.carry_first + i);  // carry_first >= 0
+    const long long Q = (long long)P << ERTRS_F;
+    const long long ntiles = (a.count + kRsTile - 1) / kRsTile;
+    const uint32_t dph = (uint32_t)kRsThreads * a.W;  // phase accumulator step between a thread's staged samples
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long long nb = a.n0 + tile * kRsTile;
+        const long long ne = min(nb + kRsTile, a.n0 + a.count);
+        const long long j_lo = a.base_k + ((nb - a.base_n) * a.M) / a.L - T / 2 + 1;
+        const long long j_hi = a.base_k + ((ne - 1 - a.base_n) * a.M) / a.L + T / 2;
+        const int nspan = (int)(j_hi - j_lo + 1);
+        __syncthreads();  // the previous tile's span is no longer read (and the tables are in place)
+        // (uint32)g * W + 2^19 for g = j_lo + i, exact mod 2^32 whatever the sign of j_lo
+        uint32_t ph = (uint32_t)(j_lo + threadIdx.x) * a.W + (1u << (31 - ERTRS_NCO_BITS));
+        for (int i = threadIdx.x; i < nspan; i += kRsThreads, ph += dph) {
+            const long long g = j_lo + i;
+            uint32_t xw = 0;
+            if (g >= 0) {
+                const uchar2 u = rs_input<F>(a, g);
+                const uint32_t e = tabE[ph >> (32 - ERTRS_NCO_BITS)];
+                const int c = (int)(short)(e & 0xffffu), s = (int)e >> 16;
+                const int si = 2 * (int)u.x - 255, sq = 2 * (int)u.y - 255;
+                const int mi = (si * c + sq * s + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
+                const int mq = (sq * c - si * s + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
+                xw = ((uint32_t)mi & 0xffffu) | ((uint32_t)mq << 16);
+            }
+            X[i] = xw;
+        }
+        __syncthreads();
+
+        long long n = nb + threadIdx.x;
+        if (n < ne) {
+            const long long nr = n - a.base_n;
+            long long k = (nr * a.M) / a.L;
+            long long phi = nr * a.M - k * a.L;
+            k += a.base_k;
+            long long q = (phi * Q) / a.L;
+            long long r = phi * Q - q * a.L;
+            for (int it = 0; it < kRsPerThread && n < ne; it++) {
+                const int p = (int)(q >> ERTRS_F), w = (int)(q & ((1 << ERTRS_F) - 1));
+                const int32_t* A = tabA + p * T;
+                const uint32_t* D = tabD + p * T2;
+                const long long j0 = k - T / 2 + 1;
+                const uint32_t* x = X + (int)(j0 - j_lo);
+                const int tc = T / 2 - 1 + (p >= P / 2 ? 1 : 0);
+                int csum = 0, ai = 0, aq = 0;
+#pragma unroll 4
+                for (int m = 0; m < T2; m++) {
+                    const int2 a01 = *reinterpret_cast<const int2*>(A + 2 * m);
+                    const uint32_t dp = D[m];
+                    const int c0 = (a01.x + ((int)(dp << 16) >> 16) * w) >> ERTRS_F;
+                    const int c1 = (a01.y + ((int)dp >> 16) * w) >> ERTRS_F;
+                    const uint32_t x0 = x[2 * m], x1 = x[2 * m + 1];
+                    csum += c0 + c1;
+                    ai += c0 * (int)(short)(x0 & 0xffffu) + c1 * (int)(short)(x1 & 0xffffu);
+                    aq += c0 * ((int)x0 >> 16) + c1 * ((int)x1 >> 16);
+                }
+                const int delta = (1 << ERTRS_S) - csum;
+                const uint32_t xc = x[tc];
+                ai += delta * (int)(short)(xc & 0xffffu);
+                aq += delta * ((int)xc >> 16);
+                const int ui = min(255, max(0, (ai + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
+                const int uq = min(255, max(0, (aq + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
+                const uchar2 o = make_uchar2((unsigned char)ui, (unsigned char)uq);
+                const long long i = n - a.n0;
+                *reinterpret_cast<uchar2*>(a.out + 2 * i) = o;
+                if (i >= a.split) *reinterpret_cast<uchar2*>(a.out2 + 2 * (i - a.split)) = o;
+                n += kRsThreads;
+                k += a.step_k;
+                phi += a.step_phi;
+                q += a.step_q;
+                r += a.step_r;
+                if (r >= a.L) { r -= a.L; q++; }
+                if (phi >= a.L) { phi -= a.L; k++; q -= Q; }
+            }
+        }
+    }
+}
+
 // Persistent grid over tiles of kRsTile outputs.  Each CTA keeps the table in shared memory and stages the input
 // span of a tile as words X[j] = int8 bytes (v_I[j], v_I[j+1], v_Q[j], v_Q[j+1]), v = u - 128, so that one dp2a
 // per component applies two taps: with s = 2v + 1 and sum_t c_t = 2^S, acc = 2 * sum_t c_t * v_t + 2^S.  Thread t
 // computes outputs t, t + 256, ... of the tile.  Outputs whose window reaches before the stream start (s = 0 there)
 // take a per-tap path.  F: the input format; the history and the carried samples are uint8 after conversion.
-template <int F>
+// TUNED: the mixing instance (resample_tuned).
+template <int F, bool TUNED>
 __global__ void __launch_bounds__(kRsThreads) resample_kernel(const int32_t* __restrict__ g_A,
                                                               const uint32_t* __restrict__ g_D, RsArgs a) {
     extern __shared__ __align__(16) int32_t rs_smem[];
+    if constexpr (TUNED) {
+        resample_tuned<F>(g_A, g_D, a, rs_smem);
+        return;
+    }
     const int T = a.T, T2 = a.T / 2;
     int32_t* tabA = rs_smem;
     uint32_t* tabD = reinterpret_cast<uint32_t*>(rs_smem + ERTRS_P * T);
@@ -171,10 +274,11 @@ __global__ void __launch_bounds__(kRsThreads) resample_kernel(const int32_t* __r
     }
 }
 
-// Shared memory of one CTA: the table (A and D) and the words of the largest input span of a tile.
-inline size_t rs_smem_bytes(int T, long long L, long long M) {
+// Shared memory of one CTA: the table (A and D) of P sub-phases, the words of the largest input span of a tile and,
+// for a tuned instance, the mixer table E.
+inline size_t rs_smem_bytes(int P, int T, long long L, long long M, bool tuned) {
     const long long span = ((kRsTile - 1) * M + L - 1) / L + 1 + T + 1;
-    return (size_t)ERTRS_P * T * 6 + (size_t)span * 4;
+    return (size_t)P * T * 6 + (size_t)span * 4 + (tuned ? (size_t)ERTRS_NCO_N * 4 : 0);
 }
 
 }  // namespace ert

@@ -42,6 +42,7 @@ int ertgpu_decode_sharded(ertgpu_handle* const* handles, int32_t nhandles, const
     for (int32_t r = 0; r < nhandles; r++) {  // shards are cut at decoder blocks of uint8 input: no resampling or converting handles
         ertgpu_resampler_info ri;
         if (ertgpu_get_resampler(handles[r], &ri, nullptr, 0, nullptr) == ERTGPU_OK) return ERTGPU_EINVAL;
+        if (ertgpu_get_tuning(handles[r], nullptr) == ERTGPU_OK) return ERTGPU_EINVAL;  // tuned, even at the native rate
         int32_t fmt = ERTGPU_FORMAT_CU8;
         if (ertgpu_get_input_format(handles[r], &fmt, nullptr) != ERTGPU_OK || fmt != ERTGPU_FORMAT_CU8) return ERTGPU_EINVAL;
     }

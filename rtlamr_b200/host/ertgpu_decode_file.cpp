@@ -5,7 +5,13 @@
 //   ertgpu_decode_file [-msgtype=scm,idm|all] [-symbollength=72] [-blockdedup=true] [-blocks=4096] [-device=0]
 //                      [-filterid=1,2] [-filtertype=4,5] [-unique=true] [-format=plain|csv|json|xml]
 //                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ]
-//                      [-sampleformat=cu8|cs8|cs16|cf32|wav] [-samplescale=G] FILE|- [FILE ...]
+//                      [-sampleformat=cu8|cs8|cs16|cf32|wav] [-samplescale=G] [-capturefreq=HZ [-centerfreq=HZ]]
+//                      FILE|- [FILE ...]
+// -capturefreq names the frequency the capture was recorded centred at; -centerfreq (rtlamr's flag) the channel to
+// receive, by default the protocols' CenterFreq (912.6 MHz, or 912.38 MHz for r900 alone).  The channel is mixed to
+// 0 Hz exactly inside the GPU resampler, whose lowpass is then the channel filter; a tuned capture may be at up to 10
+// times 32768 * -symbollength.  Without -capturefreq nothing is translated; -centerfreq alone is a usage error, and
+// so is -samplefile with -capturefreq.
 // -samplerate is rtlamr's (rtltcp's) flag name; here it names the capture's sample rate.  The default,
 // 32768 * -symbollength, decodes the bytes as they are; any other rate within 1/4 ... 4 times it is resampled
 // exactly on the GPU first, and Block / Idx then count resampled samples.
@@ -26,12 +32,14 @@
 // Several files are a batch of independent streams through ONE decoder (buffers, tables and kernels set up once):
 // each starts from zeroed history with block numbers from 0, exactly as if it were decoded alone.  They share the
 // sample file, whose offsets keep growing from one file to the next.
+#include <cerrno>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <ctime>
 #include <iostream>
+#include <tuple>
 #include <vector>
 
 #include "receiver.hpp"
@@ -45,6 +53,7 @@ int main(int argc, char** argv) {
     long long blocks = 4096, samplerate = 0;
     bool block_dedup = true, quiet = false, unique = false, single = false;
     std::string filterid, filtertype, format = "plain", samplefile, duration, sampleformat = "cu8", samplescale;
+    std::string capturefreq, centerfreq;
     bool have_scale = false;
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
@@ -53,6 +62,8 @@ int main(int argc, char** argv) {
         else if (a.rfind("-device=", 0) == 0) device = atoi(a.c_str() + 8);
         else if (a.rfind("-samplerate=", 0) == 0) samplerate = atoll(a.c_str() + 12);
         else if (a.rfind("-sampleformat=", 0) == 0) sampleformat = a.substr(14);
+        else if (a.rfind("-capturefreq=", 0) == 0) capturefreq = a.substr(13);
+        else if (a.rfind("-centerfreq=", 0) == 0) centerfreq = a.substr(12);
         else if (a.rfind("-samplescale=", 0) == 0) {
             samplescale = a.substr(13);
             have_scale = true;
@@ -75,9 +86,27 @@ int main(int argc, char** argv) {
         fprintf(stderr, "usage: %s [-msgtype=scm,scm+,idm,netidm,r900,r900bcd|all] [-symbollength=N] [-blockdedup=true|false] "
                         "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
                         "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|wav] [-samplescale=G] "
-                        "[-quiet] FILE|- [FILE ...]\n", argv[0]);
+                        "[-capturefreq=HZ [-centerfreq=HZ]] [-quiet] FILE|- [FILE ...]\n", argv[0]);
         return 2;
     }
+    // -capturefreq / -centerfreq: whole Hz, > 0 and >= 0
+    long long capture_hz = 0, center_hz = 0;
+    for (auto [flag, text, out, min] : {std::make_tuple("-capturefreq", &capturefreq, &capture_hz, 1LL),
+                                        std::make_tuple("-centerfreq", &centerfreq, &center_hz, 0LL)}) {
+        if (text->empty()) continue;
+        char* end = nullptr;
+        errno = 0;
+        *out = strtoll(text->c_str(), &end, 10);
+        if (*end || errno || *out < min) {
+            fprintf(stderr, "invalid value \"%s\" for flag %s: a frequency in Hz%s\n", text->c_str(), flag, min ? " > 0" : "");
+            return 2;
+        }
+    }
+    if (!centerfreq.empty() && capturefreq.empty()) {
+        fprintf(stderr, "-centerfreq needs -capturefreq: the frequency at the centre of the capture\n");
+        return 2;
+    }
+    const bool tuned = capture_hz > 0;
     const bool csv = format == "csv", json = format == "json", xml = format == "xml";
     int64_t limit_ns = 0;
     try {
@@ -141,6 +170,10 @@ int main(int argc, char** argv) {
     }
     // -samplerate names the capture's rate; the default DataRate*ChipLength (32768 * -symbollength) resamples nothing
     const bool resampling = samplerate != 0 && samplerate != 32768LL * chip;
+    if (tuned && !samplefile.empty() && samplefile != "/dev/null") {
+        fprintf(stderr, "-samplefile does not take tuned (-capturefreq) input\n");
+        return 2;
+    }
     if ((resampling || fmt != ERTGPU_FORMAT_CU8) && !samplefile.empty() && samplefile != "/dev/null") {
         fprintf(stderr, "-samplefile needs uint8 (cu8) input at 32768 * -symbollength = %lld Hz; this input is %s at %lld Hz\n",
                 32768LL * chip, fmt == ERTGPU_FORMAT_CU8 ? "cu8" : fmt == ERTGPU_FORMAT_CS8 ? "cs8" : fmt == ERTGPU_FORMAT_CS16 ? "cs16" : "cf32",
@@ -156,7 +189,7 @@ int main(int argc, char** argv) {
         }
     }
     try {
-        receiver::Receiver rcvr(msgtype, chip, device, blocks, resampling ? samplerate : 0, fmt, scale);
+        receiver::Receiver rcvr(msgtype, chip, device, blocks, resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz);
         fputs(rcvr.decoder().Log().c_str(), stderr);
         if (sample) rcvr.SetSampleFile(sample);
         if (limit_ns) rcvr.SetDeadline(start + std::chrono::nanoseconds(limit_ns));

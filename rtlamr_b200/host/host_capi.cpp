@@ -47,10 +47,23 @@ erthost* erthost_new_rate(const char* msgtypes_csv, int chip_length, int device,
                               errbuf, errcap);
 }
 
+erthost* erthost_new_tuned(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
+                           long long input_rate, int format, float scale, long long capture_freq, long long center_freq,
+                           char* errbuf, int errcap);
+
 // The same for IQ in sample format `format` (ERTGPU_FORMAT_*) with gain `scale` (0: the format's default);
 // erthost_decode then counts the format's bytes per sample.
 erthost* erthost_new_format(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
                             long long input_rate, int format, float scale, char* errbuf, int errcap) {
+    return erthost_new_tuned(msgtypes_csv, chip_length, device, max_blocks, max_cands, input_rate, format, scale, 0, 0,
+                             errbuf, errcap);
+}
+
+// The same for a capture recorded centred at capture_freq Hz (0: no translation), decoding the channel at center_freq
+// (0: the protocols' CenterFreq) (protocol::Decoder::SetInputTuning).
+erthost* erthost_new_tuned(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
+                           long long input_rate, int format, float scale, long long capture_freq, long long center_freq,
+                           char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;   // released only on success: a throwing NewParser / Allocate must not leak the handle
     try {
         protocol::RegisterStockParsers();
@@ -61,6 +74,7 @@ erthost* erthost_new_format(const char* msgtypes_csv, int chip_length, int devic
             if (name.empty()) continue;
             h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
         }
+        if (capture_freq > 0 || center_freq != 0) h->d.SetInputTuning(capture_freq, center_freq);
         if (input_rate > 0) h->d.SetInputRate(input_rate);
         if (format != ERTGPU_FORMAT_CU8 || scale != 0.0f) h->d.SetInputFormat(format, scale);
         h->d.Allocate(device, max_blocks, max_cands);

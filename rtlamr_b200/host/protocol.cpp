@@ -579,7 +579,10 @@ void Decoder::RegisterProtocol(ParserPtr p) {
 
 void Decoder::Allocate(int device, int64_t maxBlocksPerCall, int64_t maxCandidates) {
     int rc = ertgpu_allocate(h_, device, maxBlocksPerCall, maxCandidates);
+    if (rc == ERTGPU_EINVAL && tuned_) throw std::invalid_argument(ertgpu_last_error(h_));  // the channel at the native rate
     if (rc != ERTGPU_OK) raise(h_, rc, "Allocate");
+    // a tuned handle at the decoder's own rate gets its resampler here
+    resampling_ = ertgpu_get_resampler(h_, &rs_, nullptr, 0, nullptr) == ERTGPU_OK;
     ertgpu_decoder_config c;
     ertgpu_get_config(h_, &c);
     Cfg.SymbolLength = c.symbol_length;  // decode.go:132-141
@@ -604,6 +607,14 @@ void Decoder::SetInputRate(int64_t hz) {
     if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
     if (rc != ERTGPU_OK) raise(h_, rc, "SetInputRate");
     resampling_ = ertgpu_get_resampler(h_, &rs_, nullptr, 0, nullptr) == ERTGPU_OK;
+}
+
+void Decoder::SetInputTuning(int64_t captureHz, int64_t centerHz) {
+    if (allocated_) throw std::logic_error("SetInputTuning after Allocate");
+    int rc = ertgpu_set_input_tuning(h_, captureHz, centerHz);
+    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
+    if (rc != ERTGPU_OK) raise(h_, rc, "SetInputTuning");
+    tuned_ = true;
 }
 
 void Decoder::SetInputFormat(int32_t format, float scale) {
@@ -676,7 +687,12 @@ void Decoder::Dispatch(const ertgpu_candidate* cands, size_t n, std::vector<Mess
 
 std::string Decoder::Log() const {  // decode.go:73-90
     std::string s;
-    s += "CenterFreq: " + u(Cfg.CenterFreq) + "\nSampleRate: " + u((uint64_t)Cfg.SampleRate) + "\nDataRate: " + u((uint64_t)Cfg.DataRate);
+    ertgpu_tuning_info t;
+    if (tuned_ && ertgpu_get_tuning(h_, &t) == ERTGPU_OK)  // the channel decoded, and the capture's centre
+        s += "CenterFreq: " + std::to_string(t.center_hz) + "\nCaptureFreq: " + std::to_string(t.capture_center_hz);
+    else
+        s += "CenterFreq: " + u(Cfg.CenterFreq);
+    s += "\nSampleRate: " + u((uint64_t)Cfg.SampleRate) + "\nDataRate: " + u((uint64_t)Cfg.DataRate);
     s += "\nChipLength: " + u((uint64_t)Cfg.ChipLength) + "\nPreambleSymbols: " + u((uint64_t)Cfg.PreambleSymbols);
     s += "\nPreambleLength: " + u((uint64_t)Cfg.PreambleLength) + "\nPacketSymbols: " + u((uint64_t)Cfg.PacketSymbols);
     s += "\nPacketLength: " + u((uint64_t)Cfg.PacketLength) + "\nProtocols: ";

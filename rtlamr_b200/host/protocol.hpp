@@ -142,6 +142,11 @@ public:
     // (ertgpu_set_input_rate).  Throws std::invalid_argument for a rate outside [1/4, 4] x the decoder's.
     void SetInputRate(int64_t hz);
     bool Resampling() const { return resampling_; }
+    // The IQ fed to Decode was recorded centred at captureHz; decode the channel at centerHz (0: Cfg.CenterFreq), mixed
+    // to 0 Hz inside the GPU resampler (ertgpu_set_input_tuning).  After the last RegisterProtocol, before
+    // SetInputRate and Allocate.  Throws std::invalid_argument for bad frequencies or call order; Allocate throws it
+    // too when the channel does not fit a capture at the decoder's own rate.
+    void SetInputTuning(int64_t captureHz, int64_t centerHz = 0);
     // The IQ fed to Decode is in format ERTGPU_FORMAT_* (not part of the reference, which takes uint8 IQ only): before
     // Allocate; each component is converted on the GPU to the decoder's byte with gain `scale` (0: the format's
     // default; ertgpu_set_input_format).  Throws std::invalid_argument for an unknown format or a bad scale.
@@ -171,6 +176,7 @@ private:
     std::vector<ertgpu_candidate> cands_;
     bool allocated_ = false;
     bool resampling_ = false;
+    bool tuned_ = false;
     ertgpu_resampler_info rs_{};
     int64_t input_samples_ = 0;  // since Allocate / Reset
     int sample_bytes_ = 2;       // bytes per input IQ sample

@@ -15,7 +15,7 @@ namespace receiver {
 Digest NewDigest(const protocol::Message& m) { return Digest(m.MsgType(), m.MeterType(), m.MeterID(), m.Checksum()); }
 
 Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, int64_t sampleRate,
-                   int32_t format, float scale) {
+                   int32_t format, float scale, int64_t captureFreq, int64_t centerFreq) {
     protocol::RegisterStockParsers();
     std::string list = msgtypes == "all" ? "scm,scm+,idm,r900" : msgtypes;  // main.go:67-73
     std::stringstream ss(list);
@@ -24,6 +24,7 @@ Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int6
         if (!name.empty()) d_.RegisterProtocol(protocol::NewParser(name, chipLength));  // main.go:77-82
     if (blocksPerCall <= 0) blocksPerCall = 4096;
     blocks_per_call_ = blocksPerCall;
+    if (captureFreq > 0) d_.SetInputTuning(captureFreq, centerFreq);
     if (sampleRate > 0) d_.SetInputRate(sampleRate);
     if (format != ERTGPU_FORMAT_CU8) d_.SetInputFormat(format, scale);
     d_.Allocate(device, blocksPerCall, 0);  // main.go:86
