@@ -101,6 +101,13 @@ static inline int ertrs_plan(int64_t rate_in, int64_t rate_out, ertgpu_resampler
     return 0;
 }
 
+/* Number of outputs whose window lies inside the first x input samples (k_n + T/2 <= x - 1). */
+static inline int64_t ertrs_out_end(const ertgpu_resampler_info* info, int64_t x) {
+    const int64_t a = x - info->T / 2;
+    if (a <= 0) return 0;
+    return (int64_t)(((__int128)a * info->L + info->M - 1) / info->M);
+}
+
 /*
  * Tuned input (ertgpu_set_input_tuning): the channel at offset D = center - capture_center Hz from the
  * capture's centre is mixed to 0 Hz as the resampler stages its input, so the same lowpass is the channel

@@ -3,8 +3,8 @@
 // (protocol/decode.go:45-63).
 //
 // Device data layout (all per handle):
-//   iq      : the call's interleaved uint8 I,Q bytes (caller's device buffer or a staging chunk; the resampler's or
-//             the format conversion's output buffer when the handle has an input rate or format)
+//   iq      : the call's interleaved uint8 I,Q bytes (caller's device buffer or a staging chunk; the input stage's
+//             output buffer when the handle has an input rate or format, input_stage.cuh)
 //   hist[2] : last PKL samples of the previous call (ping-pong) -- replaces the Signal tail
 //             (decode.go:165) and the r900 parser's private signal history (r900.go:169)
 //   plane[2]: packed quantizer output, 1 bit per sample, MSB first, laid out as
@@ -17,8 +17,6 @@
 
 #include <algorithm>
 #include <atomic>
-#include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -30,12 +28,11 @@
 #include <thread>
 #include <vector>
 
-#include "convert.cuh"
 #include "copy_pool.hpp"
 #include "demod_fast.cuh"
 #include "demod_generic.cuh"
 #include "ert_common.cuh"
-#include "resample.cuh"
+#include "input_stage.cuh"
 #include "search.cuh"
 #include "synth.cuh"
 
@@ -120,63 +117,15 @@ struct ertgpu_handle {
     int64_t stage_n = 0;
     std::vector<ertgpu_candidate> results;
 
-    // input-rate resampler (ertgpu_set_input_rate); on only when the input rate differs from the decoder's
-    int64_t rate_in = 0;
-    bool rs_on = false;
-    ertgpu_resampler_info rs{};
-    std::vector<int16_t> rs_table;
-    int32_t* d_rs_A = nullptr;       // the table as the kernel reads it (rs_pack_table)
-    uint32_t* d_rs_D = nullptr;
-    uint8_t* d_rs_hist[2] = {nullptr, nullptr};  // input samples the next outputs still read
-    int rs_cur_hist = 0;
-    uint8_t* d_rs_out[2] = {nullptr, nullptr};   // [partial block | new outputs]; the demod reads whole blocks of it
-    int rs_cur_out = 0;
-    size_t rs_out_bytes = 0;
-    size_t rs_smem = 0;
-    int rs_grid = 0;
-    int64_t rs_in_total = 0;    // input samples received since the stream start
-    int64_t rs_out_next = 0;    // first output not yet computed
-    int64_t rs_hist_first = 0;  // first input sample held in d_rs_hist[rs_cur_hist]
-    int64_t rs_hist_n = 0;
-    int64_t rs_pend = 0;        // outputs at the front of d_rs_out[rs_cur_out] that wait for a whole block
-
-    // tuned input (ertgpu_set_input_tuning): the channel at center_hz of a capture centred at capture_hz
-    bool tuned = false;
-    int64_t capture_hz = 0, center_hz = 0;
-    uint32_t nco_step = 0;      // W at the input rate in effect
-    bool rs_mix = false;        // the resampler runs its tuned instance (W != 0 or P != ERTRS_P)
-    uint32_t* d_rs_E = nullptr; // the mixer table (ertrs_nco_table)
-
-    // input format (ertgpu_set_input_format); ERTGPU_FORMAT_CU8 converts nothing
-    int32_t fmt = ERTGPU_FORMAT_CU8;
-    float fmt_scale = 0.0f;
-    int sample_bytes = 2;
-    uint8_t* d_cvt = nullptr;   // native rate, other formats: the converted uint8 IQ of the call's blocks
+    InputStage in{err};  // input format, rate and tuning, and the kernel in front of the pipeline
 };
 
 namespace {
 
-int fail(ertgpu_handle* h, int code, const char* fmt, ...) {
-    if (h) {
-        char buf[512];
-        va_list ap;
-        va_start(ap, fmt);
-        vsnprintf(buf, sizeof(buf), fmt, ap);
-        va_end(ap);
-        h->err = buf;
-    }
-    return code;
-}
+template <class... A>
+int fail(ertgpu_handle* h, int code, const char* fmt, A... args) { return h ? ert::fail(h->err, code, fmt, args...) : code; }
 
-#define CUDA_TRY(h, expr)                                                                       \
-    do {                                                                                        \
-        cudaError_t e__ = (expr);                                                               \
-        if (e__ != cudaSuccess) {                                                               \
-            cudaGetLastError();                                                                 \
-            return fail(h, e__ == cudaErrorMemoryAllocation ? ERTGPU_ENOMEM : ERTGPU_ECUDA,     \
-                        "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-        }                                                                                       \
-    } while (0)
+int64_t decoder_rate(const ertgpu_handle* h) { return (int64_t)h->cfg.data_rate * h->cfg.chip_length; }
 
 // decode.go:377-379
 int32_t next_pow2(int32_t v) {
@@ -243,15 +192,7 @@ void free_device(ertgpu_handle* h) {
     dfree(h->d_out);
     dfree(h->d_counters);
     dfree(h->d_tap);
-    dfree(h->d_rs_A);
-    dfree(h->d_rs_D);
-    dfree(h->d_rs_E);
-    dfree(h->d_cvt);
-    for (int k = 0; k < 2; k++) {
-        dfree(h->d_rs_hist[k]);
-        dfree(h->d_rs_out[k]);
-    }
-    h->rs_out_bytes = 0;
+    h->in.release();
     if (h->h_counters) cudaFreeHost(h->h_counters);
     h->h_counters = nullptr;
     if (h->stream) cudaStreamDestroy(h->stream);
@@ -335,24 +276,11 @@ int launch_search(ertgpu_handle* h, const uint32_t* plane, const SearchParams& s
     return ERTGPU_OK;
 }
 
-int launch_resample(ertgpu_handle* h, const RsArgs& a, cudaStream_t st);
-int launch_convert(ertgpu_handle* h, const uint8_t* in, uint8_t* out, int64_t nsamples, cudaStream_t st);
-
-// "cs16" for the kernel labels of ertgpu_last_kernels
-const char* fmt_name(int f) {
-    return f == ERTGPU_FORMAT_CS8 ? "cs8" : f == ERTGPU_FORMAT_CS16 ? "cs16" : f == ERTGPU_FORMAT_CF32 ? "cf32" : "cu8";
-}
-
-std::string resample_label(const ertgpu_handle* h) {
-    if (h->rs_mix) return std::string("resample_kernel<") + fmt_name(h->fmt) + ",tuned>";
-    return h->fmt == ERTGPU_FORMAT_CU8 ? "resample_kernel" : std::string("resample_kernel<") + fmt_name(h->fmt) + ">";
-}
-
-// Enqueue the whole per-call pipeline for `nblocks` blocks whose IQ bytes are at d_iq.  With rs, the resampler step
-// that writes those bytes runs first; with cvt_in, the format conversion of the call's input at cvt_in into d_iq (either
-// one's time counts as demod time).
-int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uint32_t flags,
-                     cudaStream_t st, const RsArgs* rs = nullptr, const uint8_t* cvt_in = nullptr) {
+// Enqueue the whole per-call pipeline for the s.nblocks blocks whose IQ bytes are at s.iq, behind the input stage's
+// kernel that writes them (its time counts as demod time).
+int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaStream_t st) {
+    const uint8_t* d_iq = s.iq;
+    const int64_t nblocks = s.nblocks;
     const DevCfg& c = h->dcfg;
     uint32_t* plane = h->d_plane[h->cur_plane];
     uint32_t* plane_next = h->d_plane[h->cur_plane ^ 1];
@@ -377,13 +305,7 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
         h->stage_unread++;
     }
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[0], st));
-    if (rs) {
-        int rc = launch_resample(h, *rs, st);
-        if (rc) return rc;
-    } else if (cvt_in) {
-        int rc = launch_convert(h, cvt_in, const_cast<uint8_t*>(d_iq), nblocks * c.BS, st);
-        if (rc) return rc;
-    }
+    if (const int rc = h->in.launch(s, st, &h->launches)) return rc;
     // 1. magnitude + matched filter + quantize + pack
     if (h->demod_variant != 0) {
         int w_used = 0;
@@ -510,8 +432,7 @@ int enqueue_pipeline(ertgpu_handle* h, const uint8_t* d_iq, int64_t nblocks, uin
         h->launches++;
         h->kernels += ";extract_words_kernel<" + std::to_string(short_packets ? 4 : kFullK) + ">";
     }
-    if (rs) h->kernels += ";" + resample_label(h);
-    else if (cvt_in) h->kernels += std::string(";convert_kernel<") + fmt_name(h->fmt) + ">";
+    if (h->in.mode != InputStage::kPass) h->kernels += ";" + h->in.label();
 
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[3], st));
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[4], st));
@@ -627,149 +548,25 @@ int prepare_staging(ertgpu_handle* h, size_t bytes, const void* iq, bool* pageab
     return ERTGPU_OK;
 }
 
-// ---- input-rate resampler (include/ertgpu_resample.h) ----
-
-// The resample_kernel instance of an input format, untuned or tuned.
-decltype(&resample_kernel<ERTGPU_FORMAT_CU8, false>) resample_kernel_of(int f, bool tuned) {
-    switch (f) {
-        case ERTGPU_FORMAT_CS8: return tuned ? resample_kernel<ERTGPU_FORMAT_CS8, true> : resample_kernel<ERTGPU_FORMAT_CS8, false>;
-        case ERTGPU_FORMAT_CS16: return tuned ? resample_kernel<ERTGPU_FORMAT_CS16, true> : resample_kernel<ERTGPU_FORMAT_CS16, false>;
-        case ERTGPU_FORMAT_CF32: return tuned ? resample_kernel<ERTGPU_FORMAT_CF32, true> : resample_kernel<ERTGPU_FORMAT_CF32, false>;
-        default: return tuned ? resample_kernel<ERTGPU_FORMAT_CU8, true> : resample_kernel<ERTGPU_FORMAT_CU8, false>;
-    }
-}
-
-int launch_resample(ertgpu_handle* h, const RsArgs& a, cudaStream_t st) {
-    if (a.count <= 0 && a.carry_n <= 0) return ERTGPU_OK;
-    const long long tiles = (a.count + kRsTile - 1) / kRsTile;
-    const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(tiles, h->rs_grid));
-    resample_kernel_of(h->fmt, h->rs_mix)<<<grid, kRsThreads, h->rs_smem, st>>>(h->d_rs_A, h->d_rs_D, a);
-    CUDA_TRY(h, cudaGetLastError());
-    h->launches++;
-    return ERTGPU_OK;
-}
-
-// Native-rate conversion of nsamples (a multiple of 8) IQ samples of the handle's format at `in` into uint8 IQ at out.
-int launch_convert(ertgpu_handle* h, const uint8_t* in, uint8_t* out, int64_t nsamples, cudaStream_t st) {
-    const long long groups = nsamples / 8;
-    const unsigned grid = (unsigned)std::max<long long>(
-        1, std::min<long long>((groups + kCvtThreads - 1) / kCvtThreads, (long long)h->sm_count * 8));
-    switch (h->fmt) {
-        case ERTGPU_FORMAT_CS8: convert_kernel<ERTGPU_FORMAT_CS8><<<grid, kCvtThreads, 0, st>>>(in, out, groups, h->fmt_scale); break;
-        case ERTGPU_FORMAT_CS16: convert_kernel<ERTGPU_FORMAT_CS16><<<grid, kCvtThreads, 0, st>>>(in, out, groups, h->fmt_scale); break;
-        default: convert_kernel<ERTGPU_FORMAT_CF32><<<grid, kCvtThreads, 0, st>>>(in, out, groups, h->fmt_scale); break;
-    }
-    CUDA_TRY(h, cudaGetLastError());
-    h->launches++;
-    return ERTGPU_OK;
-}
-
-// Number of outputs whose window lies inside the first x input samples (k_n + T/2 <= x - 1).
-int64_t rs_out_end(const ertgpu_handle* h, int64_t x) {
-    const int64_t a = x - h->rs.T / 2;
-    if (a <= 0) return 0;
-    return (int64_t)(((__int128)a * h->rs.L + h->rs.M - 1) / h->rs.M);
-}
-
-int64_t rs_k(const ertgpu_handle* h, int64_t n) { return (int64_t)((__int128)n * h->rs.M / h->rs.L); }
-
-// Most input samples the next step may take so that it completes at most max_blocks decoder blocks.
-int64_t rs_max_input(const ertgpu_handle* h) {
-    const int64_t cap_out = (h->max_blocks + 1) * (int64_t)h->cfg.block_size - 1 - h->rs_pend;
-    return h->rs.T / 2 + rs_k(h, h->rs_out_next + cap_out) - h->rs_in_total;
-}
-
-// One step over c new input samples at d_in (device): every output whose window is complete.  *nblocks = whole
-// decoder blocks the step completes.  Nothing of the handle changes until rs_commit.
-void rs_plan_step(const ertgpu_handle* h, const uint8_t* d_in, int64_t c, RsArgs* a, int64_t* nblocks) {
-    const int64_t BS = h->cfg.block_size, L = h->rs.L, M = h->rs.M, T = h->rs.T;
-    const int64_t in_new = h->rs_in_total + c;
-    const int64_t ne = rs_out_end(h, in_new);
-    const int64_t cnt = ne - h->rs_out_next;
-    *nblocks = (h->rs_pend + cnt) / BS;
-    memset(a, 0, sizeof(*a));
-    a->hist = h->d_rs_hist[h->rs_cur_hist];
-    a->cur = d_in;
-    a->hist_first = h->rs_hist_first;
-    a->hist_n = h->rs_hist_n;
-    a->cur_n = c;
-    a->n0 = h->rs_out_next;
-    a->count = cnt;
-    a->split = *nblocks > 0 ? *nblocks * BS - h->rs_pend : LLONG_MAX;
-    a->base_n = (h->rs_out_next / L) * L;
-    a->base_k = (h->rs_out_next / L) * M;
-    a->out = h->d_rs_out[h->rs_cur_out] + 2 * h->rs_pend;
-    a->out2 = h->d_rs_out[h->rs_cur_out ^ 1];
-    const int64_t first = std::min(in_new, std::max<int64_t>(0, rs_k(h, ne) - T / 2 + 1));
-    a->carry_dst = h->d_rs_hist[h->rs_cur_hist ^ 1];
-    a->carry_first = first;
-    a->carry_n = in_new - first;
-    a->L = L;
-    a->M = M;
-    a->T = (int)T;
-    a->scale = h->fmt_scale;
-    a->E = h->d_rs_E;
-    a->W = h->nco_step;
-    a->P = h->rs.P;
-    const int64_t Q = (int64_t)h->rs.P << ERTRS_F, step = kRsThreads * M;
-    a->step_k = step / L;
-    a->step_phi = step % L;
-    a->step_q = (int64_t)(((__int128)a->step_phi * Q) / L);
-    a->step_r = (int64_t)(((__int128)a->step_phi * Q) % L);
-}
-
-void rs_commit(ertgpu_handle* h, const RsArgs& a, int64_t nblocks) {
-    h->rs_in_total += a.cur_n;
-    h->rs_out_next += a.count;
-    h->rs_hist_first = a.carry_first;
-    h->rs_hist_n = a.carry_n;
-    h->rs_cur_hist ^= 1;
-    const int64_t total = h->rs_pend + a.count;
-    if (nblocks > 0) {
-        h->rs_cur_out ^= 1;  // the outputs past the last whole block are already at the front of the other buffer
-        h->rs_pend = total - nblocks * (int64_t)h->cfg.block_size;
-    } else {
-        h->rs_pend = total;
-    }
-}
-
-void rs_reset_stream(ertgpu_handle* h) {
-    h->rs_in_total = h->rs_out_next = h->rs_hist_first = h->rs_hist_n = h->rs_pend = 0;
-}
-
-// Whole decoder blocks that the next n input samples complete.
-int64_t step_blocks(const ertgpu_handle* h, int64_t n) {
-    if (!h->rs_on) return n / h->cfg.block_size;
-    RsArgs a;
-    int64_t nb = 0;
-    rs_plan_step(h, nullptr, n, &a, &nb);
-    return nb;
-}
-
-// Enqueue the work for the next n input samples, at d_in on the device, on st: the pipeline over the whole blocks
-// they complete, behind the resampler step that produces those blocks when the handle resamples, or behind the
-// conversion of the input format at the decoder's own rate.
+// Enqueue the work for the next n input samples, at d_in on the device, on st: the input stage's step and the pipeline
+// over the whole blocks it completes.
 int enqueue_step(ertgpu_handle* h, const uint8_t* d_in, int64_t n, uint32_t flags, cudaStream_t st) {
-    if (!h->rs_on && h->d_cvt) return enqueue_pipeline(h, h->d_cvt, n / h->cfg.block_size, flags, st, nullptr, d_in);
-    if (!h->rs_on) return enqueue_pipeline(h, d_in, n / h->cfg.block_size, flags, st);
-    RsArgs a;
-    int64_t nb = 0;
-    rs_plan_step(h, d_in, n, &a, &nb);
+    const InputStep s = h->in.plan(d_in, n);
     int rc;
-    if (nb > 0) {
-        rc = enqueue_pipeline(h, h->d_rs_out[h->rs_cur_out], nb, flags, st, &a);
-    } else {  // no pipeline: the launch alone is pending, with no counters to read
+    if (s.nblocks > 0) {
+        rc = enqueue_pipeline(h, s, flags, st);
+    } else {  // no pipeline: the stage's launch alone is pending, with no counters to read
         h->launches = 0;
-        rc = launch_resample(h, a, st);
+        rc = h->in.launch(s, st, &h->launches);
         if (rc == ERTGPU_OK && h->launches) {
             h->pending = true;
             h->pending_counts = false;
             h->pending_stream = st;
-            if (h->kernels.empty()) h->kernels = resample_label(h);  // otherwise the last pipeline's list stays
+            if (h->kernels.empty()) h->kernels = h->in.label();  // otherwise the last pipeline's list stays
         }
     }
     if (rc) return rc;
-    rs_commit(h, a, nb);
+    h->in.commit(s);
     return ERTGPU_OK;
 }
 
@@ -781,31 +578,14 @@ void begin_call(ertgpu_handle* h) {
     h->total_hits = h->total_valid = 0;
 }
 
-// The start of both decode calls.  The input is checked before anything is collected, so that a rejected call leaves
-// the stream as it was: with s bytes per IQ sample, a resampling handle takes whole IQ samples (s-byte aligned on the
-// device), a native one whole blocks of BlockSize * s bytes (16-byte aligned on the device), and a device call
-// completes at most max_blocks_per_call blocks.  Then the previous call's work is collected and this call's results
+// The start of both decode calls.  The input is checked by the input stage's rules before anything is collected, so
+// that a rejected call leaves the stream as it was.  Then the previous call's work is collected and this call's results
 // start empty.
 int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
-    if (h && h->rs_on && nbytes % h->sample_bytes)
-        return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of %d-byte IQ samples", nbytes, h->sample_bytes);
+    if (const int rc = h ? h->in.check_samples(nbytes) : ERTGPU_OK) return rc;
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     if (!iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
-    const int align = h->rs_on ? h->sample_bytes : 16;
-    if (device && (reinterpret_cast<uintptr_t>(iq) & (align - 1)) != 0)
-        return fail(h, ERTGPU_EINVAL, "device input must be %d-byte aligned", align);
-    const size_t bs2 = (size_t)h->cfg.block_size2;
-    if (!h->rs_on && h->fmt == ERTGPU_FORMAT_CU8 && nbytes % bs2)
-        return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize2 %zu", nbytes, bs2);
-    const size_t bsf = (size_t)h->cfg.block_size * h->sample_bytes;
-    if (!h->rs_on && nbytes % bsf)
-        return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize * %d = %zu", nbytes, h->sample_bytes, bsf);
-    if (device) {
-        const int64_t nb = step_blocks(h, (int64_t)(nbytes / h->sample_bytes));
-        if (nb > h->max_blocks)
-            return fail(h, ERTGPU_ESIZE, "%zu input bytes complete %lld blocks, more than max_blocks_per_call %lld", nbytes,
-                        (long long)nb, (long long)h->max_blocks);
-    }
+    if (const int rc = h->in.check_call(iq, nbytes, device)) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
     if (h->pending) {
         int rc = collect(h);
@@ -880,8 +660,8 @@ int ertgpu_stock_protocol(const char* msgtype, int32_t chip_length, ertgpu_proto
 int ertgpu_register_protocol(ertgpu_handle* h, const ertgpu_protocol* p) {
     if (!h || !p) return ERTGPU_EINVAL;
     if (h->allocated) return fail(h, ERTGPU_EINVAL, "register_protocol after allocate");
-    if (h->rate_in) return fail(h, ERTGPU_EINVAL, "register_protocol after set_input_rate");
-    if (h->tuned) return fail(h, ERTGPU_EINVAL, "register_protocol after set_input_tuning");
+    if (h->in.rate_in) return fail(h, ERTGPU_EINVAL, "register_protocol after set_input_rate");
+    if (h->in.tuned) return fail(h, ERTGPU_EINVAL, "register_protocol after set_input_tuning");
     if (h->protos.size() >= ERTGPU_MAX_PROTOCOLS) return fail(h, ERTGPU_EINVAL, "too many protocols");
     const size_t n = strnlen(p->preamble, sizeof(p->preamble));
     if (n == 0 || n > ERTGPU_MAX_PREAMBLE) return fail(h, ERTGPU_EINVAL, "bad preamble length %zu", n);
@@ -923,14 +703,9 @@ int ertgpu_allocate(ertgpu_handle* h, int32_t device, int64_t max_blocks_per_cal
     return rc;
 }
 
-static int configure_rate(ertgpu_handle* h, int64_t hz);
-
 static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_per_call, int64_t max_candidates) {
     if (h->protos.empty()) return fail(h, ERTGPU_EINVAL, "no protocol registered");
-    if (h->tuned && !h->rate_in) {  // a tuned handle at the decoder's own rate: the channel must lie inside it
-        const int rc = configure_rate(h, (int64_t)h->cfg.data_rate * h->cfg.chip_length);
-        if (rc) return rc;
-    }
+    if (const int rc = h->in.plan_native(decoder_rate(h))) return rc;
 
     // decode.go:131-141
     ertgpu_decoder_config& c = h->cfg;
@@ -1059,44 +834,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->device);
     if (h->sm_count < 1) h->sm_count = 132;
 
-    if (h->rs_on) {
-        const ertgpu_resampler_info& r = h->rs;
-        std::vector<int32_t> A((size_t)r.P * r.T);
-        std::vector<uint32_t> D((size_t)r.P * (r.T / 2));
-        rs_pack_table(h->rs_table.data(), r.P, r.T, A.data(), D.data());
-        CUDA_TRY(h, cudaMalloc(&h->d_rs_A, A.size() * sizeof(int32_t)));
-        CUDA_TRY(h, cudaMemcpy(h->d_rs_A, A.data(), A.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-        CUDA_TRY(h, cudaMalloc(&h->d_rs_D, D.size() * sizeof(uint32_t)));
-        CUDA_TRY(h, cudaMemcpy(h->d_rs_D, D.data(), D.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        if (h->rs_mix) {
-            std::vector<uint32_t> E(ERTRS_NCO_N);
-            ertrs_nco_table(E.data());
-            CUDA_TRY(h, cudaMalloc(&h->d_rs_E, E.size() * sizeof(uint32_t)));
-            CUDA_TRY(h, cudaMemcpy(h->d_rs_E, E.data(), E.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        }
-        for (int k = 0; k < 2; k++) {
-            CUDA_TRY(h, cudaMalloc(&h->d_rs_hist[k], (size_t)r.T * 2 + 16));
-            // a step completes at most max_blocks blocks: less than (max_blocks + 1) * BS outputs are buffered
-            h->rs_out_bytes = (size_t)(max_blocks_per_call + 1) * c.block_size2 + 64;
-            CUDA_TRY(h, cudaMalloc(&h->d_rs_out[k], h->rs_out_bytes));
-        }
-        h->rs_smem = rs_smem_bytes(r.P, r.T, r.L, r.M, h->rs_mix);
-        {   // a property of the kernel, not of the handle: every handle on the device gets the largest any table needs
-            static OncePerDevice once;
-            if (once.first(h->device))
-                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF32; f++)
-                    for (int tuned = 0; tuned < 2; tuned++)
-                        CUDA_TRY(h, cudaFuncSetAttribute(resample_kernel_of(f, tuned), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        }
-        if (h->rs_smem > 227 * 1024) return fail(h, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", h->rs_smem);
-        int per_sm = 0;
-        CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel_of(h->fmt, h->rs_mix), kRsThreads, h->rs_smem));
-        h->rs_grid = std::max(1, per_sm) * h->sm_count;
-        h->rs_cur_hist = h->rs_cur_out = 0;
-        rs_reset_stream(h);
-    } else if (h->fmt != ERTGPU_FORMAT_CU8) {
-        CUDA_TRY(h, cudaMalloc(&h->d_cvt, (size_t)max_blocks_per_call * c.block_size2));   // 256-byte aligned
-    }
+    if (const int rc = h->in.allocate(h->device, c.block_size, max_blocks_per_call, h->sm_count)) return rc;
     h->cur_plane = h->cur_hist = 0;
     h->hist_valid = 0;
     h->block_counter = 0;
@@ -1120,40 +858,8 @@ int ertgpu_reset(ertgpu_handle* h) {
     h->fresh = true;
     h->hist_valid = 0;
     h->block_counter = 0;
-    rs_reset_stream(h);
+    h->in.reset_stream();
     begin_call(h);
-    return ERTGPU_OK;
-}
-
-// The resampler for input at hz: ertrs_plan, or ertrs_plan_tuned and the NCO step on a tuned handle.  It runs when
-// the rates differ or a tuned handle mixes; the tuned instance when it mixes or its plan has P != ERTRS_P.
-static int configure_rate(ertgpu_handle* h, int64_t hz) {
-    const int64_t rate_out = (int64_t)h->cfg.data_rate * h->cfg.chip_length;
-    ertgpu_resampler_info info{};
-    uint32_t w = 0;
-    if (h->tuned) {
-        const int64_t off = h->center_hz - h->capture_hz;
-        if (ertrs_plan_tuned(hz, rate_out, off, &info) != 0)
-            return fail(h, ERTGPU_EINVAL,
-                        "input rate %lld Hz, channel offset %lld Hz: the decoder rate %lld Hz must be within 1/10 ... 4 "
-                        "times the input rate, and |offset| + 0.4 * min(rates) at most half the input rate",
-                        (long long)hz, (long long)off, (long long)rate_out);
-        w = ertrs_nco_step(off, hz);
-    } else if (ertrs_plan(hz, rate_out, &info) != 0) {
-        return fail(h, ERTGPU_EINVAL, "input rate %lld Hz: the decoder rate %lld Hz must be within 1/4 ... 4 times it",
-                    (long long)hz, (long long)rate_out);
-    }
-    const bool on = hz != rate_out || w != 0;
-    std::vector<int16_t> table;
-    if (on) {
-        table.resize((size_t)(info.P + 1) * info.T);
-        if (ertrs_build_table(&info, table.data()) != 0) return fail(h, ERTGPU_EINVAL, "resampler table does not fit int16");
-    }
-    h->rs_on = on;
-    h->rs_mix = on && (w != 0 || info.P != ERTRS_P);
-    h->nco_step = w;
-    h->rs = info;
-    h->rs_table.swap(table);
     return ERTGPU_OK;
 }
 
@@ -1161,69 +867,36 @@ int ertgpu_set_input_rate(ertgpu_handle* h, int64_t hz) {
     if (!h) return ERTGPU_EINVAL;
     if (h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_rate after allocate");
     if (h->protos.empty()) return fail(h, ERTGPU_EINVAL, "set_input_rate before register_protocol");
-    const int rc = configure_rate(h, hz);
-    if (rc) return rc;
-    h->rate_in = hz;
-    return ERTGPU_OK;
+    return h->in.set_rate(hz, decoder_rate(h));
 }
 
 int ertgpu_set_input_tuning(ertgpu_handle* h, int64_t capture_center_hz, int64_t center_hz) {
     if (!h) return ERTGPU_EINVAL;
     if (h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_tuning after allocate");
     if (h->protos.empty()) return fail(h, ERTGPU_EINVAL, "set_input_tuning before register_protocol");
-    if (h->rate_in) return fail(h, ERTGPU_EINVAL, "set_input_tuning after set_input_rate");
-    if (capture_center_hz <= 0 || center_hz < 0)
-        return fail(h, ERTGPU_EINVAL, "capture centre %lld Hz must be > 0 and channel %lld Hz >= 0",
-                    (long long)capture_center_hz, (long long)center_hz);
-    h->tuned = true;
-    h->capture_hz = capture_center_hz;
-    h->center_hz = center_hz ? center_hz : (int64_t)h->cfg.center_freq;  // decode.go:105: the last CenterFreq
-    return ERTGPU_OK;
+    return h->in.set_tuning(capture_center_hz, center_hz, (int64_t)h->cfg.center_freq, decoder_rate(h));
 }
 
 int ertgpu_get_tuning(const ertgpu_handle* h, ertgpu_tuning_info* info) {
-    if (!h || !h->tuned) return ERTGPU_EINVAL;
-    if (info) {
-        const int64_t rate = h->rate_in ? h->rate_in : (int64_t)h->cfg.data_rate * h->cfg.chip_length;
-        info->capture_center_hz = h->capture_hz;
-        info->center_hz = h->center_hz;
-        info->offset_hz = h->center_hz - h->capture_hz;
-        // W at the input rate in effect (the decoder's own until set_input_rate)
-        const int64_t ad = info->offset_hz < 0 ? -info->offset_hz : info->offset_hz;
-        info->nco_step = ad <= rate ? ertrs_nco_step(info->offset_hz, rate) : 0;
-        info->nco_bits = ERTRS_NCO_BITS;
-    }
-    return ERTGPU_OK;
+    return h ? h->in.tuning(info) : ERTGPU_EINVAL;
 }
 
 int ertgpu_set_input_format(ertgpu_handle* h, int32_t format, float scale) {
     if (!h) return ERTGPU_EINVAL;
     if (h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_format after allocate");
-    if (format < ERTGPU_FORMAT_CU8 || format > ERTGPU_FORMAT_CF32) return fail(h, ERTGPU_EINVAL, "unknown input format %d", format);
-    if (!std::isfinite(scale) || scale < 0.0f) return fail(h, ERTGPU_EINVAL, "input scale %g is not a finite value >= 0", (double)scale);
-    if (format == ERTGPU_FORMAT_CU8 && scale != 0.0f) return fail(h, ERTGPU_EINVAL, "cu8 input is not scaled (scale %g)", (double)scale);
-    if (scale == 0.0f)
-        scale = format == ERTGPU_FORMAT_CS8 ? 1.0f : format == ERTGPU_FORMAT_CS16 ? 1.0f / 256.0f : format == ERTGPU_FORMAT_CF32 ? 128.0f : 0.0f;
-    h->fmt = format;
-    h->fmt_scale = scale;
-    h->sample_bytes = fmt_sample_bytes(format);
-    return ERTGPU_OK;
+    return h->in.set_format(format, scale);
 }
 
 int ertgpu_get_input_format(const ertgpu_handle* h, int32_t* format, float* scale) {
     if (!h) return ERTGPU_EINVAL;
-    if (format) *format = h->fmt;
-    if (scale) *scale = h->fmt_scale;
+    if (format) *format = h->in.fmt;
+    if (scale) *scale = h->in.scale;
     return ERTGPU_OK;
 }
 
 int ertgpu_get_resampler(const ertgpu_handle* h, ertgpu_resampler_info* info, int16_t* table, size_t cap,
                          size_t* n_out) {
-    if (!h || !h->rs_on) return ERTGPU_EINVAL;
-    if (info) *info = h->rs;
-    if (n_out) *n_out = h->rs_table.size();
-    if (table && cap >= h->rs_table.size()) memcpy(table, h->rs_table.data(), h->rs_table.size() * sizeof(int16_t));
-    return ERTGPU_OK;
+    return h ? h->in.resampler(info, table, cap, n_out) : ERTGPU_EINVAL;
 }
 
 int ertgpu_set_demod_variant(ertgpu_handle* h, int32_t variant) {
@@ -1238,7 +911,7 @@ int ertgpu_set_demod_variant(ertgpu_handle* h, int32_t variant) {
 int ertgpu_decode_device_async(ertgpu_handle* h, const void* d_iq, size_t nbytes, uint32_t flags, void* stream) {
     const int rc = begin_decode(h, d_iq, nbytes, true);
     if (rc || nbytes == 0) return rc;
-    return enqueue_step(h, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / h->sample_bytes), flags,
+    return enqueue_step(h, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / h->in.sample_bytes), flags,
                         stream ? (cudaStream_t)stream : h->stream);
 }
 
@@ -1254,25 +927,18 @@ int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t f
                   size_t cap, size_t* n_out) {
     int rc = begin_decode(h, iq, nbytes, false);
     if (rc) return rc;
-    const size_t s = (size_t)h->sample_bytes;
-    const int64_t total = (int64_t)(nbytes / s), BS = h->cfg.block_size;
+    const size_t s = (size_t)h->in.sample_bytes;
+    const int64_t total = (int64_t)(nbytes / s);
     if (total == 0) return deliver(h, out, cap, n_out);
 
-    // Staging chunks (allocated on first use) of s bytes per sample: the H2D copy of chunk i+1 overlaps the kernels of
-    // chunk i.  32 MiB of whole decoder blocks natively; a resampling chunk also covers the filter's look-ahead, and the step that takes it
-    // completes at most max_blocks blocks (rs_max_input).  Decimating by more than 4 (tuned handles, up to 10) the
-    // chunk grows with M / L, so that it still reaches max_blocks blocks.
-    const int64_t ratio = h->rs_on ? std::max<int64_t>(4, (h->rs.M + h->rs.L - 1) / h->rs.L) : 4;
-    const int64_t chunk = h->rs_on ? std::min<int64_t>(16 << 20, ratio * (h->max_blocks + 1) * BS + h->rs.T + 8)
-                                   : BS * std::min<int64_t>(h->max_blocks, std::max<int64_t>(1, (32 << 20) / h->cfg.block_size2));
+    // Staging chunks of s bytes per sample (allocated on first use): the H2D copy of chunk i+1 overlaps chunk i's kernels.
     bool pageable = true;
-    rc = prepare_staging(h, (size_t)chunk * s, iq, &pageable);
+    rc = prepare_staging(h, (size_t)h->in.chunk() * s, iq, &pageable);
     if (rc) return rc;
     int64_t done = 0, launches = 0;
     for (int64_t i = 0; done < total; i++) {
         const int k = (int)(i & 1);
-        int64_t c = std::min(chunk, total - done);
-        if (h->rs_on) c = std::min(c, rs_max_input(h));
+        const int64_t c = h->in.next_chunk(total - done);
         if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // the kernels that read d_stage[k] (and its H2D) are done
         const uint8_t* src = iq + (size_t)done * s;
         if (pageable) {
@@ -1370,7 +1036,7 @@ int ertgpu_tap(ertgpu_handle* h, int32_t which, int64_t block, void* dst, size_t
         CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), qd, bytes.size(), cudaMemcpyDeviceToHost, h->stream));
         CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     } else if (which == ERTGPU_TAP_RESAMPLED) {
-        if (!h->rs_on && h->fmt == ERTGPU_FORMAT_CU8) return fail(h, ERTGPU_EINVAL, "the handle neither resamples nor converts its input");
+        if (h->in.mode == InputStage::kPass) return fail(h, ERTGPU_EINVAL, "the handle neither resamples nor converts its input");
         bytes.resize((size_t)c.BS * 2);
         CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), h->last_iq + (size_t)b * c.BS * 2, bytes.size(), cudaMemcpyDeviceToHost, h->stream));
         CUDA_TRY(h, cudaStreamSynchronize(h->stream));

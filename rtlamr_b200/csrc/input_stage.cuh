@@ -1,0 +1,396 @@
+// input_stage.cuh -- the input stage of a libertgpu handle: everything between the caller's bytes and the uint8 IQ blocks
+// the demod reads.  It owns the input's format, rate and tuning (ertgpu_set_input_*), the mode they resolve to, the
+// resampler's plan, tables and stream position, and it launches the one kernel in front of the pipeline:
+// convert_kernel<F> (convert.cuh) or resample_kernel<F, TUNED> (resample.cuh).  Host code only.
+#pragma once
+
+#include <algorithm>
+#include <climits>
+#include <cmath>
+#include <cstdarg>
+#include <cstdio>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "convert.cuh"
+#include "demod_fast.cuh"  // OncePerDevice
+#include "resample.cuh"
+
+namespace ert {
+
+// The message goes to err; returns code.
+inline int fail(std::string& err, int code, const char* fmt, ...) {
+    char buf[512];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf, sizeof(buf), fmt, ap);
+    va_end(ap);
+    err = buf;
+    return code;
+}
+
+// `sink`: whatever fail() takes (a handle, an error string)
+#define CUDA_TRY(sink, expr)                                                                    \
+    do {                                                                                        \
+        cudaError_t e__ = (expr);                                                               \
+        if (e__ != cudaSuccess) {                                                               \
+            cudaGetLastError();                                                                 \
+            return fail(sink, e__ == cudaErrorMemoryAllocation ? ERTGPU_ENOMEM : ERTGPU_ECUDA,  \
+                        "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
+        }                                                                                       \
+    } while (0)
+
+// One step of the stage: input samples at rs.cur on the device, and the whole uint8 blocks they complete.
+struct InputStep {
+    const uint8_t* iq = nullptr;  // the blocks the pipeline reads: rs.cur itself in pass-through mode
+    int64_t nblocks = 0;
+    RsArgs rs{};                  // the kernel's arguments (convert_kernel reads rs.cur only)
+};
+
+struct InputStage {
+    // kPass: uint8 IQ at the decoder's rate, read where the caller put it.  kConvert: another format at that rate,
+    // convert_kernel<F> into d_out[0].  kResample(Tuned): resample_kernel<F, false (true)> into d_out[cur_out]; the tuned
+    // instance runs for a tuned capture or a plan with P != ERTRS_P.
+    enum Mode { kPass, kConvert, kResample, kResampleTuned };
+
+    explicit InputStage(std::string& err) : err_(err) {}
+
+    // configuration, resolved into `mode` by each setter
+    int32_t fmt = ERTGPU_FORMAT_CU8;
+    float scale = 0.0f;
+    int sample_bytes = 2;
+    int64_t rate_in = 0;        // set_rate's rate (0: none)
+    bool tuned = false;         // set_tuning: the channel at center_hz of a capture centred at capture_hz
+    int64_t capture_hz = 0, center_hz = 0;
+    uint32_t nco_step = 0;      // W at the input rate in effect
+    Mode mode = kPass;
+    ertgpu_resampler_info rs{};
+    std::vector<int16_t> table;
+
+    // decoder geometry (allocate)
+    int64_t block = 0, max_blocks = 0;
+
+    // device state
+    int32_t* d_A = nullptr;     // the table as the kernel reads it (rs_pack_table)
+    uint32_t* d_D = nullptr;
+    uint32_t* d_E = nullptr;    // the mixer table (ertrs_nco_table)
+    uint8_t* d_hist[2] = {nullptr, nullptr};  // input samples the next outputs still read
+    int cur_hist = 0;
+    uint8_t* d_out[2] = {nullptr, nullptr};   // [partial block | new outputs]; the demod reads whole blocks of it
+    int cur_out = 0;
+    int64_t in_total = 0;       // input samples received since the stream start
+    int64_t out_next = 0;       // first output not yet computed
+    int64_t hist_first = 0, hist_n = 0;  // the input samples held in d_hist[cur_hist]
+    int64_t pend = 0;           // outputs at the front of d_out[cur_out] that wait for a whole block
+    size_t smem = 0;
+    int grid = 0;               // most CTAs of one launch
+
+    bool resamples() const { return mode >= kResample; }
+
+    // ---- configuration (the handle is not allocated; rate_out = DataRate * ChipLength) ----
+    int set_rate(int64_t hz, int64_t rate_out) {
+        if (const int rc = configure_rate(hz, rate_out)) return rc;
+        rate_in = hz;
+        return ERTGPU_OK;
+    }
+
+    // center_hz 0: default_center_hz, the decoder's CenterFreq
+    int set_tuning(int64_t capture_center_hz, int64_t channel_hz, int64_t default_center_hz, int64_t rate_out) {
+        if (rate_in) return fail(err_, ERTGPU_EINVAL, "set_input_tuning after set_input_rate");
+        if (capture_center_hz <= 0 || channel_hz < 0)
+            return fail(err_, ERTGPU_EINVAL, "capture centre %lld Hz must be > 0 and channel %lld Hz >= 0",
+                        (long long)capture_center_hz, (long long)channel_hz);
+        tuned = true;
+        capture_hz = capture_center_hz;
+        center_hz = channel_hz ? channel_hz : default_center_hz;  // decode.go:105: the last CenterFreq
+        const int64_t off = center_hz - capture_hz, ad = off < 0 ? -off : off;
+        nco_step = ad <= rate_out ? ertrs_nco_step(off, rate_out) : 0;  // at the decoder's rate until set_rate
+        return ERTGPU_OK;
+    }
+
+    int set_format(int32_t format, float g) {
+        if (format < ERTGPU_FORMAT_CU8 || format > ERTGPU_FORMAT_CF32) return fail(err_, ERTGPU_EINVAL, "unknown input format %d", format);
+        if (!std::isfinite(g) || g < 0.0f) return fail(err_, ERTGPU_EINVAL, "input scale %g is not a finite value >= 0", (double)g);
+        if (format == ERTGPU_FORMAT_CU8 && g != 0.0f) return fail(err_, ERTGPU_EINVAL, "cu8 input is not scaled (scale %g)", (double)g);
+        if (g == 0.0f)
+            g = format == ERTGPU_FORMAT_CS8 ? 1.0f : format == ERTGPU_FORMAT_CS16 ? 1.0f / 256.0f : format == ERTGPU_FORMAT_CF32 ? 128.0f : 0.0f;
+        fmt = format;
+        scale = g;
+        sample_bytes = fmt_sample_bytes(format);
+        if (!resamples()) mode = fmt == ERTGPU_FORMAT_CU8 ? kPass : kConvert;
+        return ERTGPU_OK;
+    }
+
+    // At allocate: a tuned handle at the decoder's own rate gets its plan here, and the channel must lie inside it.
+    int plan_native(int64_t rate_out) { return tuned && !rate_in ? configure_rate(rate_out, rate_out) : ERTGPU_OK; }
+
+    int tuning(ertgpu_tuning_info* info) const {
+        if (!tuned) return ERTGPU_EINVAL;
+        if (info) {
+            info->capture_center_hz = capture_hz;
+            info->center_hz = center_hz;
+            info->offset_hz = center_hz - capture_hz;
+            info->nco_step = nco_step;
+            info->nco_bits = ERTRS_NCO_BITS;
+        }
+        return ERTGPU_OK;
+    }
+
+    int resampler(ertgpu_resampler_info* info, int16_t* dst, size_t cap, size_t* n_out) const {
+        if (!resamples()) return ERTGPU_EINVAL;
+        if (info) *info = rs;
+        if (n_out) *n_out = table.size();
+        if (dst && cap >= table.size()) memcpy(dst, table.data(), table.size() * sizeof(int16_t));
+        return ERTGPU_OK;
+    }
+
+    // ---- device buffers ----
+    // Blocks of block_size samples, a step completes at most max_blocks_per_step of them; sm_count SMs.
+    int allocate(int device, int64_t block_size, int64_t max_blocks_per_step, int sm_count) {
+        block = block_size;
+        max_blocks = max_blocks_per_step;
+        reset_stream();
+        if (mode == kPass) return ERTGPU_OK;
+        if (mode == kConvert) {
+            grid = sm_count * 8;
+            CUDA_TRY(err_, cudaMalloc(&d_out[0], (size_t)max_blocks * block * 2));  // 256-byte aligned
+            return ERTGPU_OK;
+        }
+        const bool mix = mode == kResampleTuned;
+        std::vector<int32_t> A((size_t)rs.P * rs.T);
+        std::vector<uint32_t> D((size_t)rs.P * (rs.T / 2));
+        rs_pack_table(table.data(), rs.P, rs.T, A.data(), D.data());
+        CUDA_TRY(err_, cudaMalloc(&d_A, A.size() * sizeof(int32_t)));
+        CUDA_TRY(err_, cudaMemcpy(d_A, A.data(), A.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+        CUDA_TRY(err_, cudaMalloc(&d_D, D.size() * sizeof(uint32_t)));
+        CUDA_TRY(err_, cudaMemcpy(d_D, D.data(), D.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        if (mix) {
+            std::vector<uint32_t> E(ERTRS_NCO_N);
+            ertrs_nco_table(E.data());
+            CUDA_TRY(err_, cudaMalloc(&d_E, E.size() * sizeof(uint32_t)));
+            CUDA_TRY(err_, cudaMemcpy(d_E, E.data(), E.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        }
+        for (int k = 0; k < 2; k++) {
+            CUDA_TRY(err_, cudaMalloc(&d_hist[k], (size_t)rs.T * 2 + 16));
+            // a step completes at most max_blocks blocks: less than (max_blocks + 1) * BS outputs are buffered
+            CUDA_TRY(err_, cudaMalloc(&d_out[k], (size_t)(max_blocks + 1) * block * 2 + 64));
+        }
+        smem = rs_smem_bytes(rs.P, rs.T, rs.L, rs.M, mix);
+        {   // a property of the kernel, not of the handle: every handle on the device gets the largest any table needs
+            static OncePerDevice once;
+            if (once.first(device))
+                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF32; f++)
+                    for (int t = 0; t < 2; t++)
+                        CUDA_TRY(err_, cudaFuncSetAttribute(resample_kernel_of(f, t), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        }
+        if (smem > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", smem);
+        int per_sm = 0;
+        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel_of(fmt, mix), kRsThreads, smem));
+        grid = std::max(1, per_sm) * sm_count;
+        return ERTGPU_OK;
+    }
+
+    void release() {
+        auto dfree = [](auto*& p) { if (p) cudaFree(p); p = nullptr; };
+        dfree(d_A);
+        dfree(d_D);
+        dfree(d_E);
+        for (int k = 0; k < 2; k++) {
+            dfree(d_hist[k]);
+            dfree(d_out[k]);
+        }
+    }
+
+    void reset_stream() { in_total = out_next = hist_first = hist_n = pend = cur_hist = cur_out = 0; }
+
+    // ---- calls ----
+    // Before anything else of a decode call: a resampling stage takes whole IQ samples of s bytes.
+    int check_samples(size_t nbytes) const {
+        if (resamples() && nbytes % sample_bytes)
+            return fail(err_, ERTGPU_ESIZE, "nbytes %zu is not a whole number of %d-byte IQ samples", nbytes, sample_bytes);
+        return ERTGPU_OK;
+    }
+
+    // The rest of a call's input rules: device input is s-byte aligned when resampling, 16-byte aligned otherwise; a
+    // native stage takes whole blocks of BlockSize * s bytes; a device call completes at most max_blocks blocks.
+    int check_call(const void* iq, size_t nbytes, bool device) const {
+        const int align = resamples() ? sample_bytes : 16;
+        if (device && (reinterpret_cast<uintptr_t>(iq) & (align - 1)) != 0)
+            return fail(err_, ERTGPU_EINVAL, "device input must be %d-byte aligned", align);
+        const size_t bs2 = (size_t)block * 2;
+        if (mode == kPass && nbytes % bs2)
+            return fail(err_, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize2 %zu", nbytes, bs2);
+        const size_t bsf = (size_t)block * sample_bytes;
+        if (!resamples() && nbytes % bsf)
+            return fail(err_, ERTGPU_ESIZE, "nbytes %zu is not a multiple of BlockSize * %d = %zu", nbytes, sample_bytes, bsf);
+        if (device) {
+            const int64_t nb = plan(nullptr, (int64_t)(nbytes / sample_bytes)).nblocks;
+            if (nb > max_blocks)
+                return fail(err_, ERTGPU_ESIZE, "%zu input bytes complete %lld blocks, more than max_blocks_per_call %lld", nbytes,
+                            (long long)nb, (long long)max_blocks);
+        }
+        return ERTGPU_OK;
+    }
+
+    // Input samples per staging chunk of ertgpu_decode.  32 MiB of whole decoder blocks natively; a resampling chunk also
+    // covers the filter's look-ahead.  Decimating by more than 4 (tuned handles, up to 10) the chunk grows with M / L,
+    // so that it still reaches max_blocks blocks.
+    int64_t chunk() const {
+        if (!resamples()) return block * std::min<int64_t>(max_blocks, std::max<int64_t>(1, (32 << 20) / (block * 2)));
+        const int64_t ratio = std::max<int64_t>(4, (rs.M + rs.L - 1) / rs.L);
+        return std::min<int64_t>(16 << 20, ratio * (max_blocks + 1) * block + rs.T + 8);
+    }
+
+    // The next chunk when `left` input samples remain: when resampling, the step that takes it completes at most
+    // max_blocks blocks.
+    int64_t next_chunk(int64_t left) const {
+        const int64_t c = std::min(chunk(), left);
+        return resamples() ? std::min(c, max_input()) : c;
+    }
+
+    // The step over n new input samples at d_in (device).  Nothing of the stage changes until commit.
+    InputStep plan(const uint8_t* d_in, int64_t n) const {
+        InputStep s;
+        s.rs.cur = d_in;
+        if (!resamples()) {
+            s.iq = mode == kPass ? d_in : d_out[0];
+            s.nblocks = n / block;
+            return s;
+        }
+        // every output whose window is complete
+        const int64_t L = rs.L, M = rs.M, T = rs.T;
+        const int64_t in_new = in_total + n;
+        const int64_t ne = ertrs_out_end(&rs, in_new);
+        const int64_t cnt = ne - out_next;
+        s.nblocks = (pend + cnt) / block;
+        s.iq = d_out[cur_out];
+        RsArgs* a = &s.rs;
+        a->hist = d_hist[cur_hist];
+        a->hist_first = hist_first;
+        a->hist_n = hist_n;
+        a->cur_n = n;
+        a->n0 = out_next;
+        a->count = cnt;
+        a->split = s.nblocks > 0 ? s.nblocks * block - pend : LLONG_MAX;
+        a->base_n = (out_next / L) * L;
+        a->base_k = (out_next / L) * M;
+        a->out = d_out[cur_out] + 2 * pend;
+        a->out2 = d_out[cur_out ^ 1];
+        const int64_t first = std::min(in_new, std::max<int64_t>(0, k_of(ne) - T / 2 + 1));
+        a->carry_dst = d_hist[cur_hist ^ 1];
+        a->carry_first = first;
+        a->carry_n = in_new - first;
+        a->L = L;
+        a->M = M;
+        a->T = (int)T;
+        a->scale = scale;
+        a->E = d_E;
+        a->W = nco_step;
+        a->P = rs.P;
+        const int64_t Q = (int64_t)rs.P << ERTRS_F, step = kRsThreads * M;
+        a->step_k = step / L;
+        a->step_phi = step % L;
+        a->step_q = (int64_t)(((__int128)a->step_phi * Q) / L);
+        a->step_r = (int64_t)(((__int128)a->step_phi * Q) % L);
+        return s;
+    }
+
+    // Enqueue the step's kernel on st, if it has one, and count it in *launches.
+    int launch(const InputStep& s, cudaStream_t st, int64_t* launches) const {
+        if (mode == kPass || (resamples() && s.rs.count <= 0 && s.rs.carry_n <= 0)) return ERTGPU_OK;
+        if (mode == kConvert) {
+            const long long groups = s.nblocks * block / 8;
+            const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>((groups + kCvtThreads - 1) / kCvtThreads, grid));
+            switch (fmt) {
+                case ERTGPU_FORMAT_CS8: convert_kernel<ERTGPU_FORMAT_CS8><<<g, kCvtThreads, 0, st>>>(s.rs.cur, d_out[0], groups, scale); break;
+                case ERTGPU_FORMAT_CS16: convert_kernel<ERTGPU_FORMAT_CS16><<<g, kCvtThreads, 0, st>>>(s.rs.cur, d_out[0], groups, scale); break;
+                default: convert_kernel<ERTGPU_FORMAT_CF32><<<g, kCvtThreads, 0, st>>>(s.rs.cur, d_out[0], groups, scale); break;
+            }
+        } else {
+            const long long tiles = (s.rs.count + kRsTile - 1) / kRsTile;
+            const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid));
+            resample_kernel_of(fmt, mode == kResampleTuned)<<<g, kRsThreads, smem, st>>>(d_A, d_D, s.rs);
+        }
+        CUDA_TRY(err_, cudaGetLastError());
+        ++*launches;
+        return ERTGPU_OK;
+    }
+
+    // The step's kernel is enqueued: advance the stream position.
+    void commit(const InputStep& s) {
+        if (!resamples()) return;
+        const RsArgs& a = s.rs;
+        in_total += a.cur_n;
+        out_next += a.count;
+        hist_first = a.carry_first;
+        hist_n = a.carry_n;
+        cur_hist ^= 1;
+        pend += a.count - s.nblocks * block;
+        if (s.nblocks > 0) cur_out ^= 1;  // the outputs past the last whole block are already at the front of the other buffer
+    }
+
+    // The stage's kernel as ertgpu_last_kernels names it ("" in pass-through mode).
+    std::string label() const {
+        const char* f = fmt == ERTGPU_FORMAT_CS8 ? "cs8" : fmt == ERTGPU_FORMAT_CS16 ? "cs16" : fmt == ERTGPU_FORMAT_CF32 ? "cf32" : "cu8";
+        switch (mode) {
+            case kPass: return "";
+            case kConvert: return std::string("convert_kernel<") + f + ">";
+            case kResample: return fmt == ERTGPU_FORMAT_CU8 ? "resample_kernel" : std::string("resample_kernel<") + f + ">";
+            default: return std::string("resample_kernel<") + f + ",tuned>";
+        }
+    }
+
+private:
+    std::string& err_;  // the handle's last error
+
+    // The resampler for input at hz: ertrs_plan, or ertrs_plan_tuned and the NCO step on a tuned handle.  It runs when
+    // the rates differ or a tuned handle mixes; the tuned instance when it mixes or its plan has P != ERTRS_P.
+    int configure_rate(int64_t hz, int64_t rate_out) {
+        ertgpu_resampler_info info{};
+        uint32_t w = 0;
+        if (tuned) {
+            const int64_t off = center_hz - capture_hz;
+            if (ertrs_plan_tuned(hz, rate_out, off, &info) != 0)
+                return fail(err_, ERTGPU_EINVAL,
+                            "input rate %lld Hz, channel offset %lld Hz: the decoder rate %lld Hz must be within 1/10 ... 4 "
+                            "times the input rate, and |offset| + 0.4 * min(rates) at most half the input rate",
+                            (long long)hz, (long long)off, (long long)rate_out);
+            w = ertrs_nco_step(off, hz);
+        } else if (ertrs_plan(hz, rate_out, &info) != 0) {
+            return fail(err_, ERTGPU_EINVAL, "input rate %lld Hz: the decoder rate %lld Hz must be within 1/4 ... 4 times it",
+                        (long long)hz, (long long)rate_out);
+        }
+        const bool on = hz != rate_out || w != 0;
+        std::vector<int16_t> t;
+        if (on) {
+            t.resize((size_t)(info.P + 1) * info.T);
+            if (ertrs_build_table(&info, t.data()) != 0) return fail(err_, ERTGPU_EINVAL, "resampler table does not fit int16");
+        }
+        mode = !on ? (fmt == ERTGPU_FORMAT_CU8 ? kPass : kConvert) : w != 0 || info.P != ERTRS_P ? kResampleTuned : kResample;
+        nco_step = w;
+        rs = info;
+        table.swap(t);
+        return ERTGPU_OK;
+    }
+
+    // The resample_kernel instance of an input format, untuned or tuned.
+    static decltype(&resample_kernel<ERTGPU_FORMAT_CU8, false>) resample_kernel_of(int f, bool mix) {
+        switch (f) {
+            case ERTGPU_FORMAT_CS8: return mix ? resample_kernel<ERTGPU_FORMAT_CS8, true> : resample_kernel<ERTGPU_FORMAT_CS8, false>;
+            case ERTGPU_FORMAT_CS16: return mix ? resample_kernel<ERTGPU_FORMAT_CS16, true> : resample_kernel<ERTGPU_FORMAT_CS16, false>;
+            case ERTGPU_FORMAT_CF32: return mix ? resample_kernel<ERTGPU_FORMAT_CF32, true> : resample_kernel<ERTGPU_FORMAT_CF32, false>;
+            default: return mix ? resample_kernel<ERTGPU_FORMAT_CU8, true> : resample_kernel<ERTGPU_FORMAT_CU8, false>;
+        }
+    }
+
+    int64_t k_of(int64_t n) const { return (int64_t)((__int128)n * rs.M / rs.L); }
+
+    // Most input samples the next step may take so that it completes at most max_blocks decoder blocks.
+    int64_t max_input() const {
+        const int64_t cap_out = (max_blocks + 1) * block - 1 - pend;
+        return rs.T / 2 + k_of(out_next + cap_out) - in_total;
+    }
+};
+
+}  // namespace ert

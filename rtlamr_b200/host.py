@@ -40,16 +40,8 @@ def lib():
             raise FileNotFoundError(f"{LIB_PATH} missing: run __graft_entry__.build()")
         L = C.CDLL(LIB_PATH)
         L.erthost_new.restype = C.c_void_p
-        L.erthost_new.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_char_p, C.c_int]
-        L.erthost_new_rate.restype = C.c_void_p
-        L.erthost_new_rate.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_char_p,
-                                       C.c_int]
-        L.erthost_new_format.restype = C.c_void_p
-        L.erthost_new_format.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_int,
-                                         C.c_float, C.c_char_p, C.c_int]
-        L.erthost_new_tuned.restype = C.c_void_p
-        L.erthost_new_tuned.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_int,
-                                        C.c_float, C.c_longlong, C.c_longlong, C.c_char_p, C.c_int]
+        L.erthost_new.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_int, C.c_float,
+                                  C.c_longlong, C.c_longlong, C.c_char_p, C.c_int]
         L.erthost_wav_probe.argtypes = [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
                                         C.POINTER(C.c_longlong), C.c_char_p, C.c_int]
         L.erthost_free.argtypes = [C.c_void_p]
@@ -181,24 +173,15 @@ class Receiver:
     def __init__(self, msgtypes: str, chip_length: int = 72, device: int = 0, max_blocks: int = 0, max_cands: int = 0,
                  input_rate: int = 0, input_format: int = 0, input_scale: float = 0.0, capture_freq: int = 0,
                  center_freq: int = 0):
-        """input_rate > 0: the IQ given to decode() is sampled at that rate (erthost_new_rate); any rate other than
-        DataRate * ChipLength is resampled on the GPU and decode() then takes any whole number of IQ samples.
-        input_format / input_scale: the IQ's sample format (capi.FORMAT_*) and gain (erthost_new_format).
+        """The input arguments are protocol::Decoder::SetInput's.  input_rate > 0: the IQ given to decode() is sampled at
+        that rate; any rate other than DataRate * ChipLength is resampled on the GPU and decode() then takes any whole
+        number of IQ samples.  input_format / input_scale: the IQ's sample format (capi.FORMAT_*) and gain.
         capture_freq > 0: the IQ was recorded centred there; the channel at center_freq (0: the protocols' CenterFreq) is
-        decoded (erthost_new_tuned)."""
+        decoded."""
         self._L = lib()
         err = C.create_string_buffer(512)
-        if capture_freq or center_freq:
-            self._h = self._L.erthost_new_tuned(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate,
-                                                input_format, input_scale, capture_freq, center_freq, err, 512)
-        elif input_format or input_scale:
-            self._h = self._L.erthost_new_format(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate,
-                                                 input_format, input_scale, err, 512)
-        elif input_rate:
-            self._h = self._L.erthost_new_rate(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate,
-                                               err, 512)
-        else:
-            self._h = self._L.erthost_new(msgtypes.encode(), chip_length, device, max_blocks, max_cands, err, 512)
+        self._h = self._L.erthost_new(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate, input_format,
+                                      input_scale, capture_freq, center_freq, err, 512)
         if not self._h:
             raise RuntimeError(err.value.decode())
         v = (C.c_int32 * 12)()

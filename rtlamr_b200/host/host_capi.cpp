@@ -29,41 +29,12 @@ struct erthost {
     std::string err;
 };
 
-erthost* erthost_new_format(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
-                            long long input_rate, int format, float scale, char* errbuf, int errcap);
-
-// main.go:59-86: NewDecoder; for each -msgtype NewParser + RegisterProtocol; Allocate
+// main.go:59-86: NewDecoder; for each -msgtype NewParser + RegisterProtocol; Allocate.  The input arguments are
+// protocol::Input's (all 0: uint8 IQ at the decoder's own rate): IQ sampled at input_rate Hz, in sample format `format`
+// (ERTGPU_FORMAT_*) with gain `scale`, recorded centred at capture_freq Hz with the channel at center_freq.
 erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
+                     long long input_rate, int format, float scale, long long capture_freq, long long center_freq,
                      char* errbuf, int errcap) {
-    return erthost_new_format(msgtypes_csv, chip_length, device, max_blocks, max_cands, 0, ERTGPU_FORMAT_CU8, 0.0f, errbuf,
-                              errcap);
-}
-
-// The same for IQ sampled at input_rate Hz (0: the decoder's own DataRate * ChipLength); erthost_decode then takes
-// any whole number of IQ samples.
-erthost* erthost_new_rate(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
-                          long long input_rate, char* errbuf, int errcap) {
-    return erthost_new_format(msgtypes_csv, chip_length, device, max_blocks, max_cands, input_rate, ERTGPU_FORMAT_CU8, 0.0f,
-                              errbuf, errcap);
-}
-
-erthost* erthost_new_tuned(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
-                           long long input_rate, int format, float scale, long long capture_freq, long long center_freq,
-                           char* errbuf, int errcap);
-
-// The same for IQ in sample format `format` (ERTGPU_FORMAT_*) with gain `scale` (0: the format's default);
-// erthost_decode then counts the format's bytes per sample.
-erthost* erthost_new_format(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
-                            long long input_rate, int format, float scale, char* errbuf, int errcap) {
-    return erthost_new_tuned(msgtypes_csv, chip_length, device, max_blocks, max_cands, input_rate, format, scale, 0, 0,
-                             errbuf, errcap);
-}
-
-// The same for a capture recorded centred at capture_freq Hz (0: no translation), decoding the channel at center_freq
-// (0: the protocols' CenterFreq) (protocol::Decoder::SetInputTuning).
-erthost* erthost_new_tuned(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
-                           long long input_rate, int format, float scale, long long capture_freq, long long center_freq,
-                           char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;   // released only on success: a throwing NewParser / Allocate must not leak the handle
     try {
         protocol::RegisterStockParsers();
@@ -74,9 +45,7 @@ erthost* erthost_new_tuned(const char* msgtypes_csv, int chip_length, int device
             if (name.empty()) continue;
             h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
         }
-        if (capture_freq > 0 || center_freq != 0) h->d.SetInputTuning(capture_freq, center_freq);
-        if (input_rate > 0) h->d.SetInputRate(input_rate);
-        if (format != ERTGPU_FORMAT_CU8 || scale != 0.0f) h->d.SetInputFormat(format, scale);
+        h->d.SetInput({input_rate, format, scale, capture_freq, center_freq});
         h->d.Allocate(device, max_blocks, max_cands);
         return h.release();
     } catch (const std::exception& e) {

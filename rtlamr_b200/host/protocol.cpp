@@ -8,6 +8,8 @@
 #include <mutex>
 #include <set>
 
+#include "../../include/ertgpu_resample.h"
+
 namespace {
 
 std::string sprintf_str(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
@@ -579,7 +581,7 @@ void Decoder::RegisterProtocol(ParserPtr p) {
 
 void Decoder::Allocate(int device, int64_t maxBlocksPerCall, int64_t maxCandidates) {
     int rc = ertgpu_allocate(h_, device, maxBlocksPerCall, maxCandidates);
-    if (rc == ERTGPU_EINVAL && tuned_) throw std::invalid_argument(ertgpu_last_error(h_));  // the channel at the native rate
+    if (rc == ERTGPU_EINVAL && ertgpu_get_tuning(h_, nullptr) == ERTGPU_OK) throw std::invalid_argument(ertgpu_last_error(h_));  // the channel at the native rate
     if (rc != ERTGPU_OK) raise(h_, rc, "Allocate");
     // a tuned handle at the decoder's own rate gets its resampler here
     resampling_ = ertgpu_get_resampler(h_, &rs_, nullptr, 0, nullptr) == ERTGPU_OK;
@@ -601,47 +603,31 @@ void Decoder::Reset() {
     input_samples_ = 0;
 }
 
-void Decoder::SetInputRate(int64_t hz) {
-    if (allocated_) throw std::logic_error("SetInputRate after Allocate");
-    int rc = ertgpu_set_input_rate(h_, hz);
-    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
-    if (rc != ERTGPU_OK) raise(h_, rc, "SetInputRate");
-    resampling_ = ertgpu_get_resampler(h_, &rs_, nullptr, 0, nullptr) == ERTGPU_OK;
-}
-
-void Decoder::SetInputTuning(int64_t captureHz, int64_t centerHz) {
-    if (allocated_) throw std::logic_error("SetInputTuning after Allocate");
-    int rc = ertgpu_set_input_tuning(h_, captureHz, centerHz);
-    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
-    if (rc != ERTGPU_OK) raise(h_, rc, "SetInputTuning");
-    tuned_ = true;
-}
-
-void Decoder::SetInputFormat(int32_t format, float scale) {
-    if (allocated_) throw std::logic_error("SetInputFormat after Allocate");
-    int rc = ertgpu_set_input_format(h_, format, scale);
-    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
-    if (rc != ERTGPU_OK) raise(h_, rc, "SetInputFormat");
-    sample_bytes_ = format == ERTGPU_FORMAT_CS16 ? 4 : format == ERTGPU_FORMAT_CF32 ? 8 : 2;
+void Decoder::SetInput(const Input& in) {
+    if (allocated_) throw std::logic_error("SetInput after Allocate");
+    const auto check = [this](int rc) {
+        if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
+        if (rc != ERTGPU_OK) raise(h_, rc, "SetInput");
+    };
+    if (in.CaptureFreq > 0 || in.CenterFreq != 0) check(ertgpu_set_input_tuning(h_, in.CaptureFreq, in.CenterFreq));
+    if (in.SampleRate > 0) check(ertgpu_set_input_rate(h_, in.SampleRate));
+    if (in.Format != ERTGPU_FORMAT_CU8 || in.Scale != 0.0f) {
+        check(ertgpu_set_input_format(h_, in.Format, in.Scale));
+        sample_bytes_ = in.Format == ERTGPU_FORMAT_CS16 ? 4 : in.Format == ERTGPU_FORMAT_CF32 ? 8 : 2;
+    }
 }
 
 int64_t Decoder::BlocksDecoded() const {
     if (!allocated_ || Cfg.BlockSize <= 0) return 0;
-    if (!resampling_) return input_samples_ / Cfg.BlockSize;
-    // outputs whose filter window lies inside the input so far (include/ertgpu_resample.h)
-    const int64_t a = input_samples_ - rs_.T / 2;
-    if (a <= 0) return 0;
-    const int64_t outputs = (int64_t)(((__int128)a * rs_.L + rs_.M - 1) / rs_.M);
-    return outputs / Cfg.BlockSize;
+    return (resampling_ ? ertrs_out_end(&rs_, input_samples_) : input_samples_) / Cfg.BlockSize;
 }
 
 std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
     if (!allocated_) throw std::logic_error("Decode before Allocate");
-    const size_t s = (size_t)sample_bytes_;
-    if (resampling_ ? (len % s) != 0 : (len % ((size_t)Cfg.BlockSize * s)) != 0)
+    if (len % InputQuantum())
         throw std::length_error(resampling_ ? "input is not a whole number of IQ samples"
-                                            : s == 2 ? "input is not a whole number of BlockSize2-byte blocks"
-                                                     : "input is not a whole number of blocks");
+                                            : sample_bytes_ == 2 ? "input is not a whole number of BlockSize2-byte blocks"
+                                                                 : "input is not a whole number of blocks");
     size_t n = 0;
     if (cands_.size() < 1024) cands_.resize(1024);
     int rc = ertgpu_decode(h_, input, len, ERTGPU_DECODE_ONLY_VALID, cands_.data(), cands_.size(), &n);
@@ -650,7 +636,7 @@ std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
         rc = ertgpu_fetch(h_, cands_.data(), cands_.size(), &n);
     }
     if (rc != ERTGPU_OK) raise(h_, rc, "Decode");
-    input_samples_ += (int64_t)(len / s);
+    input_samples_ += (int64_t)(len / sample_bytes_);
 
     std::vector<MessagePtr> out;
     Dispatch(cands_.data(), n, out);
@@ -688,7 +674,7 @@ void Decoder::Dispatch(const ertgpu_candidate* cands, size_t n, std::vector<Mess
 std::string Decoder::Log() const {  // decode.go:73-90
     std::string s;
     ertgpu_tuning_info t;
-    if (tuned_ && ertgpu_get_tuning(h_, &t) == ERTGPU_OK)  // the channel decoded, and the capture's centre
+    if (ertgpu_get_tuning(h_, &t) == ERTGPU_OK)  // the channel decoded, and the capture's centre
         s += "CenterFreq: " + std::to_string(t.center_hz) + "\nCaptureFreq: " + std::to_string(t.capture_center_hz);
     else
         s += "CenterFreq: " + u(Cfg.CenterFreq);

@@ -125,6 +125,15 @@ using NewParserFunc = std::function<ParserPtr(int chipLength)>;  // parse.go:21
 void RegisterParser(const std::string& name, NewParserFunc fn);  // parse.go:28-39 (throws like Go panics)
 ParserPtr NewParser(const std::string& name, int chipLength);    // parse.go:42-51 (throws invalid_argument)
 
+// The IQ fed to Decode (not part of the reference, which decodes uint8 IQ at DataRate*ChipLength only).  Every field's
+// default leaves the input as the reference takes it.
+struct Input {
+    int64_t SampleRate = 0;             // Hz; another rate than DataRate*ChipLength is resampled (ertgpu_set_input_rate)
+    int32_t Format = ERTGPU_FORMAT_CU8; // converted on the GPU with gain Scale, 0: the format's default (ertgpu_set_input_format)
+    float Scale = 0.0f;
+    int64_t CaptureFreq = 0, CenterFreq = 0;  // the capture's centre and the channel, 0: Cfg.CenterFreq (ertgpu_set_input_tuning)
+};
+
 // decode.go:45-63.  Signal/Quantized are not materialised on the host: the parity taps of the C ABI
 // expose them (ertgpu_tap).
 class Decoder {
@@ -137,26 +146,17 @@ public:
     Decoder& operator=(const Decoder&) = delete;
 
     void RegisterProtocol(ParserPtr p);  // decode.go:100-128
-    // The IQ fed to Decode is sampled at hz (not part of the reference, which decodes at DataRate*ChipLength
-    // only): between RegisterProtocol and Allocate; hz != DataRate*ChipLength resamples on the GPU
-    // (ertgpu_set_input_rate).  Throws std::invalid_argument for a rate outside [1/4, 4] x the decoder's.
-    void SetInputRate(int64_t hz);
-    bool Resampling() const { return resampling_; }
-    // The IQ fed to Decode was recorded centred at captureHz; decode the channel at centerHz (0: Cfg.CenterFreq), mixed
-    // to 0 Hz inside the GPU resampler (ertgpu_set_input_tuning).  After the last RegisterProtocol, before
-    // SetInputRate and Allocate.  Throws std::invalid_argument for bad frequencies or call order; Allocate throws it
-    // too when the channel does not fit a capture at the decoder's own rate.
-    void SetInputTuning(int64_t captureHz, int64_t centerHz = 0);
-    // The IQ fed to Decode is in format ERTGPU_FORMAT_* (not part of the reference, which takes uint8 IQ only): before
-    // Allocate; each component is converted on the GPU to the decoder's byte with gain `scale` (0: the format's
-    // default; ertgpu_set_input_format).  Throws std::invalid_argument for an unknown format or a bad scale.
-    void SetInputFormat(int32_t format, float scale = 0.0f);
+    // The IQ fed to Decode, between the last RegisterProtocol and Allocate: sets the tuning when CaptureFreq > 0 or
+    // CenterFreq != 0, then the rate when SampleRate > 0, then the format when Format != cu8 or Scale != 0.  A bad value
+    // throws std::invalid_argument, and so does Allocate when the channel does not fit a capture at the decoder's rate.
+    void SetInput(const Input& in);
     int BytesPerSample() const { return sample_bytes_; }
+    // Decode takes multiples of this many bytes: whole IQ samples when resampling, whole blocks otherwise.
+    size_t InputQuantum() const { return (size_t)sample_bytes_ * (resampling_ ? 1 : (size_t)Cfg.BlockSize); }
     void Allocate(int device = 0, int64_t maxBlocksPerCall = 0, int64_t maxCandidates = 0);  // decode.go:131-160
-    // decode.go:163-197 for N = len/BlockSize2 consecutive blocks; throws std::length_error when len is
-    // not a multiple of BlockSize2 (the reference panics with a slice-bounds error, decode.go:222).  With an
-    // input rate, len is any whole number of IQ samples and the blocks are those of the resampled stream.  With an
-    // input format of s bytes per sample, len counts s bytes per sample (BlockSize * s per block).
+    // decode.go:163-197 for N = len/BlockSize2 consecutive blocks; throws std::length_error when len is not a multiple
+    // of InputQuantum() (BlockSize2 for uint8 IQ at the decoder's rate: the reference panics with a slice-bounds error,
+    // decode.go:222).  When resampling, the blocks are those of the resampled stream.
     std::vector<MessagePtr> Decode(const uint8_t* input, size_t len);
     // Whole blocks decoded since Allocate / Reset (resampled blocks with an input rate).
     int64_t BlocksDecoded() const;
@@ -176,7 +176,6 @@ private:
     std::vector<ertgpu_candidate> cands_;
     bool allocated_ = false;
     bool resampling_ = false;
-    bool tuned_ = false;
     ertgpu_resampler_info rs_{};
     int64_t input_samples_ = 0;  // since Allocate / Reset
     int sample_bytes_ = 2;       // bytes per input IQ sample

@@ -14,8 +14,8 @@ namespace receiver {
 
 Digest NewDigest(const protocol::Message& m) { return Digest(m.MsgType(), m.MeterType(), m.MeterID(), m.Checksum()); }
 
-Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, int64_t sampleRate,
-                   int32_t format, float scale, int64_t captureFreq, int64_t centerFreq) {
+Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall,
+                   const protocol::Input& input) {
     protocol::RegisterStockParsers();
     std::string list = msgtypes == "all" ? "scm,scm+,idm,r900" : msgtypes;  // main.go:67-73
     std::stringstream ss(list);
@@ -24,9 +24,7 @@ Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int6
         if (!name.empty()) d_.RegisterProtocol(protocol::NewParser(name, chipLength));  // main.go:77-82
     if (blocksPerCall <= 0) blocksPerCall = 4096;
     blocks_per_call_ = blocksPerCall;
-    if (captureFreq > 0) d_.SetInputTuning(captureFreq, centerFreq);
-    if (sampleRate > 0) d_.SetInputRate(sampleRate);
-    if (format != ERTGPU_FORMAT_CU8) d_.SetInputFormat(format, scale);
+    d_.SetInput(input);
     d_.Allocate(device, blocksPerCall, 0);  // main.go:86
     buf_bytes_ = (size_t)blocksPerCall * (size_t)d_.Cfg.BlockSize * (size_t)d_.BytesPerSample();
     for (int k = 0; k < 2; k++) {
@@ -174,15 +172,13 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
                     int64_t max_bytes) {
     Stats st;
     const size_t bs2 = (size_t)d_.Cfg.BlockSize2;
-    const size_t s = (size_t)d_.BytesPerSample(), bsf = (size_t)d_.Cfg.BlockSize * s;   // bytes per input sample, per block
-    if (s != 2 && sample_file_) throw std::logic_error("-samplefile with converted input");
+    const size_t s = (size_t)d_.BytesPerSample(), q = d_.InputQuantum();   // bytes per input sample, per Decode unit
+    if (q != bs2 && sample_file_) throw std::logic_error("-samplefile with converted or resampled input");
     uint64_t left = max_bytes < 0 ? UINT64_MAX : (uint64_t)max_bytes;
     // main.go:225-230: sampleBuf grows by one block per block until it holds more than BufferLength<<1 bytes
     sample_blocks_ = 2 * (int64_t)d_.Cfg.BufferLength / (int64_t)bs2 + 1;
     FilterChain* fc = fc_.empty() ? nullptr : &fc_;
     const auto t0 = std::chrono::steady_clock::now();
-    const bool rs = d_.Resampling();   // the decoder takes any whole number of IQ samples and keeps the rest itself
-    if (rs && sample_file_) throw std::logic_error("-samplefile with a resampling input rate");
     int k = 0;
     size_t carry = 0;  // bytes of a partial block (a partial IQ sample when resampling) kept for the next buffer
     bool eof = false;
@@ -199,11 +195,11 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
             left -= n;
         }
         eof = have < buf_bytes_;
-        const size_t whole = rs ? have / s * s : have / bsf * bsf;
+        const size_t whole = have / q * q;
         if (whole) {
             auto msgs = d_.Decode(buf_[k], whole);
             const int64_t call_first = stream_blocks_;
-            const int64_t nblocks = rs ? d_.BlocksDecoded() - stream_blocks_ : (int64_t)(whole / bsf);
+            const int64_t nblocks = d_.BlocksDecoded() - stream_blocks_;
             st.blocks += nblocks;
             st.bytes += (int64_t)whole;   // input bytes: s per input sample
             st.samples += (int64_t)(whole / s);

@@ -61,13 +61,9 @@ private:
 class Receiver {
 public:
     // msgtypes: comma list as for -msgtype ("all" = scm,scm+,idm,r900, main.go:67-73)
-    // sampleRate > 0: the capture's sample rate in Hz; a rate other than DataRate*ChipLength is resampled on the GPU
-    // (protocol::Decoder::SetInputRate) and blocks, dedup and filters then work on the resampled stream.
-    // format / scale: the input's sample format (ERTGPU_FORMAT_*) and gain (protocol::Decoder::SetInputFormat).
-    // captureFreq > 0: the capture was recorded centred there; the channel at centerFreq (0: the protocols'
-    // CenterFreq) is decoded (protocol::Decoder::SetInputTuning).
-    Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, int64_t sampleRate = 0,
-             int32_t format = ERTGPU_FORMAT_CU8, float scale = 0.0f, int64_t captureFreq = 0, int64_t centerFreq = 0);
+    // input: the capture's rate, format and tuning (protocol::Decoder::SetInput); when it is resampled, blocks, dedup
+    // and filters work on the resampled stream.
+    Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, const protocol::Input& input);
     ~Receiver();
 
     protocol::Decoder& decoder() { return d_; }
