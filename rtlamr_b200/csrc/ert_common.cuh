@@ -66,19 +66,4 @@ enum { kCntHits = 0, kCntOut = 1, kCntValid = 2, kCntTile = 3, kCntWords = 4, kC
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// Plane bit order: stream bit g lives in word g>>5 at bit position 31-(g&31)
-// (MSB first, like the reference's packed bytes, decode.go:259-265).
-__device__ __forceinline__ uint32_t plane_bit(const uint32_t* __restrict__ plane, long long pos) {
-    return (plane[pos >> 5] >> (31 - (int)(pos & 31))) & 1u;
-}
-
-// 32 consecutive plane bits starting at bit `pos`, first bit in the MSB.
-__device__ __forceinline__ uint32_t plane_window(const uint32_t* __restrict__ plane, long long pos) {
-    long long w = pos >> 5;
-    int sh = (int)(pos & 31);
-    uint32_t hi = plane[w];
-    if (sh == 0) return hi;
-    return __funnelshift_l(plane[w + 1], hi, sh);
-}
-
 }  // namespace ert

@@ -7,10 +7,11 @@
 //             output buffer when the handle has an input rate or format, input_stage.cuh)
 //   hist[2] : last PKL samples of the previous call (ping-pong) -- replaces the Signal tail
 //             (decode.go:165) and the r900 parser's private signal history (r900.go:169)
-//   plane[2]: packed quantizer output, 1 bit per sample, MSB first, laid out as
+//   plane[2]: packed quantizer output, 1 bit per sample, MSB first (bit g is bit 31-(g&31) of word g>>5, like
+//             the reference's packed bytes, decode.go:259-265), laid out as
 //             [hist_words of history | BS/32 words per block of the call] (ping-pong) --
 //             replaces Decoder.Quantized (1 byte per bit) and Decoder.packed
-//   hits    : (start, preamble) pairs found by search_kernel
+//   hits    : (start, preamble) pairs found by the Search kernel (search_slide_kernel or search_generic_kernel)
 //   out     : ertgpu_candidate records produced by extract_kernel
 #include <ctype.h>
 #include <sched.h>
@@ -263,19 +264,6 @@ int launch_slide(ertgpu_handle* h, const uint32_t* plane, const SlideParams& sl,
     return ERTGPU_OK;
 }
 
-// Search by the per-bit-load kernel; mode = search_mode().
-template <int NPRE>
-int launch_search(ertgpu_handle* h, const uint32_t* plane, const SearchParams& sp, int mode, bool pdl, cudaStream_t st) {
-    const auto kern = mode == 1 ? search_kernel<NPRE, 1> : mode == 2 ? search_kernel<NPRE, 2> : search_kernel<NPRE, 0>;
-    const long long tiles = (sp.nwords + kSearchTile - 1) / kSearchTile;
-    unsigned grid = (unsigned)std::min<long long>(tiles, (long long)h->sm_count * 4);
-    if (grid < 1) grid = 1;
-    CUDA_TRY(h, launch_dep(pdl, kern, dim3(grid), dim3(kSearchThreads), 0, st, plane, sp, h->d_hits, h->d_words,
-                           h->cand_cap, h->d_counters));
-    h->kernels += ";search_kernel<" + std::to_string(NPRE) + "," + std::to_string(mode) + ">";
-    return ERTGPU_OK;
-}
-
 // Enqueue the whole per-call pipeline for the s.nblocks blocks whose IQ bytes are at s.iq, behind the input stage's
 // kernel that writes them (its time counts as demod time).
 int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaStream_t st) {
@@ -328,9 +316,9 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
     h->launches++;
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[1], st));
 
-    // 2. preamble search over every start position of the call
+    // 2. preamble search over every start position of the call: the sliding-window kernel where the geometry fits
+    //    it, search_generic_kernel for every other geometry
     {
-        SearchParams sp;
         SlideParams sl;
         int rc = ERTGPU_OK;
         if (make_slide_params(c, p0, nwords, &sl)) {
@@ -359,14 +347,6 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
                     rc = launch_slide<4, 0xF953u, 0x16A3u, 0x5555u, 0x0000u>(h, plane, sl, pdl, st);
                 else
                     rc = launch_slide<4>(h, plane, sl, pdl, st);
-            }
-        } else if (make_search_params(c, p0, nwords, &sp)) {
-            const int mode = search_mode(c, p0);
-            switch (c.npre) {
-                case 1: rc = launch_search<1>(h, plane, sp, mode, pdl, st); break;
-                case 2: rc = launch_search<2>(h, plane, sp, mode, pdl, st); break;
-                case 3: rc = launch_search<3>(h, plane, sp, mode, pdl, st); break;
-                default: rc = launch_search<4>(h, plane, sp, mode, pdl, st); break;
             }
         } else {
             const int nthr = 256;
@@ -794,7 +774,13 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     CUDA_TRY(h, cudaMalloc(&h->d_crc, tables.size() * sizeof(uint16_t)));
     CUDA_TRY(h, cudaMemcpy(h->d_crc, tables.data(), tables.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
 
-    h->plane_words = (size_t)d.hist_words + (size_t)max_blocks_per_call * d.words_per_block + kSearchTile + kSearchMaxHalo + kSlideMaxLoad + 8;
+    // Slack behind the largest call's words, for the Search kernels' reads past the call's last word:
+    //  * search_slide_kernel's last tile starts at a word below nwords and loads load_words <= kSlideMaxLoad words;
+    //  * search_generic_kernel (and extract_words_kernel) read the word under plane bit p0 + 32*w + k*SL and the next
+    //    one, w < nwords; with p0 + PKL = 32*hist_words that stays inside the call's words while k < PK.  Only a
+    //    preamble longer than the packet, which the ABI allows, reads past them: 1 + (nbits - 1 - PK)*SL/32 words,
+    //    at most 1696 (32 bits, PK = 1, SL = 1808 at chip length 904, the largest demod_generic_kernel takes).
+    h->plane_words = (size_t)d.hist_words + (size_t)max_blocks_per_call * d.words_per_block + kSlideMaxLoad + 8;
     for (int k = 0; k < 2; k++) {
         CUDA_TRY(h, cudaMalloc(&h->d_plane[k], h->plane_words * sizeof(uint32_t)));
         CUDA_TRY(h, cudaMemset(h->d_plane[k], 0, h->plane_words * sizeof(uint32_t)));

@@ -22,32 +22,7 @@
 
 namespace ert {
 
-// ---- Search, per-bit-load form -------------------------------------------------------------
-//
-// (The kernel for geometries the sliding-window kernel further down does not cover -- SL % 16 != 0 such as
-// chip length 78, SL outside [64, 192], preambles shorter than 16 bits.)
-// A CTA stages a tile of the bit-plane (kSearchTile words of start positions + the halo the last
-// preamble bit reaches) in shared memory; a thread then tests 32 consecutive start positions at a
-// time.  For preamble bit k every start of the word looks at the SAME relative window: word offset
-// offw[k] and bit shift shk[k] are launch constants, so one test is 2 LDS + 1 funnel shift + 1 LOP3
-// per registered preamble (the window is shared by all preambles).  The first kSearchProbe bits are
-// tested unconditionally (no divergence: 1/256 of the starts survive on noise), the remaining bits
-// only for words that still have a live start.
-constexpr int kSearchThreads = 256;
-constexpr int kSearchTile = 2048;   // words of starts per CTA iteration
-constexpr int kSearchProbe = 12;    // preamble bits tested unconditionally
-constexpr int kSearchMaxPre = 4;
-constexpr int kSearchMaxHalo = 168; // words: (127 + 31*SL)/32 + 2 for SL <= 160
-
-struct SearchParams {
-    int32_t offb[ERTGPU_MAX_PREAMBLE];              // 4 * ((sh0 + k*SL) >> 5): byte offset of the window's first word
-    int32_t shk[ERTGPU_MAX_PREAMBLE];               // (sh0 + k*SL) & 31
-    uint32_t inv[kSearchMaxPre][ERTGPU_MAX_PREAMBLE];  // 0 where P[k]=1, ~0 where P[k]=0
-    int32_t nbits[kSearchMaxPre];
-    int32_t npre;
-    int32_t halo_words;
-    long long nwords;  // words of starts
-};
+constexpr int kSearchMaxPre = 4;  // preambles the sliding-window kernel takes in one pass
 
 __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
     uint32_t v;
@@ -82,77 +57,6 @@ __device__ __forceinline__ void emit_hit_word(uint32_t m, long long gw, int p, R
             hits[slot] = h;
         }
         slot++;
-    }
-}
-
-// The plane's first start lies in the first 4 words (p0 < 128), so tile t starts at plane word t*kSearchTile:
-// 16-byte aligned, fetched with one cp.async.bulk per tile into a 2-stage ring (the plane is
-// allocated with kSearchTile + kSearchMaxHalo words of slack so the last tile can over-read).
-// MODE 0: any geometry.  MODE 1: every window is word aligned (first start in bit 0 of a word and
-// SL % 32 == 0).  MODE 2: SL % 32 == 16: even preamble bits are word aligned, odd ones sit half a word in.
-// Every chip length the reference CLI accepts gives MODE 1 or 2 (SL = 2*CL, CL a multiple of 8).
-template <int NPRE, int MODE>
-__global__ void __launch_bounds__(kSearchThreads)
-search_kernel(const uint32_t* __restrict__ plane, SearchParams sp, RawHit* __restrict__ hits, HitWord* __restrict__ words,
-              unsigned long long hit_cap, unsigned long long* __restrict__ hit_count) {
-    __shared__ __align__(128) uint32_t buf[2][kSearchTile + kSearchMaxHalo];
-    __shared__ __align__(8) unsigned long long bars[2];
-    const long long ntiles = (sp.nwords + kSearchTile - 1) / kSearchTile;
-    const uint32_t bar0 = smem_u32(&bars[0]);
-    const uint32_t nload_bytes = (uint32_t)((kSearchTile + sp.halo_words + 3) & ~3) * 4u;
-    if (threadIdx.x == 0) {
-        mbar_init(bar0, 1);
-        mbar_init(bar0 + 8, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    pdl_launch_dependents();
-    pdl_wait();
-    __syncthreads();
-    auto issue = [&](long long tile, int st) {
-        mbar_arrive_expect_tx(bar0 + 8 * st, nload_bytes);
-        bulk_g2s(smem_u32(&buf[st][0]), plane + tile * kSearchTile, nload_bytes, bar0 + 8 * st);
-    };
-    if (threadIdx.x == 0 && blockIdx.x < ntiles) issue(blockIdx.x, 0);
-    uint32_t phases = 0;
-    int it = 0;
-    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, it++) {
-        const int st = it & 1;
-        const long long next = tile + gridDim.x;
-        if (threadIdx.x == 0 && next < ntiles) issue(next, st ^ 1);  // that stage was released by the barrier below
-        mbar_wait(bar0 + 8 * st, (phases >> st) & 1u);
-        phases ^= 1u << st;
-        const long long t0 = tile * kSearchTile;
-        const int nhere = (int)((sp.nwords - t0 < kSearchTile) ? (sp.nwords - t0) : kSearchTile);
-        const uint32_t base = smem_u32(&buf[st][0]);
-        for (int j = threadIdx.x; j < nhere; j += kSearchThreads) {
-            const uint32_t row = base + 4u * (uint32_t)j;
-            uint32_t m[NPRE];
-#pragma unroll
-            for (int p = 0; p < NPRE; p++) m[p] = 0xFFFFFFFFu;
-#pragma unroll
-            for (int k = 0; k < kSearchProbe; k++) {
-                const uint32_t a = row + (uint32_t)sp.offb[k];
-                uint32_t x;
-                if (MODE == 1 || (MODE == 2 && (k & 1) == 0)) x = lds_u32(a);
-                else if (MODE == 2) x = __byte_perm(lds_u32(a + 4), lds_u32(a), 0x5432);  // 16 bits in
-                else x = __funnelshift_l(lds_u32(a + 4), lds_u32(a), sp.shk[k]);
-#pragma unroll
-                for (int p = 0; p < NPRE; p++) m[p] &= x ^ sp.inv[p][k];
-            }
-#pragma unroll
-            for (int p = 0; p < NPRE; p++) {
-                uint32_t mm = m[p];
-                if (mm == 0) continue;
-                for (int k = kSearchProbe; k < sp.nbits[p] && mm; k++) {
-                    const uint32_t a = row + (uint32_t)sp.offb[k];
-                    const uint32_t x = __funnelshift_l(lds_u32(a + 4), lds_u32(a), sp.shk[k]);
-                    mm &= x ^ sp.inv[p][k];
-                }
-                if (mm == 0) continue;
-                emit_hit_word(mm, t0 + j, p, hits, words, hit_cap, hit_count);
-            }
-        }
-        __syncthreads();  // everyone is done with buf[st]: it may be refilled next iteration
     }
 }
 
@@ -340,40 +244,9 @@ inline bool make_slide_params(const DevCfg& c, long long p0, long long nwords, S
     return true;
 }
 
-// host: fill the launch constants.  p0 = plane bit of start 0 (must lie in word 0).
-inline bool make_search_params(const DevCfg& c, long long p0, long long nwords, SearchParams* sp) {
-    if (c.npre > kSearchMaxPre || p0 < 0 || p0 >= 128) return false;
-    memset(sp, 0, sizeof(*sp));
-    const int sh0 = (int)p0;
-    int maxbits = 0;
-    for (int p = 0; p < c.npre; p++) {
-        if (c.pre_nbits[p] < kSearchProbe) return false;
-        sp->nbits[p] = c.pre_nbits[p];
-        if (c.pre_nbits[p] > maxbits) maxbits = c.pre_nbits[p];
-        for (int k = 0; k < ERTGPU_MAX_PREAMBLE; k++)
-            sp->inv[p][k] = (k < c.pre_nbits[p]) ? (c.pre_bits[p][k] ? 0u : 0xFFFFFFFFu) : 0u;
-    }
-    for (int k = 0; k < ERTGPU_MAX_PREAMBLE; k++) {
-        const long long off = sh0 + (long long)k * c.SL;
-        sp->offb[k] = (int32_t)((off >> 5) * 4);
-        sp->shk[k] = (int32_t)(off & 31);
-    }
-    sp->npre = c.npre;
-    sp->halo_words = (int32_t)(((sh0 + (long long)(maxbits - 1) * c.SL) >> 5) + 2);  // sh0 < 128 covers word0
-    if (sp->halo_words > kSearchMaxHalo) return false;
-    sp->nwords = nwords;
-    return true;
-}
-
-// which specialisation of search_kernel fits the geometry
-inline int search_mode(const DevCfg& c, long long p0) {
-    if ((p0 & 31) != 0) return 0;
-    if (c.SL % 32 == 0) return 1;
-    if (c.SL % 32 == 16) return 2;
-    return 0;
-}
-
-// slow path kept for more than kSearchMaxPre preambles or very short preambles
+// ---- Search for every other geometry: SL % 16 != 0 (e.g. chip length 78), SL outside [64, 192], more than
+// kSearchMaxPre preambles, preambles shorter than 16 bits, halos beyond kSlideMaxLoad.  One thread per word of
+// starts, every preamble bit read from global memory: exact for any geometry.
 __device__ __forceinline__ uint32_t plane_window2(const uint32_t* __restrict__ plane, long long pos) {
     const long long w = pos >> 5;
     return __funnelshift_l(plane[w + 1], plane[w], (int)(pos & 31));

@@ -128,9 +128,6 @@ def search_label(preambles, SL, p0):
         stock = (npre == 1 and pats[0] in (0xF953, 0x16A3, 0x5555, 0x0000)) or pats == STOCK_PATTERNS.get(npre)
         return f"search_slide_kernel<{npre},{'true' if SL % 32 == 16 else 'false'}" + \
             ("," + ", ".join("0x%04Xu" % v for v in pats) if stock else "") + ">"
-    if npre <= 4 and p0 < 128 and min(nbits) >= 12 and ((p0 + (max(nbits) - 1) * SL) >> 5) + 2 <= 168:
-        mode = 0 if p0 % 32 else (1 if SL % 32 == 0 else 2 if SL % 32 == 16 else 0)
-        return f"search_kernel<{npre},{mode}>"
     return "search_generic_kernel"
 
 
@@ -315,8 +312,8 @@ def test_search_label_restatement():
     assert lab("scm,scm+,idm,r900", 72) == "search_slide_kernel<4,true,0xF953u, 0x16A3u, 0x5555u, 0x0000u>"
     assert lab("scm,scm+", 72) == "search_slide_kernel<2,true>"
     assert lab("scm", 64) == "search_slide_kernel<1,false,0xF953u>"
-    assert lab("scm", 78) == "search_kernel<1,0>" and lab("scm", 16) == "search_kernel<1,1>"
-    assert lab("scm", 24) == "search_kernel<1,2>" and lab("idm", 100) == "search_generic_kernel"
+    assert lab("scm", 78) == "search_generic_kernel" and lab("scm", 16) == "search_generic_kernel"
+    assert lab("scm", 24) == "search_generic_kernel" and lab("idm", 100) == "search_generic_kernel"
 
 
 # ---------------------------------------------------------------- 1. instance matrix
@@ -325,7 +322,9 @@ MATRIX = [("scm", 40), ("scm+", 56), ("idm", 88), ("r900", 40), ("scm,idm", 88),
           ("idm,scm,scm+", 40), ("scm,scm+,idm,r900", 56), ("r900,scm,scm+,idm", 72),
           ("scm", 48), ("scm+", 32), ("netidm", 64), ("r900bcd", 96), ("scm,r900", 80), ("scm,scm+,idm", 32),
           ("scm+,idm,r900", 48), ("scm,scm+,idm,r900", 80), ("idm,scm,scm+,r900", 96), ("scm,scm+", 64),
-          ("scm", 78), ("scm,scm+,idm,r900", 78), ("idm", 100)]
+          ("idm", 100)]
+# SL = 156, not a multiple of 16: the sliding-window Search does not take it and search_generic_kernel runs
+ODD_SL_MATRIX = [("scm", 78), ("scm,scm+,idm,r900", 78)]
 
 
 @gpu
@@ -367,6 +366,13 @@ def test_instance_matrix(built, mt, cl):
     for b, q in r900q.items():
         assert np.array_equal(h.tap(capi.TAP_R900_QUANTIZED, b), q), b
     h.close()
+
+
+@gpu
+@pytest.mark.parametrize("mt,cl", ODD_SL_MATRIX)
+def test_odd_symbol_length_matrix(built, mt, cl):
+    """The instance-matrix checks on a symbol length that is not a multiple of 16 (search_generic_kernel)."""
+    test_instance_matrix(built, mt, cl)
 
 
 def synth_stream_any(mt, cl, nsamples):
@@ -703,13 +709,13 @@ def test_launch_switches_have_the_expected_shape():
 
 
 @gpu
-def test_every_instance_was_seen(built):
-    """Runs last: every demod_fast instance at both plane alignments, every slide instance, and the other Search
-    kernels were launched by the tests above."""
+def test_every_kernel_instance_was_seen(built):
+    """Runs last: every demod_fast instance at both plane alignments, every slide instance, and search_generic_kernel
+    were launched by the tests above."""
     if not SEEN_DEMOD:
         pytest.skip("collects what the other tests of this file launched: run the whole file")
     cls, demod, slide = expected_instances()
     missing = sorted((d, ph) for d in demod for ph in (0, 4) if (d, ph) not in SEEN_DEMOD)
     assert not missing, missing
     assert not sorted(slide - SEEN_SEARCH), sorted(slide - SEEN_SEARCH)
-    assert any(s.startswith("search_kernel<") for s in SEEN_SEARCH) and "search_generic_kernel" in SEEN_SEARCH
+    assert "search_generic_kernel" in SEEN_SEARCH

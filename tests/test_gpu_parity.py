@@ -155,22 +155,23 @@ def _variant_is_bit_exact(sample_iq, kernel=None, ntiles=None):
 
 
 # Search instance each geometry reaches by default (the second entry of last_kernels()): the sliding-window kernel for
-# the stock geometries, with the stock preamble sets' patterns as compile-time constants; search_kernel<NPRE, MODE>
-# where it does not fit (SL % 16 != 0, SL outside [64, 192]); search_generic_kernel where the halo of search_kernel
-# is too large
+# the stock geometries, with the stock preamble sets' patterns as compile-time constants; search_generic_kernel for
+# every geometry it does not fit (SL % 16 != 0, SL outside [64, 192], more than 4 preambles, preambles under 16 bits)
 SEARCH_KERNEL = {("scm", 72): "search_slide_kernel<1,true,0xF953u>",    # SL 144: odd bits half a word in
                  ("scm,scm+,idm", 72): "search_slide_kernel<3,true,0xF953u, 0x16A3u, 0x5555u>",
                  ("scm,scm+,idm,r900", 72): "search_slide_kernel<4,true,0xF953u, 0x16A3u, 0x5555u, 0x0000u>",
                  ("scm,scm+", 72): "search_slide_kernel<2,true>",        # no stock set: patterns read at run time
                  ("r900", 72): "search_slide_kernel<1,true,0x0000u>",
                  ("scm", 64): "search_slide_kernel<1,false,0xF953u>",   # SL 128
-                 ("scm", 78): "search_kernel<1,0>",         # SL 156: SL % 16 != 0, SL % 32 == 28
-                 ("scm", 16): "search_kernel<1,1>",         # SL 32 < 64, first start word aligned
-                 ("scm", 24): "search_kernel<1,2>",         # SL 48 < 64, SL % 32 == 16
-                 ("idm", 100): "search_generic_kernel"}     # SL 200: a 32-bit preamble's halo of 195 words is too large
+                 ("scm", 78): "search_generic_kernel",      # SL 156: SL % 16 != 0, SL % 32 == 28
+                 ("scm", 16): "search_generic_kernel",      # SL 32 < 64, SL % 32 == 0
+                 ("scm", 24): "search_generic_kernel",      # SL 48 < 64, SL % 32 == 16
+                 ("idm", 100): "search_generic_kernel"}     # SL 200 > 192
+# symbol lengths below 64 or not a multiple of 16: each residue of SL mod 32 a chip length can give (0, 16, other)
+SHORT_OR_ODD_SL = [("scm", 78), ("scm", 16), ("scm", 24)]
 
 
-@pytest.mark.parametrize("mt,cl", list(SEARCH_KERNEL))
+@pytest.mark.parametrize("mt,cl", [g for g in SEARCH_KERNEL if g not in SHORT_OR_ODD_SL])
 def test_legacy_search_kernel_agrees(built, mt, cl):
     """Every Search kernel finds the oracle's candidates on a geometry that reaches it by default."""
     iq, _, _ = synth_stream(mt, cl, 1 << 21, spacing=1 << 18)
@@ -181,6 +182,12 @@ def test_legacy_search_kernel_agrees(built, mt, cl):
     assert h.last_kernels().split(";")[1] == SEARCH_KERNEL[(mt, cl)], h.last_kernels()
     compare_candidates(h, got, o, cands)
     h.close()
+
+
+@pytest.mark.parametrize("mt,cl", SHORT_OR_ODD_SL)
+def test_short_or_odd_symbol_search_agrees(built, mt, cl):
+    """search_generic_kernel finds the oracle's candidates where the sliding-window Search does not run."""
+    test_legacy_search_kernel_agrees(built, mt, cl)
 
 
 @pytest.mark.parametrize("mt,cl", [("r900", 72), ("scm,scm+,idm,r900", 72), ("r900bcd", 32)])
