@@ -117,6 +117,17 @@ typedef struct {
 #define ERTGPU_FORMAT_CS8 1  /* interleaved int8 I,Q (hackrf_transfer): 2 bytes per sample        */
 #define ERTGPU_FORMAT_CS16 2 /* interleaved little-endian int16 I,Q: 4 bytes per sample              */
 #define ERTGPU_FORMAT_CF32 3 /* interleaved little-endian float32 I,Q: 8 bytes per sample            */
+/* The other complex SigMF datatypes, named by their SigMF names; x is the component the scale multiplies. */
+#define ERTGPU_FORMAT_CS16BE 16 /* ci16_be: big-endian int16, 4 bytes per sample, x = v          */
+#define ERTGPU_FORMAT_CF32BE 17 /* cf32_be: big-endian float32, 8 bytes per sample, x = v        */
+#define ERTGPU_FORMAT_CU16 18   /* cu16_le: little-endian uint16, 4 bytes, x = v - 2^15          */
+#define ERTGPU_FORMAT_CU16BE 19 /* cu16_be: big-endian uint16, 4 bytes, x = v - 2^15             */
+#define ERTGPU_FORMAT_CS32 20   /* ci32_le: little-endian int32, 8 bytes, x = v                  */
+#define ERTGPU_FORMAT_CS32BE 21 /* ci32_be: big-endian int32, 8 bytes, x = v                     */
+#define ERTGPU_FORMAT_CU32 22   /* cu32_le: little-endian uint32, 8 bytes, x = v - 2^31          */
+#define ERTGPU_FORMAT_CU32BE 23 /* cu32_be: big-endian uint32, 8 bytes, x = v - 2^31             */
+#define ERTGPU_FORMAT_CF64 24   /* cf64_le: little-endian float64, 16 bytes, x = v               */
+#define ERTGPU_FORMAT_CF64BE 25 /* cf64_be: big-endian float64, 16 bytes, x = v                  */
 
 typedef struct ertgpu_handle ertgpu_handle;
 
@@ -206,8 +217,10 @@ int ertgpu_get_tuning(const ertgpu_handle *h, ertgpu_tuning_info *info);
  * ertgpu_allocate (its order relative to ertgpu_set_input_rate is free).  Each component x is
  * converted on the GPU to the byte the decoder reads,
  *     u = (isnan(p) ? 0 : clamp(rint(p), -128, 127)) + 128,   p = fl32(x * scale)
- * (one float32 multiply, both roundings to nearest even).  scale == 0 selects the format's
- * default: 1 for cs8, 2^-8 for cs16, 2^7 for cf32, which map full scale to full scale.
+ * (one float32 multiply, both roundings to nearest even).  The 32-bit integer and float64 formats,
+ * whose x is not exact in float32, take p = fl64(x * (double)scale) instead and clamp and round it
+ * in double.  scale == 0 selects the format's default: 1 for cs8, 2^-8 for the 16-bit formats,
+ * 2^7 for the float formats, 2^-24 for the 32-bit integer formats, which map full scale to full scale.
  * ERTGPU_FORMAT_CU8 (or never calling this) changes nothing; it takes no scale.  ERTGPU_EINVAL
  * for an unknown format, a negative or non-finite scale, cu8 with a scale other than 0, or a
  * call after ertgpu_allocate.  With s bytes per IQ sample, a handle that resamples takes any

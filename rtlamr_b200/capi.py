@@ -21,7 +21,12 @@ DECODE_ONLY_VALID = 1
 CAND_HAS_R900 = 1
 TAP_SIGNAL, TAP_CSUM, TAP_QUANTIZED, TAP_PACKED, TAP_R900_QUANTIZED, TAP_RESAMPLED = range(6)
 FORMAT_CU8, FORMAT_CS8, FORMAT_CS16, FORMAT_CF32 = range(4)
-FORMAT_BYTES = {FORMAT_CU8: 2, FORMAT_CS8: 2, FORMAT_CS16: 4, FORMAT_CF32: 8}  # bytes per IQ sample
+# the other complex SigMF datatypes: ci16_be, cf32_be, cu16_le, cu16_be, ci32_le, ci32_be, cu32_le, cu32_be, cf64_le, cf64_be
+(FORMAT_CS16BE, FORMAT_CF32BE, FORMAT_CU16, FORMAT_CU16BE, FORMAT_CS32, FORMAT_CS32BE, FORMAT_CU32, FORMAT_CU32BE, FORMAT_CF64,
+ FORMAT_CF64BE) = range(16, 26)
+FORMAT_BYTES = {FORMAT_CU8: 2, FORMAT_CS8: 2, FORMAT_CS16: 4, FORMAT_CF32: 8,   # bytes per IQ sample
+                FORMAT_CS16BE: 4, FORMAT_CF32BE: 8, FORMAT_CU16: 4, FORMAT_CU16BE: 4, FORMAT_CS32: 8, FORMAT_CS32BE: 8,
+                FORMAT_CU32: 8, FORMAT_CU32BE: 8, FORMAT_CF64: 16, FORMAT_CF64BE: 16}
 
 
 class Protocol(C.Structure):

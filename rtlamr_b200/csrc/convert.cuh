@@ -1,9 +1,15 @@
-// Input-format conversion: signed 8-bit, signed 16-bit and float32 IQ (ertgpu_set_input_format) -> the uint8 IQ the
-// decoder reads.  One formula for every format: u = clamp(rint(fl32(x * g)), -128, 127) + 128, NaN -> 128.
+// Input-format conversion: every complex SigMF datatype (ertgpu_set_input_format) -> the uint8 IQ the decoder reads.
+// One formula for every format: u = clamp(rint(p), -128, 127) + 128, NaN -> 128, with p = fl32(x * g) where the
+// component x is exact in float32 (8- and 16-bit integers, float32) and p = fl64(x * (double)g) where it is not (32-bit
+// integers, float64).  x is the stored value, less 2^15 or 2^31 for the unsigned formats; a big-endian value is byte
+// permuted first.
 #pragma once
 
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
+#include <utility>
 
 #include "../../include/ertgpu.h"
 
@@ -11,7 +17,54 @@ namespace ert {
 
 // bytes per IQ sample of a format
 __host__ __device__ constexpr int fmt_sample_bytes(int f) {
-    return f == ERTGPU_FORMAT_CS16 ? 4 : f == ERTGPU_FORMAT_CF32 ? 8 : 2;
+    return f == ERTGPU_FORMAT_CS16 || f == ERTGPU_FORMAT_CS16BE || f == ERTGPU_FORMAT_CU16 || f == ERTGPU_FORMAT_CU16BE ? 4
+           : f == ERTGPU_FORMAT_CF64 || f == ERTGPU_FORMAT_CF64BE                                                      ? 16
+           : f == ERTGPU_FORMAT_CF32 || f >= ERTGPU_FORMAT_CF32BE                                                      ? 8
+                                                                                                                      : 2;
+}
+
+// Every input format, and f(std::integral_constant<int, F>{}) for the one equal to `format`; false when none is.
+using AllFormats = std::integer_sequence<int, ERTGPU_FORMAT_CU8, ERTGPU_FORMAT_CS8, ERTGPU_FORMAT_CS16, ERTGPU_FORMAT_CF32,
+                                         ERTGPU_FORMAT_CS16BE, ERTGPU_FORMAT_CF32BE, ERTGPU_FORMAT_CU16, ERTGPU_FORMAT_CU16BE,
+                                         ERTGPU_FORMAT_CS32, ERTGPU_FORMAT_CS32BE, ERTGPU_FORMAT_CU32, ERTGPU_FORMAT_CU32BE,
+                                         ERTGPU_FORMAT_CF64, ERTGPU_FORMAT_CF64BE>;
+template <typename Fn, int... Fs>
+bool fmt_visit_in(int format, Fn&& f, std::integer_sequence<int, Fs...>) {
+    return ((format == Fs ? (f(std::integral_constant<int, Fs>{}), true) : false) || ...);
+}
+template <typename Fn>
+bool fmt_visit(int format, Fn&& f) { return fmt_visit_in(format, f, AllFormats{}); }
+
+// The name of a format: its SigMF datatype, or cu8 / cs8 / cs16 / cf32 for the first four.
+inline const char* fmt_name(int f) {
+    switch (f) {
+        case ERTGPU_FORMAT_CU8: return "cu8";
+        case ERTGPU_FORMAT_CS8: return "cs8";
+        case ERTGPU_FORMAT_CS16: return "cs16";
+        case ERTGPU_FORMAT_CF32: return "cf32";
+        case ERTGPU_FORMAT_CS16BE: return "ci16_be";
+        case ERTGPU_FORMAT_CF32BE: return "cf32_be";
+        case ERTGPU_FORMAT_CU16: return "cu16_le";
+        case ERTGPU_FORMAT_CU16BE: return "cu16_be";
+        case ERTGPU_FORMAT_CS32: return "ci32_le";
+        case ERTGPU_FORMAT_CS32BE: return "ci32_be";
+        case ERTGPU_FORMAT_CU32: return "cu32_le";
+        case ERTGPU_FORMAT_CU32BE: return "cu32_be";
+        case ERTGPU_FORMAT_CF64: return "cf64_le";
+        case ERTGPU_FORMAT_CF64BE: return "cf64_be";
+        default: return nullptr;
+    }
+}
+
+// The default gain of a format, which maps full scale to full scale (0 for cu8, which is not scaled).
+inline float fmt_default_scale(int f) {
+    switch (f) {
+        case ERTGPU_FORMAT_CU8: return 0.0f;
+        case ERTGPU_FORMAT_CS8: return 1.0f;
+        case ERTGPU_FORMAT_CS16: case ERTGPU_FORMAT_CS16BE: case ERTGPU_FORMAT_CU16: case ERTGPU_FORMAT_CU16BE: return 1.0f / 256.0f;
+        case ERTGPU_FORMAT_CS32: case ERTGPU_FORMAT_CS32BE: case ERTGPU_FORMAT_CU32: case ERTGPU_FORMAT_CU32BE: return 1.0f / 16777216.0f;
+        default: return 128.0f;   // float32 and float64
+    }
 }
 
 // One IQ component x (int8, int16 or float32, exact in float32) times g as the decoder's byte.  The product is one
@@ -24,8 +77,67 @@ __device__ __forceinline__ uint32_t fmt_byte(float x, float g) {
 }
 
 // The bytes of IQ sample j of format F (F != cu8) at src: I in the low byte, Q in the high byte.
+// The same in double for the components float32 cannot hold: p = fl64(x * (double)g), one multiply rounded to nearest
+// even, then clamped and rounded half to even in double.
+__device__ __forceinline__ uint32_t fmt_byte_d(double x, float g) {
+    const double p = __dmul_rn(x, (double)g);
+    if (p != p) return 128u;
+    return (uint32_t)(__double2int_rn(fmin(fmax(p, -128.0), 127.0)) + 128);
+}
+
+// The SigMF formats after the first four.  Component c (0: I of the first sample, 1: its Q, 2: I of the next, ...) as the
+// decoder's byte, from the little-endian 32-bit words x of the samples' bytes.
+template <int F>
+__device__ __forceinline__ uint32_t fmt_comp(const uint32_t* x, int c, float g) {
+    constexpr bool be = F == ERTGPU_FORMAT_CS16BE || F == ERTGPU_FORMAT_CF32BE || F == ERTGPU_FORMAT_CU16BE ||
+                        F == ERTGPU_FORMAT_CS32BE || F == ERTGPU_FORMAT_CU32BE || F == ERTGPU_FORMAT_CF64BE;
+    constexpr bool un = F == ERTGPU_FORMAT_CU16 || F == ERTGPU_FORMAT_CU16BE || F == ERTGPU_FORMAT_CU32 || F == ERTGPU_FORMAT_CU32BE;
+    constexpr int S = fmt_sample_bytes(F);
+    if constexpr (S == 4) {         // 16-bit: one word per sample, I in the low half
+        uint32_t w = x[c >> 1];
+        if constexpr (be) w = __byte_perm(w, 0, 0x2301);
+        if constexpr (un) w ^= 0x80008000u;   // v - 2^15 as int16
+        return fmt_byte((float)(int16_t)((c & 1) ? w >> 16 : w & 0xffffu), g);
+    } else if constexpr (S == 8) {  // 32-bit: one word per component
+        uint32_t w = x[c];
+        if constexpr (be) w = __byte_perm(w, 0, 0x0123);
+        if constexpr (F == ERTGPU_FORMAT_CF32BE) {
+            return fmt_byte(__uint_as_float(w), g);
+        } else {
+            if constexpr (un) w ^= 0x80000000u;   // v - 2^31 as int32
+            return fmt_byte_d((double)(int32_t)w, g);
+        }
+    } else {                        // float64: two words per component
+        uint32_t lo = x[2 * c], hi = x[2 * c + 1];
+        if constexpr (be) {
+            const uint32_t t = __byte_perm(lo, 0, 0x0123);
+            lo = __byte_perm(hi, 0, 0x0123);
+            hi = t;
+        }
+        return fmt_byte_d(__hiloint2double((int)hi, (int)lo), g);
+    }
+}
+
 template <int F>
 __device__ __forceinline__ uchar2 fmt_sample(const uint8_t* src, long long j, float g) {
+    if constexpr (F != ERTGPU_FORMAT_CS8 && F != ERTGPU_FORMAT_CS16 && F != ERTGPU_FORMAT_CF32) {
+        constexpr int S = fmt_sample_bytes(F);
+        uint32_t x[S / 4];
+        if constexpr (S == 4) {
+            x[0] = *reinterpret_cast<const uint32_t*>(src + 4 * j);
+        } else if constexpr (S == 8) {
+            const uint2 v = *reinterpret_cast<const uint2*>(src + 8 * j);
+            x[0] = v.x;
+            x[1] = v.y;
+        } else {
+            const uint4 v = *reinterpret_cast<const uint4*>(src + 16 * j);
+            x[0] = v.x;
+            x[1] = v.y;
+            x[2] = v.z;
+            x[3] = v.w;
+        }
+        return make_uchar2((unsigned char)fmt_comp<F>(x, 0, g), (unsigned char)fmt_comp<F>(x, 1, g));
+    }
     float i, q;
     if constexpr (F == ERTGPU_FORMAT_CS8) {
         const char2 v = *reinterpret_cast<const char2*>(src + 2 * j);
@@ -46,7 +158,8 @@ __device__ __forceinline__ uchar2 fmt_sample(const uint8_t* src, long long j, fl
 constexpr int kCvtThreads = 256;
 
 // Native-rate conversion of ngroups groups of 8 IQ samples (16 output bytes each) from `in` (16-byte aligned, format
-// F) to `out` (16-byte aligned).  Grid-stride loop; each group is one, two or four 16-byte loads and one 16-byte store.
+// F) to `out` (16-byte aligned).  Grid-stride loop; each group is one, two, four or eight 16-byte loads and one 16-byte
+// store.
 template <int F>
 __global__ void __launch_bounds__(kCvtThreads) convert_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out,
                                                               long long ngroups, float g) {
@@ -75,6 +188,19 @@ __global__ void __launch_bounds__(kCvtThreads) convert_kernel(const uint8_t* __r
                 w[k] = fmt_byte((float)(int16_t)(a & 0xffffu), g) | fmt_byte((float)(int16_t)(a >> 16), g) << 8 |
                        fmt_byte((float)(int16_t)(b & 0xffffu), g) << 16 | fmt_byte((float)(int16_t)(b >> 16), g) << 24;
             }
+        } else if constexpr (F != ERTGPU_FORMAT_CF32) {
+            uint32_t x[4 * kLoads];
+#pragma unroll
+            for (int k = 0; k < kLoads; k++) {
+                x[4 * k] = v[k].x;
+                x[4 * k + 1] = v[k].y;
+                x[4 * k + 2] = v[k].z;
+                x[4 * k + 3] = v[k].w;
+            }
+#pragma unroll
+            for (int k = 0; k < 4; k++)
+                w[k] = fmt_comp<F>(x, 4 * k, g) | fmt_comp<F>(x, 4 * k + 1, g) << 8 | fmt_comp<F>(x, 4 * k + 2, g) << 16 |
+                       fmt_comp<F>(x, 4 * k + 3, g) << 24;
         } else {
 #pragma unroll
             for (int k = 0; k < 4; k++)

@@ -110,11 +110,10 @@ struct InputStage {
     }
 
     int set_format(int32_t format, float g) {
-        if (format < ERTGPU_FORMAT_CU8 || format > ERTGPU_FORMAT_CF32) return fail(err_, ERTGPU_EINVAL, "unknown input format %d", format);
+        if (!fmt_name(format)) return fail(err_, ERTGPU_EINVAL, "unknown input format %d", format);
         if (!std::isfinite(g) || g < 0.0f) return fail(err_, ERTGPU_EINVAL, "input scale %g is not a finite value >= 0", (double)g);
         if (format == ERTGPU_FORMAT_CU8 && g != 0.0f) return fail(err_, ERTGPU_EINVAL, "cu8 input is not scaled (scale %g)", (double)g);
-        if (g == 0.0f)
-            g = format == ERTGPU_FORMAT_CS8 ? 1.0f : format == ERTGPU_FORMAT_CS16 ? 1.0f / 256.0f : format == ERTGPU_FORMAT_CF32 ? 128.0f : 0.0f;
+        if (g == 0.0f) g = fmt_default_scale(format);
         fmt = format;
         scale = g;
         sample_bytes = fmt_sample_bytes(format);
@@ -180,8 +179,8 @@ struct InputStage {
         {   // a property of the kernel, not of the handle: every handle on the device gets the largest any table needs
             static OncePerDevice once;
             if (once.first(device))
-                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF32; f++)
-                    for (int t = 0; t < 2; t++)
+                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF64BE; f++)
+                    for (int t = 0; t < 2 && fmt_name(f); t++)
                         CUDA_TRY(err_, cudaFuncSetAttribute(resample_kernel_of(f, t), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         }
         if (smem > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", smem);
@@ -302,11 +301,10 @@ struct InputStage {
         if (mode == kConvert) {
             const long long groups = s.nblocks * block / 8;
             const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>((groups + kCvtThreads - 1) / kCvtThreads, grid));
-            switch (fmt) {
-                case ERTGPU_FORMAT_CS8: convert_kernel<ERTGPU_FORMAT_CS8><<<g, kCvtThreads, 0, st>>>(s.rs.cur, d_out[0], groups, scale); break;
-                case ERTGPU_FORMAT_CS16: convert_kernel<ERTGPU_FORMAT_CS16><<<g, kCvtThreads, 0, st>>>(s.rs.cur, d_out[0], groups, scale); break;
-                default: convert_kernel<ERTGPU_FORMAT_CF32><<<g, kCvtThreads, 0, st>>>(s.rs.cur, d_out[0], groups, scale); break;
-            }
+            fmt_visit(fmt, [&](auto f) {
+                if constexpr (f() != ERTGPU_FORMAT_CU8)
+                    convert_kernel<f()><<<g, kCvtThreads, 0, st>>>(s.rs.cur, d_out[0], groups, scale);
+            });
         } else {
             const long long tiles = (s.rs.count + kRsTile - 1) / kRsTile;
             const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid));
@@ -332,7 +330,7 @@ struct InputStage {
 
     // The stage's kernel as ertgpu_last_kernels names it ("" in pass-through mode).
     std::string label() const {
-        const char* f = fmt == ERTGPU_FORMAT_CS8 ? "cs8" : fmt == ERTGPU_FORMAT_CS16 ? "cs16" : fmt == ERTGPU_FORMAT_CF32 ? "cf32" : "cu8";
+        const char* f = fmt_name(fmt);
         switch (mode) {
             case kPass: return "";
             case kConvert: return std::string("convert_kernel<") + f + ">";
@@ -376,12 +374,9 @@ private:
 
     // The resample_kernel instance of an input format, untuned or tuned.
     static decltype(&resample_kernel<ERTGPU_FORMAT_CU8, false>) resample_kernel_of(int f, bool mix) {
-        switch (f) {
-            case ERTGPU_FORMAT_CS8: return mix ? resample_kernel<ERTGPU_FORMAT_CS8, true> : resample_kernel<ERTGPU_FORMAT_CS8, false>;
-            case ERTGPU_FORMAT_CS16: return mix ? resample_kernel<ERTGPU_FORMAT_CS16, true> : resample_kernel<ERTGPU_FORMAT_CS16, false>;
-            case ERTGPU_FORMAT_CF32: return mix ? resample_kernel<ERTGPU_FORMAT_CF32, true> : resample_kernel<ERTGPU_FORMAT_CF32, false>;
-            default: return mix ? resample_kernel<ERTGPU_FORMAT_CU8, true> : resample_kernel<ERTGPU_FORMAT_CU8, false>;
-        }
+        decltype(&resample_kernel<ERTGPU_FORMAT_CU8, false>) k = nullptr;
+        fmt_visit(f, [&](auto F) { k = mix ? resample_kernel<F(), true> : resample_kernel<F(), false>; });
+        return k;
     }
 
     int64_t k_of(int64_t n) const { return (int64_t)((__int128)n * rs.M / rs.L); }

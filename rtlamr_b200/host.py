@@ -44,6 +44,10 @@ def lib():
                                   C.c_longlong, C.c_longlong, C.c_char_p, C.c_int]
         L.erthost_wav_probe.argtypes = [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
                                         C.POINTER(C.c_longlong), C.c_char_p, C.c_int]
+        ll, pll = C.c_longlong, C.POINTER(C.c_longlong)
+        L.erthost_sigmf_probe.argtypes = [C.c_char_p, C.POINTER(C.c_int), pll, pll, C.c_char_p, C.c_int, pll, pll, pll, pll,
+                                          C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.c_char_p, C.c_int]
+        L.erthost_sigmf_block_time.argtypes = [C.c_char_p, ll, ll, ll, pll, C.c_char_p, C.c_int]
         L.erthost_free.argtypes = [C.c_void_p]
         L.erthost_error.restype = C.c_char_p
         L.erthost_error.argtypes = [C.c_void_p]
@@ -162,6 +166,35 @@ def wav_probe(path) -> dict:
     if L.erthost_wav_probe(os.fsencode(path), C.byref(fmt), C.byref(rate), C.byref(off), C.byref(size), err, 512) != 0:
         raise ValueError(err.value.decode())
     return {"format": fmt.value, "rate": rate.value, "data_offset": off.value, "data_size": size.value}
+
+
+def sigmf_probe(path) -> dict:
+    """erthost_sigmf_probe: the metadata of a SigMF recording (NAME.sigmf-meta, NAME.sigmf-data or NAME): format =
+    capi.FORMAT_*, rate in Hz, frequency in Hz or None, the data file's path and its number of samples, and the capture
+    segments, each {"start", "header_bytes", "datetime_ns" (None: not dated)}.  Raises ValueError naming the field."""
+    L = lib()
+    fmt, rate, freq, samples, nseg = C.c_int(0), C.c_longlong(0), C.c_longlong(0), C.c_longlong(0), C.c_int(0)
+    data, err = C.create_string_buffer(4096), C.create_string_buffer(512)
+    cap = 1024
+    starts, hdr, dt = (C.c_longlong * cap)(), (C.c_longlong * cap)(), (C.c_longlong * cap)()
+    dated = (C.c_int * cap)()
+    if L.erthost_sigmf_probe(os.fsencode(path), C.byref(fmt), C.byref(rate), C.byref(freq), data, 4096, C.byref(samples),
+                             starts, hdr, dt, dated, cap, C.byref(nseg), err, 512) != 0:
+        raise ValueError(err.value.decode())
+    segs = [{"start": starts[k], "header_bytes": hdr[k], "datetime_ns": dt[k] if dated[k] else None}
+            for k in range(min(nseg.value, cap))]
+    return {"format": fmt.value, "rate": rate.value, "frequency": freq.value or None, "data_path": os.fsdecode(data.value),
+            "samples": samples.value, "segments": segs}
+
+
+def sigmf_block_time(path, block: int, block_size: int, rate_out: int) -> int:
+    """erthost_sigmf_block_time: the time in ns since the Unix epoch at which a live receiver would have finished decoder
+    block `block` of the recording (block_size samples at rate_out Hz).  Raises ValueError when no segment is dated."""
+    L = lib()
+    ns, err = C.c_longlong(0), C.create_string_buffer(512)
+    if L.erthost_sigmf_block_time(os.fsencode(path), block, block_size, rate_out, C.byref(ns), err, 512) != 0:
+        raise ValueError(err.value.decode())
+    return ns.value
 
 
 class Receiver:

@@ -1,11 +1,11 @@
-// ertgpu_decode_file -- decode an IQ capture (raw uint8 IQ as rtl_sdr and rtlamr -samplefile write it, raw int8,
-// int16 or float32 IQ, or a baseband WAV recording) or stdin through the C++ mirror of rtlamr's receive loop
+// ertgpu_decode_file -- decode an IQ capture (raw uint8 IQ as rtl_sdr and rtlamr -samplefile write it, raw IQ of any
+// complex SigMF datatype, a baseband WAV recording or a SigMF recording) or stdin through the C++ mirror of rtlamr's receive loop
 // (receiver.hpp) on the GPU and print one line per message in rtlamr's plain format without the time fields
 // (protocol/parse.go:119-121 StringNoOffset).
 //   ertgpu_decode_file [-msgtype=scm,idm|all] [-symbollength=72] [-blockdedup=true] [-blocks=4096] [-device=0]
 //                      [-filterid=1,2] [-filtertype=4,5] [-unique=true] [-format=plain|csv|json|xml]
 //                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ]
-//                      [-sampleformat=cu8|cs8|cs16|cf32|wav] [-samplescale=G] [-capturefreq=HZ [-centerfreq=HZ]]
+//                      [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|cf64_be|wav|sigmf] [-samplescale=G] [-capturefreq=HZ [-centerfreq=HZ]]
 //                      FILE|- [FILE ...]
 // -capturefreq names the frequency the capture was recorded centred at; -centerfreq (rtlamr's flag) the channel to
 // receive, by default the protocols' CenterFreq (912.6 MHz, or 912.38 MHz for r900 alone).  The channel is mixed to
@@ -17,10 +17,17 @@
 // exactly on the GPU first, and Block / Idx then count resampled samples.
 // -sampleformat names the capture's samples: cu8 (the default: uint8, rtl_sdr), cs8 (int8, hackrf_transfer), cs16
 // (little-endian int16: airspy_rx, rx_sdr, SoapySDR), cf32 (little-endian float32: GNU Radio, gqrx) or wav (SDR#,
-// SDR++, SDRuno, HDSDR: each file's header gives the format and the rate; wav.hpp).  Other formats are converted to
-// uint8 on the GPU, u = clamp(rint(x * G), -128, 127) + 128; -samplescale=G is that gain (default 1 for cs8, 2^-8 for
-// cs16, 2^7 for cf32: full scale to full scale; a 12-bit Airspy wants 0.0625).  A WAV file is never detected by its
-// content or name.  -samplefile takes only uint8 input at 32768 * -symbollength (an 8-bit WAV at that rate is uint8).
+// SDR++, SDRuno, HDSDR: each file's header gives the format and the rate; wav.hpp).  Every complex SigMF datatype name
+// (ci8, ci16_le, ci16_be, cu16_le, cu16_be, ci32_le, ci32_be, cu32_le, cu32_be, cf32_le, cf32_be, cf64_le, cf64_be; cu8)
+// names raw samples of that type too.  -sampleformat=sigmf reads SigMF recordings (sigmf.hpp): FILE is NAME.sigmf-meta,
+// NAME.sigmf-data or NAME, and the metadata gives the format, the rate and the capture frequency (-centerfreq then picks
+// the channel as with -capturefreq); -samplerate or -capturefreq that disagree with it are usage errors.  When a capture
+// segment carries a core:datetime, the csv, json and xml Time is the moment a live receiver would have finished the
+// message's block (sigmf::BlockTime) instead of the wall clock.  Other formats are converted to uint8 on the GPU,
+// u = clamp(rint(x * G), -128, 127) + 128; -samplescale=G is that gain (default 1 for cs8, 2^-8 for the 16-bit formats,
+// 2^-24 for the 32-bit integers, 2^7 for the floats: full scale to full scale; a 12-bit Airspy wants 0.0625).  A WAV or
+// SigMF file is never detected by its content or name.  -samplefile takes only untuned uint8 input at
+// 32768 * -symbollength (an 8-bit WAV at that rate is uint8).
 // -filterid / -filtertype / -unique, -format, -samplefile, -single and -duration are rtlamr's flags of the same names
 // (flags.go:37-58,69-70,140-170; the filter chain runs before the cross-block dedup, main.go:236-260).  With -format=csv a
 // line is LogMessage.Record() (parse.go:123-129: time, offset, length, then the message's own record) through Go's
@@ -43,6 +50,7 @@
 #include <vector>
 
 #include "receiver.hpp"
+#include "sigmf.hpp"
 #include "wav.hpp"
 
 int main(int argc, char** argv) {
@@ -85,7 +93,8 @@ int main(int argc, char** argv) {
     if (files.empty()) {
         fprintf(stderr, "usage: %s [-msgtype=scm,scm+,idm,netidm,r900,r900bcd|all] [-symbollength=N] [-blockdedup=true|false] "
                         "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
-                        "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|wav] [-samplescale=G] "
+                        "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|wav|sigmf] "
+                        "[-samplescale=G] "
                         "[-capturefreq=HZ [-centerfreq=HZ]] [-quiet] FILE|- [FILE ...]\n", argv[0]);
         return 2;
     }
@@ -102,11 +111,6 @@ int main(int argc, char** argv) {
             return 2;
         }
     }
-    if (!centerfreq.empty() && capturefreq.empty()) {
-        fprintf(stderr, "-centerfreq needs -capturefreq: the frequency at the centre of the capture\n");
-        return 2;
-    }
-    const bool tuned = capture_hz > 0;
     const bool csv = format == "csv", json = format == "json", xml = format == "xml";
     int64_t limit_ns = 0;
     try {
@@ -115,13 +119,14 @@ int main(int argc, char** argv) {
         fprintf(stderr, "invalid value \"%s\" for flag -duration: %s\n", duration.c_str(), e.what());
         return 2;
     }
-    const bool wav_in = sampleformat == "wav";
+    const bool wav_in = sampleformat == "wav", sigmf_in = sampleformat == "sigmf";
     int32_t fmt = ERTGPU_FORMAT_CU8;
     if (sampleformat == "cs8") fmt = ERTGPU_FORMAT_CS8;
     else if (sampleformat == "cs16") fmt = ERTGPU_FORMAT_CS16;
     else if (sampleformat == "cf32") fmt = ERTGPU_FORMAT_CF32;
-    else if (sampleformat != "cu8" && !wav_in) {
-        fprintf(stderr, "invalid value \"%s\" for flag -sampleformat: cu8, cs8, cs16, cf32 or wav\n", sampleformat.c_str());
+    else if (!wav_in && !sigmf_in && (fmt = sigmf::FormatOf(sampleformat)) < 0) {
+        fprintf(stderr, "invalid value \"%s\" for flag -sampleformat: cu8, cs8, cs16, cf32, a complex SigMF datatype "
+                        "(ci16_be, cf64_le, ...), wav or sigmf\n", sampleformat.c_str());
         return 2;
     }
     float scale = 0.0f;
@@ -164,6 +169,44 @@ int main(int argc, char** argv) {
         samplerate = wav_hdr[0].rate;
         fmt = wav_hdr[0].format;
     }
+    // sigmf: every recording's metadata, before anything else
+    std::vector<sigmf::Recording> rec(files.size());
+    if (sigmf_in) {
+        for (size_t fi = 0; fi < files.size(); fi++) {
+            if (files[fi] == "-") {
+                fprintf(stderr, "-sampleformat=sigmf reads NAME.sigmf-meta beside NAME.sigmf-data, not stdin\n");
+                return 2;
+            }
+            try {
+                rec[fi] = sigmf::Read(files[fi]);
+            } catch (const std::exception& e) {
+                fprintf(stderr, "%s: %s\n", files[fi].c_str(), e.what());
+                return 1;
+            }
+            if (rec[fi].rate != rec[0].rate || rec[fi].format != rec[0].format || rec[fi].frequency != rec[0].frequency) {
+                fprintf(stderr, "%s: %s at %lld Hz, %lld Hz, but %s: %s at %lld Hz, %lld Hz: the files of a batch share one decoder\n",
+                        files[0].c_str(), sigmf::FormatName(rec[0].format), (long long)rec[0].rate, (long long)rec[0].frequency,
+                        files[fi].c_str(), sigmf::FormatName(rec[fi].format), (long long)rec[fi].rate, (long long)rec[fi].frequency);
+                return 2;
+            }
+        }
+        if (samplerate != 0 && samplerate != rec[0].rate) {
+            fprintf(stderr, "-samplerate=%lld disagrees with the SigMF core:sample_rate %lld Hz\n", samplerate, (long long)rec[0].rate);
+            return 2;
+        }
+        if (capture_hz != 0 && rec[0].frequency != 0 && capture_hz != rec[0].frequency) {
+            fprintf(stderr, "-capturefreq=%lld disagrees with the SigMF core:frequency %lld Hz\n", capture_hz, (long long)rec[0].frequency);
+            return 2;
+        }
+        samplerate = rec[0].rate;
+        fmt = rec[0].format;
+        if (rec[0].frequency) capture_hz = rec[0].frequency;
+    }
+    if (!centerfreq.empty() && capture_hz == 0) {
+        fprintf(stderr, "-centerfreq needs -capturefreq: the frequency at the centre of the capture\n");
+        return 2;
+    }
+    const bool tuned = capture_hz > 0;
     if (have_scale && fmt == ERTGPU_FORMAT_CU8) {
         fprintf(stderr, "-samplescale does not apply to uint8 (cu8) input\n");
         return 2;
@@ -176,7 +219,7 @@ int main(int argc, char** argv) {
     }
     if ((resampling || fmt != ERTGPU_FORMAT_CU8) && !samplefile.empty() && samplefile != "/dev/null") {
         fprintf(stderr, "-samplefile needs uint8 (cu8) input at 32768 * -symbollength = %lld Hz; this input is %s at %lld Hz\n",
-                32768LL * chip, fmt == ERTGPU_FORMAT_CU8 ? "cu8" : fmt == ERTGPU_FORMAT_CS8 ? "cs8" : fmt == ERTGPU_FORMAT_CS16 ? "cs16" : "cf32",
+                32768LL * chip, sigmf::FormatName(fmt),
                 samplerate ? samplerate : 32768LL * chip);
         return 2;
     }
@@ -209,7 +252,7 @@ int main(int argc, char** argv) {
         if (unique) rcvr.filters().Add(std::make_shared<receiver::UniqueFilter>());
         for (size_t fi = 0; fi < files.size(); fi++) {
             const std::string& file = files[fi];
-            FILE* in = file == "-" ? stdin : fopen(file.c_str(), "rb");
+            FILE* in = sigmf_in ? sigmf::OpenSamples(rec[fi]) : file == "-" ? stdin : fopen(file.c_str(), "rb");
             if (!in) {
                 perror(file.c_str());
                 return 1;
@@ -220,10 +263,17 @@ int main(int argc, char** argv) {
                 if (quiet) return;
                 if (csv || json || xml) {
                     receiver::LogMessage lm;
-                    timespec ts{};
-                    clock_gettime(CLOCK_REALTIME, &ts);
-                    lm.unix_seconds = (int64_t)ts.tv_sec;
-                    lm.nanos = (int32_t)ts.tv_nsec;
+                    if (sigmf_in && sigmf::Dated(rec[fi])) {
+                        const protocol::PacketConfig& c = rcvr.decoder().Cfg;
+                        const int64_t ns = sigmf::BlockTime(rec[fi], m.Block, c.BlockSize, c.SampleRate);
+                        lm.unix_seconds = ns / 1000000000 - (ns % 1000000000 < 0);
+                        lm.nanos = (int32_t)(ns - lm.unix_seconds * 1000000000);
+                    } else {
+                        timespec ts{};
+                        clock_gettime(CLOCK_REALTIME, &ts);
+                        lm.unix_seconds = (int64_t)ts.tv_sec;
+                        lm.nanos = (int32_t)ts.tv_nsec;
+                    }
                     lm.Offset = offset;
                     lm.Length = length;
                     lm.Message = &m;

@@ -8,6 +8,7 @@
 
 #include "protocol.hpp"
 #include "receiver.hpp"
+#include "sigmf.hpp"
 #include "wav.hpp"
 
 extern "C" {
@@ -270,6 +271,47 @@ int erthost_wav_probe(const char* path, int* format, long long* rate, long long*
         return 0;
     } catch (const std::exception& e) {
         fclose(f);
+        if (errbuf && errcap > 0) snprintf(errbuf, (size_t)errcap, "%s", e.what());
+        return -1;
+    }
+}
+
+// The metadata of the SigMF recording at `path` (NAME.sigmf-meta, NAME.sigmf-data or NAME; sigmf.hpp): *format =
+// ERTGPU_FORMAT_*, *rate and *frequency in Hz (0: none given), the data file's path and *samples, and per capture segment
+// its first sample, header bytes and datetime in ns (dated[k] = 0: none), the first seg_cap of *nseg.  Returns 0, or -1
+// with the message in errbuf.
+int erthost_sigmf_probe(const char* path, int* format, long long* rate, long long* frequency, char* data_path, int data_cap,
+                        long long* samples, long long* starts, long long* header_bytes, long long* datetime_ns, int* dated,
+                        int seg_cap, int* nseg, char* errbuf, int errcap) {
+    try {
+        const sigmf::Recording r = sigmf::Read(path);
+        *format = r.format;
+        *rate = r.rate;
+        *frequency = r.frequency;
+        snprintf(data_path, (size_t)data_cap, "%s", r.data_path.c_str());
+        *samples = r.samples;
+        *nseg = (int)r.segments.size();
+        for (int k = 0; k < *nseg && k < seg_cap; k++) {
+            starts[k] = r.segments[k].sample_start;
+            header_bytes[k] = r.segments[k].header_bytes;
+            datetime_ns[k] = r.segments[k].datetime_ns;
+            dated[k] = r.segments[k].dated;
+        }
+        return 0;
+    } catch (const std::exception& e) {
+        if (errbuf && errcap > 0) snprintf(errbuf, (size_t)errcap, "%s", e.what());
+        return -1;
+    }
+}
+
+// sigmf::BlockTime of decoder block `block` (block_size samples at rate_out Hz) of the recording at `path`, in *ns.
+// Returns 0, or -1 with the message in errbuf (also when no segment is dated).
+int erthost_sigmf_block_time(const char* path, long long block, long long block_size, long long rate_out, long long* ns,
+                             char* errbuf, int errcap) {
+    try {
+        *ns = sigmf::BlockTime(sigmf::Read(path), block, block_size, rate_out);
+        return 0;
+    } catch (const std::exception& e) {
         if (errbuf && errcap > 0) snprintf(errbuf, (size_t)errcap, "%s", e.what());
         return -1;
     }

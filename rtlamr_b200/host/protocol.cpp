@@ -613,7 +613,7 @@ void Decoder::SetInput(const Input& in) {
     if (in.SampleRate > 0) check(ertgpu_set_input_rate(h_, in.SampleRate));
     if (in.Format != ERTGPU_FORMAT_CU8 || in.Scale != 0.0f) {
         check(ertgpu_set_input_format(h_, in.Format, in.Scale));
-        sample_bytes_ = in.Format == ERTGPU_FORMAT_CS16 ? 4 : in.Format == ERTGPU_FORMAT_CF32 ? 8 : 2;
+        sample_bytes_ = FormatBytes(in.Format);
     }
 }
 

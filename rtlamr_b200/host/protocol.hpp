@@ -127,6 +127,16 @@ ParserPtr NewParser(const std::string& name, int chipLength);    // parse.go:42-
 
 // The IQ fed to Decode (not part of the reference, which decodes uint8 IQ at DataRate*ChipLength only).  Every field's
 // default leaves the input as the reference takes it.
+// Bytes per IQ sample of an ERTGPU_FORMAT_*.
+inline int FormatBytes(int32_t f) {
+    switch (f) {
+        case ERTGPU_FORMAT_CU8: case ERTGPU_FORMAT_CS8: return 2;
+        case ERTGPU_FORMAT_CS16: case ERTGPU_FORMAT_CS16BE: case ERTGPU_FORMAT_CU16: case ERTGPU_FORMAT_CU16BE: return 4;
+        case ERTGPU_FORMAT_CF64: case ERTGPU_FORMAT_CF64BE: return 16;
+        default: return 8;
+    }
+}
+
 struct Input {
     int64_t SampleRate = 0;             // Hz; another rate than DataRate*ChipLength is resampled (ertgpu_set_input_rate)
     int32_t Format = ERTGPU_FORMAT_CU8; // converted on the GPU with gain Scale, 0: the format's default (ertgpu_set_input_format)

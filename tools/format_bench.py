@@ -1,13 +1,13 @@
 """Cost of the input-format conversion: scm at chip length 72 on about 1 GiB of decoder-rate uint8 IQ (512 Mi samples),
-fed as cs16 and cf32 at the decoder's rate (convert_kernel) and at 2.4 MS/s (resample_kernel<F>), each arm alternated
-with the same samples as uint8 (cu8).
+fed in each format of --formats (cs16 and cf32 by default, or any complex SigMF datatype name) at the decoder's rate
+(convert_kernel) and at 2.4 MS/s (resample_kernel<F>), each arm alternated with the same samples as uint8 (cu8).
 
 Prints one JSON line with the card's name and power limit (read in the same run) and, per arm:
   - the conversion kernel's time (torch.profiler) and, natively, its read + write bytes/s as a fraction of the H100 SXM
     data sheet's 3.35 TB/s;
   - the device-resident step (CUDA events around ertgpu_decode_device_async);
-  - end to end from pinned host memory (ertgpu_decode).
-Usage: python tools/format_bench.py [--reps 5] [--formats cs16,cf32]"""
+  - end to end from pinned host memory (ertgpu_decode), unless --no-e2e.
+Usage: python tools/format_bench.py [--reps 5] [--formats cs16,cf32,ci16_be,...,cf64_be] [--samples N] [--no-e2e]"""
 import argparse
 import json
 import os
@@ -24,7 +24,12 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from resample_bench import power_limit_w  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
-FORMATS = {"cs16": capi.FORMAT_CS16, "cf32": capi.FORMAT_CF32}
+FORMATS = {"cs16": capi.FORMAT_CS16, "cf32": capi.FORMAT_CF32, "ci16_be": capi.FORMAT_CS16BE, "cf32_be": capi.FORMAT_CF32BE,
+           "cu16_le": capi.FORMAT_CU16, "cu16_be": capi.FORMAT_CU16BE, "ci32_le": capi.FORMAT_CS32,
+           "ci32_be": capi.FORMAT_CS32BE, "cu32_le": capi.FORMAT_CU32, "cu32_be": capi.FORMAT_CU32BE,
+           "cf64_le": capi.FORMAT_CF64, "cf64_be": capi.FORMAT_CF64BE}
+BIG_ENDIAN = {capi.FORMAT_CS16BE, capi.FORMAT_CF32BE, capi.FORMAT_CU16BE, capi.FORMAT_CS32BE, capi.FORMAT_CU32BE,
+              capi.FORMAT_CF64BE}
 
 
 def encode_on_device(u8: torch.Tensor, fmt: int) -> torch.Tensor:
@@ -32,7 +37,17 @@ def encode_on_device(u8: torch.Tensor, fmt: int) -> torch.Tensor:
     v = u8.to(torch.int16) - 128
     if fmt == capi.FORMAT_CS16:
         return (v * 256).view(torch.uint8)
-    return (v.to(torch.float32) / 128).view(torch.uint8)
+    if fmt == capi.FORMAT_CF32:
+        return (v.to(torch.float32) / 128).view(torch.uint8)
+    k = capi.FORMAT_BYTES[fmt] // 2   # bytes per component
+    if fmt in (capi.FORMAT_CF32BE, capi.FORMAT_CF64, capi.FORMAT_CF64BE):
+        b = (v.to(torch.float32 if k == 4 else torch.float64) / 128).view(torch.uint8).view(-1, k)
+    else:
+        x = v.to(torch.int64) * (1 << (8 * k - 8))
+        if fmt in (capi.FORMAT_CU16, capi.FORMAT_CU16BE, capi.FORMAT_CU32, capi.FORMAT_CU32BE):
+            x += 1 << (8 * k - 1)
+        b = x.view(torch.uint8).view(-1, 8)[:, :k]   # the low k bytes, little-endian
+    return (b.flip(1) if fmt in BIG_ENDIAN else b).contiguous().view(-1)
 
 
 def main():
@@ -40,6 +55,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--samples", type=int, default=1 << 29, help="decoder-rate IQ samples (2^29 = 1 GiB of uint8)")
     ap.add_argument("--formats", default="cs16,cf32")
+    ap.add_argument("--no-e2e", action="store_true", help="skip the end-to-end arms from pinned host memory")
     args = ap.parse_args()
     cl, flags = 72, capi.DECODE_ONLY_VALID
     rate_out = 32768 * cl
@@ -55,10 +71,12 @@ def main():
         for name in args.formats.split(","):
             fmt = FORMATS[name]
             d = encode_on_device(u8, fmt)
-            host = torch.empty(d.numel(), dtype=torch.uint8).pin_memory()
-            host.copy_(d)
-            host_u8 = torch.empty(u8.numel(), dtype=torch.uint8).pin_memory()
-            host_u8.copy_(u8)
+            host = host_u8 = None
+            if not args.no_e2e:
+                host = torch.empty(d.numel(), dtype=torch.uint8).pin_memory()
+                host.copy_(d)
+                host_u8 = torch.empty(u8.numel(), dtype=torch.uint8).pin_memory()
+                host_u8.copy_(u8)
             torch.cuda.synchronize()
             h = capi.new_decoder("scm", cl, max_blocks_per_call=out_blocks, max_candidates=1 << 20, input_rate=rate_in,
                                  input_format=fmt)
@@ -104,10 +122,12 @@ def main():
                 us = [e.device_time for e in prof.events() if want in e.name]
                 kern_us[k] = float(np.sum(us)) if us else None
 
-            for k, (dec, _b, hbuf) in arms.items():
-                e2e(dec, hbuf)
-            t_e2e = {k: [] for k in arms}
-            for _ in range(args.reps):
+            t_e2e = {k: [float("nan")] for k in arms}
+            if not args.no_e2e:
+                for k, (dec, _b, hbuf) in arms.items():
+                    e2e(dec, hbuf)
+                t_e2e = {k: [] for k in arms}
+            for _ in range(0 if args.no_e2e else args.reps):
                 for k, (dec, _b, hbuf) in arms.items():
                     t_e2e[k].append(e2e(dec, hbuf))
 
