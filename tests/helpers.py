@@ -64,6 +64,92 @@ PREAMBLES = {"scm": "111110010101001100000", "scm+": "0001011010100011", "idm": 
              "r900bcd": "00000000000000001110010101100100"}
 
 
+def _names(msgtypes):
+    return [m.strip() for m in msgtypes.split(",") if m.strip()] if isinstance(msgtypes, str) else list(msgtypes)
+
+
+def r900_preamble_id(msgtypes):
+    """preamble_id of the r900 preamble among the distinct preambles in registration order (decode.go:121-124)."""
+    order = []
+    for m in _names(msgtypes):
+        if PREAMBLES[m] not in order:
+            order.append(PREAMBLES[m])
+    return order.index(PREAMBLES["r900"])
+
+
+def _feed(o, iq, chunk=128):
+    """Decode whole blocks in chunks whose candidate arrays stay small (the oracle's state runs on across calls)."""
+    bs2, out = o.cfg.block_size2, []
+    for a in range(0, iq.size // bs2, chunk):
+        part = iq[a * bs2:(a + chunk) * bs2]
+        n = part.size // bs2
+        out += o.decode(part, cand_cap=4096 + 512 * n, msg_cap=256 + 16 * n)[0]
+    return out
+
+
+def oracle_r900_digits(mt, cl, iq, first_block=0, cuts=()):
+    """{(block, idx, preamble_id): 42 digits as bytes} for every r900-preamble candidate the oracle finds in `iq` (whole
+    blocks, the stream's first bytes: nothing in front of them), blocks numbered from `first_block`.  Digit k is the r900
+    parser's quantized[idx + PL - SL + 4*k*CL] (r900.go:187-193) after the candidate's own block: a first pass finds those
+    blocks, a second one feeds the oracle in segments ending at each of them (and at the blocks in `cuts`)."""
+    search = oracle.SEARCH_GO if (2 * cl) % 8 == 0 else oracle.SEARCH_EXACT
+    pid = r900_preamble_id(mt)
+    o = oracle.Oracle(mt, cl, search)
+    bs2 = o.cfg.block_size2
+    iq = whole_blocks(iq, bs2)
+    ends = sorted({c.block for c in _feed(o, iq) if c.preamble_id == pid} | set(cuts))
+    o.close()
+    o = oracle.Oracle(mt, cl, search)
+    c = o.cfg
+    pos = c.preamble_length - c.symbol_length + 4 * cl * np.arange(42)
+    out, prev = {}, 0
+    for b in ends:
+        cands = _feed(o, iq[prev * bs2:(b + 1) * bs2])
+        prev = b + 1
+        hits = [x for x in cands if x.preamble_id == pid and x.block == b]
+        if hits:
+            q = o.r900_quantized()
+            for x in hits:
+                out[(x.block + first_block, x.idx, pid)] = q[x.idx + pos].tobytes()
+    o.close()
+    return out
+
+
+def r900_symbols(digits):
+    """The 21 symbols of 42 base-6 digits (r900.go:188-197); None if one exceeds 31 (the parser drops the candidate)."""
+    sym = [digits[2 * k] * 6 + digits[2 * k + 1] for k in range(21)]
+    return None if max(sym) > 31 else sym
+
+
+def compare_r900_digits(got, msgtypes, want):
+    """Every GPU record against oracle_r900_digits: a record of the r900 preamble carries CAND_HAS_R900 and exactly the
+    oracle's 42 digits, every other record neither; the r900 records are exactly the oracle's r900 candidates; and every
+    r900 / r900bcd bit of check_mask is screen_expected of the ORACLE's digits.  Returns (records compared, of those
+    failing the screen)."""
+    names = _names(msgtypes)
+    pid = r900_preamble_id(names)
+    bits = [i for i, m in enumerate(names) if m in ("r900", "r900bcd")]
+    rmask = sum(1 << i for i in bits)
+    is_r = got["preamble_id"] == pid
+    other = got[~is_r]
+    assert not (other["flags"] & capi.CAND_HAS_R900).any() and not other["r900_digits"].any()
+    assert not (other["check_mask"] & rmask).any()
+    rec = got[is_r]
+    keys = list(zip(rec["block"].tolist(), rec["idx"].tolist(), rec["preamble_id"].tolist()))
+    assert len(set(keys)) == len(keys)
+    assert set(keys) == set(want), (len(set(keys) - set(want)), len(set(want) - set(keys)),
+                                    sorted(set(keys) ^ set(want))[:8])
+    assert (rec["flags"] & capi.CAND_HAS_R900).all()
+    fails = 0
+    for r, k in zip(rec, keys):
+        d = want[k]
+        assert r["r900_digits"].tobytes() == d, (k, list(r["r900_digits"]), list(d))
+        ok = screen_expected("r900", b"", d)
+        fails += not ok
+        assert int(r["check_mask"]) & rmask == (rmask if ok else 0), (k, int(r["check_mask"]), ok)
+    return len(keys), fails
+
+
 def assert_check_masks_exact(got, msgtypes):
     """BOTH directions: bit i of check_mask is set iff the candidate is filed under parser i's preamble and
     passes that parser's integrity check (recomputed here from the returned bytes / digits)."""

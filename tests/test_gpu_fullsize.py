@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 
 import oracle
-from helpers import assert_check_masks_exact, cand_key_gpu, cand_key_oracle
+from helpers import assert_check_masks_exact, cand_key_gpu, cand_key_oracle, compare_r900_digits, oracle_r900_digits
 from rtlamr_b200 import capi, shard, synth
 
 pytestmark = pytest.mark.gpu
@@ -130,6 +130,9 @@ def test_windows_match_the_oracle_bit_for_bit(big):
         assert have == want, (b.name, w0, len(have), len(want))
         total_cands += len(want)
         assert_check_masks_exact(sel, b.mt)
+        if "r900" in b.msgtypes:   # every r900 candidate's 42 digits against the r900 parser fed the window, halo included
+            digits = {k: v for k, v in oracle_r900_digits(b.mt, CL, iq, first_block=f0).items() if k[0] >= w0}
+            assert compare_r900_digits(sel, b.mt, digits)[0] > 0
         # the parsers' verdicts: every message the oracle's parsers emit sits on a candidate with that bit set
         protos = oracle.proto_ids(b.mt)
         masks = {(int(r["block"]), int(r["idx"])): int(r["check_mask"]) for r in sel}
