@@ -232,6 +232,29 @@ int ertgpu_set_input_format(ertgpu_handle *h, int32_t format, float scale);
 /* The format and the scale in effect (the default filled in). */
 int ertgpu_get_input_format(const ertgpu_handle *h, int32_t *format, float *scale);
 
+/* The level of a converted input (include/ertgpu_level.h has the rule): a histogram of e = floor(log2 |x|) over the
+ * components x of the samples measured, and the gain the rule picks from it. */
+typedef struct {
+    int64_t components, zeros, nans; /* components measured (2 per IQ sample); of them zero (+-0) and NaN         */
+    int64_t bins[256];   /* bins[e + 128]: components with 2^e <= |x| < 2^(e+1), e clamped to [-128, 127]; +-inf in bins[255] */
+    int32_t exponent;    /* k of the rule (log2 of the format's default gain when no component is non-zero and non-NaN) */
+    float scale;         /* 2^k, or the format's default                                                                 */
+} ertgpu_input_level;
+
+/* Measure nbytes of samples in HOST memory (pinned or pageable) in the handle's input format: *out gets their
+ * histogram and the gain ertgpu_level.h's rule picks.  Any whole number of IQ samples is accepted (otherwise
+ * ERTGPU_ESIZE); they are copied through the handle's staging buffers and counted on the GPU on the handle's device
+ * and stream.  Nothing of the decode stream changes: a decode after a measure returns exactly what it returns
+ * without it.  Nothing is applied either: ertgpu_set_input_scale does that.  ERTGPU_EINVAL before ertgpu_allocate
+ * and for ERTGPU_FORMAT_CU8. */
+int ertgpu_measure_input(ertgpu_handle *h, const void *samples, size_t nbytes, ertgpu_input_level *out);
+
+/* Change the gain of an allocated, converting handle (scale as for ertgpu_set_input_format, 0: the format's default),
+ * at a stream start only: after ertgpu_allocate or ertgpu_reset and before the next decode call.  The gain stays for
+ * the stream and survives ertgpu_reset.  ERTGPU_EINVAL otherwise, for ERTGPU_FORMAT_CU8, and for a negative or
+ * non-finite scale. */
+int ertgpu_set_input_scale(ertgpu_handle *h, float scale);
+
 /* The resampler of a handle with an input rate: *info, and the (P+1)*T int16 prototype table
  * when table != NULL and cap (entries) is large enough; *n_out = number of table entries.
  * ERTGPU_EINVAL when the handle does not resample. */

@@ -63,6 +63,11 @@ class TuningInfo(C.Structure):
                 ("nco_step", C.c_uint32), ("nco_bits", C.c_int32)]
 
 
+class InputLevel(C.Structure):
+    _fields_ = [("components", C.c_int64), ("zeros", C.c_int64), ("nans", C.c_int64), ("bins", C.c_int64 * 256),
+                ("exponent", C.c_int32), ("scale", C.c_float)]
+
+
 class Shard(C.Structure):
     _fields_ = [("first_block", C.c_int64), ("last_block", C.c_int64), ("first_fed_block", C.c_int64)]
 
@@ -89,7 +94,7 @@ EXPORTS = [
     "ertgpu_host_alloc", "ertgpu_host_free", "ertgpu_synth_fill",
     "ertgpu_bind_host_thread", "ertgpu_last_kernels", "ertgpu_plan_shards", "ertgpu_decode_sharded",
     "ertgpu_set_input_rate", "ertgpu_get_resampler", "ertgpu_set_input_format", "ertgpu_get_input_format",
-    "ertgpu_set_input_tuning", "ertgpu_get_tuning",
+    "ertgpu_set_input_tuning", "ertgpu_get_tuning", "ertgpu_measure_input", "ertgpu_set_input_scale",
 ]
 
 _lib = None
@@ -148,6 +153,8 @@ def lib() -> C.CDLL:
     L.ertgpu_get_input_format.argtypes = [vp, C.POINTER(i32), C.POINTER(C.c_float)]
     L.ertgpu_set_input_tuning.argtypes = [vp, i64, i64]
     L.ertgpu_get_tuning.argtypes = [vp, C.POINTER(TuningInfo)]
+    L.ertgpu_measure_input.argtypes = [vp, vp, sz, C.POINTER(InputLevel)]
+    L.ertgpu_set_input_scale.argtypes = [vp, C.c_float]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the library does not export it
     _lib = L
@@ -214,6 +221,23 @@ class Handle:
         f, g = C.c_int32(0), C.c_float(0)
         self._check(self._L.ertgpu_get_input_format(self._h, C.byref(f), C.byref(g)))
         return f.value, g.value
+
+    def measure_input(self, buf) -> dict:
+        """ertgpu_measure_input on a HOST buffer (numpy array of any dtype, or an address/size pair) of whole samples in
+        the handle's format: {"components", "zeros", "nans", "bins" (int64[256], bins[e + 128]), "exponent", "scale"}."""
+        if isinstance(buf, tuple):
+            addr, nbytes = buf
+        else:
+            buf = np.ascontiguousarray(buf)
+            addr, nbytes = buf.ctypes.data, buf.nbytes
+        lv = InputLevel()
+        self._check(self._L.ertgpu_measure_input(self._h, addr, nbytes, C.byref(lv)))
+        return {"components": lv.components, "zeros": lv.zeros, "nans": lv.nans,
+                "bins": np.array(lv.bins[:], dtype=np.int64), "exponent": lv.exponent, "scale": lv.scale}
+
+    def set_input_scale(self, scale: float):
+        """ertgpu_set_input_scale: the gain of the stream that starts now (after allocate or reset, before decode)."""
+        self._check(self._L.ertgpu_set_input_scale(self._h, float(scale)))
 
     def resampler(self):
         """ertgpu_get_resampler: (info dict, int16 table of (P+1)*T entries)."""

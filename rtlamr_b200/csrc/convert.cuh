@@ -76,7 +76,6 @@ __device__ __forceinline__ uint32_t fmt_byte(float x, float g) {
     return (uint32_t)(__float2int_rn(fminf(fmaxf(p, -128.0f), 127.0f)) + 128);
 }
 
-// The bytes of IQ sample j of format F (F != cu8) at src: I in the low byte, Q in the high byte.
 // The same in double for the components float32 cannot hold: p = fl64(x * (double)g), one multiply rounded to nearest
 // even, then clamped and rounded half to even in double.
 __device__ __forceinline__ uint32_t fmt_byte_d(double x, float g) {
@@ -85,27 +84,32 @@ __device__ __forceinline__ uint32_t fmt_byte_d(double x, float g) {
     return (uint32_t)(__double2int_rn(fmin(fmax(p, -128.0), 127.0)) + 128);
 }
 
-// The SigMF formats after the first four.  Component c (0: I of the first sample, 1: its Q, 2: I of the next, ...) as the
-// decoder's byte, from the little-endian 32-bit words x of the samples' bytes.
+// Component c (0: I of the first sample, 1: its Q, 2: I of the next, ...) of format F (F != cu8) from the little-endian
+// 32-bit words x of the samples' bytes: the value x the gain multiplies, as the type that holds it exactly (int8_t,
+// int16_t, int32_t, float or double).  It is the stored value, byte permuted first for a big-endian format, less 2^15 or
+// 2^31 for an unsigned one.  convert_kernel, resample_kernel and level_kernel read every component through this.
 template <int F>
-__device__ __forceinline__ uint32_t fmt_comp(const uint32_t* x, int c, float g) {
+__device__ __forceinline__ auto fmt_x(const uint32_t* x, int c) {
     constexpr bool be = F == ERTGPU_FORMAT_CS16BE || F == ERTGPU_FORMAT_CF32BE || F == ERTGPU_FORMAT_CU16BE ||
                         F == ERTGPU_FORMAT_CS32BE || F == ERTGPU_FORMAT_CU32BE || F == ERTGPU_FORMAT_CF64BE;
     constexpr bool un = F == ERTGPU_FORMAT_CU16 || F == ERTGPU_FORMAT_CU16BE || F == ERTGPU_FORMAT_CU32 || F == ERTGPU_FORMAT_CU32BE;
     constexpr int S = fmt_sample_bytes(F);
-    if constexpr (S == 4) {         // 16-bit: one word per sample, I in the low half
+    static_assert(F != ERTGPU_FORMAT_CU8, "cu8 is not converted");
+    if constexpr (S == 2) {         // cs8: four components per word
+        return (int8_t)(x[c >> 2] >> (8 * (c & 3)));
+    } else if constexpr (S == 4) {  // 16-bit: one word per sample, I in the low half
         uint32_t w = x[c >> 1];
         if constexpr (be) w = __byte_perm(w, 0, 0x2301);
         if constexpr (un) w ^= 0x80008000u;   // v - 2^15 as int16
-        return fmt_byte((float)(int16_t)((c & 1) ? w >> 16 : w & 0xffffu), g);
+        return (int16_t)((c & 1) ? w >> 16 : w & 0xffffu);
     } else if constexpr (S == 8) {  // 32-bit: one word per component
         uint32_t w = x[c];
         if constexpr (be) w = __byte_perm(w, 0, 0x0123);
-        if constexpr (F == ERTGPU_FORMAT_CF32BE) {
-            return fmt_byte(__uint_as_float(w), g);
+        if constexpr (F == ERTGPU_FORMAT_CF32 || F == ERTGPU_FORMAT_CF32BE) {
+            return __uint_as_float(w);
         } else {
             if constexpr (un) w ^= 0x80000000u;   // v - 2^31 as int32
-            return fmt_byte_d((double)(int32_t)w, g);
+            return (int32_t)w;
         }
     } else {                        // float64: two words per component
         uint32_t lo = x[2 * c], hi = x[2 * c + 1];
@@ -114,45 +118,50 @@ __device__ __forceinline__ uint32_t fmt_comp(const uint32_t* x, int c, float g) 
             lo = __byte_perm(hi, 0, 0x0123);
             hi = t;
         }
-        return fmt_byte_d(__hiloint2double((int)hi, (int)lo), g);
+        return __hiloint2double((int)hi, (int)lo);
     }
 }
 
+// A component as the decoder's byte: float32 arithmetic for the types float32 holds exactly, double for the others.
+__device__ __forceinline__ uint32_t fmt_byte_x(int8_t x, float g) { return fmt_byte((float)x, g); }
+__device__ __forceinline__ uint32_t fmt_byte_x(int16_t x, float g) { return fmt_byte((float)x, g); }
+__device__ __forceinline__ uint32_t fmt_byte_x(float x, float g) { return fmt_byte(x, g); }
+__device__ __forceinline__ uint32_t fmt_byte_x(int32_t x, float g) { return fmt_byte_d((double)x, g); }
+__device__ __forceinline__ uint32_t fmt_byte_x(double x, float g) { return fmt_byte_d(x, g); }
+
+template <int F>
+__device__ __forceinline__ uint32_t fmt_comp(const uint32_t* x, int c, float g) { return fmt_byte_x(fmt_x<F>(x, c), g); }
+
+// The bytes of IQ sample j of format F (F != cu8) at src: I in the low byte, Q in the high byte.
 template <int F>
 __device__ __forceinline__ uchar2 fmt_sample(const uint8_t* src, long long j, float g) {
-    if constexpr (F != ERTGPU_FORMAT_CS8 && F != ERTGPU_FORMAT_CS16 && F != ERTGPU_FORMAT_CF32) {
-        constexpr int S = fmt_sample_bytes(F);
-        uint32_t x[S / 4];
-        if constexpr (S == 4) {
-            x[0] = *reinterpret_cast<const uint32_t*>(src + 4 * j);
-        } else if constexpr (S == 8) {
-            const uint2 v = *reinterpret_cast<const uint2*>(src + 8 * j);
-            x[0] = v.x;
-            x[1] = v.y;
-        } else {
-            const uint4 v = *reinterpret_cast<const uint4*>(src + 16 * j);
-            x[0] = v.x;
-            x[1] = v.y;
-            x[2] = v.z;
-            x[3] = v.w;
-        }
-        return make_uchar2((unsigned char)fmt_comp<F>(x, 0, g), (unsigned char)fmt_comp<F>(x, 1, g));
-    }
-    float i, q;
+    constexpr int S = fmt_sample_bytes(F);
+    uint32_t x[(S + 3) / 4];
+    // cs8, cs16 and cf32 are loaded as the vector of their components, which the compiler reads in place
     if constexpr (F == ERTGPU_FORMAT_CS8) {
         const char2 v = *reinterpret_cast<const char2*>(src + 2 * j);
-        i = (float)v.x;
-        q = (float)v.y;
+        x[0] = (uint32_t)(uint8_t)v.x | (uint32_t)(uint8_t)v.y << 8;
     } else if constexpr (F == ERTGPU_FORMAT_CS16) {
         const short2 v = *reinterpret_cast<const short2*>(src + 4 * j);
-        i = (float)v.x;
-        q = (float)v.y;
-    } else {
+        x[0] = (uint32_t)(uint16_t)v.x | (uint32_t)(uint16_t)v.y << 16;
+    } else if constexpr (F == ERTGPU_FORMAT_CF32) {
         const float2 v = *reinterpret_cast<const float2*>(src + 8 * j);
-        i = v.x;
-        q = v.y;
+        x[0] = __float_as_uint(v.x);
+        x[1] = __float_as_uint(v.y);
+    } else if constexpr (S == 4) {
+        x[0] = *reinterpret_cast<const uint32_t*>(src + 4 * j);
+    } else if constexpr (S == 8) {
+        const uint2 v = *reinterpret_cast<const uint2*>(src + 8 * j);
+        x[0] = v.x;
+        x[1] = v.y;
+    } else {
+        const uint4 v = *reinterpret_cast<const uint4*>(src + 16 * j);
+        x[0] = v.x;
+        x[1] = v.y;
+        x[2] = v.z;
+        x[3] = v.w;
     }
-    return make_uchar2((unsigned char)fmt_byte(i, g), (unsigned char)fmt_byte(q, g));
+    return make_uchar2((unsigned char)fmt_comp<F>(x, 0, g), (unsigned char)fmt_comp<F>(x, 1, g));
 }
 
 constexpr int kCvtThreads = 256;
@@ -170,42 +179,26 @@ __global__ void __launch_bounds__(kCvtThreads) convert_kernel(const uint8_t* __r
         uint4 v[kLoads];
 #pragma unroll
         for (int k = 0; k < kLoads; k++) v[k] = __ldcs(src + k);   // read once: do not keep it in L2
-        uint32_t w[4];
-        if constexpr (F == ERTGPU_FORMAT_CS8) {
-            const uint32_t x[4] = {v[0].x, v[0].y, v[0].z, v[0].w};
+        uint32_t x[4 * kLoads];
 #pragma unroll
-            for (int k = 0; k < 4; k++) {
+        for (int k = 0; k < kLoads; k++) {
+            x[4 * k] = v[k].x;
+            x[4 * k + 1] = v[k].y;
+            x[4 * k + 2] = v[k].z;
+            x[4 * k + 3] = v[k].w;
+        }
+        uint32_t w[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            if constexpr (F == ERTGPU_FORMAT_CS8) {
                 uint32_t o = 0;
 #pragma unroll
-                for (int b = 0; b < 4; b++) o |= fmt_byte((float)(int8_t)(x[k] >> (8 * b)), g) << (8 * b);
+                for (int b = 0; b < 4; b++) o |= fmt_comp<F>(x, 4 * k + b, g) << (8 * b);
                 w[k] = o;
-            }
-        } else if constexpr (F == ERTGPU_FORMAT_CS16) {
-            const uint32_t x[8] = {v[0].x, v[0].y, v[0].z, v[0].w, v[1].x, v[1].y, v[1].z, v[1].w};
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                const uint32_t a = x[2 * k], b = x[2 * k + 1];
-                w[k] = fmt_byte((float)(int16_t)(a & 0xffffu), g) | fmt_byte((float)(int16_t)(a >> 16), g) << 8 |
-                       fmt_byte((float)(int16_t)(b & 0xffffu), g) << 16 | fmt_byte((float)(int16_t)(b >> 16), g) << 24;
-            }
-        } else if constexpr (F != ERTGPU_FORMAT_CF32) {
-            uint32_t x[4 * kLoads];
-#pragma unroll
-            for (int k = 0; k < kLoads; k++) {
-                x[4 * k] = v[k].x;
-                x[4 * k + 1] = v[k].y;
-                x[4 * k + 2] = v[k].z;
-                x[4 * k + 3] = v[k].w;
-            }
-#pragma unroll
-            for (int k = 0; k < 4; k++)
+            } else {
                 w[k] = fmt_comp<F>(x, 4 * k, g) | fmt_comp<F>(x, 4 * k + 1, g) << 8 | fmt_comp<F>(x, 4 * k + 2, g) << 16 |
                        fmt_comp<F>(x, 4 * k + 3, g) << 24;
-        } else {
-#pragma unroll
-            for (int k = 0; k < 4; k++)
-                w[k] = fmt_byte(__uint_as_float(v[k].x), g) | fmt_byte(__uint_as_float(v[k].y), g) << 8 |
-                       fmt_byte(__uint_as_float(v[k].z), g) << 16 | fmt_byte(__uint_as_float(v[k].w), g) << 24;
+            }
         }
         reinterpret_cast<uint4*>(out)[grp] = make_uint4(w[0], w[1], w[2], w[3]);
     }

@@ -29,6 +29,7 @@
 #include <thread>
 #include <vector>
 
+#include "../../include/ertgpu_level.h"
 #include "copy_pool.hpp"
 #include "demod_fast.cuh"
 #include "demod_generic.cuh"
@@ -95,6 +96,7 @@ struct ertgpu_handle {
     bool uncopied = false;      // a pipeline is synchronised, its candidates still only on the device
     unsigned long long uncopied_n = 0;
     bool fresh = true;          // next pipeline must see zeroed history (start of stream / after reset)
+    bool started = false;       // a decode call was accepted since allocate / reset (ertgpu_set_input_scale)
     cudaStream_t pending_stream = nullptr;
     const uint8_t* last_iq = nullptr;
     const uint8_t* last_hist = nullptr;
@@ -567,6 +569,7 @@ int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
     if (!iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
     if (const int rc = h->in.check_call(iq, nbytes, device)) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
+    h->started = true;
     if (h->pending) {
         int rc = collect(h);
         if (rc) return rc;
@@ -824,6 +827,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     h->cur_plane = h->cur_hist = 0;
     h->hist_valid = 0;
     h->block_counter = 0;
+    h->started = false;
     return ERTGPU_OK;
 }
 
@@ -844,6 +848,7 @@ int ertgpu_reset(ertgpu_handle* h) {
     h->fresh = true;
     h->hist_valid = 0;
     h->block_counter = 0;
+    h->started = false;
     h->in.reset_stream();
     begin_call(h);
     return ERTGPU_OK;
@@ -877,6 +882,59 @@ int ertgpu_get_input_format(const ertgpu_handle* h, int32_t* format, float* scal
     if (!h) return ERTGPU_EINVAL;
     if (format) *format = h->in.fmt;
     if (scale) *scale = h->in.scale;
+    return ERTGPU_OK;
+}
+
+int ertgpu_set_input_scale(ertgpu_handle* h, float scale) {
+    if (!h) return ERTGPU_EINVAL;
+    if (!h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_scale before allocate: ertgpu_set_input_format takes the scale");
+    if (h->started) return fail(h, ERTGPU_EINVAL, "set_input_scale after a decode call: the gain changes only at a stream start");
+    return h->in.set_scale(scale);
+}
+
+// Each chunk is copied to d_stage[k] and counted by level_kernel on the handle's stream; pageable input is staged through
+// h_stage[k] as in ertgpu_decode.  The counters live in the input stage and are zeroed first; nothing the decode reads
+// or keeps between calls is touched.
+int ertgpu_measure_input(ertgpu_handle* h, const void* samples, size_t nbytes, ertgpu_input_level* out) {
+    if (!h || !h->allocated) return ERTGPU_EINVAL;
+    if (h->in.fmt == ERTGPU_FORMAT_CU8) return fail(h, ERTGPU_EINVAL, "cu8 input is not measured: it takes no gain");
+    if (!out || (!samples && nbytes)) return fail(h, ERTGPU_EINVAL, "null argument");
+    const size_t s = (size_t)h->in.sample_bytes;
+    if (nbytes % s) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of %zu-byte IQ samples", nbytes, s);
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaMemsetAsync(h->in.d_level, 0, kLvCounters * sizeof(unsigned long long), h->stream));
+    const int64_t total = (int64_t)(nbytes / s);
+    if (total) {
+        bool pageable = true;
+        if (const int rc = prepare_staging(h, (size_t)h->in.chunk() * s, samples, &pageable)) return rc;
+        const int64_t chunk = (int64_t)(h->stage_bytes / s);
+        const uint8_t* src0 = static_cast<const uint8_t*>(samples);
+        int64_t done = 0;
+        for (int64_t i = 0; done < total; i++) {
+            const int k = (int)(i & 1);
+            const int64_t c = std::min(chunk, total - done);
+            if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // d_stage[k] and h_stage[k] are free again
+            const uint8_t* src = src0 + (size_t)done * s;
+            if (pageable) {
+                h->copy_pool->copy(h->h_stage[k], src, (size_t)c * s);
+                src = h->h_stage[k];
+            }
+            CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * s, cudaMemcpyHostToDevice, h->stream));
+            if (const int rc = h->in.launch_level(h->d_stage[k], c, h->stream)) return rc;
+            CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
+            done += c;
+        }
+    }
+    unsigned long long cnt[kLvCounters];
+    CUDA_TRY(h, cudaMemcpyAsync(cnt, h->in.d_level, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    memset(out, 0, sizeof(*out));
+    out->components = 2 * total;
+    out->zeros = (int64_t)cnt[kLvZero];
+    out->nans = (int64_t)cnt[kLvNan];
+    for (int b = 0; b < ERTLV_BINS; b++) out->bins[b] = (int64_t)cnt[b];
+    out->exponent = ertlv_exponent(out->bins, out->components, out->zeros, out->nans, ilogbf(fmt_default_scale(h->in.fmt)));
+    out->scale = ldexpf(1.0f, out->exponent);
     return ERTGPU_OK;
 }
 

@@ -1,7 +1,8 @@
 // input_stage.cuh -- the input stage of a libertgpu handle: everything between the caller's bytes and the uint8 IQ blocks
 // the demod reads.  It owns the input's format, rate and tuning (ertgpu_set_input_*), the mode they resolve to, the
 // resampler's plan, tables and stream position, and it launches the one kernel in front of the pipeline:
-// convert_kernel<F> (convert.cuh) or resample_kernel<F, TUNED> (resample.cuh).  Host code only.
+// convert_kernel<F> (convert.cuh) or resample_kernel<F, TUNED> (resample.cuh).  It also measures the level of its input
+// with level_kernel<F> (level.cuh) for ertgpu_measure_input.  Host code only.
 #pragma once
 
 #include <algorithm>
@@ -15,6 +16,7 @@
 
 #include "convert.cuh"
 #include "demod_fast.cuh"  // OncePerDevice
+#include "level.cuh"
 #include "resample.cuh"
 
 namespace ert {
@@ -85,6 +87,8 @@ struct InputStage {
     int64_t pend = 0;           // outputs at the front of d_out[cur_out] that wait for a whole block
     size_t smem = 0;
     int grid = 0;               // most CTAs of one launch
+    unsigned long long* d_level = nullptr;  // level_kernel's kLvCounters counters (converted input only)
+    int level_grid = 0;
 
     bool resamples() const { return mode >= kResample; }
 
@@ -121,6 +125,14 @@ struct InputStage {
         return ERTGPU_OK;
     }
 
+    // The gain of a converted input, as set_format takes it; the caller allows it at a stream start only.
+    int set_scale(float g) {
+        if (fmt == ERTGPU_FORMAT_CU8) return fail(err_, ERTGPU_EINVAL, "cu8 input is not scaled");
+        if (!std::isfinite(g) || g < 0.0f) return fail(err_, ERTGPU_EINVAL, "input scale %g is not a finite value >= 0", (double)g);
+        scale = g == 0.0f ? fmt_default_scale(fmt) : g;
+        return ERTGPU_OK;
+    }
+
     // At allocate: a tuned handle at the decoder's own rate gets its plan here, and the channel must lie inside it.
     int plan_native(int64_t rate_out) { return tuned && !rate_in ? configure_rate(rate_out, rate_out) : ERTGPU_OK; }
 
@@ -150,6 +162,10 @@ struct InputStage {
         block = block_size;
         max_blocks = max_blocks_per_step;
         reset_stream();
+        if (fmt != ERTGPU_FORMAT_CU8) {
+            CUDA_TRY(err_, cudaMalloc(&d_level, kLvCounters * sizeof(unsigned long long)));
+            level_grid = sm_count * 4;
+        }
         if (mode == kPass) return ERTGPU_OK;
         if (mode == kConvert) {
             grid = sm_count * 8;
@@ -195,6 +211,7 @@ struct InputStage {
         dfree(d_A);
         dfree(d_D);
         dfree(d_E);
+        dfree(d_level);
         for (int k = 0; k < 2; k++) {
             dfree(d_hist[k]);
             dfree(d_out[k]);
@@ -312,6 +329,17 @@ struct InputStage {
         }
         CUDA_TRY(err_, cudaGetLastError());
         ++*launches;
+        return ERTGPU_OK;
+    }
+
+    // Enqueue level_kernel over n input samples at d_in (device, 16-byte aligned) on st: their counts are added to d_level.
+    int launch_level(const uint8_t* d_in, int64_t n, cudaStream_t st) const {
+        const long long nbytes = n * sample_bytes, groups = (nbytes + 15) / 16;
+        const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>((groups + kLvThreads - 1) / kLvThreads, level_grid));
+        fmt_visit(fmt, [&](auto f) {
+            if constexpr (f() != ERTGPU_FORMAT_CU8) level_kernel<f()><<<g, kLvThreads, 0, st>>>(d_in, nbytes, d_level);
+        });
+        CUDA_TRY(err_, cudaGetLastError());
         return ERTGPU_OK;
     }
 

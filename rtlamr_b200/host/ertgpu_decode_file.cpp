@@ -5,7 +5,7 @@
 //   ertgpu_decode_file [-msgtype=scm,idm|all] [-symbollength=72] [-blockdedup=true] [-blocks=4096] [-device=0]
 //                      [-filterid=1,2] [-filtertype=4,5] [-unique=true] [-format=plain|csv|json|xml]
 //                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ]
-//                      [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|cf64_be|wav|sigmf] [-samplescale=G] [-capturefreq=HZ [-centerfreq=HZ]]
+//                      [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|cf64_be|wav|sigmf] [-samplescale=G|auto] [-capturefreq=HZ [-centerfreq=HZ]]
 //                      FILE|- [FILE ...]
 // -capturefreq names the frequency the capture was recorded centred at; -centerfreq (rtlamr's flag) the channel to
 // receive, by default the protocols' CenterFreq (912.6 MHz, or 912.38 MHz for r900 alone).  The channel is mixed to
@@ -25,7 +25,11 @@
 // segment carries a core:datetime, the csv, json and xml Time is the moment a live receiver would have finished the
 // message's block (sigmf::BlockTime) instead of the wall clock.  Other formats are converted to uint8 on the GPU,
 // u = clamp(rint(x * G), -128, 127) + 128; -samplescale=G is that gain (default 1 for cs8, 2^-8 for the 16-bit formats,
-// 2^-24 for the 32-bit integers, 2^7 for the floats: full scale to full scale; a 12-bit Airspy wants 0.0625).  A WAV or
+// 2^-24 for the 32-bit integers, 2^7 for the floats: full scale to full scale; a 12-bit Airspy wants 0.0625).
+// -samplescale=auto picks G = 2^k per stream (each file of a batch, or stdin) from the stream's first 2^22 samples, after
+// a WAV header or SigMF core:header_bytes: the largest k in [-120, 120] at which at most one component in 65 536 clips
+// (include/ertgpu_level.h).  The gain then stays fixed for the whole stream; it does not follow the level the way a tuner's
+// AGC does.  k, G and the number of samples measured go to stderr; stdout is exactly that of -samplescale=G.  A WAV or
 // SigMF file is never detected by its content or name.  -samplefile takes only untuned uint8 input at
 // 32768 * -symbollength (an 8-bit WAV at that rate is uint8).
 // -filterid / -filtertype / -unique, -format, -samplefile, -single and -duration are rtlamr's flags of the same names
@@ -62,7 +66,7 @@ int main(int argc, char** argv) {
     bool block_dedup = true, quiet = false, unique = false, single = false;
     std::string filterid, filtertype, format = "plain", samplefile, duration, sampleformat = "cu8", samplescale;
     std::string capturefreq, centerfreq;
-    bool have_scale = false;
+    bool have_scale = false, auto_scale = false;
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
         if (a.rfind("-msgtype=", 0) == 0) msgtype = a.substr(9);
@@ -94,7 +98,7 @@ int main(int argc, char** argv) {
         fprintf(stderr, "usage: %s [-msgtype=scm,scm+,idm,netidm,r900,r900bcd|all] [-symbollength=N] [-blockdedup=true|false] "
                         "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
                         "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|wav|sigmf] "
-                        "[-samplescale=G] "
+                        "[-samplescale=G|auto] "
                         "[-capturefreq=HZ [-centerfreq=HZ]] [-quiet] FILE|- [FILE ...]\n", argv[0]);
         return 2;
     }
@@ -130,11 +134,13 @@ int main(int argc, char** argv) {
         return 2;
     }
     float scale = 0.0f;
-    if (have_scale) {
+    if (samplescale == "auto") {
+        auto_scale = true;
+    } else if (have_scale) {
         char* end = nullptr;
         scale = strtof(samplescale.c_str(), &end);
         if (samplescale.empty() || *end || !std::isfinite(scale) || scale <= 0.0f) {
-            fprintf(stderr, "invalid value \"%s\" for flag -samplescale: a finite gain > 0\n", samplescale.c_str());
+            fprintf(stderr, "invalid value \"%s\" for flag -samplescale: a finite gain > 0, or auto\n", samplescale.c_str());
             return 2;
         }
     }
@@ -232,7 +238,7 @@ int main(int argc, char** argv) {
         }
     }
     try {
-        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz});
+        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale});
         fputs(rcvr.decoder().Log().c_str(), stderr);
         if (sample) rcvr.SetSampleFile(sample);
         if (limit_ns) rcvr.SetDeadline(start + std::chrono::nanoseconds(limit_ns));
@@ -258,6 +264,11 @@ int main(int argc, char** argv) {
                 return 1;
             }
             if (fi) rcvr.Reset();
+            if (auto_scale)
+                rcvr.SetLevelReport([&](const ertgpu_input_level& lv) {
+                    fprintf(stderr, "%s%s-samplescale=auto: 2^%d = %.9g from %lld samples\n", files.size() > 1 ? file.c_str() : "",
+                            files.size() > 1 ? ": " : "", lv.exponent, (double)lv.scale, (long long)(lv.components / 2));
+                });
             if (wav_in && in != stdin) wav_hdr[fi] = wav::ReadHeader(in);   // the same header as above: to the samples
             auto st = rcvr.Run(in, block_dedup, [&](const protocol::Message& m, int64_t offset, int length) {
                 if (quiet) return;

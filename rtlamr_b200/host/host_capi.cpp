@@ -1,11 +1,13 @@
 // host_capi.cpp -- a small C surface over the C++ protocol mirror so that the Python parity tests
 // (and a CLI) can drive Decoder/Parser exactly like rtlamr's main.go does (main.go:59-86,235).
+#include <algorithm>
 #include <cerrno>
 #include <cstdio>
 #include <cstring>
 #include <memory>
 #include <sstream>
 
+#include "../../include/ertgpu_level.h"
 #include "protocol.hpp"
 #include "receiver.hpp"
 #include "sigmf.hpp"
@@ -28,14 +30,18 @@ struct erthost_msg {
 struct erthost {
     protocol::Decoder d;
     std::string err;
+    bool started = false;        // a decode call since erthost_new / erthost_reset
+    bool measured = false;       // `level` holds the measurement of this stream's start
+    ertgpu_input_level level{};
 };
 
 // main.go:59-86: NewDecoder; for each -msgtype NewParser + RegisterProtocol; Allocate.  The input arguments are
 // protocol::Input's (all 0: uint8 IQ at the decoder's own rate): IQ sampled at input_rate Hz, in sample format `format`
-// (ERTGPU_FORMAT_*) with gain `scale`, recorded centred at capture_freq Hz with the channel at center_freq.
+// (ERTGPU_FORMAT_*) with gain `scale`, recorded centred at capture_freq Hz with the channel at center_freq.  auto_scale:
+// the gain of each stream is measured from the first min(len, ERTLV_WINDOW) samples of its first erthost_decode call.
 erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
                      long long input_rate, int format, float scale, long long capture_freq, long long center_freq,
-                     char* errbuf, int errcap) {
+                     int auto_scale, char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;   // released only on success: a throwing NewParser / Allocate must not leak the handle
     try {
         protocol::RegisterStockParsers();
@@ -46,7 +52,7 @@ erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long
             if (name.empty()) continue;
             h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
         }
-        h->d.SetInput({input_rate, format, scale, capture_freq, center_freq});
+        h->d.SetInput({input_rate, format, scale, capture_freq, center_freq, auto_scale != 0});
         h->d.Allocate(device, max_blocks, max_cands);
         return h.release();
     } catch (const std::exception& e) {
@@ -90,6 +96,7 @@ int erthost_config(const erthost* h, int32_t* out12) {
 int erthost_reset(erthost* h) {
     try {
         h->d.Reset();
+        h->started = h->measured = false;
         return 0;
     } catch (const std::exception& e) {
         h->err = e.what();
@@ -215,6 +222,13 @@ long long erthost_encode(erthost* h, const ertgpu_candidate* cands, long long n,
 
 long long erthost_decode(erthost* h, const uint8_t* iq, size_t len, erthost_msg* out, long long cap) {
     try {
+        if (h->d.AutoScale() && !h->started && len % h->d.InputQuantum() == 0) {
+            const size_t s = (size_t)h->d.BytesPerSample();
+            h->level = h->d.Measure(iq, std::min(len / s, (size_t)ERTLV_WINDOW) * s);
+            h->measured = true;
+            h->d.SetScale(h->level.scale);
+        }
+        h->started = true;
         auto msgs = h->d.Decode(iq, len);
         return fill_msgs(msgs, out, cap);
     } catch (const std::length_error& e) {
@@ -315,6 +329,17 @@ int erthost_sigmf_block_time(const char* path, long long block, long long block_
         if (errbuf && errcap > 0) snprintf(errbuf, (size_t)errcap, "%s", e.what());
         return -1;
     }
+}
+
+// The level measured at the start of the current stream (auto_scale): *exponent = k, *scale = 2^k, *components, and the
+// 256 bins when bins != NULL.  Returns 0, or -1 when nothing was measured yet.
+int erthost_level(const erthost* h, int* exponent, float* scale, long long* components, long long* bins) {
+    if (!h->measured) return -1;
+    *exponent = h->level.exponent;
+    *scale = h->level.scale;
+    *components = h->level.components;
+    if (bins) memcpy(bins, h->level.bins, sizeof(h->level.bins));
+    return 0;
 }
 
 int erthost_log(const erthost* h, char* buf, int cap) {

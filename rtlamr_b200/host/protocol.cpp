@@ -611,10 +611,26 @@ void Decoder::SetInput(const Input& in) {
     };
     if (in.CaptureFreq > 0 || in.CenterFreq != 0) check(ertgpu_set_input_tuning(h_, in.CaptureFreq, in.CenterFreq));
     if (in.SampleRate > 0) check(ertgpu_set_input_rate(h_, in.SampleRate));
+    if (in.AutoScale && in.Format == ERTGPU_FORMAT_CU8) throw std::invalid_argument("automatic gain does not apply to uint8 (cu8) input");
     if (in.Format != ERTGPU_FORMAT_CU8 || in.Scale != 0.0f) {
         check(ertgpu_set_input_format(h_, in.Format, in.Scale));
         sample_bytes_ = FormatBytes(in.Format);
     }
+    auto_scale_ = in.AutoScale;
+}
+
+ertgpu_input_level Decoder::Measure(const uint8_t* samples, size_t len) {
+    if (!allocated_) throw std::logic_error("Measure before Allocate");
+    ertgpu_input_level lv{};
+    const int rc = ertgpu_measure_input(h_, samples, len, &lv);
+    if (rc != ERTGPU_OK) raise(h_, rc, "Measure");
+    return lv;
+}
+
+void Decoder::SetScale(float scale) {
+    const int rc = ertgpu_set_input_scale(h_, scale);
+    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
+    if (rc != ERTGPU_OK) raise(h_, rc, "SetScale");
 }
 
 int64_t Decoder::BlocksDecoded() const {

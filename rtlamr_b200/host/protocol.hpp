@@ -142,6 +142,10 @@ struct Input {
     int32_t Format = ERTGPU_FORMAT_CU8; // converted on the GPU with gain Scale, 0: the format's default (ertgpu_set_input_format)
     float Scale = 0.0f;
     int64_t CaptureFreq = 0, CenterFreq = 0;  // the capture's centre and the channel, 0: Cfg.CenterFreq (ertgpu_set_input_tuning)
+    // The gain of each stream is measured from its first samples (ertgpu_measure_input) and set before its first Decode
+    // (ertgpu_set_input_scale); Scale is the gain until then.  Not for cu8.  The Decoder only carries the flag: whoever
+    // feeds it (receiver::Receiver::Run, erthost_decode) measures and sets the gain.
+    bool AutoScale = false;
 };
 
 // decode.go:45-63.  Signal/Quantized are not materialised on the host: the parity taps of the C ABI
@@ -161,6 +165,11 @@ public:
     // throws std::invalid_argument, and so does Allocate when the channel does not fit a capture at the decoder's rate.
     void SetInput(const Input& in);
     int BytesPerSample() const { return sample_bytes_; }
+    bool AutoScale() const { return auto_scale_; }
+    // ertgpu_measure_input on len bytes of whole IQ samples: their level and the gain its rule picks.
+    ertgpu_input_level Measure(const uint8_t* samples, size_t len);
+    // ertgpu_set_input_scale: the gain of the stream that starts now (after Allocate or Reset, before Decode).
+    void SetScale(float scale);
     // Decode takes multiples of this many bytes: whole IQ samples when resampling, whole blocks otherwise.
     size_t InputQuantum() const { return (size_t)sample_bytes_ * (resampling_ ? 1 : (size_t)Cfg.BlockSize); }
     void Allocate(int device = 0, int64_t maxBlocksPerCall = 0, int64_t maxCandidates = 0);  // decode.go:131-160
@@ -189,6 +198,7 @@ private:
     ertgpu_resampler_info rs_{};
     int64_t input_samples_ = 0;  // since Allocate / Reset
     int sample_bytes_ = 2;       // bytes per input IQ sample
+    bool auto_scale_ = false;
 };
 
 void RegisterStockParsers();  // the effect of the reference's blank imports (main.go:37-44)

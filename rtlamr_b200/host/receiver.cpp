@@ -10,6 +10,8 @@
 #include <sstream>
 #include <stdexcept>
 
+#include "../../include/ertgpu_level.h"
+
 namespace receiver {
 
 Digest NewDigest(const protocol::Message& m) { return Digest(m.MsgType(), m.MeterType(), m.MeterID(), m.Checksum()); }
@@ -179,6 +181,33 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
     sample_blocks_ = 2 * (int64_t)d_.Cfg.BufferLength / (int64_t)bs2 + 1;
     FilterChain* fc = fc_.empty() ? nullptr : &fc_;
     const auto t0 = std::chrono::steady_clock::now();
+    // Automatic gain: the stream's first min(stream, ERTLV_WINDOW) samples are read and measured before its first Decode,
+    // the gain is set, and then those same bytes are decoded, followed by the rest.  Nothing is read twice (stdin works),
+    // and the window does not depend on the size of a Decode call.
+    std::vector<uint8_t> window;
+    size_t window_pos = 0;
+    if (d_.AutoScale()) {
+        window.resize((size_t)std::min<uint64_t>((uint64_t)ERTLV_WINDOW * s, left));
+        size_t have = 0;
+        while (have < window.size()) {
+            const size_t n = fread(window.data() + have, 1, window.size() - have, in);
+            if (n == 0) break;
+            have += n;
+        }
+        window.resize(have);
+        level_ = d_.Measure(window.data(), have / s * s);
+        d_.SetScale(level_.scale);
+        if (level_report_) level_report_(level_);
+    }
+    const auto read = [&](uint8_t* dst, size_t n) -> size_t {
+        if (window_pos < window.size()) {
+            const size_t m = std::min(n, window.size() - window_pos);
+            memcpy(dst, window.data() + window_pos, m);
+            window_pos += m;
+            return m;
+        }
+        return fread(dst, 1, n, in);
+    };
     int k = 0;
     size_t carry = 0;  // bytes of a partial block (a partial IQ sample when resampling) kept for the next buffer
     bool eof = false;
@@ -189,7 +218,7 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
         }
         size_t have = carry;
         while (have < buf_bytes_ && left) {
-            const size_t n = fread(buf_[k] + have, 1, (size_t)std::min<uint64_t>(buf_bytes_ - have, left), in);
+            const size_t n = read(buf_[k] + have, (size_t)std::min<uint64_t>(buf_bytes_ - have, left));
             if (n == 0) break;
             have += n;
             left -= n;

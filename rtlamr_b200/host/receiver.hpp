@@ -83,8 +83,13 @@ public:
     }
     // -duration: checked before every read, so a call already read is decoded and reported in full.
     void SetDeadline(std::chrono::steady_clock::time_point t) { deadline_ = t; }
+    // Input::AutoScale: `report` sees each stream's level and gain once it is measured, before the stream is decoded.
+    void SetLevelReport(std::function<void(const ertgpu_input_level&)> report) { level_report_ = std::move(report); }
+    // The level measured at the start of the last stream (Input::AutoScale; all zero otherwise).
+    const ertgpu_input_level& Level() const { return level_; }
 
-    // Run over a FILE* until EOF, -single or the deadline.  `emit` is called once per reported message (after the
+    // Run over a FILE* until EOF, -single or the deadline.  With Input::AutoScale the stream's gain is set from its first
+    // min(stream, ERTLV_WINDOW) samples (include/ertgpu_level.h) before anything is decoded; it stays for the stream.  `emit` is called once per reported message (after the
     // cross-block dedup when block_dedup) with its LogMessage Offset and Length (0 without a sample file).  max_bytes >= 0
     // stops reading after that many bytes (the data chunk of a WAV file).
     Stats Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&, int64_t, int)>& emit,
@@ -114,6 +119,8 @@ private:
     bool single_ = false;
     UintMap* single_ids_ = nullptr;
     std::chrono::steady_clock::time_point deadline_ = std::chrono::steady_clock::time_point::max();
+    std::function<void(const ertgpu_input_level&)> level_report_;
+    ertgpu_input_level level_{};
 
     void DumpSampleBuf(const uint8_t* call, int64_t call_first, int64_t block);
     void KeepHistory(const uint8_t* call, size_t nblocks);
