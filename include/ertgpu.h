@@ -170,7 +170,27 @@ int ertgpu_stock_protocol(const char *msgtype, int32_t chip_length, ertgpu_proto
 /* Decoder.Allocate (decode.go:131-160): derive SymbolLength, BlockSize, ...,
  * select the CUDA device, allocate device buffers for up to
  * max_blocks_per_call blocks per decode call and max_candidates candidates.
- * max_blocks_per_call <= 0 or max_candidates <= 0 pick defaults. */
+ * max_blocks_per_call <= 0 or max_candidates <= 0 pick defaults.
+ *
+ * Before any device call it returns ERTGPU_EINVAL, with a message naming the
+ * rule, for a merged configuration (PS, PK, CL, SL, PL, PKL, BS, BUF of
+ * decode.go:131-141; n = bits of a registered preamble) in which the reference
+ * reads something it did not compute for the candidate at hand:
+ *   R1  8*ceil((BS+PL)/8) <= BUF: Search packs that many Quantized bits
+ *       (decode.go:259-265);
+ *   R2  for every preamble, n - 1 <= PK and (n-1)*(SL>>3) + BS/8 <=
+ *       ceil((BS+PL)/8): the exact pass and the byte pre-filter stay inside
+ *       Quantized and packed (decode.go:268-325);
+ *   R3  with an ERTGPU_CHECK_R900 protocol, PK >= PS + 83: every payload digit
+ *       lies below BUF - 4*CL, the positions the r900 filter writes
+ *       (r900.go:117,187-193).  This also rejects PK = PS+81 and PS+82, where
+ *       the reference reads digits it never wrote (zeros) instead of panicking;
+ *       decoding them would need a zero-digit branch in two r900 kernels;
+ *   R4  when PK % 8 != 0, no ERTGPU_CHECK_CRC16 range [crc_from, crc_to)
+ *       holds byte PK>>3: in the reference that byte still carries the
+ *       previous candidate's high bits (decode.go:363-366), so its CRC
+ *       verdict depends on the order the preambles are searched in.
+ * Every stock -msgtype set passes these rules at any chip length. */
 int ertgpu_allocate(ertgpu_handle *h, int32_t device, int64_t max_blocks_per_call,
                     int64_t max_candidates);
 

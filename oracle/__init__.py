@@ -22,6 +22,9 @@ SCM, SCMPLUS, IDM, NETIDM, R900, R900BCD = range(6)
 PROTO_NAMES = ["scm", "scm+", "idm", "netidm", "r900", "r900bcd"]
 SEARCH_GO, SEARCH_EXACT = 0, 1
 MAX_PKT = 96
+PARSER_NONE = -1
+CHECK_R900 = 3    # ERTGPU_CHECK_R900 of include/ertgpu.h
+PANIC = -2        # ert_oracle_decode: the reference indexes a slice past its length here
 
 
 def build(force: bool = False) -> str:
@@ -39,6 +42,17 @@ class Cfg(C.Structure):
         "data_rate", "block_size", "block_size2", "chip_length", "symbol_length", "sample_rate",
         "preamble_symbols", "packet_symbols", "preamble_length", "packet_length",
         "buffer_length")] + [("center_freq", C.c_uint32)]
+
+
+class Proto(C.Structure):
+    """ert_oracle_proto: one parser's PacketConfig and the parser run on its candidates."""
+    _fields_ = [("preamble", C.c_char * 33), ("data_rate", C.c_int32), ("chip_length", C.c_int32),
+                ("preamble_symbols", C.c_int32), ("packet_symbols", C.c_int32), ("center_freq", C.c_uint32),
+                ("parser", C.c_int32)]
+
+
+class ReferencePanic(RuntimeError):
+    """The reference decoder would index a slice past its length on this input (it panics there)."""
 
 
 class Cand(C.Structure):
@@ -84,6 +98,8 @@ def lib():
         L = C.CDLL(_LIB_PATH)
         L.ert_oracle_new.restype = C.c_void_p
         L.ert_oracle_new.argtypes = [C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32]
+        L.ert_oracle_new_protocols.restype = C.c_void_p
+        L.ert_oracle_new_protocols.argtypes = [C.POINTER(Proto), C.c_int32, C.c_int32]
         L.ert_oracle_free.argtypes = [C.c_void_p]
         L.ert_oracle_config.restype = C.POINTER(Cfg)
         L.ert_oracle_config.argtypes = [C.c_void_p]
@@ -174,16 +190,37 @@ def bench_threads(msgtypes, chip_length: int, iq, nthreads: int, repeats: int = 
 class Oracle:
     """One protocol.Decoder with its registered parsers (decode.go:65-160)."""
 
-    def __init__(self, msgtypes="scm", chip_length: int = 72, search: int = SEARCH_GO):
-        ids = proto_ids(msgtypes)
-        arr = (C.c_int32 * len(ids))(*ids)
+    def __init__(self, msgtypes="scm", chip_length: int = 72, search: int = SEARCH_GO, _protocols=None):
         self._L = lib()
-        self._h = self._L.ert_oracle_new(arr, len(ids), chip_length, search)
+        if _protocols is None:
+            ids = proto_ids(msgtypes)
+            arr = (C.c_int32 * len(ids))(*ids)
+            self._h = self._L.ert_oracle_new(arr, len(ids), chip_length, search)
+        else:
+            ids = [p.parser for p in _protocols]
+            arr = (Proto * len(ids))(*_protocols)
+            self._h = self._L.ert_oracle_new_protocols(arr, len(ids), search)
         if not self._h:
             raise ValueError("ert_oracle_new failed")
         self.protos = ids
         self.cfg = self._L.ert_oracle_config(self._h).contents
         self.npreambles = self._L.ert_oracle_npreambles(self._h)
+
+    @classmethod
+    def from_protocols(cls, protocols, search: int = SEARCH_GO, parsers=None):
+        """A decoder with the libertgpu protocol structs `protocols` (rtlamr_b200.capi.Protocol) registered in order.
+        parsers[i] is the parser run on protocol i's candidates (an ERT_* id or PARSER_NONE); by default the stock
+        parser of the protocol's name, else the r900 DSP parser for an r900 check, else none."""
+        out = []
+        for i, p in enumerate(protocols):
+            if parsers is not None:
+                parser = parsers[i]
+            else:
+                name = bytes(p.name).split(b"\0")[0].decode()
+                parser = PROTO_NAMES.index(name) if name in PROTO_NAMES else R900 if p.check_kind == CHECK_R900 else PARSER_NONE
+            out.append(Proto(bytes(p.preamble).split(b"\0")[0], p.data_rate, p.chip_length, p.preamble_symbols,
+                             p.packet_symbols, p.center_freq, parser))
+        return cls(search=search, _protocols=out)
 
     def close(self):
         if self._h:
@@ -208,6 +245,8 @@ class Oracle:
         nc, nm = C.c_int32(0), C.c_int32(0)
         rc = self._L.ert_oracle_decode_stream(self._h, iq.ctypes.data, nblocks, cands, cand_cap,
                                               C.byref(nc), msgs, msg_cap, C.byref(nm))
+        if rc == PANIC:
+            raise ReferencePanic("the reference indexes a slice past its length on this input")
         if rc != 0:
             raise OverflowError(f"oracle caps too small: {nc.value} candidates, {nm.value} messages")
         co = [Candidate(c.block, c.idx, c.preamble_id, bytes(c.bytes[:c.nbytes]))

@@ -45,7 +45,7 @@ static const proto_desc PROTO[ERT_NPROTO] = {
 typedef struct {
     uint8_t bits[MAX_PREAMBLE_BITS]; /* numeric 0/1, decode.go:113-118 */
     int32_t nbits;
-    int32_t parsers[ERT_NPROTO]; /* protocol ids sharing this preamble, decode.go:124 */
+    int32_t parsers[ERT_ORACLE_MAX_PROTOS]; /* registration indices sharing this preamble, decode.go:124 */
     int32_t nparsers;
 } preamble_entry;
 
@@ -62,6 +62,7 @@ struct ert_oracle {
     ert_oracle_cfg cfg;
     int32_t search_mode;
     int64_t block; /* number of Decode calls so far */
+    int panicked;  /* the reference indexed past a slice: it has died */
 
     float lut[256];
 
@@ -74,10 +75,11 @@ struct ert_oracle {
     int32_t npkt;
     int32_t *idx_a, *idx_b; /* sIdxA/sIdxB, decode.go:156-157 (sized 8x for the expand step) */
 
-    preamble_entry pre[ERT_NPROTO];
+    preamble_entry pre[ERT_ORACLE_MAX_PROTOS];
     int32_t npre;
 
-    r900_state r900[2]; /* [0]=r900, [1]=r900bcd: each registered parser owns its buffers */
+    int32_t parser[ERT_ORACLE_MAX_PROTOS];   /* ERT_* or ERT_PARSER_NONE, by registration index */
+    r900_state r900[ERT_ORACLE_MAX_PROTOS]; /* by registration index: each registered r900 parser owns its buffers */
 
     uint16_t bch[256];   /* crc.NewTable(0x6F63) */
     uint16_t ccitt[256]; /* crc.NewTable(0x1021) */
@@ -187,33 +189,64 @@ static int32_t next_pow2(int32_t v) {
 
 static int32_t imax(int32_t a, int32_t b) { return a > b ? a : b; }
 
+/* bits of a preamble string in a 33-byte field (MAX_PREAMBLE_BITS + 1 when unterminated) */
+static int32_t preamble_len(const char *s) {
+    int32_t n = 0;
+    while (n <= MAX_PREAMBLE_BITS && s[n]) n++;
+    return n;
+}
+
 /* ------------------------------------------------------------------ */
 /* construction: NewDecoder, RegisterProtocol, Allocate                */
 /* ------------------------------------------------------------------ */
 ert_oracle *ert_oracle_new(const int32_t *protos, int32_t nprotos, int32_t chip_length,
                            int32_t search_mode) {
-    if (!protos || nprotos <= 0 || nprotos > ERT_NPROTO || chip_length <= 0) return NULL;
+    if (!protos || nprotos <= 0 || nprotos > ERT_ORACLE_MAX_PROTOS || chip_length <= 0) return NULL;
+    ert_oracle_proto p[ERT_ORACLE_MAX_PROTOS];
+    memset(p, 0, sizeof(p));
+    for (int i = 0; i < nprotos; i++) {
+        const int32_t id = protos[i];
+        if (id < 0 || id >= ERT_NPROTO) return NULL;
+        const proto_desc *d = &PROTO[id];
+        strcpy(p[i].preamble, d->preamble);
+        p[i].data_rate = d->data_rate;
+        p[i].chip_length = chip_length;
+        p[i].preamble_symbols = d->preamble_symbols;
+        p[i].packet_symbols = d->packet_symbols;
+        p[i].center_freq = d->center_freq;
+        p[i].parser = id;
+    }
+    return ert_oracle_new_protocols(p, nprotos, search_mode);
+}
+
+ert_oracle *ert_oracle_new_protocols(const ert_oracle_proto *protos, int32_t nprotos, int32_t search_mode) {
+    if (!protos || nprotos <= 0 || nprotos > ERT_ORACLE_MAX_PROTOS) return NULL;
+    for (int i = 0; i < nprotos; i++) {
+        const ert_oracle_proto *p = &protos[i];
+        const int32_t n = preamble_len(p->preamble);
+        if (n == 0 || n > MAX_PREAMBLE_BITS || p->chip_length <= 0 || p->preamble_symbols <= 0 ||
+            p->packet_symbols <= 0 || (p->packet_symbols + 7) / 8 > ERT_ORACLE_MAX_PKT ||
+            p->parser < ERT_PARSER_NONE || p->parser >= ERT_NPROTO)
+            return NULL;
+        for (int32_t k = 0; k < n; k++)
+            if (p->preamble[k] != '0' && p->preamble[k] != '1') return NULL;
+    }
     ert_oracle *o = (ert_oracle *)calloc(1, sizeof(*o));
     if (!o) return NULL;
     o->search_mode = search_mode;
 
     /* decode.go:100-128 RegisterProtocol, in the caller's order */
     for (int i = 0; i < nprotos; i++) {
-        int32_t id = protos[i];
-        if (id < 0 || id >= ERT_NPROTO) {
-            free(o);
-            return NULL;
-        }
-        const proto_desc *p = &PROTO[id];
+        const ert_oracle_proto *p = &protos[i];
         o->cfg.center_freq = p->center_freq;                                         /* :105 */
         o->cfg.data_rate = imax(o->cfg.data_rate, p->data_rate);                     /* :106 */
-        o->cfg.chip_length = imax(o->cfg.chip_length, chip_length);                  /* :107 */
+        o->cfg.chip_length = imax(o->cfg.chip_length, p->chip_length);               /* :107 */
         o->cfg.preamble_symbols = imax(o->cfg.preamble_symbols, p->preamble_symbols); /* :108 */
         o->cfg.packet_symbols = imax(o->cfg.packet_symbols, p->packet_symbols);      /* :109 */
 
         preamble_entry e;
         memset(&e, 0, sizeof(e));
-        e.nbits = (int32_t)strlen(p->preamble);
+        e.nbits = preamble_len(p->preamble);
         for (int k = 0; k < e.nbits; k++) e.bits[k] = (uint8_t)(p->preamble[k] == '1'); /* :113-118 */
         int found = -1;
         for (int j = 0; j < o->npre; j++)
@@ -223,9 +256,9 @@ ert_oracle *ert_oracle_new(const int32_t *protos, int32_t nprotos, int32_t chip_
             found = o->npre++;
             o->pre[found] = e;
         }
-        o->pre[found].parsers[o->pre[found].nparsers++] = id; /* :124 */
-        if (id == ERT_R900) o->r900[0].active = 1;
-        if (id == ERT_R900BCD) o->r900[1].active = 1;
+        o->pre[found].parsers[o->pre[found].nparsers++] = i; /* :124 */
+        o->parser[i] = p->parser;
+        if (p->parser == ERT_R900 || p->parser == ERT_R900BCD) o->r900[i].active = 1;
     }
 
     /* decode.go:131-141 Allocate */
@@ -250,7 +283,7 @@ ert_oracle *ert_oracle_new(const int32_t *protos, int32_t nprotos, int32_t chip_
     make_maglut(o->lut);
 
     /* r900.go:161-166 once.Do: buffers sized from the merged decoder config */
-    for (int k = 0; k < 2; k++) {
+    for (int k = 0; k < ERT_ORACLE_MAX_PROTOS; k++) {
         if (!o->r900[k].active) continue;
         o->r900[k].signal = (float *)calloc((size_t)c->buffer_length, sizeof(float));
         o->r900[k].csum = (float *)calloc((size_t)c->buffer_length + 1, sizeof(float));
@@ -271,7 +304,7 @@ void ert_oracle_free(ert_oracle *o) {
     free(o->packed);
     free(o->idx_a);
     free(o->idx_b);
-    for (int k = 0; k < 2; k++) {
+    for (int k = 0; k < ERT_ORACLE_MAX_PROTOS; k++) {
         free(o->r900[k].signal);
         free(o->r900[k].csum);
         free(o->r900[k].quantized);
@@ -317,22 +350,26 @@ void ert_oracle_dsp_only(ert_oracle *o, const uint8_t *input) {
 /* ------------------------------------------------------------------ */
 /* Search: decode.go:255-348                                           */
 /* ------------------------------------------------------------------ */
-static void pack_quantized(ert_oracle *o) {
-    /* :259-265 */
+/* Every index below is checked against the length Go's slice has; past it the reference panics and the search
+ * returns ERT_ORACLE_PANIC without reading. */
+static int32_t pack_quantized(ert_oracle *o) {
+    /* :259-265: d.Quantized[bIdx<<3 : (bIdx+1)<<3] */
+    if ((int64_t)o->npacked * 8 > o->cfg.buffer_length) return ERT_ORACLE_PANIC;
     for (int32_t b = 0; b < o->npacked; b++) {
         uint8_t v = 0;
         for (int k = 0; k < 8; k++) v = (uint8_t)((v << 1) | o->quantized[(b << 3) + k]);
         o->packed[b] = v;
     }
+    return 0;
 }
 
-/* returns number of indices left in o->idx_a */
+/* returns number of indices left in o->idx_a, or ERT_ORACLE_PANIC */
 static int32_t search_go(ert_oracle *o, const preamble_entry *p) {
     const ert_oracle_cfg *c = &o->cfg;
     const int32_t sym_len_byte = c->symbol_length >> 3; /* :256 */
     int32_t *a = o->idx_a, *b = o->idx_b, na = 0, nb = 0;
 
-    pack_quantized(o);
+    if (pack_quantized(o)) return ERT_ORACLE_PANIC;
 
     for (int32_t k = 0; k < p->nbits; k++) {
         uint8_t mask = (uint8_t)((p->bits[k] ^ 1) * 0xFF); /* :270 */
@@ -342,9 +379,12 @@ static int32_t search_go(ert_oracle *o, const preamble_entry *p) {
             for (int32_t qi = 0; qi < (c->block_size >> 3); qi++) /* :277 */
                 if (o->packed[qi] != mask) a[na++] = qi;
         } else {
-            nb = 0; /* searchPassByte :330-338 */
-            for (int32_t j = 0; j < na; j++)
+            nb = 0; /* searchPassByte :330-338 over d.packed[offset:] (:287) */
+            if (offset > o->npacked) return ERT_ORACLE_PANIC;
+            for (int32_t j = 0; j < na; j++) {
+                if (offset + a[j] >= o->npacked) return ERT_ORACLE_PANIC;
                 if (o->packed[offset + a[j]] != mask) b[nb++] = a[j];
+            }
             int32_t *t = a; a = b; b = t; na = nb;
             if (na == 0) return 0; /* :290-292 */
         }
@@ -358,6 +398,8 @@ static int32_t search_go(ert_oracle *o, const preamble_entry *p) {
 
     /* :313-325 exact pass, searchPass :340-348 */
     for (int32_t k = 0; k < p->nbits; k++) {
+        /* d.Quantized[offset : offset+BlockSize] (:315) */
+        if ((int64_t)k * c->symbol_length + c->block_size > c->buffer_length) return ERT_ORACLE_PANIC;
         const uint8_t *sig = o->quantized + k * c->symbol_length;
         nb = 0;
         for (int32_t j = 0; j < na; j++)
@@ -372,11 +414,13 @@ static int32_t search_go(ert_oracle *o, const preamble_entry *p) {
 static int32_t search_exact(ert_oracle *o, const preamble_entry *p) {
     const ert_oracle_cfg *c = &o->cfg;
     int32_t n = 0;
-    pack_quantized(o); /* keeps the `packed` tap identical in both modes */
+    if (pack_quantized(o)) return ERT_ORACLE_PANIC; /* keeps the `packed` tap identical in both modes */
     for (int32_t i = 0; i < c->block_size; i++) {
         int ok = 1;
-        for (int32_t k = 0; k < p->nbits && ok; k++)
+        for (int32_t k = 0; k < p->nbits && ok; k++) {
+            if ((int64_t)i + (int64_t)k * c->symbol_length >= c->buffer_length) return ERT_ORACLE_PANIC;
             ok = o->quantized[i + k * c->symbol_length] == p->bits[k];
+        }
         if (ok) o->idx_a[n++] = i;
     }
     return n;
@@ -559,8 +603,8 @@ static void r900_filter(ert_oracle *o, r900_state *r) {
     }
 }
 
-static void parse_r900(ert_oracle *o, int32_t proto, r900_state *r, const ert_oracle_cand *pk,
-                       int32_t npk, msg_sink *sink) {
+static int32_t parse_r900(ert_oracle *o, int32_t proto, r900_state *r, const ert_oracle_cand *pk,
+                          int32_t npk, msg_sink *sink) {
     const ert_oracle_cfg *c = &o->cfg;
     /* :168-170 slide own history, append the decoder's new magnitudes */
     memmove(r->signal, r->signal + c->block_size, (size_t)(c->buffer_length - c->block_size) * sizeof(float));
@@ -575,6 +619,11 @@ static void parse_r900(ert_oracle *o, int32_t proto, r900_state *r, const ert_or
         uint8_t symbols[21 + 16];
         memset(symbols, 0, sizeof(symbols));
         int bad = 0;
+        /* p.quantized[payloadIdx + 41*4*ChipLength] is the last digit :189-192 reads */
+        if ((int64_t)payload + 41ll * 4 * c->chip_length >= c->buffer_length) {
+            free(seen.keys);
+            return ERT_ORACLE_PANIC;
+        }
         for (int32_t k = 0; k < 21; k++) { /* :188-207: two base-6 digits per symbol */
             int32_t d0 = r->quantized[payload + (2 * k) * 4 * c->chip_length];
             int32_t d1 = r->quantized[payload + (2 * k + 1) * 4 * c->chip_length];
@@ -627,6 +676,7 @@ static void parse_r900(ert_oracle *o, int32_t proto, r900_state *r, const ert_or
         emit(sink, &m);
     }
     free(seen.keys);
+    return 0;
 }
 
 /* ------------------------------------------------------------------ */
@@ -640,6 +690,7 @@ int32_t ert_oracle_decode(ert_oracle *o, const uint8_t *input, ert_oracle_cand *
     int32_t nc = ncands ? *ncands : 0;
     msg_sink sink = {msgs, msg_cap, nmsgs ? *nmsgs : 0, 0};
 
+    if (o->panicked) return ERT_ORACLE_PANIC;
     ert_oracle_dsp_only(o, input);
 
     ert_oracle_cand *local = NULL;
@@ -648,6 +699,10 @@ int32_t ert_oracle_decode(ert_oracle *o, const uint8_t *input, ert_oracle_cand *
     for (int32_t pi = 0; pi < o->npre; pi++) { /* :177 (Go map order is random; ours is fixed) */
         const preamble_entry *p = &o->pre[pi];
         int32_t n = (o->search_mode == ERT_SEARCH_GO) ? search_go(o, p) : search_exact(o, p);
+        if (n < 0) {
+            o->panicked = 1;
+            break;
+        }
 
         if (n > local_cap) {
             local_cap = n;
@@ -658,6 +713,10 @@ int32_t ert_oracle_decode(ert_oracle *o, const uint8_t *input, ert_oracle_cand *
         for (int32_t j = 0; j < n; j++) {
             int32_t qi = o->idx_a[j];
             if (qi > c->block_size) continue; /* :358 */
+            if (qi + (int64_t)(c->packet_symbols - 1) * c->symbol_length >= c->buffer_length) {
+                o->panicked = 1;
+                break;
+            }
             for (int32_t s = 0; s < c->packet_symbols; s++) { /* :363-366, pkt never cleared */
                 o->pkt[s >> 3] = (uint8_t)(o->pkt[s >> 3] << 1);
                 o->pkt[s >> 3] |= o->quantized[qi + s * c->symbol_length];
@@ -670,6 +729,7 @@ int32_t ert_oracle_decode(ert_oracle *o, const uint8_t *input, ert_oracle_cand *
             d->nbytes = o->npkt;
             memcpy(d->bytes, o->pkt, (size_t)o->npkt);
         }
+        if (o->panicked) break;
         for (int32_t j = 0; j < npk; j++) {
             if (cands && nc < cand_cap)
                 cands[nc] = local[j];
@@ -677,21 +737,26 @@ int32_t ert_oracle_decode(ert_oracle *o, const uint8_t *input, ert_oracle_cand *
                 overflow = 1;
             nc++;
         }
-        for (int32_t k = 0; k < p->nparsers; k++) { /* :185-187 */
-            switch (p->parsers[k]) {
+        for (int32_t k = 0; k < p->nparsers && !o->panicked; k++) { /* :185-187 */
+            const int32_t i = p->parsers[k];
+            switch (o->parser[i]) {
             case ERT_SCM: parse_scm(o, local, npk, &sink); break;
             case ERT_SCMPLUS: parse_scmplus(o, local, npk, &sink); break;
             case ERT_IDM: parse_idm_like(o, ERT_IDM, local, npk, &sink); break;
             case ERT_NETIDM: parse_idm_like(o, ERT_NETIDM, local, npk, &sink); break;
-            case ERT_R900: parse_r900(o, ERT_R900, &o->r900[0], local, npk, &sink); break;
-            case ERT_R900BCD: parse_r900(o, ERT_R900BCD, &o->r900[1], local, npk, &sink); break;
+            case ERT_R900:
+            case ERT_R900BCD:
+                if (parse_r900(o, o->parser[i], &o->r900[i], local, npk, &sink)) o->panicked = 1;
+                break;
             }
         }
+        if (o->panicked) break;
     }
     free(local);
     o->block++;
     if (ncands) *ncands = nc;
     if (nmsgs) *nmsgs = sink.n;
+    if (o->panicked) return ERT_ORACLE_PANIC;
     return (overflow || sink.overflow) ? -1 : 0;
 }
 
@@ -699,10 +764,12 @@ int32_t ert_oracle_decode_stream(ert_oracle *o, const uint8_t *input, int64_t nb
                                  ert_oracle_cand *cands, int32_t cand_cap, int32_t *ncands,
                                  ert_oracle_msg *msgs, int32_t msg_cap, int32_t *nmsgs) {
     int32_t rc = 0;
-    for (int64_t b = 0; b < nblocks; b++)
-        if (ert_oracle_decode(o, input + (size_t)b * (size_t)o->cfg.block_size2, cands, cand_cap,
-                              ncands, msgs, msg_cap, nmsgs) != 0)
-            rc = -1;
+    for (int64_t b = 0; b < nblocks; b++) {
+        const int32_t r = ert_oracle_decode(o, input + (size_t)b * (size_t)o->cfg.block_size2, cands, cand_cap,
+                                            ncands, msgs, msg_cap, nmsgs);
+        if (r == ERT_ORACLE_PANIC) return r;
+        if (r != 0) rc = -1;
+    }
     return rc;
 }
 
@@ -727,5 +794,7 @@ const uint8_t *ert_oracle_packed(const ert_oracle *o, int32_t *n) {
 }
 const uint8_t *ert_oracle_r900_quantized(const ert_oracle *o, int32_t *n) {
     if (n) *n = o->cfg.buffer_length;
-    return o->r900[0].active ? o->r900[0].quantized : (o->r900[1].active ? o->r900[1].quantized : NULL);
+    for (int k = 0; k < ERT_ORACLE_MAX_PROTOS; k++)
+        if (o->r900[k].active) return o->r900[k].quantized; /* every r900 parser filters the same signal */
+    return NULL;
 }

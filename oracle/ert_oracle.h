@@ -86,8 +86,26 @@ typedef struct {
 
 typedef struct ert_oracle ert_oracle;
 
-/* NewDecoder + RegisterProtocol for every id in protos[] (in that order) +
- * Allocate (decode.go:65-71,100-128,131-160).  Returns NULL on bad input. */
+#define ERT_ORACLE_MAX_PROTOS 8 /* protocols one decoder registers (ERTGPU_MAX_PROTOCOLS) */
+#define ERT_PARSER_NONE (-1)    /* candidates only: no parser runs on them */
+
+/* One parser's PacketConfig (decode.go:27-42) and the parser that runs on its
+ * candidates: a stock ERT_* parser (ERT_R900 / ERT_R900BCD: the r900 DSP parser,
+ * r900.go:160-245) or ERT_PARSER_NONE. */
+typedef struct {
+    char preamble[33]; /* '0'/'1', 1..32 bits */
+    int32_t data_rate, chip_length;
+    int32_t preamble_symbols, packet_symbols;
+    uint32_t center_freq;
+    int32_t parser;
+} ert_oracle_proto;
+
+/* NewDecoder + RegisterProtocol for every entry of p[] (in that order, merged
+ * per protocol as decode.go:100-128 does, ChipLength included) + Allocate
+ * (decode.go:131-160).  Returns NULL on bad input. */
+ert_oracle *ert_oracle_new_protocols(const ert_oracle_proto *p, int32_t n, int32_t search_mode);
+
+/* The same for the stock parsers protos[] (ERT_* ids), all at one chip length. */
 ert_oracle *ert_oracle_new(const int32_t *protos, int32_t nprotos, int32_t chip_length,
                            int32_t search_mode);
 void ert_oracle_free(ert_oracle *o);
@@ -98,7 +116,12 @@ int32_t ert_oracle_npreambles(const ert_oracle *o);
 /* One Decoder.Decode(input) call (decode.go:163-197) on block_size2 bytes,
  * followed by every registered parser's Parse.  Candidates and messages of
  * this block are appended to the caller's arrays (up to the caps); the
- * return value is 0, or -1 if a cap was hit (counts are still exact). */
+ * return value is 0, or -1 if a cap was hit (counts are still exact), or
+ * ERT_ORACLE_PANIC when the reference would index a slice past its length
+ * here (Search's packing, byte pre-filter or exact pass, Slice, the r900 digit
+ * reads): nothing is read out of bounds, the block's results are incomplete
+ * and every later call returns ERT_ORACLE_PANIC too (the reference has died). */
+#define ERT_ORACLE_PANIC (-2)
 int32_t ert_oracle_decode(ert_oracle *o, const uint8_t *input, ert_oracle_cand *cands,
                           int32_t cand_cap, int32_t *ncands, ert_oracle_msg *msgs,
                           int32_t msg_cap, int32_t *nmsgs);

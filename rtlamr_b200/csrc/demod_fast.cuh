@@ -108,6 +108,17 @@ constexpr int fast_body_len(int CL) {
     return L;
 }
 
+// The fast kernel reads two bodies of L samples from one block (a shorter block: PreambleSymbols = 1 at chip length 32,
+// 56 or 64) ...
+constexpr bool fast_block_fits(int L, int BS) { return 2 * L <= BS; }
+// ... and a lead-in of 2L samples from the history of PacketLength samples, with bulk copies from 2*PacketLength - 4L
+// bytes into the history, which must be 16-byte aligned (a shorter packet: PacketSymbols = 1; PacketLength % 8 != 0: an
+// odd PacketSymbols at chip length 78).  Geometries that do not fit take demod_generic_kernel.
+constexpr bool fast_history_fits(int L, int PacketLength) { return PacketLength >= 2 * L && PacketLength % 8 == 0; }
+constexpr bool fast_geometry_fits(int L, int BS, int PacketLength) {
+    return fast_block_fits(L, BS) && fast_history_fits(L, PacketLength);
+}
+
 template <int CL>
 struct FastGeom {
     static constexpr int L = fast_body_len(CL);
@@ -505,7 +516,7 @@ int launch_demod_fast_cw(const uint8_t* iq, const uint8_t* hist, int hist_sample
             if (e != cudaSuccess) return (int)e;
         }
     }
-    if (2 * G::kRowBytes > 2 * BS || hist_samples < 2 * G::L) return (int)cudaErrorInvalidValue;
+    if (!fast_geometry_fits(G::L, BS, hist_samples)) return (int)cudaErrorInvalidValue;
     // the IQ bytes of the call as a 2D uint8 tensor: [nblocks rows][BlockSize2 bytes]
     EncodeTiledFn enc = encode_tiled_fn();
     if (!enc) return (int)cudaErrorNotSupported;
@@ -542,12 +553,18 @@ int launch_demod_fast_cw(const uint8_t* iq, const uint8_t* hist, int hist_sample
 // chip lengths with a specialised kernel: every value the reference CLI accepts (flags.go:127-132
 // allows 8,32,40,...,96) except 8, plus 78, the rate the reference's sample.bin fixture was captured at
 // (nothing in the kernel needs CL to be a multiple of 8: only L is).  Anything else uses the generic kernel.
+// Two arguments: the instance of a chip length and block size (fast_block_fits), whatever the packet.
 inline int demod_fast_variant(int CL, int BS) {
-    (void)BS;
     switch (CL) {
-        case 32: case 40: case 48: case 56: case 64: case 72: case 78: case 80: case 88: case 96: return CL;
+        case 32: case 40: case 48: case 56: case 64: case 72: case 78: case 80: case 88: case 96:
+            return fast_block_fits(fast_body_len(CL), BS) ? CL : 0;
         default: return 0;
     }
+}
+// The instance a decoder runs: the same, if its packet length also gives the lead-in history (fast_history_fits).
+inline int demod_fast_variant(int CL, int BS, int PacketLength) {
+    const int v = demod_fast_variant(CL, BS);
+    return v != 0 && fast_history_fits(fast_body_len(CL), PacketLength) ? v : 0;
 }
 
 inline int launch_demod_fast(int variant, const uint8_t* iq, const uint8_t* hist, int hist_samples,

@@ -167,6 +167,39 @@ void make_gf32(Gf32* g) {
     g->log[0] = 31;
 }
 
+// The merged configurations the reference decodes: every index it takes for a candidate lies inside what it computed
+// for that candidate (include/ertgpu.h, ertgpu_allocate).  Anything else is ERTGPU_EINVAL, naming the rule.
+int check_decodable(ertgpu_handle* h) {
+    const ertgpu_decoder_config& c = h->cfg;
+    const int64_t BS = c.block_size, PL = c.preamble_length, SL = c.symbol_length, CL = c.chip_length;
+    const int64_t PS = c.preamble_symbols, PK = c.packet_symbols, BUF = c.buffer_length;
+    const int64_t npacked = (BS + PL + 7) >> 3;  // len(d.packed), decode.go:159
+    // R1: Search packs d.packed from Quantized[8*i : 8*i+8] (decode.go:259-265)
+    if (8 * npacked > BUF)
+        return fail(h, ERTGPU_EINVAL, "R1: Search packs %lld Quantized bits of %lld (PreambleSymbols %lld, PacketSymbols %lld)",
+                    (long long)(8 * npacked), (long long)BUF, (long long)PS, (long long)PK);
+    bool r900 = false;
+    for (const ertgpu_protocol& p : h->protos) {
+        const int64_t n = (int64_t)strnlen(p.preamble, sizeof(p.preamble));
+        // R2: the exact pass reads Quantized[(n-1)*SL : (n-1)*SL + BS] (decode.go:313-318), the byte pre-filter
+        // d.packed[(n-1)*(SL>>3) + BS/8 - 1] (decode.go:268-287)
+        if (n - 1 > PK || (n - 1) * (SL >> 3) + BS / 8 > npacked)
+            return fail(h, ERTGPU_EINVAL, "R2: the Search of the %lld-bit preamble %s reads past Quantized (PacketSymbols %lld)",
+                        (long long)n, p.preamble, (long long)PK);
+        r900 = r900 || p.check_kind == ERTGPU_CHECK_R900;
+        // R4: the partial last byte holds the previous candidate's bits in the reference (decode.go:363-366)
+        if (p.check_kind == ERTGPU_CHECK_CRC16 && (PK & 7) && p.crc_from <= (PK >> 3) && (PK >> 3) < p.crc_to)
+            return fail(h, ERTGPU_EINVAL, "R4: CRC range [%d, %d) of %.16s holds the partial last byte %lld (PacketSymbols %lld)",
+                        p.crc_from, p.crc_to, p.name, (long long)(PK >> 3), (long long)PK);
+    }
+    // R3: the last r900 payload digit (r900.go:187-193) lies below BufferLength - 4*ChipLength, the last position the
+    // r900 filter writes (r900.go:117): PacketSymbols >= PreambleSymbols + 83
+    if (r900 && BS - 1 + PL - SL + 4 * (ERTGPU_R900_DIGITS - 1) * CL >= BUF - 4 * CL)
+        return fail(h, ERTGPU_EINVAL, "R3: r900 payload digits need PacketSymbols >= PreambleSymbols + 83 (%lld < %lld)",
+                    (long long)PK, (long long)(PS + 83));
+    return ERTGPU_OK;
+}
+
 void free_device(ertgpu_handle* h) {
     if (!h->allocated) return;
     cudaSetDevice(h->device);
@@ -701,6 +734,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     c.buffer_length = c.packet_length + c.block_size;
     c.packet_bytes = (c.packet_symbols + 7) >> 3;
     if (c.block_size < 32) return fail(h, ERTGPU_EINVAL, "block size %d below 32", c.block_size);
+    if (const int rc = check_decodable(h)) return rc;
 
     DevCfg& d = h->dcfg;
     memset(&d, 0, sizeof(d));
@@ -780,9 +814,9 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     // Slack behind the largest call's words, for the Search kernels' reads past the call's last word:
     //  * search_slide_kernel's last tile starts at a word below nwords and loads load_words <= kSlideMaxLoad words;
     //  * search_generic_kernel (and extract_words_kernel) read the word under plane bit p0 + 32*w + k*SL and the next
-    //    one, w < nwords; with p0 + PKL = 32*hist_words that stays inside the call's words while k < PK.  Only a
-    //    preamble longer than the packet, which the ABI allows, reads past them: 1 + (nbits - 1 - PK)*SL/32 words,
-    //    at most 1696 (32 bits, PK = 1, SL = 1808 at chip length 904, the largest demod_generic_kernel takes).
+    //    one, w < nwords; with p0 + PKL = 32*hist_words the bits they use lie inside the call's words while k <= PK
+    //    (the next word may be the first one behind them).  Rule R2 (check_decodable) keeps every preamble at most
+    //    PK + 1 bits long, so no Search result depends on bits past the call's words.
     h->plane_words = (size_t)d.hist_words + (size_t)max_blocks_per_call * d.words_per_block + kSlideMaxLoad + 8;
     for (int k = 0; k < 2; k++) {
         CUDA_TRY(h, cudaMalloc(&h->d_plane[k], h->plane_words * sizeof(uint32_t)));
@@ -819,7 +853,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     h->tap_floats = (size_t)std::max(d.BS + d.SL, d.BUF) * 2 + 16;
     CUDA_TRY(h, cudaMalloc(&h->d_tap, h->tap_floats * sizeof(float)));
 
-    h->demod_variant = demod_fast_variant(d.CL, d.BS);
+    h->demod_variant = demod_fast_variant(d.CL, d.BS, d.PKL);
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->device);
     if (h->sm_count < 1) h->sm_count = 132;
 
@@ -946,7 +980,7 @@ int ertgpu_get_resampler(const ertgpu_handle* h, ertgpu_resampler_info* info, in
 int ertgpu_set_demod_variant(ertgpu_handle* h, int32_t variant) {
     // test hook: 0 forces the generic kernel, -1 restores the automatic choice
     if (!h || !h->allocated) return ERTGPU_EINVAL;
-    if (variant < 0) h->demod_variant = demod_fast_variant(h->dcfg.CL, h->dcfg.BS);
+    if (variant < 0) h->demod_variant = demod_fast_variant(h->dcfg.CL, h->dcfg.BS, h->dcfg.PKL);
     else if (variant == 0) h->demod_variant = 0;
     else return ERTGPU_EINVAL;
     return ERTGPU_OK;

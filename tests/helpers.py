@@ -40,23 +40,31 @@ def synth_stream(msgtypes, cl, nsamples, seed=0x5EED0001, spacing=1 << 19, pkt_s
 
 
 # ---- the integrity screens, restated with the oracle's own crc/gf functions (crc/crc.go, r900/gf/gf.go) ----
-def screen_expected(proto_name: str, data: bytes, digits=None) -> bool:
-    """What bit i of check_mask must be for a candidate filed under parser `proto_name`:
-    scm/scm.go:76, scmplus/scmplus.go:77, idm/idm.go:77-87, netidm/netidm.go:88-98, r900/r900.go:199-221."""
-    if proto_name == "scm":
+def screen_expected(proto, data: bytes, digits=None) -> bool:
+    """What bit i of check_mask must be for a candidate filed under parser `proto` (a stock name or a capi.Protocol):
+    scm/scm.go:76, scmplus/scmplus.go:77, idm/idm.go:77-87, netidm/netidm.go:88-98, r900/r900.go:199-221; a protocol
+    struct's own CRC16 (init, polynomial, residue over bytes [crc_from, crc_to)) or ERTGPU_CHECK_NONE (always set)."""
+    if not isinstance(proto, str):
+        kind = proto.check_kind
+        if kind == capi.CHECK_NONE:
+            return True
+        if kind == capi.CHECK_CRC16:
+            return oracle.crc_checksum(proto.crc_init, data[proto.crc_from:proto.crc_to], proto.crc_poly) == proto.crc_residue
+        proto = {capi.CHECK_IDM: "idm", capi.CHECK_R900: "r900"}[kind]
+    if proto == "scm":
         return oracle.crc_checksum(0, data[2:12], 0x6F63) == 0
-    if proto_name == "scm+":
+    if proto == "scm+":
         return oracle.crc_checksum(0xFFFF, data[2:16], 0x1021) == 0x1D0F
-    if proto_name in ("idm", "netidm"):
+    if proto in ("idm", "netidm"):
         return (oracle.crc_checksum(0xFFFF, data[4:92], 0x1021) == 0x1D0F
                 and oracle.crc_checksum(0xFFFF, data[9:13] + data[88:90], 0x1021) == 0x1D0F)
-    if proto_name in ("r900", "r900bcd"):
+    if proto in ("r900", "r900bcd"):
         sym = [digits[2 * k] * 6 + digits[2 * k + 1] for k in range(21)]
         if max(sym) > 31:
             return False
         msg = bytes(sym[:16]) + bytes(10) + bytes(sym[16:])
         return oracle.gf32_syndrome(msg, 5, 29) == bytes(5)
-    raise ValueError(proto_name)
+    raise ValueError(proto)
 
 
 PREAMBLES = {"scm": "111110010101001100000", "scm+": "0001011010100011", "idm": "01010101010101010001011010100011",
@@ -150,26 +158,94 @@ def compare_r900_digits(got, msgtypes, want):
     return len(keys), fails
 
 
+def preamble_of(proto) -> str:
+    """The preamble of a stock name or a capi.Protocol."""
+    return PREAMBLES[proto] if isinstance(proto, str) else bytes(proto.preamble).split(b"\0")[0].decode()
+
+
+def _is_r900(proto) -> bool:
+    return proto in ("r900", "r900bcd") if isinstance(proto, str) else proto.check_kind == capi.CHECK_R900
+
+
 def assert_check_masks_exact(got, msgtypes):
     """BOTH directions: bit i of check_mask is set iff the candidate is filed under parser i's preamble and
-    passes that parser's integrity check (recomputed here from the returned bytes / digits)."""
+    passes that parser's integrity check (recomputed here from the returned bytes / digits).  msgtypes: stock names
+    or capi.Protocol structs, in registration order."""
     if isinstance(msgtypes, str):
         msgtypes = [m.strip() for m in msgtypes.split(",") if m.strip()]
-    pre_ids, order = {}, []
+    pre_ids, order = [], []
     for m in msgtypes:          # distinct preambles in registration order (decode.go:121-124)
-        if PREAMBLES[m] not in order:
-            order.append(PREAMBLES[m])
-        pre_ids[m] = order.index(PREAMBLES[m])
+        if preamble_of(m) not in order:
+            order.append(preamble_of(m))
+        pre_ids.append(order.index(preamble_of(m)))
     cache = {}
     for r in got:
         data, dig, pid = r["bytes"].tobytes(), r["r900_digits"].tobytes(), int(r["preamble_id"])
         want = 0
         for i, m in enumerate(msgtypes):
-            if pre_ids[m] != pid:
+            if pre_ids[i] != pid:
                 continue
-            key = (m, data if m not in ("r900", "r900bcd") else dig)
+            key = (i, data if not _is_r900(m) else dig)
             if key not in cache:
                 cache[key] = screen_expected(m, data, list(dig))
             if cache[key]:
                 want |= 1 << i
         assert int(r["check_mask"]) == want, (int(r["block"]), int(r["idx"]), pid, int(r["check_mask"]), want)
+
+
+# ---- custom protocol configurations (ertgpu_protocol) and the rules ertgpu_allocate applies to them ----
+def make_protocol(preamble, cl, ps, pk, check=capi.CHECK_NONE, crc=(0xFFFF, 0x1021, 0x1D0F), crc_range=(0, 0),
+                  name="custom"):
+    """A capi.Protocol: `preamble` a '0'/'1' string, ChipLength cl, PreambleSymbols ps, PacketSymbols pk, a check kind
+    and, for CHECK_CRC16 / CHECK_IDM, (init, polynomial, residue) over bytes [crc_range)."""
+    p = capi.Protocol()
+    p.name, p.preamble = name.encode(), preamble.encode()
+    p.data_rate, p.chip_length, p.preamble_symbols, p.packet_symbols = 32768, cl, ps, pk
+    p.center_freq, p.check_kind = 912600155, check
+    p.crc_init, p.crc_poly, p.crc_residue = crc
+    p.crc_from, p.crc_to = crc_range
+    return p
+
+
+def merged_geometry(protos):
+    """Decoder.Cfg after RegisterProtocol of every protocol and Allocate (decode.go:100-141)."""
+    cl = max(p.chip_length for p in protos)
+    ps = max(p.preamble_symbols for p in protos)
+    pk = max(p.packet_symbols for p in protos)
+    sl = 2 * cl
+    pl, pkl = ps * sl, pk * sl
+    bs = 1 << max(0, (pl - 1).bit_length())
+    return {"CL": cl, "SL": sl, "PS": ps, "PK": pk, "PL": pl, "PKL": pkl, "BS": bs, "BUF": pkl + bs}
+
+
+def rule_violated(protos):
+    """The first rule of ertgpu_allocate (include/ertgpu.h) the merged configuration breaks, in the order the library
+    checks them ("BS": block size below 32, then R1, R2 / R4 per protocol in registration order, R3), or None."""
+    g = merged_geometry(protos)
+    BS, PL, SL, CL, PS, PK, BUF = g["BS"], g["PL"], g["SL"], g["CL"], g["PS"], g["PK"], g["BUF"]
+    if BS < 32:
+        return "BS"
+    npacked = -(-(BS + PL) // 8)
+    if 8 * npacked > BUF:
+        return "R1"
+    for p in protos:
+        n = len(preamble_of(p))
+        if n - 1 > PK or (n - 1) * (SL >> 3) + BS // 8 > npacked:
+            return "R2"
+        if p.check_kind == capi.CHECK_CRC16 and PK % 8 and p.crc_from <= PK >> 3 < p.crc_to:
+            return "R4"
+    if any(p.check_kind == capi.CHECK_R900 for p in protos) and BS - 1 + PL - SL + 164 * CL >= BUF - 4 * CL:
+        return "R3"
+    return None
+
+
+def allocate_verdict(protos, max_blocks=1, max_cands=1):
+    """(return code of ertgpu_allocate, its message) for the protocols registered in order; never decodes."""
+    h = capi.Handle()
+    try:
+        for p in protos:
+            h.register(p)
+        rc = h._L.ertgpu_allocate(h._h, 0, max_blocks, max_cands)
+        return rc, (h._L.ertgpu_last_error(h._h) or b"").decode()
+    finally:
+        h.close()
