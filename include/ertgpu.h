@@ -142,6 +142,16 @@ typedef struct {
     int32_t F;  /* bits of the sub-phase interpolation weight   */
 } ertgpu_resampler_info;
 
+/* The first stage of a decimating tuned handle (ertgpu_allow_input_decimation; include/ertgpu_resample.h has the
+ * arithmetic): mix, lowpass and keep every D-th sample, R_in -> R_mid = R_in / D.  D = 1 means no first stage. */
+typedef struct {
+    int64_t rate_in, rate_out; /* the capture's rate and the decoder's rate R_out             */
+    int32_t D;                 /* decimation of the first stage                              */
+    int32_t T1;                /* its taps (0 when D = 1)                                    */
+    int32_t S;                 /* the taps sum to 2^S                                        */
+    int32_t reserved;
+} ertgpu_decimator_info;
+
 /* The tuning of a handle (ertgpu_set_input_tuning; include/ertgpu_resample.h has the arithmetic). */
 typedef struct {
     int64_t capture_center_hz; /* the frequency at the centre of the capture                    */
@@ -207,7 +217,8 @@ int ertgpu_reset(ertgpu_handle *h);
  * R_out = DataRate * ChipLength (and its geometry, blocks, Idx and taps); when hz != R_out the
  * input is converted to R_out by an exact integer resampler on the GPU, and Block / Idx refer to
  * the resampled stream.  hz == R_out (or never calling this) changes nothing.  R_out / hz must
- * lie in [1/4, 4] ([1/10, 4] on a handle tuned by ertgpu_set_input_tuning), otherwise ERTGPU_EINVAL.  With resampling, ertgpu_decode and
+ * lie in [1/4, 4] ([1/10, 4] on a handle tuned by ertgpu_set_input_tuning, [1/256, 4] on one that also called
+ * ertgpu_allow_input_decimation), otherwise ERTGPU_EINVAL.  With resampling, ertgpu_decode and
  * ertgpu_decode_device_async take any whole number of IQ samples (nbytes even, else
  * ERTGPU_ESIZE): the handle carries the input history, the outputs still waiting for look-ahead
  * and the partial output block across calls and decodes every whole block it has.
@@ -229,6 +240,23 @@ int ertgpu_set_input_rate(ertgpu_handle *h, int64_t hz);
  * ERTGPU_TAP_RESAMPLED returns the mixed and filtered bytes; ertgpu_decode_sharded rejects tuned
  * handles.  Several channels of one capture are several handles fed the same bytes. */
 int ertgpu_set_input_tuning(ertgpu_handle *h, int64_t capture_center_hz, int64_t center_hz);
+
+/* Let a tuned handle take captures at up to 256 times the decoder's rate R_out.  Call it after
+ * ertgpu_set_input_tuning and before ertgpu_set_input_rate and ertgpu_allocate; otherwise, and on an untuned handle,
+ * ERTGPU_EINVAL.  Up to 10:1 nothing changes: the handle runs the tuned resampler alone, with the same plan, bytes and
+ * kernels.  Above 10:1, up to 256:1, the input goes through two stages on the GPU (include/ertgpu_resample.h):
+ * decimate_kernel mixes the channel to 0 Hz, lowpasses and keeps every D-th sample, D = ceil(R_in / (4 R_out)), and the
+ * untuned uint8 resample_kernel takes R_mid = R_in / D to R_out.  The channel must lie inside the capture,
+ * |offset| + 0.4 R_out <= 0.5 R_in.  ertgpu_last_kernels names both kernels (demod first, decimate_kernel<F> and
+ * resample_kernel<cu8> last), ERTGPU_TAP_RESAMPLED returns the bytes at R_out, ertgpu_get_resampler describes the
+ * second stage and ertgpu_reset restarts both and the mixer's phase. */
+int ertgpu_allow_input_decimation(ertgpu_handle *h);
+
+/* The first stage of a handle that allows decimation, once its rate is known (after ertgpu_set_input_rate, or after
+ * ertgpu_allocate at the decoder's own rate): *info, and the T1 int16 taps when taps != NULL and cap (entries) is
+ * large enough; *n_out = T1.  D = 1 and T1 = 0 when the handle does not decimate.  ERTGPU_EINVAL otherwise. */
+int ertgpu_get_decimator(const ertgpu_handle *h, ertgpu_decimator_info *info, int16_t *taps, size_t cap,
+                         size_t *n_out);
 
 /* The tuning of a handle; ERTGPU_EINVAL when ertgpu_set_input_tuning was not called. */
 int ertgpu_get_tuning(const ertgpu_handle *h, ertgpu_tuning_info *info);

@@ -37,6 +37,7 @@
 #define ERTRS_NCO_BITS 12 /* log2 of the entries of the mixer table E     */
 #define ERTRS_NCO_N (1 << ERTRS_NCO_BITS)
 #define ERTRS_E_S 14      /* |E[k]| ~ 2^E_S                                */
+#define ERTRS_MAX_D 64    /* largest stage-1 decimation (R_in <= 256 R_out) */
 
 static inline int64_t ertrs_gcd(int64_t a, int64_t b) {
     while (b) {
@@ -131,6 +132,74 @@ static inline int ertrs_plan_tuned(int64_t rate_in, int64_t rate_out, int64_t of
     if (ad > rate_in || 10 * ad + 4 * lo > 5 * rate_in) return -1;
     ertrs_fill_plan(rate_in, rate_out, info);
     info->P = info->T <= 96 ? 256 : info->T <= 160 ? 128 : 64;
+    return 0;
+}
+
+/*
+ * Decimating tuned input (ertgpu_allow_input_decimation): above 10:1 the channel goes through two stages.
+ *   Stage 1 mixes and decimates by D: the tuned formula above with L = 1, M = D and a single table row, so every output
+ *     has phase 0 and no coefficient is interpolated.  Output n reads the T1 mixed samples s' at nD - T1/2 + 1 ...
+ *     nD + T1/2 (s' = 0 before the stream start):  u_mid = clamp((sum_t h_t s'_t + 2^(S+8)) >> (S+1), 0, 255).
+ *     h is a Kaiser-windowed (70 dB) sinc with its passband edge at 0.4 R_out, its stopband edge at R_mid - 0.6 R_out
+ *     and the cut-off midway, R_mid = R_in / D; T1 (even) is the Kaiser estimate for that transition band.  The int16
+ *     taps are symmetric about tap T1/2 - 1 (h_t = h_{T1-2-t}, h_{T1-1} = 0) and sum to exactly 2^S (the residual goes
+ *     to the centre tap).
+ *   Stage 2 is the untuned uint8 resampler of ertrs_fill_plan(R_in, D * R_out): the same L/M, T and table as
+ *     R_mid -> R_out, fed with the stage-1 bytes.
+ */
+
+/* The plan of a handle that allows decimation.  R_in <= 10 R_out: D = 1, T1 = 0 and *info is ertrs_plan_tuned's.
+ * 10 R_out < R_in <= 256 R_out: D = ceil(R_in / (4 R_out)) (so 3 R_out < R_mid <= 4 R_out), the channel inside the
+ * capture (|offset| + 0.4 R_out <= 0.5 R_in), and *info the second stage's plan.  Returns 0 or -1. */
+static inline int ertrs_plan_decimated(int64_t rate_in, int64_t rate_out, int64_t offset_hz, ertgpu_decimator_info* dec,
+                                       ertgpu_resampler_info* info) {
+    if (rate_in <= 0 || rate_out <= 0) return -1;
+    dec->rate_in = rate_in;
+    dec->rate_out = rate_out;
+    dec->S = ERTRS_S;
+    dec->reserved = 0;
+    if (rate_in <= 10 * rate_out) {
+        dec->D = 1;
+        dec->T1 = 0;
+        return ertrs_plan_tuned(rate_in, rate_out, offset_hz, info);
+    }
+    if (rate_in > ERTRS_MAX_D * 4 * rate_out) return -1;
+    const int64_t ad = offset_hz < 0 ? -offset_hz : offset_hz;
+    if (10 * ad + 4 * rate_out > 5 * rate_in) return -1;
+    const int64_t D = (rate_in + 4 * rate_out - 1) / (4 * rate_out);
+    const double width = ((double)rate_in / (double)D - (double)rate_out) / (double)rate_in; /* cycles per input sample */
+    const double n = (ERTRS_ATTEN_DB - 7.95) / (14.36 * width);
+    int32_t T1 = 2 * (int32_t)((n + 1.999999) / 2.0);
+    if (T1 < 8) T1 = 8;
+    dec->D = (int32_t)D;
+    dec->T1 = T1;
+    ertrs_fill_plan(rate_in, D * rate_out, info);
+    return 0;
+}
+
+/* The stage-1 taps h_0 .. h_{T1-1} of a plan with D >= 2.  Returns 0, or -1 if a tap does not fit int16. */
+static inline int ertrs_build_decimator(const ertgpu_decimator_info* dec, int16_t* taps) {
+    const int32_t T1 = dec->T1, c = T1 / 2 - 1;
+    const double half = 0.5 * (double)T1;
+    const double mid = (double)dec->rate_in / (double)dec->D;
+    const double fc = 0.5 * (mid - 0.2 * (double)dec->rate_out) / (double)dec->rate_in; /* cycles per input sample */
+    const double beta = 0.1102 * (ERTRS_ATTEN_DB - 8.7);
+    int64_t sum = 0;
+    for (int32_t t = 0; t <= c; t++) { /* d = t - c <= 0; the other half mirrors it */
+        const double d = (double)(t - c), z = d / half;
+        const double w = ertrs_i0(beta * __builtin_sqrt(1.0 - z * z)) / ertrs_i0(beta);
+        const double x = 2.0 * fc * d;
+        const double sinc = x == 0.0 ? 1.0 : ertrs_sinpi(x) / (3.14159265358979323846 * x);
+        const double v = (double)(1 << dec->S) * 2.0 * fc * sinc * w;
+        const double r = v >= 0 ? (double)(int64_t)(v + 0.5) : -(double)(int64_t)(-v + 0.5);
+        if (r > 32767.0 || r < -32768.0) return -1;
+        taps[t] = taps[T1 - 2 - t] = (int16_t)r;
+        sum += t == c ? (int64_t)taps[t] : 2 * (int64_t)taps[t];
+    }
+    taps[T1 - 1] = 0;
+    const int64_t cc = taps[c] + ((1 << dec->S) - sum);
+    if (cc > 32767 || cc < -32768) return -1;
+    taps[c] = (int16_t)cc;
     return 0;
 }
 

@@ -58,6 +58,11 @@ class ResamplerInfo(C.Structure):
                 ("T", C.c_int32), ("P", C.c_int32), ("S", C.c_int32), ("F", C.c_int32)]
 
 
+class DecimatorInfo(C.Structure):
+    _fields_ = [("rate_in", C.c_int64), ("rate_out", C.c_int64), ("D", C.c_int32), ("T1", C.c_int32), ("S", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 class TuningInfo(C.Structure):
     _fields_ = [("capture_center_hz", C.c_int64), ("center_hz", C.c_int64), ("offset_hz", C.c_int64),
                 ("nco_step", C.c_uint32), ("nco_bits", C.c_int32)]
@@ -95,6 +100,7 @@ EXPORTS = [
     "ertgpu_bind_host_thread", "ertgpu_last_kernels", "ertgpu_plan_shards", "ertgpu_decode_sharded",
     "ertgpu_set_input_rate", "ertgpu_get_resampler", "ertgpu_set_input_format", "ertgpu_get_input_format",
     "ertgpu_set_input_tuning", "ertgpu_get_tuning", "ertgpu_measure_input", "ertgpu_set_input_scale",
+    "ertgpu_allow_input_decimation", "ertgpu_get_decimator",
 ]
 
 _lib = None
@@ -155,6 +161,8 @@ def lib() -> C.CDLL:
     L.ertgpu_get_tuning.argtypes = [vp, C.POINTER(TuningInfo)]
     L.ertgpu_measure_input.argtypes = [vp, vp, sz, C.POINTER(InputLevel)]
     L.ertgpu_set_input_scale.argtypes = [vp, C.c_float]
+    L.ertgpu_allow_input_decimation.argtypes = [vp]
+    L.ertgpu_get_decimator.argtypes = [vp, C.POINTER(DecimatorInfo), vp, sz, C.POINTER(sz)]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the library does not export it
     _lib = L
@@ -204,6 +212,19 @@ class Handle:
         """ertgpu_set_input_tuning: the IQ was recorded centred at capture_hz; decode the channel at center_hz (0: the
         decoder's CenterFreq).  After the protocols, before the rate and allocate."""
         self._check(self._L.ertgpu_set_input_tuning(self._h, int(capture_hz), int(center_hz)))
+
+    def allow_input_decimation(self):
+        """ertgpu_allow_input_decimation: a tuned handle may take captures at up to 256 times the decoder's rate (after
+        the tuning, before the rate and allocate)."""
+        self._check(self._L.ertgpu_allow_input_decimation(self._h))
+
+    def decimator(self):
+        """ertgpu_get_decimator: (info dict, int16 taps of the first stage, T1 entries)."""
+        info, n = DecimatorInfo(), C.c_size_t(0)
+        self._check(self._L.ertgpu_get_decimator(self._h, C.byref(info), None, 0, C.byref(n)))
+        taps = np.zeros(n.value, dtype=np.int16)
+        self._check(self._L.ertgpu_get_decimator(self._h, C.byref(info), taps.ctypes.data, taps.size, C.byref(n)))
+        return {k: getattr(info, k) for k, _ in DecimatorInfo._fields_}, taps
 
     def tuning(self):
         """ertgpu_get_tuning as a dict."""
@@ -342,7 +363,8 @@ def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per
     (reference main.go:64-86).  input_rate > 0: the IQ is sampled at that rate (ertgpu_set_input_rate);
     input_format / input_scale: its sample format and gain (ertgpu_set_input_format, not called for plain cu8);
     capture_freq > 0: the IQ was recorded centred there, and the channel at center_freq (0: the protocols'
-    CenterFreq) is decoded (ertgpu_set_input_tuning, before the rate)."""
+    CenterFreq) is decoded (ertgpu_set_input_tuning, before the rate), at up to 256 times the decoder's rate
+    (ertgpu_allow_input_decimation)."""
     if isinstance(msgtypes, str):
         msgtypes = [m.strip() for m in msgtypes.split(",") if m.strip()]
     h = Handle()
@@ -350,6 +372,7 @@ def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per
         h.register(stock_protocol(m, chip_length))
     if capture_freq or center_freq:
         h.set_input_tuning(capture_freq, center_freq)
+        h.allow_input_decimation()
     if input_rate:
         h.set_input_rate(input_rate)
     if input_format != FORMAT_CU8 or input_scale:

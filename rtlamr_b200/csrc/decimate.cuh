@@ -1,0 +1,126 @@
+// Stage 1 of a decimating tuned input (ertgpu_allow_input_decimation): IQ at R_in -> uint8 IQ at R_mid = R_in / D,
+// the channel mixed to 0 Hz and lowpassed on the way, as include/ertgpu_resample.h states it (all integer).  The
+// untuned uint8 resample_kernel (resample.cuh) then takes R_mid to R_out.  Input of another format (convert.cuh) is
+// converted to uint8 as it is staged, exactly as resample_kernel does.
+#pragma once
+
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "../../include/ertgpu_resample.h"
+#include "convert.cuh"
+
+namespace ert {
+
+constexpr int kDcThreads = 256;
+constexpr int kDcSpanWords = 20480;  // most input samples one tile stages (80 KiB, so that two CTAs fit an SM)
+constexpr int kDcMaxPer = 16;        // most outputs per thread and tile
+
+struct DcArgs {
+    // input samples [hist_first, hist_first + hist_n) are in hist (uint8), the next cur_n ones in cur (the handle's format)
+    const uint8_t* hist;
+    const uint8_t* cur;
+    long long hist_first, hist_n, cur_n;
+    // outputs [n0, n0 + count): output n0 + i goes to out[2i..2i+1]
+    long long n0, count;
+    uint8_t* out;
+    // input samples [carry_first, carry_first + carry_n) are copied to carry_dst (the next call's history)
+    uint8_t* carry_dst;
+    long long carry_first, carry_n;
+    int D, T1;
+    int per;      // outputs of a thread per tile: a tile is kDcThreads * per outputs
+    float scale;  // g of the input format (not read for uint8 input)
+    const uint32_t* E;  // the mixer table (ertrs_nco_table) and its step W at R_in
+    uint32_t W;
+};
+
+// Outputs a thread computes per tile, so that a tile's input span, (kDcThreads * per - 1) * D + T1 samples, fits
+// kDcSpanWords (for every D <= ERTRS_MAX_D).
+inline int dc_per_thread(int D, int T1) {
+    const int per = (kDcSpanWords - T1) / (kDcThreads * D);
+    return per < 1 ? 1 : per > kDcMaxPer ? kDcMaxPer : per;
+}
+
+// Staged word i sits at i + i / 32: lanes that read words D apart then hit different banks for every D <= 32.
+__device__ __forceinline__ int dc_skew(int i) { return i + (i >> 5); }
+
+// Shared memory of one CTA: E, the taps h_0 .. h_{T1/2-1} as int32 and the skewed span of the largest tile.
+inline size_t dc_smem_bytes(int D, int T1, int per) {
+    const long long span = ((long long)kDcThreads * per - 1) * D + T1;
+    return ((size_t)ERTRS_NCO_N + (size_t)(T1 / 2) + (size_t)(span + (span >> 5) + 1)) * 4;
+}
+
+// Input sample g as uint8 IQ: from the history as it is, from cur converted from format F.
+template <int F>
+__device__ __forceinline__ uchar2 dc_input(const DcArgs& a, long long g) {  // g >= 0
+    const long long e = a.hist_first + a.hist_n;
+    if (g < e) return *reinterpret_cast<const uchar2*>(a.hist + 2 * (g - a.hist_first));
+    if constexpr (F == ERTGPU_FORMAT_CU8) return *reinterpret_cast<const uchar2*>(a.cur + 2 * (g - e));
+    else return fmt_sample<F>(a.cur, g - e, a.scale);
+}
+
+// Persistent grid over tiles of kDcThreads * per outputs.  Each CTA keeps E and the taps in shared memory and stages a
+// tile's input span once, each sample mixed by E[k_g] into one word of int16 s'_I | s'_Q << 16 (s' = 0 before the
+// stream start).  Thread t computes outputs t, t + 256, ... of the tile, each whole: the symmetric taps are folded, so
+// an output takes T1/2 - 1 pair sums and the centre tap, two multiply-adds per pair.
+template <int F>
+__global__ void __launch_bounds__(kDcThreads) decimate_kernel(const int16_t* __restrict__ g_taps, DcArgs a) {
+    extern __shared__ __align__(16) uint32_t dc_smem[];
+    const int T1 = a.T1, c = a.T1 / 2 - 1, D = a.D;
+    uint32_t* tabE = dc_smem;
+    int* taps = reinterpret_cast<int*>(dc_smem + ERTRS_NCO_N);
+    uint32_t* X = dc_smem + ERTRS_NCO_N + T1 / 2;
+    for (int i = threadIdx.x; i < ERTRS_NCO_N; i += kDcThreads) tabE[i] = a.E[i];
+    for (int i = threadIdx.x; i <= c; i += kDcThreads) taps[i] = g_taps[i];
+    if (blockIdx.x == 0)
+        for (long long i = threadIdx.x; i < a.carry_n; i += kDcThreads)
+            *reinterpret_cast<uchar2*>(a.carry_dst + 2 * i) = dc_input<F>(a, a.carry_first + i);  // carry_first >= 0
+    const long long tile_n = (long long)kDcThreads * a.per;
+    const long long ntiles = (a.count + tile_n - 1) / tile_n;
+    const uint32_t dph = (uint32_t)kDcThreads * a.W;  // phase accumulator step between a thread's staged samples
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long long nb = a.n0 + tile * tile_n;
+        const long long ne = min(nb + tile_n, a.n0 + a.count);
+        const long long j_lo = nb * D - T1 / 2 + 1;
+        const int nspan = (int)((ne - 1 - nb) * D + T1);
+        __syncthreads();  // the previous tile's span is no longer read (and E and the taps are in place)
+        // (uint32)g * W + 2^19 for g = j_lo + i, exact mod 2^32 whatever the sign of j_lo
+        uint32_t ph = (uint32_t)(j_lo + threadIdx.x) * a.W + (1u << (31 - ERTRS_NCO_BITS));
+        for (int i = threadIdx.x; i < nspan; i += kDcThreads, ph += dph) {
+            const long long g = j_lo + i;
+            uint32_t xw = 0;
+            if (g >= 0) {
+                const uchar2 u = dc_input<F>(a, g);
+                const uint32_t e = tabE[ph >> (32 - ERTRS_NCO_BITS)];
+                const int ce = (int)(short)(e & 0xffffu), se = (int)e >> 16;
+                const int si = 2 * (int)u.x - 255, sq = 2 * (int)u.y - 255;
+                const int mi = (si * ce + sq * se + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
+                const int mq = (sq * ce - si * se + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
+                xw = ((uint32_t)mi & 0xffffu) | ((uint32_t)mq << 16);
+            }
+            X[dc_skew(i)] = xw;
+        }
+        __syncthreads();
+
+        const int nloc = (int)(ne - nb);
+        for (int m = threadIdx.x; m < nloc; m += kDcThreads) {
+            const int o = m * D;  // the output's first tap reads staged word o
+            int ai = 0, aq = 0;
+#pragma unroll 4
+            for (int t = 0; t < c; t++) {
+                const uint32_t x0 = X[dc_skew(o + t)], x1 = X[dc_skew(o + T1 - 2 - t)];
+                const int h = taps[t];
+                ai += h * ((int)(short)(x0 & 0xffffu) + (int)(short)(x1 & 0xffffu));
+                aq += h * (((int)x0 >> 16) + ((int)x1 >> 16));
+            }
+            const uint32_t xc = X[dc_skew(o + c)];
+            ai += taps[c] * (int)(short)(xc & 0xffffu);
+            aq += taps[c] * ((int)xc >> 16);
+            const int ui = min(255, max(0, (ai + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
+            const int uq = min(255, max(0, (aq + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
+            *reinterpret_cast<uchar2*>(a.out + 2 * (nb - a.n0 + m)) = make_uchar2((unsigned char)ui, (unsigned char)uq);
+        }
+    }
+}
+
+}  // namespace ert

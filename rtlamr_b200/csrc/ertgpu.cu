@@ -902,6 +902,16 @@ int ertgpu_set_input_tuning(ertgpu_handle* h, int64_t capture_center_hz, int64_t
     return h->in.set_tuning(capture_center_hz, center_hz, (int64_t)h->cfg.center_freq, decoder_rate(h));
 }
 
+int ertgpu_allow_input_decimation(ertgpu_handle* h) {
+    if (!h) return ERTGPU_EINVAL;
+    if (h->allocated) return fail(h, ERTGPU_EINVAL, "allow_input_decimation after allocate");
+    return h->in.allow_decimation();
+}
+
+int ertgpu_get_decimator(const ertgpu_handle* h, ertgpu_decimator_info* info, int16_t* taps, size_t cap, size_t* n_out) {
+    return h ? h->in.decimator(info, taps, cap, n_out) : ERTGPU_EINVAL;
+}
+
 int ertgpu_get_tuning(const ertgpu_handle* h, ertgpu_tuning_info* info) {
     return h ? h->in.tuning(info) : ERTGPU_EINVAL;
 }

@@ -1,8 +1,9 @@
 // input_stage.cuh -- the input stage of a libertgpu handle: everything between the caller's bytes and the uint8 IQ blocks
 // the demod reads.  It owns the input's format, rate and tuning (ertgpu_set_input_*), the mode they resolve to, the
 // resampler's plan, tables and stream position, and it launches the one kernel in front of the pipeline:
-// convert_kernel<F> (convert.cuh) or resample_kernel<F, TUNED> (resample.cuh).  It also measures the level of its input
-// with level_kernel<F> (level.cuh) for ertgpu_measure_input.  Host code only.
+// convert_kernel<F> (convert.cuh) or resample_kernel<F, TUNED> (resample.cuh), or the two of a decimating handle:
+// decimate_kernel<F> (decimate.cuh) into resample_kernel<cu8, false>.  It also measures the level of its input with
+// level_kernel<F> (level.cuh) for ertgpu_measure_input.  Host code only.
 #pragma once
 
 #include <algorithm>
@@ -15,6 +16,7 @@
 #include <vector>
 
 #include "convert.cuh"
+#include "decimate.cuh"
 #include "demod_fast.cuh"  // OncePerDevice
 #include "level.cuh"
 #include "resample.cuh"
@@ -48,13 +50,15 @@ struct InputStep {
     const uint8_t* iq = nullptr;  // the blocks the pipeline reads: rs.cur itself in pass-through mode
     int64_t nblocks = 0;
     RsArgs rs{};                  // the kernel's arguments (convert_kernel reads rs.cur only)
+    DcArgs dc{};                  // decimate_kernel's (kDecimate): rs.cur is then its output
 };
 
 struct InputStage {
     // kPass: uint8 IQ at the decoder's rate, read where the caller put it.  kConvert: another format at that rate,
     // convert_kernel<F> into d_out[0].  kResample(Tuned): resample_kernel<F, false (true)> into d_out[cur_out]; the tuned
-    // instance runs for a tuned capture or a plan with P != ERTRS_P.
-    enum Mode { kPass, kConvert, kResample, kResampleTuned };
+    // instance runs for a tuned capture or a plan with P != ERTRS_P.  kDecimate: decimate_kernel<F> into d_mid, then
+    // resample_kernel<cu8, false> from d_mid into d_out[cur_out] (a tuned handle that allows decimation, above 10:1).
+    enum Mode { kPass, kConvert, kResample, kResampleTuned, kDecimate };
 
     explicit InputStage(std::string& err) : err_(err) {}
 
@@ -66,9 +70,12 @@ struct InputStage {
     bool tuned = false;         // set_tuning: the channel at center_hz of a capture centred at capture_hz
     int64_t capture_hz = 0, center_hz = 0;
     uint32_t nco_step = 0;      // W at the input rate in effect
+    bool decimation = false;    // allow_decimation: a tuned handle may take up to 256:1
     Mode mode = kPass;
-    ertgpu_resampler_info rs{};
+    ertgpu_resampler_info rs{};  // the resampler (the second stage in kDecimate)
     std::vector<int16_t> table;
+    ertgpu_decimator_info dec{};  // the first stage (decimation allowed and a plan made; D = 1: none)
+    std::vector<int16_t> taps;
 
     // decoder geometry (allocate)
     int64_t block = 0, max_blocks = 0;
@@ -89,6 +96,15 @@ struct InputStage {
     int grid = 0;               // most CTAs of one launch
     unsigned long long* d_level = nullptr;  // level_kernel's kLvCounters counters (converted input only)
     int level_grid = 0;
+    // the first stage of kDecimate: its taps, input history and output (the second stage's input), and stream position
+    int16_t* d_taps = nullptr;
+    uint8_t* d_hist1[2] = {nullptr, nullptr};
+    int cur_hist1 = 0;
+    uint8_t* d_mid = nullptr;
+    int64_t in1_total = 0;      // input samples received since the stream start
+    int64_t hist1_first = 0, hist1_n = 0;  // (the first stage's next output is the second stage's in_total)
+    size_t smem1 = 0;
+    int grid1 = 0, per1 = 0;
 
     bool resamples() const { return mode >= kResample; }
 
@@ -110,6 +126,14 @@ struct InputStage {
         center_hz = channel_hz ? channel_hz : default_center_hz;  // decode.go:105: the last CenterFreq
         const int64_t off = center_hz - capture_hz, ad = off < 0 ? -off : off;
         nco_step = ad <= rate_out ? ertrs_nco_step(off, rate_out) : 0;  // at the decoder's rate until set_rate
+        return ERTGPU_OK;
+    }
+
+    // A tuned handle may take up to 256:1 (ertrs_plan_decimated), between set_tuning and set_rate.
+    int allow_decimation() {
+        if (!tuned) return fail(err_, ERTGPU_EINVAL, "allow_input_decimation before set_input_tuning");
+        if (rate_in) return fail(err_, ERTGPU_EINVAL, "allow_input_decimation after set_input_rate");
+        decimation = true;
         return ERTGPU_OK;
     }
 
@@ -156,6 +180,14 @@ struct InputStage {
         return ERTGPU_OK;
     }
 
+    int decimator(ertgpu_decimator_info* info, int16_t* dst, size_t cap, size_t* n_out) const {
+        if (!decimation || dec.rate_in == 0) return ERTGPU_EINVAL;
+        if (info) *info = dec;
+        if (n_out) *n_out = taps.size();
+        if (dst && cap >= taps.size()) memcpy(dst, taps.data(), taps.size() * sizeof(int16_t));
+        return ERTGPU_OK;
+    }
+
     // ---- device buffers ----
     // Blocks of block_size samples, a step completes at most max_blocks_per_step of them; sm_count SMs.
     int allocate(int device, int64_t block_size, int64_t max_blocks_per_step, int sm_count) {
@@ -180,7 +212,7 @@ struct InputStage {
         CUDA_TRY(err_, cudaMemcpy(d_A, A.data(), A.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
         CUDA_TRY(err_, cudaMalloc(&d_D, D.size() * sizeof(uint32_t)));
         CUDA_TRY(err_, cudaMemcpy(d_D, D.data(), D.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        if (mix) {
+        if (mix || mode == kDecimate) {
             std::vector<uint32_t> E(ERTRS_NCO_N);
             ertrs_nco_table(E.data());
             CUDA_TRY(err_, cudaMalloc(&d_E, E.size() * sizeof(uint32_t)));
@@ -201,9 +233,10 @@ struct InputStage {
         }
         if (smem > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", smem);
         int per_sm = 0;
-        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel_of(fmt, mix), kRsThreads, smem));
+        const int fmt2 = mode == kDecimate ? ERTGPU_FORMAT_CU8 : fmt;  // the second stage reads the first stage's bytes
+        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel_of(fmt2, mix), kRsThreads, smem));
         grid = std::max(1, per_sm) * sm_count;
-        return ERTGPU_OK;
+        return mode == kDecimate ? allocate_first(device, sm_count) : ERTGPU_OK;
     }
 
     void release() {
@@ -212,13 +245,19 @@ struct InputStage {
         dfree(d_D);
         dfree(d_E);
         dfree(d_level);
+        dfree(d_taps);
+        dfree(d_mid);
         for (int k = 0; k < 2; k++) {
             dfree(d_hist[k]);
             dfree(d_out[k]);
+            dfree(d_hist1[k]);
         }
     }
 
-    void reset_stream() { in_total = out_next = hist_first = hist_n = pend = cur_hist = cur_out = 0; }
+    void reset_stream() {
+        in_total = out_next = hist_first = hist_n = pend = cur_hist = cur_out = 0;
+        in1_total = hist1_first = hist1_n = cur_hist1 = 0;
+    }
 
     // ---- calls ----
     // Before anything else of a decode call: a resampling stage takes whole IQ samples of s bytes.
@@ -254,6 +293,10 @@ struct InputStage {
     // so that it still reaches max_blocks blocks.
     int64_t chunk() const {
         if (!resamples()) return block * std::min<int64_t>(max_blocks, std::max<int64_t>(1, (32 << 20) / (block * 2)));
+        if (mode == kDecimate) {  // and with the first stage's D
+            const int64_t ratio = dec.D * std::max<int64_t>(4, (rs.M + rs.L - 1) / rs.L);
+            return std::min<int64_t>(16 << 20, ratio * (max_blocks + 1) * block + dec.D * (rs.T + 8) + dec.T1 + 8);
+        }
         const int64_t ratio = std::max<int64_t>(4, (rs.M + rs.L - 1) / rs.L);
         return std::min<int64_t>(16 << 20, ratio * (max_blocks + 1) * block + rs.T + 8);
     }
@@ -273,6 +316,10 @@ struct InputStage {
             s.iq = mode == kPass ? d_in : d_out[0];
             s.nblocks = n / block;
             return s;
+        }
+        if (mode == kDecimate) {  // the second stage takes the first stage's outputs of this step
+            n = plan_first(s.dc, d_in, n);
+            s.rs.cur = d_mid;
         }
         // every output whose window is complete
         const int64_t L = rs.L, M = rs.M, T = rs.T;
@@ -314,6 +361,23 @@ struct InputStage {
 
     // Enqueue the step's kernel on st, if it has one, and count it in *launches.
     int launch(const InputStep& s, cudaStream_t st, int64_t* launches) const {
+        if (mode == kDecimate) {
+            if (s.dc.count > 0 || s.dc.carry_n > 0) {
+                const long long tiles = (s.dc.count + (long long)kDcThreads * per1 - 1) / ((long long)kDcThreads * per1);
+                const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid1));
+                decimate_kernel_of(fmt)<<<g, kDcThreads, smem1, st>>>(d_taps, s.dc);
+                CUDA_TRY(err_, cudaGetLastError());
+                ++*launches;
+            }
+            if (s.rs.count > 0 || s.rs.carry_n > 0) {
+                const long long tiles = (s.rs.count + kRsTile - 1) / kRsTile;
+                const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid));
+                resample_kernel<ERTGPU_FORMAT_CU8, false><<<g, kRsThreads, smem, st>>>(d_A, d_D, s.rs);
+                CUDA_TRY(err_, cudaGetLastError());
+                ++*launches;
+            }
+            return ERTGPU_OK;
+        }
         if (mode == kPass || (resamples() && s.rs.count <= 0 && s.rs.carry_n <= 0)) return ERTGPU_OK;
         if (mode == kConvert) {
             const long long groups = s.nblocks * block / 8;
@@ -346,6 +410,12 @@ struct InputStage {
     // The step's kernel is enqueued: advance the stream position.
     void commit(const InputStep& s) {
         if (!resamples()) return;
+        if (mode == kDecimate) {
+            in1_total += s.dc.cur_n;
+            hist1_first = s.dc.carry_first;
+            hist1_n = s.dc.carry_n;
+            cur_hist1 ^= 1;
+        }
         const RsArgs& a = s.rs;
         in_total += a.cur_n;
         out_next += a.count;
@@ -363,6 +433,7 @@ struct InputStage {
             case kPass: return "";
             case kConvert: return std::string("convert_kernel<") + f + ">";
             case kResample: return fmt == ERTGPU_FORMAT_CU8 ? "resample_kernel" : std::string("resample_kernel<") + f + ">";
+            case kDecimate: return std::string("decimate_kernel<") + f + ">;resample_kernel<cu8>";
             default: return std::string("resample_kernel<") + f + ",tuned>";
         }
     }
@@ -374,8 +445,22 @@ private:
     // the rates differ or a tuned handle mixes; the tuned instance when it mixes or its plan has P != ERTRS_P.
     int configure_rate(int64_t hz, int64_t rate_out) {
         ertgpu_resampler_info info{};
+        ertgpu_decimator_info d{};
+        std::vector<int16_t> t1;
         uint32_t w = 0;
-        if (tuned) {
+        if (tuned && decimation) {
+            const int64_t off = center_hz - capture_hz;
+            if (ertrs_plan_decimated(hz, rate_out, off, &d, &info) != 0)  // up to 10:1 the message of a tuned handle
+                return fail(err_, ERTGPU_EINVAL,
+                            "input rate %lld Hz, channel offset %lld Hz: the decoder rate %lld Hz must be within %s ... 4 "
+                            "times the input rate, and |offset| + 0.4 * min(rates) at most half the input rate",
+                            (long long)hz, (long long)off, (long long)rate_out, hz <= 10 * rate_out ? "1/10" : "1/256");
+            if (d.D > 1) {
+                t1.resize((size_t)d.T1);
+                if (ertrs_build_decimator(&d, t1.data()) != 0) return fail(err_, ERTGPU_EINVAL, "decimator taps do not fit int16");
+            }
+            w = ertrs_nco_step(off, hz);
+        } else if (tuned) {
             const int64_t off = center_hz - capture_hz;
             if (ertrs_plan_tuned(hz, rate_out, off, &info) != 0)
                 return fail(err_, ERTGPU_EINVAL,
@@ -394,10 +479,70 @@ private:
             if (ertrs_build_table(&info, t.data()) != 0) return fail(err_, ERTGPU_EINVAL, "resampler table does not fit int16");
         }
         mode = !on ? (fmt == ERTGPU_FORMAT_CU8 ? kPass : kConvert) : w != 0 || info.P != ERTRS_P ? kResampleTuned : kResample;
+        if (d.D > 1) mode = kDecimate;
         nco_step = w;
         rs = info;
         table.swap(t);
+        dec = d;
+        taps.swap(t1);
         return ERTGPU_OK;
+    }
+
+    // The first stage's plan of the step over n new input samples at d_in; returns its number of outputs.
+    int64_t plan_first(DcArgs& a, const uint8_t* d_in, int64_t n) const {
+        const int64_t D = dec.D, T1 = dec.T1;
+        const int64_t in_new = in1_total + n;
+        const int64_t ne = in_new - T1 / 2 > 0 ? (in_new - T1 / 2 + D - 1) / D : 0;  // ertrs_out_end at L = 1, M = D
+        a.hist = d_hist1[cur_hist1];
+        a.cur = d_in;
+        a.hist_first = hist1_first;
+        a.hist_n = hist1_n;
+        a.cur_n = n;
+        a.n0 = in_total;  // the first stage's next output is the second stage's next input
+        a.count = ne - in_total;
+        a.out = d_mid;
+        const int64_t first = std::min(in_new, std::max<int64_t>(0, ne * D - T1 / 2 + 1));
+        a.carry_dst = d_hist1[cur_hist1 ^ 1];
+        a.carry_first = first;
+        a.carry_n = in_new - first;
+        a.D = (int)D;
+        a.T1 = (int)T1;
+        a.per = per1;
+        a.scale = scale;
+        a.E = d_E;
+        a.W = nco_step;
+        return a.count;
+    }
+
+    // The first stage's device buffers, after the second stage's.
+    int allocate_first(int device, int sm_count) {
+        CUDA_TRY(err_, cudaMalloc(&d_taps, taps.size() * sizeof(int16_t)));
+        CUDA_TRY(err_, cudaMemcpy(d_taps, taps.data(), taps.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
+        for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_hist1[k], (size_t)(dec.T1 + dec.D + 16) * 2));
+        // A step hands the second stage fewer than (max_blocks + 1) * block * M / L + M / L + T samples (the blocks a
+        // step may complete, plus the look-ahead).
+        const int64_t mid = (int64_t)(((__int128)(max_blocks + 1) * block * rs.M + rs.L - 1) / rs.L) + rs.M / rs.L + rs.T + 64;
+        CUDA_TRY(err_, cudaMalloc(&d_mid, (size_t)mid * 2));
+        per1 = dc_per_thread(dec.D, dec.T1);
+        smem1 = dc_smem_bytes(dec.D, dec.T1, per1);
+        {
+            static OncePerDevice once;
+            if (once.first(device))
+                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF64BE; f++)
+                    if (fmt_name(f))
+                        CUDA_TRY(err_, cudaFuncSetAttribute(decimate_kernel_of(f), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        }
+        if (smem1 > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "decimator needs %zu B of shared memory", smem1);
+        int per_sm = 0;
+        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decimate_kernel_of(fmt), kDcThreads, smem1));
+        grid1 = std::max(1, per_sm) * sm_count;
+        return ERTGPU_OK;
+    }
+
+    static decltype(&decimate_kernel<ERTGPU_FORMAT_CU8>) decimate_kernel_of(int f) {
+        decltype(&decimate_kernel<ERTGPU_FORMAT_CU8>) k = nullptr;
+        fmt_visit(f, [&](auto F) { k = decimate_kernel<F()>; });
+        return k;
     }
 
     // The resample_kernel instance of an input format, untuned or tuned.
@@ -412,7 +557,9 @@ private:
     // Most input samples the next step may take so that it completes at most max_blocks decoder blocks.
     int64_t max_input() const {
         const int64_t cap_out = (max_blocks + 1) * block - 1 - pend;
-        return rs.T / 2 + k_of(out_next + cap_out) - in_total;
+        const int64_t m2 = rs.T / 2 + k_of(out_next + cap_out) - in_total;
+        // decimating: the first stage completes at most m2 outputs, ceil((in1_total + x - T1/2) / D) <= in_total + m2
+        return mode == kDecimate ? (in_total + m2) * dec.D + dec.T1 / 2 - in1_total : m2;
     }
 };
 

@@ -9,9 +9,10 @@
 //                      FILE|- [FILE ...]
 // -capturefreq names the frequency the capture was recorded centred at; -centerfreq (rtlamr's flag) the channel to
 // receive, by default the protocols' CenterFreq (912.6 MHz, or 912.38 MHz for r900 alone).  The channel is mixed to
-// 0 Hz exactly inside the GPU resampler, whose lowpass is then the channel filter; a tuned capture may be at up to 10
-// times 32768 * -symbollength.  Without -capturefreq nothing is translated; -centerfreq alone is a usage error, and
-// so is -samplefile with -capturefreq.
+// 0 Hz exactly inside the GPU resampler, whose lowpass is then the channel filter; a tuned capture may be at up to 256
+// times 32768 * -symbollength (above 10 times it is first decimated by D on the GPU, and the decoder log on stderr
+// names D and the intermediate rate).  Without -capturefreq nothing is translated; -centerfreq alone is a usage error,
+// and so is -samplefile with -capturefreq.
 // -samplerate is rtlamr's (rtltcp's) flag name; here it names the capture's sample rate.  The default,
 // 32768 * -symbollength, decodes the bytes as they are; any other rate within 1/4 ... 4 times it is resampled
 // exactly on the GPU first, and Block / Idx then count resampled samples.

@@ -609,7 +609,10 @@ void Decoder::SetInput(const Input& in) {
         if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
         if (rc != ERTGPU_OK) raise(h_, rc, "SetInput");
     };
-    if (in.CaptureFreq > 0 || in.CenterFreq != 0) check(ertgpu_set_input_tuning(h_, in.CaptureFreq, in.CenterFreq));
+    if (in.CaptureFreq > 0 || in.CenterFreq != 0) {
+        check(ertgpu_set_input_tuning(h_, in.CaptureFreq, in.CenterFreq));
+        check(ertgpu_allow_input_decimation(h_));  // up to 256:1; nothing changes up to 10:1
+    }
     if (in.SampleRate > 0) check(ertgpu_set_input_rate(h_, in.SampleRate));
     if (in.AutoScale && in.Format == ERTGPU_FORMAT_CU8) throw std::invalid_argument("automatic gain does not apply to uint8 (cu8) input");
     if (in.Format != ERTGPU_FORMAT_CU8 || in.Scale != 0.0f) {
@@ -690,10 +693,17 @@ void Decoder::Dispatch(const ertgpu_candidate* cands, size_t n, std::vector<Mess
 std::string Decoder::Log() const {  // decode.go:73-90
     std::string s;
     ertgpu_tuning_info t;
-    if (ertgpu_get_tuning(h_, &t) == ERTGPU_OK)  // the channel decoded, and the capture's centre
+    if (ertgpu_get_tuning(h_, &t) == ERTGPU_OK) {  // the channel decoded, and the capture's centre
         s += "CenterFreq: " + std::to_string(t.center_hz) + "\nCaptureFreq: " + std::to_string(t.capture_center_hz);
-    else
+        ertgpu_decimator_info d;
+        if (ertgpu_get_decimator(h_, &d, nullptr, 0, nullptr) == ERTGPU_OK && d.D > 1) {  // above 10:1: the first stage
+            char mid[64];
+            snprintf(mid, sizeof(mid), "%.3f", (double)d.rate_in / d.D);
+            s += "\nDecimation: " + std::to_string(d.D) + "\nIntermediateRate: " + mid;
+        }
+    } else {
         s += "CenterFreq: " + u(Cfg.CenterFreq);
+    }
     s += "\nSampleRate: " + u((uint64_t)Cfg.SampleRate) + "\nDataRate: " + u((uint64_t)Cfg.DataRate);
     s += "\nChipLength: " + u((uint64_t)Cfg.ChipLength) + "\nPreambleSymbols: " + u((uint64_t)Cfg.PreambleSymbols);
     s += "\nPreambleLength: " + u((uint64_t)Cfg.PreambleLength) + "\nPacketSymbols: " + u((uint64_t)Cfg.PacketSymbols);

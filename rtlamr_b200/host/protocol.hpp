@@ -161,7 +161,8 @@ public:
 
     void RegisterProtocol(ParserPtr p);  // decode.go:100-128
     // The IQ fed to Decode, between the last RegisterProtocol and Allocate: sets the tuning when CaptureFreq > 0 or
-    // CenterFreq != 0, then the rate when SampleRate > 0, then the format when Format != cu8 or Scale != 0.  A bad value
+    // CenterFreq != 0 (and allows decimation, so a tuned capture may be at up to 256 times the decoder's rate), then the
+    // rate when SampleRate > 0, then the format when Format != cu8 or Scale != 0.  A bad value
     // throws std::invalid_argument, and so does Allocate when the channel does not fit a capture at the decoder's rate.
     void SetInput(const Input& in);
     int BytesPerSample() const { return sample_bytes_; }
