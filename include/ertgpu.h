@@ -44,6 +44,7 @@ extern "C" {
 
 #define ERTGPU_MAX_PROTOCOLS 8
 #define ERTGPU_MAX_PREAMBLE 32
+#define ERTGPU_MAX_CHANNELS 64 /* most handles of one ertgpu_decode_channels call */
 #define ERTGPU_MAX_PACKET_BYTES 92 /* (PacketSymbols+7)>>3 for idm/netidm */
 #define ERTGPU_R900_DIGITS 42      /* r900.PayloadSymbols, r900/r900.go:30 */
 
@@ -238,7 +239,8 @@ int ertgpu_set_input_rate(ertgpu_handle *h, int64_t hz);
  * ertgpu_set_input_rate, or by ertgpu_allocate when the input is at the decoder's own rate.  An offset
  * of 0 decodes exactly like an untuned handle.  ertgpu_reset restarts the mixer's phase;
  * ERTGPU_TAP_RESAMPLED returns the mixed and filtered bytes; ertgpu_decode_sharded rejects tuned
- * handles.  Several channels of one capture are several handles fed the same bytes. */
+ * handles.  Several channels of one capture are several handles, fed the same bytes in one pass by
+ * ertgpu_decode_channels. */
 int ertgpu_set_input_tuning(ertgpu_handle *h, int64_t capture_center_hz, int64_t center_hz);
 
 /* Let a tuned handle take captures at up to 256 times the decoder's rate R_out.  Call it after
@@ -334,6 +336,28 @@ int ertgpu_decode(ertgpu_handle *h, const uint8_t *iq, size_t nbytes, uint32_t f
  * read with ertgpu_fetch.  d_iq must stay valid until then. */
 int ertgpu_decode_device_async(ertgpu_handle *h, const void *d_iq, size_t nbytes, uint32_t flags,
                                void *stream);
+
+/* Several channels of ONE capture in one pass: handles[0..n) are tuned to different channels of the same capture, and
+ * each decodes the nbytes of iq (HOST memory, pinned or pageable, staged as ertgpu_decode stages it) exactly as
+ * ertgpu_decode would on that handle alone: the same candidates, taps, block counts and stream state.  The input crosses
+ * the host link once per chunk, into handles[0]'s staging buffers, and every channel reads that device copy.  Above
+ * 10:1 (a first stage with D > 1) one decimate_channels_kernel converts each input sample once and runs the first stage
+ * of every channel; then each handle runs its own second stage and pipeline.  Up to 10:1 each handle's tuned resampler
+ * reads the shared copy.  Synchronous; read each handle's candidates with ertgpu_fetch(handles[c], ...).  Call splits
+ * are free: n calls on a group equal one call over the same bytes.  The rules, each broken one ERTGPU_EINVAL with the
+ * rule named in ertgpu_last_error(handles[0]):
+ *   1 <= n <= ERTGPU_MAX_CHANNELS, and no handle appears twice;
+ *   every handle is allocated, on one device, with the same protocols (and so the same chip length);
+ *   every handle is tuned (ertgpu_set_input_tuning), with the same capture centre, input rate, format and scale;
+ *   every handle is at the same stream position (fresh, or reset together, and fed together since).
+ * Otherwise every rule of ertgpu_decode holds for each handle. */
+int ertgpu_decode_channels(ertgpu_handle *const *handles, int32_t n, const uint8_t *iq, size_t nbytes, uint32_t flags);
+
+/* The same with the input in DEVICE memory of the handles' device, enqueued on `stream` (a cudaStream_t, NULL = the
+ * handles[0]'s own stream) without synchronising, as ertgpu_decode_device_async does for one handle.  d_iq must stay
+ * valid until every handle's candidates are fetched. */
+int ertgpu_decode_channels_device_async(ertgpu_handle *const *handles, int32_t n, const void *d_iq, size_t nbytes,
+                                        uint32_t flags, void *stream);
 
 /* Wait for the decode enqueued last and copy its candidates out (sorted as
  * above).  May be repeated (e.g. after ERTGPU_ECAPACITY). */

@@ -101,6 +101,7 @@ EXPORTS = [
     "ertgpu_set_input_rate", "ertgpu_get_resampler", "ertgpu_set_input_format", "ertgpu_get_input_format",
     "ertgpu_set_input_tuning", "ertgpu_get_tuning", "ertgpu_measure_input", "ertgpu_set_input_scale",
     "ertgpu_allow_input_decimation", "ertgpu_get_decimator",
+    "ertgpu_decode_channels", "ertgpu_decode_channels_device_async",
 ]
 
 _lib = None
@@ -153,6 +154,8 @@ def lib() -> C.CDLL:
     L.ertgpu_last_kernels.argtypes = [vp]
     L.ertgpu_plan_shards.argtypes = [i64, i32, i32, i32, C.POINTER(Shard)]
     L.ertgpu_decode_sharded.argtypes = [C.POINTER(vp), i32, vp, sz, u32, vp, sz, C.POINTER(sz)]
+    L.ertgpu_decode_channels.argtypes = [C.POINTER(vp), i32, vp, sz, u32]
+    L.ertgpu_decode_channels_device_async.argtypes = [C.POINTER(vp), i32, vp, sz, u32, vp]
     L.ertgpu_set_input_rate.argtypes = [vp, i64]
     L.ertgpu_get_resampler.argtypes = [vp, C.POINTER(ResamplerInfo), vp, sz, C.POINTER(sz)]
     L.ertgpu_set_input_format.argtypes = [vp, i32, C.c_float]
@@ -435,3 +438,29 @@ SYNTH_DTYPE = np.dtype([("start_sample", "<i8"), ("n_chips", "<i4"), ("chip_leng
                         ("amp_i", "<i2"), ("amp_q", "<i2"), ("chips", "u1", (192,)),
                         ("pad", "<i4")])
 assert SYNTH_DTYPE.itemsize == C.sizeof(SynthPacket) == 216
+
+
+def _channel_call(handles, call):
+    hs = (C.c_void_p * len(handles))(*[h._h if h is not None else None for h in handles])
+    rc = call(hs, len(handles))
+    if rc != OK:
+        h0 = handles[0] if handles and handles[0] is not None else None
+        msg = (lib().ertgpu_last_error(h0._h) or b"").decode() if h0 is not None and h0._h else ""
+        raise ErtGpuError(rc, msg or "ertgpu_decode_channels failed")
+
+
+def decode_channels(handles, iq, flags: int = 0, cap: int = 4096) -> list:
+    """ertgpu_decode_channels: one HOST buffer (numpy uint8 or an address/size pair) through every handle, each tuned to
+    another channel of the same capture, in one pass.  Returns each handle's candidates (ertgpu_fetch)."""
+    if isinstance(iq, tuple):
+        addr, nbytes = iq
+    else:
+        iq = np.ascontiguousarray(iq, dtype=np.uint8)
+        addr, nbytes = iq.ctypes.data, iq.size
+    _channel_call(handles, lambda hs, n: lib().ertgpu_decode_channels(hs, n, addr, nbytes, flags))
+    return [h.fetch(cap) for h in handles]
+
+
+def decode_channels_device_async(handles, d_ptr: int, nbytes: int, flags: int = 0, stream: int = 0):
+    """ertgpu_decode_channels_device_async: the same for input in device memory; read each handle with fetch()."""
+    _channel_call(handles, lambda hs, n: lib().ertgpu_decode_channels_device_async(hs, n, d_ptr, nbytes, flags, stream))

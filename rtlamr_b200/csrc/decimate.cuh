@@ -7,6 +7,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/ertgpu.h"
 #include "../../include/ertgpu_resample.h"
 #include "convert.cuh"
 
@@ -15,6 +16,7 @@ namespace ert {
 constexpr int kDcThreads = 256;
 constexpr int kDcSpanWords = 20480;  // most input samples one tile stages (80 KiB, so that two CTAs fit an SM)
 constexpr int kDcMaxPer = 16;        // most outputs per thread and tile
+constexpr int kDcChannelsSpanWords = kDcSpanWords * 2 / 3;  // decimate_channels_kernel's: X and U in the same 80 KiB
 
 struct DcArgs {
     // input samples [hist_first, hist_first + hist_n) are in hist (uint8), the next cur_n ones in cur (the handle's format)
@@ -35,9 +37,10 @@ struct DcArgs {
 };
 
 // Outputs a thread computes per tile, so that a tile's input span, (kDcThreads * per - 1) * D + T1 samples, fits
-// kDcSpanWords (for every D <= ERTRS_MAX_D).
-inline int dc_per_thread(int D, int T1) {
-    const int per = (kDcSpanWords - T1) / (kDcThreads * D);
+// span_words (for every D <= ERTRS_MAX_D).
+// decimate_channels_kernel passes a smaller span_words, so that its uint8 copy of the span fits beside it.
+inline int dc_per_thread(int D, int T1, int span_words = kDcSpanWords) {
+    const int per = (span_words - T1) / (kDcThreads * D);
     return per < 1 ? 1 : per > kDcMaxPer ? kDcMaxPer : per;
 }
 
@@ -59,10 +62,42 @@ __device__ __forceinline__ uchar2 dc_input(const DcArgs& a, long long g) {  // g
     else return fmt_sample<F>(a.cur, g - e, a.scale);
 }
 
+// The mixer: uint8 IQ u times E[ph >> (32 - NCO_BITS)], as one word of int16 s'_I | s'_Q << 16.
+__device__ __forceinline__ uint32_t dc_mix(uchar2 u, const uint32_t* tabE, uint32_t ph) {
+    const uint32_t e = tabE[ph >> (32 - ERTRS_NCO_BITS)];
+    const int ce = (int)(short)(e & 0xffffu), se = (int)e >> 16;
+    const int si = 2 * (int)u.x - 255, sq = 2 * (int)u.y - 255;
+    const int mi = (si * ce + sq * se + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
+    const int mq = (sq * ce - si * se + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
+    return ((uint32_t)mi & 0xffffu) | ((uint32_t)mq << 16);
+}
+
+// The nloc outputs of a tile from its staged span X (skewed), output m to out[2m..2m+1]: the symmetric taps are
+// folded, so an output takes T1/2 - 1 pair sums and the centre tap, two multiply-adds per pair.
+__device__ __forceinline__ void dc_filter(const uint32_t* X, const int* taps, int T1, int D, int nloc, uint8_t* out) {
+    const int c = T1 / 2 - 1;
+    for (int m = threadIdx.x; m < nloc; m += kDcThreads) {
+        const int o = m * D;  // the output's first tap reads staged word o
+        int ai = 0, aq = 0;
+#pragma unroll 4
+        for (int t = 0; t < c; t++) {
+            const uint32_t x0 = X[dc_skew(o + t)], x1 = X[dc_skew(o + T1 - 2 - t)];
+            const int h = taps[t];
+            ai += h * ((int)(short)(x0 & 0xffffu) + (int)(short)(x1 & 0xffffu));
+            aq += h * (((int)x0 >> 16) + ((int)x1 >> 16));
+        }
+        const uint32_t xc = X[dc_skew(o + c)];
+        ai += taps[c] * (int)(short)(xc & 0xffffu);
+        aq += taps[c] * ((int)xc >> 16);
+        const int ui = min(255, max(0, (ai + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
+        const int uq = min(255, max(0, (aq + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
+        *reinterpret_cast<uchar2*>(out + 2 * m) = make_uchar2((unsigned char)ui, (unsigned char)uq);
+    }
+}
+
 // Persistent grid over tiles of kDcThreads * per outputs.  Each CTA keeps E and the taps in shared memory and stages a
 // tile's input span once, each sample mixed by E[k_g] into one word of int16 s'_I | s'_Q << 16 (s' = 0 before the
-// stream start).  Thread t computes outputs t, t + 256, ... of the tile, each whole: the symmetric taps are folded, so
-// an output takes T1/2 - 1 pair sums and the centre tap, two multiply-adds per pair.
+// stream start).  Thread t computes outputs t, t + 256, ... of the tile, each whole (dc_filter).
 template <int F>
 __global__ void __launch_bounds__(kDcThreads) decimate_kernel(const int16_t* __restrict__ g_taps, DcArgs a) {
     extern __shared__ __align__(16) uint32_t dc_smem[];
@@ -88,37 +123,70 @@ __global__ void __launch_bounds__(kDcThreads) decimate_kernel(const int16_t* __r
         uint32_t ph = (uint32_t)(j_lo + threadIdx.x) * a.W + (1u << (31 - ERTRS_NCO_BITS));
         for (int i = threadIdx.x; i < nspan; i += kDcThreads, ph += dph) {
             const long long g = j_lo + i;
-            uint32_t xw = 0;
-            if (g >= 0) {
-                const uchar2 u = dc_input<F>(a, g);
-                const uint32_t e = tabE[ph >> (32 - ERTRS_NCO_BITS)];
-                const int ce = (int)(short)(e & 0xffffu), se = (int)e >> 16;
-                const int si = 2 * (int)u.x - 255, sq = 2 * (int)u.y - 255;
-                const int mi = (si * ce + sq * se + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
-                const int mq = (sq * ce - si * se + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
-                xw = ((uint32_t)mi & 0xffffu) | ((uint32_t)mq << 16);
-            }
-            X[dc_skew(i)] = xw;
+            X[dc_skew(i)] = g >= 0 ? dc_mix(dc_input<F>(a, g), tabE, ph) : 0u;
         }
         __syncthreads();
+        dc_filter(X, taps, T1, D, (int)(ne - nb), a.out + 2 * (nb - a.n0));
+    }
+}
 
-        const int nloc = (int)(ne - nb);
-        for (int m = threadIdx.x; m < nloc; m += kDcThreads) {
-            const int o = m * D;  // the output's first tap reads staged word o
-            int ai = 0, aq = 0;
-#pragma unroll 4
-            for (int t = 0; t < c; t++) {
-                const uint32_t x0 = X[dc_skew(o + t)], x1 = X[dc_skew(o + T1 - 2 - t)];
-                const int h = taps[t];
-                ai += h * ((int)(short)(x0 & 0xffffu) + (int)(short)(x1 & 0xffffu));
-                aq += h * (((int)x0 >> 16) + ((int)x1 >> 16));
-            }
-            const uint32_t xc = X[dc_skew(o + c)];
-            ai += taps[c] * (int)(short)(xc & 0xffffu);
-            aq += taps[c] * ((int)xc >> 16);
-            const int ui = min(255, max(0, (ai + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
-            const int uq = min(255, max(0, (aq + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
-            *reinterpret_cast<uchar2*>(a.out + 2 * (nb - a.n0 + m)) = make_uchar2((unsigned char)ui, (unsigned char)uq);
+// The channels of one capture that decimate_channels_kernel serves: channel c mixes with step W[c], writes its outputs
+// to out[c] and its copy of the input history to carry_dst[c].
+struct DcChannels {
+    uint32_t W[ERTGPU_MAX_CHANNELS];
+    uint8_t* out[ERTGPU_MAX_CHANNELS];
+    uint8_t* carry_dst[ERTGPU_MAX_CHANNELS];
+    int n;
+};
+
+// Shared memory of one CTA of decimate_channels_kernel: decimate_kernel's, and the tile's span as uint8 IQ.
+inline size_t dc_channels_smem_bytes(int D, int T1, int per) {
+    const long long span = ((long long)kDcThreads * per - 1) * D + T1;
+    return dc_smem_bytes(D, T1, per) + (size_t)((span + 1) / 2) * 4;
+}
+
+// decimate_kernel for ch.n channels of one capture at once.  The channels share everything of a's but W, out and
+// carry_dst (a's are not read).  A tile's input span is read and converted to uint8 IQ once, into U; then, channel by
+// channel, U is mixed with that channel's step into X and filtered into its outputs, with decimate_kernel's integer
+// formulas, so channel c's bytes are those of decimate_kernel at W[c].  The history carry is converted once and stored
+// for every channel, so that each handle keeps a history of its own.
+template <int F>
+__global__ void __launch_bounds__(kDcThreads) decimate_channels_kernel(const int16_t* __restrict__ g_taps, DcArgs a,
+                                                                       const __grid_constant__ DcChannels ch) {
+    extern __shared__ __align__(16) uint32_t dc_smem[];
+    const int T1 = a.T1, c = a.T1 / 2 - 1, D = a.D;
+    const long long tile_n = (long long)kDcThreads * a.per;
+    const long long span_max = (tile_n - 1) * D + T1;
+    uint32_t* tabE = dc_smem;
+    int* taps = reinterpret_cast<int*>(dc_smem + ERTRS_NCO_N);
+    uint32_t* X = dc_smem + ERTRS_NCO_N + T1 / 2;
+    uchar2* U = reinterpret_cast<uchar2*>(X + span_max + (span_max >> 5) + 1);
+    for (int i = threadIdx.x; i < ERTRS_NCO_N; i += kDcThreads) tabE[i] = a.E[i];
+    for (int i = threadIdx.x; i <= c; i += kDcThreads) taps[i] = g_taps[i];
+    if (blockIdx.x == 0)
+        for (long long i = threadIdx.x; i < a.carry_n; i += kDcThreads) {
+            const uchar2 u = dc_input<F>(a, a.carry_first + i);  // carry_first >= 0
+            for (int k = 0; k < ch.n; k++) *reinterpret_cast<uchar2*>(ch.carry_dst[k] + 2 * i) = u;
+        }
+    const long long ntiles = (a.count + tile_n - 1) / tile_n;
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long long nb = a.n0 + tile * tile_n;
+        const long long ne = min(nb + tile_n, a.n0 + a.count);
+        const long long j_lo = nb * D - T1 / 2 + 1;
+        const int nspan = (int)((ne - 1 - nb) * D + T1);
+        __syncthreads();  // the previous tile's U and X are no longer read (and E and the taps are in place)
+        for (int i = threadIdx.x; i < nspan; i += kDcThreads) {
+            const long long g = j_lo + i;
+            U[i] = g >= 0 ? dc_input<F>(a, g) : make_uchar2(0, 0);  // g < 0 is mixed to 0 below, whatever U holds
+        }
+        for (int k = 0; k < ch.n; k++) {
+            const uint32_t W = ch.W[k], dph = (uint32_t)kDcThreads * W;
+            __syncthreads();  // U is staged, and the previous channel's X is no longer read
+            uint32_t ph = (uint32_t)(j_lo + threadIdx.x) * W + (1u << (31 - ERTRS_NCO_BITS));
+            for (int i = threadIdx.x; i < nspan; i += kDcThreads, ph += dph)
+                X[dc_skew(i)] = j_lo + i >= 0 ? dc_mix(U[i], tabE, ph) : 0u;
+            __syncthreads();
+            dc_filter(X, taps, T1, D, (int)(ne - nb), ch.out[k] + 2 * (nb - a.n0));
         }
     }
 }

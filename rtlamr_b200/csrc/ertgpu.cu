@@ -447,7 +447,7 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
         h->launches++;
         h->kernels += ";extract_words_kernel<" + std::to_string(short_packets ? 4 : kFullK) + ">";
     }
-    if (h->in.mode != InputStage::kPass) h->kernels += ";" + h->in.label();
+    if (h->in.mode != InputStage::kPass) h->kernels += ";" + h->in.label(s.shared_first);
 
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[3], st));
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[4], st));
@@ -565,8 +565,7 @@ int prepare_staging(ertgpu_handle* h, size_t bytes, const void* iq, bool* pageab
 
 // Enqueue the work for the next n input samples, at d_in on the device, on st: the input stage's step and the pipeline
 // over the whole blocks it completes.
-int enqueue_step(ertgpu_handle* h, const uint8_t* d_in, int64_t n, uint32_t flags, cudaStream_t st) {
-    const InputStep s = h->in.plan(d_in, n);
+int run_step(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaStream_t st) {
     int rc;
     if (s.nblocks > 0) {
         rc = enqueue_pipeline(h, s, flags, st);
@@ -577,11 +576,39 @@ int enqueue_step(ertgpu_handle* h, const uint8_t* d_in, int64_t n, uint32_t flag
             h->pending = true;
             h->pending_counts = false;
             h->pending_stream = st;
-            if (h->kernels.empty()) h->kernels = h->in.label();  // otherwise the last pipeline's list stays
+            if (h->kernels.empty()) h->kernels = h->in.label(s.shared_first);  // otherwise the last pipeline's list stays
         }
     }
     if (rc) return rc;
     h->in.commit(s);
+    return ERTGPU_OK;
+}
+
+int enqueue_step(ertgpu_handle* h, const uint8_t* d_in, int64_t n, uint32_t flags, cudaStream_t st) {
+    return run_step(h, h->in.plan(d_in, n), flags, st);
+}
+
+// The same for the channels hs[0..n) of one capture (check_channels holds) over the same input.  Decimating channels
+// share one decimate_channels_kernel launch, counted in hs[0]'s launches; the rest is each handle's own step.
+int enqueue_channels(ertgpu_handle* const* hs, int n, const uint8_t* d_in, int64_t cnt, uint32_t flags, cudaStream_t st) {
+    if (n == 1 || hs[0]->in.mode != InputStage::kDecimate) {
+        for (int k = 0; k < n; k++)
+            if (const int rc = enqueue_step(hs[k], d_in, cnt, flags, st)) return rc;
+        return ERTGPU_OK;
+    }
+    InputStep steps[ERTGPU_MAX_CHANNELS];
+    for (int k = 0; k < n; k++) steps[k] = hs[k]->in.plan(d_in, cnt);
+    int64_t shared = 0;
+    if (const int rc = hs[0]->in.launch_channels(steps, n, st, &shared)) return fail(hs[0], rc, "%s", hs[0]->err.c_str());
+    for (int k = 0; k < n; k++)
+        if (const int rc = run_step(hs[k], steps[k], flags, st)) return rc;
+    ertgpu_handle* h = hs[0];
+    h->launches += shared;
+    if (shared && !h->pending) {  // the shared launch wrote every channel's history: wait for it like a stage launch
+        h->pending = true;
+        h->pending_counts = false;
+        h->pending_stream = st;
+    }
     return ERTGPU_OK;
 }
 
@@ -596,11 +623,15 @@ void begin_call(ertgpu_handle* h) {
 // The start of both decode calls.  The input is checked by the input stage's rules before anything is collected, so
 // that a rejected call leaves the stream as it was.  Then the previous call's work is collected and this call's results
 // start empty.
-int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
+int check_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
     if (const int rc = h ? h->in.check_samples(nbytes) : ERTGPU_OK) return rc;
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     if (!iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
-    if (const int rc = h->in.check_call(iq, nbytes, device)) return rc;
+    return h->in.check_call(iq, nbytes, device);
+}
+
+int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
+    if (const int rc = check_decode(h, iq, nbytes, device)) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
     h->started = true;
     if (h->pending) {
@@ -608,6 +639,50 @@ int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
         if (rc) return rc;
     }
     begin_call(h);
+    return ERTGPU_OK;
+}
+
+bool same_protocol(const ertgpu_protocol& a, const ertgpu_protocol& b) {
+    return strncmp(a.name, b.name, sizeof(a.name)) == 0 && strncmp(a.preamble, b.preamble, sizeof(a.preamble)) == 0 &&
+           a.data_rate == b.data_rate && a.chip_length == b.chip_length && a.preamble_symbols == b.preamble_symbols &&
+           a.packet_symbols == b.packet_symbols && a.center_freq == b.center_freq && a.check_kind == b.check_kind &&
+           a.crc_init == b.crc_init && a.crc_poly == b.crc_poly && a.crc_residue == b.crc_residue &&
+           a.crc_from == b.crc_from && a.crc_to == b.crc_to;
+}
+
+// The rules of ertgpu_decode_channels and then each handle's own call rules (ertgpu.h), before anything changes.  The
+// message of a broken rule goes to hs[0].
+int check_channels(ertgpu_handle* const* hs, int32_t n, const void* iq, size_t nbytes, bool device) {
+    if (!hs || n < 1) return ERTGPU_EINVAL;
+    ertgpu_handle* h0 = hs[0];
+    if (n > ERTGPU_MAX_CHANNELS) return fail(h0, ERTGPU_EINVAL, "%d channels: one call takes 1 ... %d", n, ERTGPU_MAX_CHANNELS);
+    for (int k = 0; k < n; k++) {
+        if (!hs[k] || !hs[k]->allocated) return fail(h0, ERTGPU_EINVAL, "channel %d: the handle is not allocated", k);
+        for (int j = 0; j < k; j++)
+            if (hs[j] == hs[k]) return fail(h0, ERTGPU_EINVAL, "channel %d is the handle of channel %d again", k, j);
+    }
+    for (int k = 0; k < n; k++) {
+        const ertgpu_handle* h = hs[k];
+        if (!h->in.tuned) return fail(h0, ERTGPU_EINVAL, "channel %d is not tuned (ertgpu_set_input_tuning)", k);
+        if (h->device != h0->device)
+            return fail(h0, ERTGPU_EINVAL, "channel %d is on device %d, channel 0 on device %d", k, h->device, h0->device);
+        bool same = h->protos.size() == h0->protos.size();
+        for (size_t i = 0; same && i < h->protos.size(); i++) same = same_protocol(h->protos[i], h0->protos[i]);
+        if (!same) return fail(h0, ERTGPU_EINVAL, "channel %d decodes other protocols or another chip length than channel 0", k);
+        if (h->in.fmt != h0->in.fmt || h->in.scale != h0->in.scale)
+            return fail(h0, ERTGPU_EINVAL, "channel %d has another input format or scale than channel 0", k);
+        // (the same rate gives every decimating handle the same first stage: D and T1 do not depend on the channel)
+        if (h->in.rate_in != h0->in.rate_in || h->in.capture_hz != h0->in.capture_hz)
+            return fail(h0, ERTGPU_EINVAL, "channel %d has another input rate or capture centre than channel 0", k);
+        if (h->in.received() != h0->in.received())
+            return fail(h0, ERTGPU_EINVAL, "channel %d is at input sample %lld of its stream, channel 0 at %lld: reset the channels together",
+                        k, (long long)h->in.received(), (long long)h0->in.received());
+    }
+    for (int k = 0; k < n; k++)
+        if (const int rc = check_decode(hs[k], iq, nbytes, device)) {
+            if (k) fail(h0, rc, "channel %d: %s", k, hs[k]->err.c_str());
+            return rc;
+        }
     return ERTGPU_OK;
 }
 
@@ -1051,6 +1126,69 @@ int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t f
     CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));  // a step that launched nothing still copied from iq
     h->launches = launches;
     return deliver(h, out, cap, n_out);
+}
+
+int ertgpu_decode_channels_device_async(ertgpu_handle* const* hs, int32_t n, const void* d_iq, size_t nbytes, uint32_t flags,
+                                        void* stream) {
+    if (const int rc = check_channels(hs, n, d_iq, nbytes, true)) return rc;
+    for (int k = 0; k < n; k++)
+        if (const int rc = begin_decode(hs[k], d_iq, nbytes, true)) return rc;
+    if (nbytes == 0) return ERTGPU_OK;
+    return enqueue_channels(hs, n, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / hs[0]->in.sample_bytes), flags,
+                            stream ? (cudaStream_t)stream : hs[0]->stream);
+}
+
+// ertgpu_decode's loop over hs[0]'s staging buffers and streams, with every channel's step behind each chunk's copy.
+int ertgpu_decode_channels(ertgpu_handle* const* hs, int32_t n, const uint8_t* iq, size_t nbytes, uint32_t flags) {
+    if (const int rc = check_channels(hs, n, iq, nbytes, false)) return rc;
+    for (int k = 0; k < n; k++)
+        if (const int rc = begin_decode(hs[k], iq, nbytes, false)) return rc;
+    ertgpu_handle* h = hs[0];
+    const size_t s = (size_t)h->in.sample_bytes;
+    const int64_t total = (int64_t)(nbytes / s);
+    if (total == 0) return ERTGPU_OK;
+    int64_t chunk = 0;
+    for (int k = 0; k < n; k++) chunk = std::max(chunk, hs[k]->in.chunk());
+    bool pageable = true;
+    int rc = prepare_staging(h, (size_t)chunk * s, iq, &pageable);
+    if (rc) return rc;
+    // At the decoder's own rate the channel at the capture's centre is not resampled (it only converts, if anything) and
+    // takes whole blocks: then every step does.
+    bool whole_blocks = false;
+    for (int j = 0; j < n; j++) whole_blocks |= !hs[j]->in.resamples();
+    const int64_t block = h->dcfg.BS;
+    int64_t launches[ERTGPU_MAX_CHANNELS] = {};
+    int64_t done = 0;
+    for (int64_t i = 0; done < total; i++) {
+        const int k = (int)(i & 1);
+        int64_t c = total - done;
+        for (int j = 0; j < n; j++) c = std::min(c, hs[j]->in.next_chunk(total - done));  // a step every channel takes
+        if (whole_blocks) c -= c % block;
+        if (c <= 0) return fail(h, ERTGPU_EINVAL, "no step of whole blocks fits every channel's buffers");
+        if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));
+        const uint8_t* src = iq + (size_t)done * s;
+        if (pageable) {
+            h->copy_pool->copy(h->h_stage[k], src, (size_t)c * s);
+            src = h->h_stage[k];
+        }
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * s, cudaMemcpyHostToDevice, h->copy_stream));
+        CUDA_TRY(h, cudaEventRecord(h->ev_h2d[k], h->copy_stream));
+        if (i >= 1)
+            for (int j = 0; j < n; j++)
+                if ((rc = collect(hs[j]))) return rc;
+        CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[k], 0));
+        if ((rc = enqueue_channels(hs, n, h->d_stage[k], c, flags, h->stream))) return rc;
+        for (int j = 0; j < n; j++) launches[j] += hs[j]->launches;
+        CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
+        done += c;
+    }
+    for (int j = 0; j < n; j++) {
+        if ((rc = collect(hs[j]))) return rc;
+        hs[j]->launches = launches[j];
+    }
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));
+    return ERTGPU_OK;
 }
 
 int ertgpu_last_counts(ertgpu_handle* h, int64_t* n_candidates, int64_t* n_valid) {

@@ -2,7 +2,8 @@
 // the demod reads.  It owns the input's format, rate and tuning (ertgpu_set_input_*), the mode they resolve to, the
 // resampler's plan, tables and stream position, and it launches the one kernel in front of the pipeline:
 // convert_kernel<F> (convert.cuh) or resample_kernel<F, TUNED> (resample.cuh), or the two of a decimating handle:
-// decimate_kernel<F> (decimate.cuh) into resample_kernel<cu8, false>.  It also measures the level of its input with
+// decimate_kernel<F> (decimate.cuh) into resample_kernel<cu8, false>.  The first stage of several decimating channels of
+// one capture can run as one decimate_channels_kernel<F> (launch_channels).  It also measures the level of its input with
 // level_kernel<F> (level.cuh) for ertgpu_measure_input.  Host code only.
 #pragma once
 
@@ -51,6 +52,7 @@ struct InputStep {
     int64_t nblocks = 0;
     RsArgs rs{};                  // the kernel's arguments (convert_kernel reads rs.cur only)
     DcArgs dc{};                  // decimate_kernel's (kDecimate): rs.cur is then its output
+    bool shared_first = false;    // decimate_channels_kernel ran the first stage for a group of channels (launch_channels)
 };
 
 struct InputStage {
@@ -88,7 +90,7 @@ struct InputStage {
     int cur_hist = 0;
     uint8_t* d_out[2] = {nullptr, nullptr};   // [partial block | new outputs]; the demod reads whole blocks of it
     int cur_out = 0;
-    int64_t in_total = 0;       // input samples received since the stream start
+    int64_t in_total = 0;       // input samples received since the stream start (the second stage's in kDecimate)
     int64_t out_next = 0;       // first output not yet computed
     int64_t hist_first = 0, hist_n = 0;  // the input samples held in d_hist[cur_hist]
     int64_t pend = 0;           // outputs at the front of d_out[cur_out] that wait for a whole block
@@ -105,8 +107,12 @@ struct InputStage {
     int64_t hist1_first = 0, hist1_n = 0;  // (the first stage's next output is the second stage's in_total)
     size_t smem1 = 0;
     int grid1 = 0, per1 = 0;
+    size_t smem1c = 0;          // the same for decimate_channels_kernel
+    int grid1c = 0, per1c = 0;
 
     bool resamples() const { return mode >= kResample; }
+    // Input samples received since the stream start.
+    int64_t received() const { return mode == kDecimate ? in1_total : in_total; }
 
     // ---- configuration (the handle is not allocated; rate_out = DataRate * ChipLength) ----
     int set_rate(int64_t hz, int64_t rate_out) {
@@ -362,7 +368,7 @@ struct InputStage {
     // Enqueue the step's kernel on st, if it has one, and count it in *launches.
     int launch(const InputStep& s, cudaStream_t st, int64_t* launches) const {
         if (mode == kDecimate) {
-            if (s.dc.count > 0 || s.dc.carry_n > 0) {
+            if (!s.shared_first && (s.dc.count > 0 || s.dc.carry_n > 0)) {
                 const long long tiles = (s.dc.count + (long long)kDcThreads * per1 - 1) / ((long long)kDcThreads * per1);
                 const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid1));
                 decimate_kernel_of(fmt)<<<g, kDcThreads, smem1, st>>>(d_taps, s.dc);
@@ -396,6 +402,30 @@ struct InputStage {
         return ERTGPU_OK;
     }
 
+    // Enqueue decimate_channels_kernel on st for the first stage of the n steps s[0..n) of a group of decimating
+    // channels of one capture (this stage is s[0]'s; the others share its format, gain, plan, tables and stream position),
+    // and mark each step's first stage as done.  Counted in *launches.
+    int launch_channels(InputStep* s, int n, cudaStream_t st, int64_t* launches) const {
+        const DcArgs& a = s[0].dc;
+        DcChannels ch{};
+        ch.n = n;
+        for (int k = 0; k < n; k++) {
+            ch.W[k] = s[k].dc.W;
+            ch.out[k] = s[k].dc.out;
+            ch.carry_dst[k] = s[k].dc.carry_dst;
+            s[k].shared_first = true;
+        }
+        if (a.count <= 0 && a.carry_n <= 0) return ERTGPU_OK;
+        DcArgs ac = a;
+        ac.per = per1c;
+        const long long tiles = (a.count + (long long)kDcThreads * per1c - 1) / ((long long)kDcThreads * per1c);
+        const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid1c));
+        fmt_visit(fmt, [&](auto f) { decimate_channels_kernel<f()><<<g, kDcThreads, smem1c, st>>>(d_taps, ac, ch); });
+        CUDA_TRY(err_, cudaGetLastError());
+        ++*launches;
+        return ERTGPU_OK;
+    }
+
     // Enqueue level_kernel over n input samples at d_in (device, 16-byte aligned) on st: their counts are added to d_level.
     int launch_level(const uint8_t* d_in, int64_t n, cudaStream_t st) const {
         const long long nbytes = n * sample_bytes, groups = (nbytes + 15) / 16;
@@ -409,7 +439,10 @@ struct InputStage {
 
     // The step's kernel is enqueued: advance the stream position.
     void commit(const InputStep& s) {
-        if (!resamples()) return;
+        if (!resamples()) {  // whole blocks only (check_call)
+            in_total += s.nblocks * block;
+            return;
+        }
         if (mode == kDecimate) {
             in1_total += s.dc.cur_n;
             hist1_first = s.dc.carry_first;
@@ -426,14 +459,15 @@ struct InputStage {
         if (s.nblocks > 0) cur_out ^= 1;  // the outputs past the last whole block are already at the front of the other buffer
     }
 
-    // The stage's kernel as ertgpu_last_kernels names it ("" in pass-through mode).
-    std::string label() const {
+    // The stage's kernels as ertgpu_last_kernels names them ("" in pass-through mode); `shared`: the first stage ran as
+    // decimate_channels_kernel.
+    std::string label(bool shared = false) const {
         const char* f = fmt_name(fmt);
         switch (mode) {
             case kPass: return "";
             case kConvert: return std::string("convert_kernel<") + f + ">";
             case kResample: return fmt == ERTGPU_FORMAT_CU8 ? "resample_kernel" : std::string("resample_kernel<") + f + ">";
-            case kDecimate: return std::string("decimate_kernel<") + f + ">;resample_kernel<cu8>";
+            case kDecimate: return std::string(shared ? "decimate_channels_kernel<" : "decimate_kernel<") + f + ">;resample_kernel<cu8>";
             default: return std::string("resample_kernel<") + f + ",tuned>";
         }
     }
@@ -536,6 +570,14 @@ private:
         int per_sm = 0;
         CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decimate_kernel_of(fmt), kDcThreads, smem1));
         grid1 = std::max(1, per_sm) * sm_count;
+        per1c = dc_per_thread(dec.D, dec.T1, kDcChannelsSpanWords);
+        smem1c = dc_channels_smem_bytes(dec.D, dec.T1, per1c);
+        if (smem1c > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "decimator needs %zu B of shared memory", smem1c);
+        const void* kc = nullptr;
+        fmt_visit(fmt, [&](auto f) { kc = (const void*)decimate_channels_kernel<f()>; });
+        CUDA_TRY(err_, cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kc, kDcThreads, smem1c));
+        grid1c = std::max(1, per_sm) * sm_count;
         return ERTGPU_OK;
     }
 

@@ -65,6 +65,9 @@ def lib():
         L.erthost_parse_dedup.restype = C.c_longlong
         L.erthost_parse_dedup.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.POINTER(_Msg), C.c_longlong,
                                           C.POINTER(C.c_longlong)]
+        L.erthost_parse_dedup_channels.restype = C.c_longlong
+        L.erthost_parse_dedup_channels.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_int,
+                                                   C.POINTER(_Msg), C.POINTER(C.c_int), C.c_longlong, C.POINTER(C.c_longlong)]
         L.erthost_parse_filtered.restype = C.c_longlong
         L.erthost_parse_filtered.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_char_p, C.c_char_p, C.c_int, C.c_int,
                                              C.POINTER(_Msg), C.c_longlong, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
@@ -121,6 +124,24 @@ def _parse_dedup(self, cands: np.ndarray, block_dedup: bool = True, cap: int = 4
 
 
 Parsers.parse_dedup = _parse_dedup
+
+
+def _parse_dedup_channels(self, per_channel, block_dedup: bool = True, cap: int = 4096):
+    """parse() of each channel's candidates (a list of arrays, one per channel of one capture), then the receiver's
+    cross-channel dedup in its print order (ascending block, then channel): ([(channel, message)], duplicates dropped)."""
+    cands = np.ascontiguousarray(np.concatenate(per_channel)) if per_channel else np.zeros(0, np.uint8)
+    counts = (C.c_longlong * len(per_channel))(*[len(c) for c in per_channel])
+    out, chan = (_Msg * cap)(), (C.c_int * cap)()
+    dup = C.c_longlong(0)
+    n = self._L.erthost_parse_dedup_channels(self._h, cands.ctypes.data, counts, len(per_channel), 1 if block_dedup else 0,
+                                             out, chan, cap, C.byref(dup))
+    if n < 0:
+        raise RuntimeError(self._L.erthost_error(self._h).decode())
+    n = min(n, cap)
+    return list(zip(chan[:n], _messages(out, n))), int(dup.value)
+
+
+Parsers.parse_dedup_channels = _parse_dedup_channels
 
 
 def _parse_filtered(self, cands, filterid: str = "", filtertype: str = "", unique: bool = False, block_dedup: bool = True,

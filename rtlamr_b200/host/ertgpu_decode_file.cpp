@@ -5,7 +5,7 @@
 //   ertgpu_decode_file [-msgtype=scm,idm|all] [-symbollength=72] [-blockdedup=true] [-blocks=4096] [-device=0]
 //                      [-filterid=1,2] [-filtertype=4,5] [-unique=true] [-format=plain|csv|json|xml]
 //                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ]
-//                      [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|cf64_be|wav|sigmf] [-samplescale=G|auto] [-capturefreq=HZ [-centerfreq=HZ]]
+//                      [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|cf64_be|wav|sigmf] [-samplescale=G|auto] [-capturefreq=HZ [-centerfreq=HZ[,HZ...]]]
 //                      FILE|- [FILE ...]
 // -capturefreq names the frequency the capture was recorded centred at; -centerfreq (rtlamr's flag) the channel to
 // receive, by default the protocols' CenterFreq (912.6 MHz, or 912.38 MHz for r900 alone).  The channel is mixed to
@@ -41,6 +41,13 @@
 // -single stops after the first reported message or, with -filterid, once every listed meter has reported.  -duration
 // (Go duration syntax, 0 = no limit) is checked before each read of -blocks blocks: the call in progress is decoded and
 // reported in full, so the run can last one call longer than asked.  Both end the run with exit status 0.
+// -centerfreq=F1,F2,... (with a capture frequency: -capturefreq or the SigMF metadata) decodes several channels of the
+// capture in one pass: each chunk is read and sent to the GPU once, every channel is decoded from it exactly as a run
+// with that channel alone decodes it, and the messages are printed by ascending block, then channel in the order given.
+// The cross-block dedup spans the channels: a message is dropped when its digest was seen for the previous block in any
+// channel, or for the same block in an earlier channel, so a packet where two channels overlap is printed once
+// (-blockdedup=false prints it from each).  The decoder log's CenterFreq lists every channel and the summary counts each
+// channel's messages.  -samplescale=auto measures the stream once and sets that gain on every channel.
 // Several files are a batch of independent streams through ONE decoder (buffers, tables and kernels set up once):
 // each starts from zeroed history with block numbers from 0, exactly as if it were decoded alone.  They share the
 // sample file, whose offsets keep growing from one file to the next.
@@ -54,6 +61,7 @@
 #include <tuple>
 #include <vector>
 
+#include "../../include/ertgpu_resample.h"
 #include "receiver.hpp"
 #include "sigmf.hpp"
 #include "wav.hpp"
@@ -100,22 +108,41 @@ int main(int argc, char** argv) {
                         "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
                         "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|wav|sigmf] "
                         "[-samplescale=G|auto] "
-                        "[-capturefreq=HZ [-centerfreq=HZ]] [-quiet] FILE|- [FILE ...]\n", argv[0]);
+                        "[-capturefreq=HZ [-centerfreq=HZ[,HZ...]]] [-quiet] FILE|- [FILE ...]\n", argv[0]);
         return 2;
     }
-    // -capturefreq / -centerfreq: whole Hz, > 0 and >= 0
+    // -capturefreq / -centerfreq: whole Hz, > 0 and >= 0; -centerfreq may be a comma list of channels
+    std::vector<std::string> centers;
+    for (size_t p = 0; !centerfreq.empty();) {
+        const size_t q = centerfreq.find(',', p);
+        centers.push_back(centerfreq.substr(p, q == std::string::npos ? std::string::npos : q - p));
+        if (q == std::string::npos) break;
+        p = q + 1;
+    }
     long long capture_hz = 0, center_hz = 0;
-    for (auto [flag, text, out, min] : {std::make_tuple("-capturefreq", &capturefreq, &capture_hz, 1LL),
-                                        std::make_tuple("-centerfreq", &centerfreq, &center_hz, 0LL)}) {
-        if (text->empty()) continue;
+    std::vector<long long> list;
+    std::vector<std::tuple<const char*, const std::string*, long long*, long long>> freqs = {
+        std::make_tuple("-capturefreq", &capturefreq, &capture_hz, 1LL)};
+    if (centers.size() == 1) freqs.push_back(std::make_tuple("-centerfreq", &centerfreq, &center_hz, 0LL));
+    list.resize(centers.size() > 1 ? centers.size() : 0);
+    for (size_t c = 0; c < list.size(); c++) freqs.push_back(std::make_tuple("-centerfreq", &centers[c], &list[c], 1LL));
+    for (auto [flag, text, out, min] : freqs) {
+        if (text->empty() && text == &capturefreq) continue;
         char* end = nullptr;
         errno = 0;
         *out = strtoll(text->c_str(), &end, 10);
-        if (*end || errno || *out < min) {
+        if (text->empty() || *end || errno || *out < min) {
             fprintf(stderr, "invalid value \"%s\" for flag %s: a frequency in Hz%s\n", text->c_str(), flag, min ? " > 0" : "");
             return 2;
         }
     }
+    const std::vector<int64_t> channels(list.begin(), list.end());
+    for (size_t c = 0; c < channels.size(); c++)
+        for (size_t j = 0; j < c; j++)
+            if (channels[c] == channels[j]) {
+                fprintf(stderr, "-centerfreq names the channel %lld Hz twice\n", (long long)channels[c]);
+                return 2;
+            }
     const bool csv = format == "csv", json = format == "json", xml = format == "xml";
     int64_t limit_ns = 0;
     try {
@@ -213,6 +240,20 @@ int main(int argc, char** argv) {
         fprintf(stderr, "-centerfreq needs -capturefreq: the frequency at the centre of the capture\n");
         return 2;
     }
+    if (!channels.empty() && !samplefile.empty() && samplefile != "/dev/null") {
+        fprintf(stderr, "-samplefile takes one channel, not a -centerfreq list\n");
+        return 2;
+    }
+    for (const int64_t ch : channels) {   // each channel of a list lies inside the capture (ertrs_plan_decimated's rule)
+        const int64_t rate = samplerate ? samplerate : 32768LL * chip;
+        ertgpu_decimator_info d{};
+        ertgpu_resampler_info info{};
+        if (ertrs_plan_decimated(rate, 32768LL * chip, ch - capture_hz, &d, &info) != 0) {
+            fprintf(stderr, "-centerfreq channel %lld Hz does not fit a %lld Hz capture at %lld Hz: |offset| + 0.4 * %lld Hz "
+                            "must be at most half the capture's rate\n", (long long)ch, (long long)rate, capture_hz, 32768LL * chip);
+            return 2;
+        }
+    }
     const bool tuned = capture_hz > 0;
     if (have_scale && fmt == ERTGPU_FORMAT_CU8) {
         fprintf(stderr, "-samplescale does not apply to uint8 (cu8) input\n");
@@ -239,8 +280,15 @@ int main(int argc, char** argv) {
         }
     }
     try {
-        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale});
-        fputs(rcvr.decoder().Log().c_str(), stderr);
+        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale},
+                                channels);
+        std::string log = rcvr.decoder().Log();
+        if (!channels.empty()) {   // the channels share everything of the log but CenterFreq, its first line: name them all
+            std::string names;
+            for (size_t c = 0; c < channels.size(); c++) names += (c ? "," : "") + std::to_string(channels[c]);
+            log = "CenterFreq: " + names + log.substr(log.find('\n'));
+        }
+        fputs(log.c_str(), stderr);
         if (sample) rcvr.SetSampleFile(sample);
         if (limit_ns) rcvr.SetDeadline(start + std::chrono::nanoseconds(limit_ns));
         if (single) rcvr.SetSingle(nullptr);
@@ -299,6 +347,9 @@ int main(int argc, char** argv) {
                     files.size() > 1 ? file.c_str() : "", files.size() > 1 ? ": " : "", (long long)st.messages,
                     (long long)st.duplicates, (long long)st.blocks, st.bytes / 1e6, st.seconds,
                     st.samples / 1e6 / (st.seconds > 0 ? st.seconds : 1));
+            for (size_t c = 0; c < channels.size(); c++)
+                fprintf(stderr, "%s%s%lld Hz: %lld messages\n", files.size() > 1 ? file.c_str() : "", files.size() > 1 ? ": " : "",
+                        (long long)channels[c], (long long)st.channel_messages[c]);
             if (st.stopped) break;
         }
     } catch (const std::exception& e) {

@@ -147,6 +147,40 @@ long long erthost_parse_dedup(erthost* h, const ertgpu_candidate* cands, long lo
     }
 }
 
+// erthost_parse_dedup over the candidate lists of nch channels of one capture (counts[c] candidates of channel c, one
+// list after the other in cands): each list is parsed, and the messages go through the cross-channel dedup in the order
+// the receiver prints them (ascending block, then channel).  channel_out[i]: the channel of out[i].
+long long erthost_parse_dedup_channels(erthost* h, const ertgpu_candidate* cands, const long long* counts, int nch,
+                                       int block_dedup, erthost_msg* out, int* channel_out, long long cap, long long* duplicates) {
+    try {
+        std::vector<std::vector<protocol::MessagePtr>> per((size_t)nch);
+        for (int c = 0; c < nch; c++) {
+            h->d.Dispatch(cands, (size_t)counts[c], per[(size_t)c]);
+            cands += counts[c];
+        }
+        receiver::BlockDedup dd;
+        receiver::Stats st;
+        std::vector<size_t> pos((size_t)nch, 0), cnt;
+        std::vector<protocol::MessagePtr*> at;
+        std::vector<protocol::MessagePtr> view;
+        std::vector<int> chan;
+        int64_t b = 0;
+        while (receiver::NextBlock(per, pos, at, cnt, &b))
+            dd.FilterChannels(at.data(), cnt.data(), (size_t)nch, block_dedup != 0, [&](const protocol::Message& m, size_t c) {
+                for (size_t i = 0; i < cnt[c]; i++)
+                    if (at[c][i].get() == &m) view.push_back(std::move(at[c][i]));
+                chan.push_back((int)c);
+                return true;
+            }, st);
+        if (duplicates) *duplicates = st.duplicates;
+        for (size_t i = 0; i < chan.size() && (long long)i < cap; i++) channel_out[i] = chan[i];
+        return fill_msgs(view, out, cap);
+    } catch (const std::exception& e) {
+        h->err = e.what();
+        return -1;
+    }
+}
+
 // erthost_parse, then the receive loop of main.go:236-260 on the result with a fresh memory: the filter chain in the order
 // flag.Visit builds it (main.go:97-113: filterid, filtertype, unique -- lexicographic, whatever the command line's order),
 // then the cross-block digest dedup.  filterid / filtertype: comma lists as for the flags, NULL or "" = flag not given.

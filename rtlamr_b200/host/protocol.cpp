@@ -641,6 +641,34 @@ int64_t Decoder::BlocksDecoded() const {
     return (resampling_ ? ertrs_out_end(&rs_, input_samples_) : input_samples_) / Cfg.BlockSize;
 }
 
+std::vector<std::vector<MessagePtr>> Decoder::DecodeChannels(const std::vector<Decoder*>& ds, const uint8_t* input, size_t len) {
+    if (ds.empty()) throw std::invalid_argument("DecodeChannels without a channel");
+    for (const Decoder* d : ds)
+        if (!d->allocated_) throw std::logic_error("Decode before Allocate");
+    Decoder& d0 = *ds[0];
+    if (len % d0.InputQuantum()) throw std::length_error("input is not a whole number of IQ samples");
+    std::vector<ertgpu_handle*> hs;
+    for (const Decoder* d : ds) hs.push_back(d->h_);
+    int rc = ertgpu_decode_channels(hs.data(), (int32_t)hs.size(), input, len, ERTGPU_DECODE_ONLY_VALID);
+    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(d0.h_));
+    if (rc != ERTGPU_OK) raise(d0.h_, rc, "DecodeChannels");
+    std::vector<std::vector<MessagePtr>> out(ds.size());
+    for (size_t c = 0; c < ds.size(); c++) {
+        Decoder& d = *ds[c];
+        size_t n = 0;
+        if (d.cands_.size() < 1024) d.cands_.resize(1024);
+        rc = ertgpu_fetch(d.h_, d.cands_.data(), d.cands_.size(), &n);
+        if (rc == ERTGPU_ECAPACITY && n > d.cands_.size() && std::string(ertgpu_last_error(d.h_)).find("internal") == std::string::npos) {
+            d.cands_.resize(n);
+            rc = ertgpu_fetch(d.h_, d.cands_.data(), d.cands_.size(), &n);
+        }
+        if (rc != ERTGPU_OK) raise(d.h_, rc, "DecodeChannels");
+        d.input_samples_ += (int64_t)(len / d.sample_bytes_);
+        d.Dispatch(d.cands_.data(), n, out[c]);
+    }
+    return out;
+}
+
 std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
     if (!allocated_) throw std::logic_error("Decode before Allocate");
     if (len % InputQuantum())

@@ -178,6 +178,10 @@ public:
     // of InputQuantum() (BlockSize2 for uint8 IQ at the decoder's rate: the reference panics with a slice-bounds error,
     // decode.go:222).  When resampling, the blocks are those of the resampled stream.
     std::vector<MessagePtr> Decode(const uint8_t* input, size_t len);
+    // Decode on each of ds[0..n), decoders tuned to different channels of one capture (the same protocols, input and
+    // stream position), from ONE pass over input (ertgpu_decode_channels): element c is what ds[c]->Decode returns.  A
+    // group the C ABI refuses throws std::invalid_argument.
+    static std::vector<std::vector<MessagePtr>> DecodeChannels(const std::vector<Decoder*>& ds, const uint8_t* input, size_t len);
     // Whole blocks decoded since Allocate / Reset (resampled blocks with an input rate).
     int64_t BlocksDecoded() const;
     // The second half of Decode (decode.go:177-187 + parse.go): candidates sorted by (block, preamble, idx) are

@@ -13,6 +13,7 @@
 #include <chrono>
 #include <cstdio>
 #include <functional>
+#include <memory>
 #include <set>
 #include <string>
 #include <tuple>
@@ -29,6 +30,7 @@ Digest NewDigest(const protocol::Message& m);
 
 struct Stats {
     int64_t blocks = 0, bytes = 0, samples = 0, messages = 0, duplicates = 0, filtered = 0;   // bytes, samples: input
+    std::vector<int64_t> channel_messages;   // messages reported per channel (Receiver::Run)
     double seconds = 0;
     bool stopped = false;  // -single or -duration ended the run: nothing after it is read
 };
@@ -37,7 +39,9 @@ struct Stats {
 int64_t ParseDuration(const std::string& s);
 
 // The receive loop's prev/next digest maps (main.go:221-224,244-260,292) on their own: a message whose digest was
-// reported for the previous block is dropped; a gap in the block numbers empties the memory.
+// reported for the previous block is dropped; a gap in the block numbers empties the memory.  Across the channels of
+// one capture (FilterChannels) a message is also dropped when an earlier channel reported its digest for the same
+// block, and "the previous block" means any channel's: one channel is exactly the rule above.
 class BlockDedup {
 public:
     // msgs grouped by ascending Block (what Decode returns); `emit` sees every message that is reported.  `fc` is the
@@ -48,6 +52,10 @@ public:
     // main.go:275-277); FilterBlock then returns false too.
     bool FilterBlock(protocol::MessagePtr* msgs, size_t n, bool block_dedup,
                      const std::function<bool(const protocol::Message&)>& emit, Stats& st, FilterChain* fc = nullptr);
+    // The same for ONE block's messages of nch channels, channel c's n[c] messages at msgs[c], in the order the channels
+    // were given; `emit` also sees the channel.
+    bool FilterChannels(protocol::MessagePtr* const* msgs, const size_t* n, size_t nch, bool block_dedup,
+                        const std::function<bool(const protocol::Message&, size_t)>& emit, Stats& st, FilterChain* fc = nullptr);
     void Reset() {
         prev_.clear();
         prev_block_ = -2;
@@ -58,15 +66,26 @@ private:
     int64_t prev_block_ = -2;
 };
 
+// The next block with a message in any of the channels' Decode results per[c] (each grouped by ascending Block), from
+// the cursors pos[c]: its number goes to *block and its messages of channel c to at[c] .. at[c] + n[c], and the cursors
+// move past it.  False when every channel is done.
+bool NextBlock(std::vector<std::vector<protocol::MessagePtr>>& per, std::vector<size_t>& pos,
+               std::vector<protocol::MessagePtr*>& at, std::vector<size_t>& n, int64_t* block);
+
 class Receiver {
 public:
     // msgtypes: comma list as for -msgtype ("all" = scm,scm+,idm,r900, main.go:67-73)
     // input: the capture's rate, format and tuning (protocol::Decoder::SetInput); when it is resampled, blocks, dedup
     // and filters work on the resampled stream.
-    Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, const protocol::Input& input);
+    // channels: the centre frequencies of several channels of one tuned capture (input.CenterFreq is then not read),
+    // decoded in one pass with one protocol::Decoder each: Run reads every chunk once and reports ascending blocks,
+    // channel by channel in this order, through the cross-channel dedup (BlockDedup::FilterChannels).
+    Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall, const protocol::Input& input,
+             const std::vector<int64_t>& channels = {});
     ~Receiver();
 
-    protocol::Decoder& decoder() { return d_; }
+    protocol::Decoder& decoder(size_t channel = 0) { return *d_[channel]; }
+    size_t channels() const { return d_.size(); }
     FilterChain& filters() { return fc_; }   // -filterid / -filtertype / -unique (flags.go:147-170)
 
     // -samplefile (main.go:225-230,279-284): after every block with at least one reported message, the receive loop's
@@ -104,7 +123,7 @@ public:
                 const std::function<void(const protocol::Message&)>& emit, Stats& st);
 
 private:
-    protocol::Decoder d_;
+    std::vector<std::unique_ptr<protocol::Decoder>> d_;   // one per channel
     int64_t blocks_per_call_;
     uint8_t* buf_[2] = {nullptr, nullptr};
     size_t buf_bytes_ = 0;
