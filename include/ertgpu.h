@@ -305,6 +305,39 @@ int ertgpu_measure_input(ertgpu_handle *h, const void *samples, size_t nbytes, e
  * non-finite scale. */
 int ertgpu_set_input_scale(ertgpu_handle *h, float scale);
 
+/* The wide channel path of a tuned handle (include/ertgpu_resample.h has the arithmetic).  Called before
+ * ertgpu_allocate, it makes the handle keep its input at 15 bits (s_w = rint(x * scale * 2^7)) through the mixer and
+ * the channel filter, and form the decoder's byte only from the last stage's accumulator, scaled by the channel gain
+ * 2^k, k in [0, 14].  The gain is then chosen after channel selection, so a weak channel next to a strong one is not
+ * cut to the few bits the strong one leaves it.  Every rate and offset the tuned handle takes is accepted, and a wide
+ * handle at the decoder's own rate and offset 0 still filters (L = M = 1, T = 22).  After ertgpu_allocate it changes k
+ * only at a stream start (after allocate or ertgpu_reset, before the next decode call); k survives ertgpu_reset.
+ * ertgpu_last_kernels names the wide instances (resample_kernel<F,tuned,wide>, or decimate_kernel<F,wide> and
+ * resample_kernel<mid16,tuned,wide>), ERTGPU_TAP_RESAMPLED returns the wide path's bytes.  ERTGPU_EINVAL on an
+ * untuned handle, on a handle allocated without the wide path, for k outside [0, 14], and after a decode call.
+ * Handles that never call it decode exactly as before. */
+int ertgpu_set_channel_gain(ertgpu_handle *h, int32_t k);
+
+/* The channel gain k of a wide handle; ERTGPU_EINVAL when it is not one. */
+int ertgpu_get_channel_gain(const ertgpu_handle *h, int32_t *k);
+
+/* The level of a wide handle's channel: floor(log2 |acc|) of the last stage's output accumulators, and the k the
+ * rule of include/ertgpu_resample.h (ertrs_channel_gain) picks from it. */
+typedef struct {
+    int64_t components;  /* output components measured (2 per output sample)                   */
+    int64_t zeros;       /* of them with acc = 0                                                 */
+    int64_t bins[32];    /* bins[e]: components with 2^e <= |acc| < 2^(e+1)                     */
+    int32_t k;           /* the channel gain the rule picks                                      */
+    int32_t reserved;
+} ertgpu_channel_level;
+
+/* Run the handle's wide input stage over nbytes of samples in HOST memory (pinned or pageable, any whole number of IQ
+ * samples, copied through the handle's staging buffers) as the start of a stream, and histogram the last stage's
+ * accumulators instead of forming bytes.  Nothing of the decode stream changes: its position, history, taps and the
+ * last call's counts are those before the call.  Nothing is applied either: ertgpu_set_channel_gain does that.
+ * ERTGPU_EINVAL before ertgpu_allocate and on a handle without the wide path; ERTGPU_ESIZE for a partial sample. */
+int ertgpu_measure_channel(ertgpu_handle *h, const void *samples, size_t nbytes, ertgpu_channel_level *out);
+
 /* The resampler of a handle with an input rate: *info, and the (P+1)*T int16 prototype table
  * when table != NULL and cap (entries) is large enough; *n_out = number of table entries.
  * ERTGPU_EINVAL when the handle does not resample. */
@@ -349,7 +382,9 @@ int ertgpu_decode_device_async(ertgpu_handle *h, const void *d_iq, size_t nbytes
  *   1 <= n <= ERTGPU_MAX_CHANNELS, and no handle appears twice;
  *   every handle is allocated, on one device, with the same protocols (and so the same chip length);
  *   every handle is tuned (ertgpu_set_input_tuning), with the same capture centre, input rate, format and scale;
- *   every handle is at the same stream position (fresh, or reset together, and fed together since).
+ *   every handle is at the same stream position (fresh, or reset together, and fed together since);
+ *   every handle takes the wide channel path (ertgpu_set_channel_gain), each with its own k, or none does.  Wide
+ *   handles run their first stage each on its own.
  * Otherwise every rule of ertgpu_decode holds for each handle. */
 int ertgpu_decode_channels(ertgpu_handle *const *handles, int32_t n, const uint8_t *iq, size_t nbytes, uint32_t flags);
 

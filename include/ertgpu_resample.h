@@ -233,6 +233,64 @@ static inline void ertrs_mix(int32_t si, int32_t sq, uint32_t e, int32_t* oi, in
     *oq = (sq * c - si * s + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
 }
 
+/*
+ * The wide channel path of a tuned handle (ertgpu_set_channel_gain): the input keeps 15 bits through the mixer and the
+ * channel filter, and the decoder's byte is formed only from the last stage's accumulator, with a channel gain 2^k.
+ *   Wide component  s_w = isnan(p) ? 0 : clamp(rint(p), -16383, 16383), p = (x * g) * 2^7 with convert.cuh's product
+ *                   (fl32(x * g) for components float32 holds exactly, fl64(x * (double)g) otherwise; the * 2^7 is
+ *                   exact), so s_w is 64 * (2u - 255) of the narrow path without its half-LSB offset.  cu8 gives
+ *                   exactly 64 * (2u - 255).  The input history is carried as s_w pairs.
+ *   Mixer           ertrs_mix on s_w.  |s_I C + s_Q S| <= 16383 * max_k(|C| + |S|) = 16383 * 23171 < 2^31, so
+ *                   |s'| <= 23170: one staged word of int16 s'_I | s'_Q, as on the narrow path.
+ *   Filter          the same tables, taps and interpolation into int32 accumulators.  They cannot overflow while
+ *                   (sum_t |c_t| + |delta|) * 23170 < 2^31, i.e. the taps' L1 norm stays below 5.6 * 2^S; the CPU tests
+ *                   check sum_t max(|table[p][t]|, |table[p+1][t]|) + 2T over every row pair of every plan of the
+ *                   ertrs_plan_tuned and ertrs_plan_decimated sweeps, and sum_t |h_t| of every stage-1 plan (its folded
+ *                   pair sums h * (x0 + x1) are bounded by the same |h| (|x0| + |x1|)).
+ *   Between stages  a decimating handle's stage 1 writes s_w pairs: ertrs_wide_mid(acc) = clamp((acc + 2^13) >> 14,
+ *                   +-16383).  Stage 2 is the tuned resampler on them at W = 0: E[0] = (2^14, 0), so s' = s.
+ *   Output byte     u = clamp(((acc + 2^(S+6-k) - 1) >> (S+7-k)) + 128, 0, 255) (ertrs_wide_byte): acc / 2^(S+7) is
+ *                   the channel in the decoder's byte units at k = 0, scaled by 2^k and rounded half down, so that a
+ *                   constant cu8 input u (s_w = 128 (u - 127.5)) comes out as u at k = 0, and an integer one as itself.
+ *   Channel gain    k in [0, ERTRS_GAIN_K_MAX].  At k = 14 the shift S + 7 - k is 7: one s_w unit (2^-7 of a byte at
+ *                   k = 0, the input's own quantisation step) spans 2^7 output LSBs, so a larger k only magnifies the
+ *                   input's rounding, and the shift keeps an integer rounding bias.
+ *   Auto rule       from a histogram of e = floor(log2 |acc|) of the last stage's N output components (bins[e],
+ *                   e in [0, 31]; zeros not binned): k is the largest in [0, K_MAX] at which at most floor(N / 65536)
+ *                   components would clip, counting as clipping every |acc| * 2^k >= 2^(S+14) (128 output LSBs),
+ *                   i.e. e >= S + 14 - k.  k = 0 when no component is non-zero (ertrs_channel_gain).
+ */
+#define ERTRS_WIDE_MAX 16383     /* |s_w|, and |stage-1 output|                                 */
+#define ERTRS_WIDE_BITS 7        /* s_w = rint(x * g * 2^7)                                     */
+#define ERTRS_GAIN_K_MAX 14
+#define ERTRS_GAIN_BINS 32       /* floor(log2 |acc|) of an int32                                */
+#define ERTRS_GAIN_CLIP_SHIFT 16 /* at most N >> 16 components clip                             */
+
+static inline int32_t ertrs_wide_mid(int32_t acc) {
+    const int32_t v = (acc + (1 << (ERTRS_S - 1))) >> ERTRS_S;
+    return v < -ERTRS_WIDE_MAX ? -ERTRS_WIDE_MAX : v > ERTRS_WIDE_MAX ? ERTRS_WIDE_MAX : v;
+}
+
+static inline uint8_t ertrs_wide_byte(int32_t acc, int32_t k) {
+    const int32_t sh = ERTRS_S + ERTRS_WIDE_BITS - k;
+    const int32_t v = ((acc + (1 << (sh - 1)) - 1) >> sh) + 128;
+    return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v);
+}
+
+/* k of the auto rule for bins[ERTRS_GAIN_BINS] of `components` output components */
+static inline int32_t ertrs_channel_gain(const int64_t* bins, int64_t components) {
+    int64_t nonzero = 0;
+    for (int e = 0; e < ERTRS_GAIN_BINS; e++) nonzero += bins[e];
+    if (nonzero == 0) return 0;
+    const int64_t allow = components >> ERTRS_GAIN_CLIP_SHIFT;
+    for (int32_t k = ERTRS_GAIN_K_MAX; k > 0; k--) {
+        int64_t over = 0;
+        for (int e = ERTRS_S + 14 - k; e < ERTRS_GAIN_BINS; e++) over += bins[e];
+        if (over <= allow) return k;
+    }
+    return 0;
+}
+
 /* h(d) * 2^S for the plan's window */
 static inline double ertrs_proto(const ertgpu_resampler_info* info, double d) {
     const double nu = info->rate_out < info->rate_in ? (double)info->rate_out / (double)info->rate_in : 1.0;

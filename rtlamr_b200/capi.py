@@ -68,6 +68,14 @@ class TuningInfo(C.Structure):
                 ("nco_step", C.c_uint32), ("nco_bits", C.c_int32)]
 
 
+class ChannelLevel(C.Structure):
+    _fields_ = [("components", C.c_int64), ("zeros", C.c_int64), ("bins", C.c_int64 * 32), ("k", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+CHANNEL_GAIN_K_MAX = 14
+
+
 class InputLevel(C.Structure):
     _fields_ = [("components", C.c_int64), ("zeros", C.c_int64), ("nans", C.c_int64), ("bins", C.c_int64 * 256),
                 ("exponent", C.c_int32), ("scale", C.c_float)]
@@ -102,6 +110,7 @@ EXPORTS = [
     "ertgpu_set_input_tuning", "ertgpu_get_tuning", "ertgpu_measure_input", "ertgpu_set_input_scale",
     "ertgpu_allow_input_decimation", "ertgpu_get_decimator",
     "ertgpu_decode_channels", "ertgpu_decode_channels_device_async",
+    "ertgpu_set_channel_gain", "ertgpu_get_channel_gain", "ertgpu_measure_channel",
 ]
 
 _lib = None
@@ -166,6 +175,9 @@ def lib() -> C.CDLL:
     L.ertgpu_set_input_scale.argtypes = [vp, C.c_float]
     L.ertgpu_allow_input_decimation.argtypes = [vp]
     L.ertgpu_get_decimator.argtypes = [vp, C.POINTER(DecimatorInfo), vp, sz, C.POINTER(sz)]
+    L.ertgpu_set_channel_gain.argtypes = [vp, i32]
+    L.ertgpu_get_channel_gain.argtypes = [vp, C.POINTER(i32)]
+    L.ertgpu_measure_channel.argtypes = [vp, vp, sz, C.POINTER(ChannelLevel)]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the library does not export it
     _lib = L
@@ -262,6 +274,29 @@ class Handle:
     def set_input_scale(self, scale: float):
         """ertgpu_set_input_scale: the gain of the stream that starts now (after allocate or reset, before decode)."""
         self._check(self._L.ertgpu_set_input_scale(self._h, float(scale)))
+
+    def set_channel_gain(self, k: int):
+        """ertgpu_set_channel_gain: before allocate, the wide channel path of a tuned handle with gain 2^k; after it, k
+        of the stream that starts now."""
+        self._check(self._L.ertgpu_set_channel_gain(self._h, int(k)))
+
+    def channel_gain(self) -> int:
+        """ertgpu_get_channel_gain: k of a wide handle."""
+        k = C.c_int32(0)
+        self._check(self._L.ertgpu_get_channel_gain(self._h, C.byref(k)))
+        return k.value
+
+    def measure_channel(self, buf) -> dict:
+        """ertgpu_measure_channel on a HOST buffer (numpy array, or an address/size pair) of whole samples in the
+        handle's format: {"components", "zeros", "bins" (int64[32], bins[e] for 2^e <= |acc| < 2^(e+1)), "k"}."""
+        if isinstance(buf, tuple):
+            addr, nbytes = buf
+        else:
+            buf = np.ascontiguousarray(buf)
+            addr, nbytes = buf.ctypes.data, buf.nbytes
+        lv = ChannelLevel()
+        self._check(self._L.ertgpu_measure_channel(self._h, addr, nbytes, C.byref(lv)))
+        return {"components": lv.components, "zeros": lv.zeros, "bins": np.array(lv.bins[:], dtype=np.int64), "k": lv.k}
 
     def resampler(self):
         """ertgpu_get_resampler: (info dict, int16 table of (P+1)*T entries)."""
@@ -361,13 +396,15 @@ class Handle:
 
 def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per_call: int = 0,
                 max_candidates: int = 0, input_rate: int = 0, input_format: int = FORMAT_CU8,
-                input_scale: float = 0.0, capture_freq: int = 0, center_freq: int = 0) -> Handle:
+                input_scale: float = 0.0, capture_freq: int = 0, center_freq: int = 0,
+                channel_gain: int | None = None) -> Handle:
     """NewDecoder + RegisterProtocol(NewParser(name, chip_length)) for each name + Allocate
     (reference main.go:64-86).  input_rate > 0: the IQ is sampled at that rate (ertgpu_set_input_rate);
     input_format / input_scale: its sample format and gain (ertgpu_set_input_format, not called for plain cu8);
     capture_freq > 0: the IQ was recorded centred there, and the channel at center_freq (0: the protocols'
     CenterFreq) is decoded (ertgpu_set_input_tuning, before the rate), at up to 256 times the decoder's rate
-    (ertgpu_allow_input_decimation)."""
+    (ertgpu_allow_input_decimation).  channel_gain k: the wide channel path with gain 2^k (ertgpu_set_channel_gain;
+    tuned handles only)."""
     if isinstance(msgtypes, str):
         msgtypes = [m.strip() for m in msgtypes.split(",") if m.strip()]
     h = Handle()
@@ -380,6 +417,8 @@ def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per
         h.set_input_rate(input_rate)
     if input_format != FORMAT_CU8 or input_scale:
         h.set_input_format(input_format, input_scale)
+    if channel_gain is not None:
+        h.set_channel_gain(channel_gain)
     h.allocate(device, max_blocks_per_call, max_candidates)
     return h
 

@@ -164,6 +164,52 @@ __device__ __forceinline__ uchar2 fmt_sample(const uint8_t* src, long long j, fl
     return make_uchar2((unsigned char)fmt_comp<F>(x, 0, g), (unsigned char)fmt_comp<F>(x, 1, g));
 }
 
+// The wide component of the channel path (include/ertgpu_resample.h): s_w = clamp(rint(p * 2^7), +-16383), NaN -> 0,
+// with p the product fmt_byte / fmt_byte_d form.  The * 2^7 is exact, and the clamp comes first, as in fmt_byte.
+__device__ __forceinline__ int fmt_wide(float x, float g) {
+    const float p = __fmul_rn(__fmul_rn(x, g), 128.0f);
+    if (p != p) return 0;
+    return __float2int_rn(fminf(fmaxf(p, -16383.0f), 16383.0f));
+}
+__device__ __forceinline__ int fmt_wide_d(double x, float g) {
+    const double p = __dmul_rn(__dmul_rn(x, (double)g), 128.0);
+    if (p != p) return 0;
+    return __double2int_rn(fmin(fmax(p, -16383.0), 16383.0));
+}
+__device__ __forceinline__ int fmt_wide_x(int8_t x, float g) { return fmt_wide((float)x, g); }
+__device__ __forceinline__ int fmt_wide_x(int16_t x, float g) { return fmt_wide((float)x, g); }
+__device__ __forceinline__ int fmt_wide_x(float x, float g) { return fmt_wide(x, g); }
+__device__ __forceinline__ int fmt_wide_x(int32_t x, float g) { return fmt_wide_d((double)x, g); }
+__device__ __forceinline__ int fmt_wide_x(double x, float g) { return fmt_wide_d(x, g); }
+
+// IQ sample j of format F at src as one word of int16 s_w,I | s_w,Q << 16.
+template <int F>
+__device__ __forceinline__ uint32_t fmt_wide_sample(const uint8_t* src, long long j, float g) {
+    if constexpr (F == ERTGPU_FORMAT_CU8) {
+        const uchar2 u = *reinterpret_cast<const uchar2*>(src + 2 * j);
+        return ((uint32_t)(64 * (2 * (int)u.x - 255)) & 0xffffu) | ((uint32_t)(64 * (2 * (int)u.y - 255)) << 16);
+    } else {
+        constexpr int S = fmt_sample_bytes(F);
+        uint32_t x[(S + 3) / 4];
+        if constexpr (S == 2) {
+            x[0] = *reinterpret_cast<const uint16_t*>(src + 2 * j);
+        } else if constexpr (S == 4) {
+            x[0] = *reinterpret_cast<const uint32_t*>(src + 4 * j);
+        } else if constexpr (S == 8) {
+            const uint2 v = *reinterpret_cast<const uint2*>(src + 8 * j);
+            x[0] = v.x;
+            x[1] = v.y;
+        } else {
+            const uint4 v = *reinterpret_cast<const uint4*>(src + 16 * j);
+            x[0] = v.x;
+            x[1] = v.y;
+            x[2] = v.z;
+            x[3] = v.w;
+        }
+        return ((uint32_t)fmt_wide_x(fmt_x<F>(x, 0), g) & 0xffffu) | ((uint32_t)fmt_wide_x(fmt_x<F>(x, 1), g) << 16);
+    }
+}
+
 constexpr int kCvtThreads = 256;
 
 // Native-rate conversion of ngroups groups of 8 IQ samples (16 output bytes each) from `in` (16-byte aligned, format

@@ -10,6 +10,7 @@
 #include "../../include/ertgpu.h"
 #include "../../include/ertgpu_resample.h"
 #include "convert.cuh"
+#include "resample.cuh"  // wide_input, rs_mix
 
 namespace ert {
 
@@ -73,7 +74,9 @@ __device__ __forceinline__ uint32_t dc_mix(uchar2 u, const uint32_t* tabE, uint3
 }
 
 // The nloc outputs of a tile from its staged span X (skewed), output m to out[2m..2m+1]: the symmetric taps are
-// folded, so an output takes T1/2 - 1 pair sums and the centre tap, two multiply-adds per pair.
+// folded, so an output takes T1/2 - 1 pair sums and the centre tap, two multiply-adds per pair.  WIDE: output m is the
+// word of int16 ertrs_wide_mid(acc_I) | ertrs_wide_mid(acc_Q) << 16 at out[4m..4m+3].
+template <bool WIDE = false>
 __device__ __forceinline__ void dc_filter(const uint32_t* X, const int* taps, int T1, int D, int nloc, uint8_t* out) {
     const int c = T1 / 2 - 1;
     for (int m = threadIdx.x; m < nloc; m += kDcThreads) {
@@ -89,6 +92,12 @@ __device__ __forceinline__ void dc_filter(const uint32_t* X, const int* taps, in
         const uint32_t xc = X[dc_skew(o + c)];
         ai += taps[c] * (int)(short)(xc & 0xffffu);
         aq += taps[c] * ((int)xc >> 16);
+        if constexpr (WIDE) {
+            const int wi = min(ERTRS_WIDE_MAX, max(-ERTRS_WIDE_MAX, (ai + (1 << (ERTRS_S - 1))) >> ERTRS_S));
+            const int wq = min(ERTRS_WIDE_MAX, max(-ERTRS_WIDE_MAX, (aq + (1 << (ERTRS_S - 1))) >> ERTRS_S));
+            reinterpret_cast<uint32_t*>(out)[m] = ((uint32_t)wi & 0xffffu) | ((uint32_t)wq << 16);
+            continue;
+        }
         const int ui = min(255, max(0, (ai + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
         const int uq = min(255, max(0, (aq + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
         *reinterpret_cast<uchar2*>(out + 2 * m) = make_uchar2((unsigned char)ui, (unsigned char)uq);
@@ -98,9 +107,10 @@ __device__ __forceinline__ void dc_filter(const uint32_t* X, const int* taps, in
 // Persistent grid over tiles of kDcThreads * per outputs.  Each CTA keeps E and the taps in shared memory and stages a
 // tile's input span once, each sample mixed by E[k_g] into one word of int16 s'_I | s'_Q << 16 (s' = 0 before the
 // stream start).  Thread t computes outputs t, t + 256, ... of the tile, each whole (dc_filter).
-template <int F>
-__global__ void __launch_bounds__(kDcThreads) decimate_kernel(const int16_t* __restrict__ g_taps, DcArgs a) {
-    extern __shared__ __align__(16) uint32_t dc_smem[];
+// WIDE: the first stage of the wide channel path (include/ertgpu_resample.h): the staged, carried and written samples
+// are s_w words (wide_input), written by dc_filter<true>.
+template <int F, bool WIDE>
+__device__ __forceinline__ void dc_stage(const int16_t* __restrict__ g_taps, const DcArgs& a, uint32_t* dc_smem) {
     const int T1 = a.T1, c = a.T1 / 2 - 1, D = a.D;
     uint32_t* tabE = dc_smem;
     int* taps = reinterpret_cast<int*>(dc_smem + ERTRS_NCO_N);
@@ -108,8 +118,10 @@ __global__ void __launch_bounds__(kDcThreads) decimate_kernel(const int16_t* __r
     for (int i = threadIdx.x; i < ERTRS_NCO_N; i += kDcThreads) tabE[i] = a.E[i];
     for (int i = threadIdx.x; i <= c; i += kDcThreads) taps[i] = g_taps[i];
     if (blockIdx.x == 0)
-        for (long long i = threadIdx.x; i < a.carry_n; i += kDcThreads)
-            *reinterpret_cast<uchar2*>(a.carry_dst + 2 * i) = dc_input<F>(a, a.carry_first + i);  // carry_first >= 0
+        for (long long i = threadIdx.x; i < a.carry_n; i += kDcThreads) {
+            if constexpr (WIDE) reinterpret_cast<uint32_t*>(a.carry_dst)[i] = wide_input<F>(a, a.carry_first + i);
+            else *reinterpret_cast<uchar2*>(a.carry_dst + 2 * i) = dc_input<F>(a, a.carry_first + i);  // carry_first >= 0
+        }
     const long long tile_n = (long long)kDcThreads * a.per;
     const long long ntiles = (a.count + tile_n - 1) / tile_n;
     const uint32_t dph = (uint32_t)kDcThreads * a.W;  // phase accumulator step between a thread's staged samples
@@ -123,11 +135,35 @@ __global__ void __launch_bounds__(kDcThreads) decimate_kernel(const int16_t* __r
         uint32_t ph = (uint32_t)(j_lo + threadIdx.x) * a.W + (1u << (31 - ERTRS_NCO_BITS));
         for (int i = threadIdx.x; i < nspan; i += kDcThreads, ph += dph) {
             const long long g = j_lo + i;
-            X[dc_skew(i)] = g >= 0 ? dc_mix(dc_input<F>(a, g), tabE, ph) : 0u;
+            if constexpr (WIDE) {
+                uint32_t x = 0;
+                if (g >= 0) {
+                    const uint32_t w = wide_input<F>(a, g);
+                    x = rs_mix((int)(short)(w & 0xffffu), (int)w >> 16, tabE, ph);
+                }
+                X[dc_skew(i)] = x;
+            } else {
+                X[dc_skew(i)] = g >= 0 ? dc_mix(dc_input<F>(a, g), tabE, ph) : 0u;
+            }
         }
         __syncthreads();
-        dc_filter(X, taps, T1, D, (int)(ne - nb), a.out + 2 * (nb - a.n0));
+        if constexpr (WIDE) dc_filter<true>(X, taps, T1, D, (int)(ne - nb), a.out + 4 * (nb - a.n0));
+        else dc_filter(X, taps, T1, D, (int)(ne - nb), a.out + 2 * (nb - a.n0));
     }
+}
+
+template <int F>
+__global__ void __launch_bounds__(kDcThreads) decimate_kernel(const int16_t* __restrict__ g_taps, DcArgs a) {
+    extern __shared__ __align__(16) uint32_t dc_smem[];
+    dc_stage<F, false>(g_taps, a, dc_smem);
+}
+
+// The first stage of a wide decimating handle: s_w words in, s_w words (ertrs_wide_mid) out, into resample_wide_kernel<
+// kFmtMid>.  Same shared memory and tiles as decimate_kernel.
+template <int F>
+__global__ void __launch_bounds__(kDcThreads) decimate_wide_kernel(const int16_t* __restrict__ g_taps, DcArgs a) {
+    extern __shared__ __align__(16) uint32_t dc_smem[];
+    dc_stage<F, true>(g_taps, a, dc_smem);
 }
 
 // The channels of one capture that decimate_channels_kernel serves: channel c mixes with step W[c], writes its outputs

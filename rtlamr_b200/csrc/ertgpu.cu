@@ -591,7 +591,7 @@ int enqueue_step(ertgpu_handle* h, const uint8_t* d_in, int64_t n, uint32_t flag
 // The same for the channels hs[0..n) of one capture (check_channels holds) over the same input.  Decimating channels
 // share one decimate_channels_kernel launch, counted in hs[0]'s launches; the rest is each handle's own step.
 int enqueue_channels(ertgpu_handle* const* hs, int n, const uint8_t* d_in, int64_t cnt, uint32_t flags, cudaStream_t st) {
-    if (n == 1 || hs[0]->in.mode != InputStage::kDecimate) {
+    if (n == 1 || hs[0]->in.mode != InputStage::kDecimate || hs[0]->in.wide) {  // wide: per handle (DESIGN §3.12)
         for (int k = 0; k < n; k++)
             if (const int rc = enqueue_step(hs[k], d_in, cnt, flags, st)) return rc;
         return ERTGPU_OK;
@@ -674,6 +674,9 @@ int check_channels(ertgpu_handle* const* hs, int32_t n, const void* iq, size_t n
         // (the same rate gives every decimating handle the same first stage: D and T1 do not depend on the channel)
         if (h->in.rate_in != h0->in.rate_in || h->in.capture_hz != h0->in.capture_hz)
             return fail(h0, ERTGPU_EINVAL, "channel %d has another input rate or capture centre than channel 0", k);
+        if (h->in.wide != h0->in.wide)
+            return fail(h0, ERTGPU_EINVAL, "channel %d %s the wide channel path and channel 0 %s: every channel of a group takes it or none does",
+                        k, h->in.wide ? "takes" : "does not take", h0->in.wide ? "does" : "does not");
         if (h->in.received() != h0->in.received())
             return fail(h0, ERTGPU_EINVAL, "channel %d is at input sample %lld of its stream, channel 0 at %lld: reset the channels together",
                         k, (long long)h->in.received(), (long long)h0->in.received());
@@ -1009,6 +1012,77 @@ int ertgpu_set_input_scale(ertgpu_handle* h, float scale) {
     if (!h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_scale before allocate: ertgpu_set_input_format takes the scale");
     if (h->started) return fail(h, ERTGPU_EINVAL, "set_input_scale after a decode call: the gain changes only at a stream start");
     return h->in.set_scale(scale);
+}
+
+int ertgpu_set_channel_gain(ertgpu_handle* h, int32_t k) {
+    if (!h) return ERTGPU_EINVAL;
+    if (h->allocated && h->started)
+        return fail(h, ERTGPU_EINVAL, "set_channel_gain after a decode call: the gain changes only at a stream start");
+    return h->in.set_channel_gain(k, h->allocated);
+}
+
+int ertgpu_get_channel_gain(const ertgpu_handle* h, int32_t* k) {
+    if (!h || !h->in.wide) return ERTGPU_EINVAL;
+    if (k) *k = h->in.gain;
+    return ERTGPU_OK;
+}
+
+// ertgpu_measure_input's staging, with the input stage's own steps (begin_measure: from a stream start, on the
+// measurement's histories) counting into d_clevel.  The steps end on the handle's stream before the position comes back.
+int ertgpu_measure_channel(ertgpu_handle* h, const void* samples, size_t nbytes, ertgpu_channel_level* out) {
+    if (!h || !h->allocated) return ERTGPU_EINVAL;
+    if (!h->in.wide) return fail(h, ERTGPU_EINVAL, "measure_channel: the handle does not take the wide channel path");
+    if (!out || (!samples && nbytes)) return fail(h, ERTGPU_EINVAL, "null argument");
+    const size_t s = (size_t)h->in.sample_bytes;
+    if (nbytes % s) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of %zu-byte IQ samples", nbytes, s);
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    if (const int rc = collect_sync(h)) return rc;  // the stream's own last step is done with the histories
+    CUDA_TRY(h, cudaMemsetAsync(h->in.d_clevel, 0, ERTRS_GAIN_BINS * sizeof(unsigned long long), h->stream));
+    const int64_t total = (int64_t)(nbytes / s);
+    int64_t outputs = 0;
+    int rc = ERTGPU_OK;
+    const InputStage::Position pos = h->in.begin_measure();
+    if (total) {
+        bool pageable = true;
+        rc = prepare_staging(h, (size_t)h->in.chunk() * s, samples, &pageable);
+        const uint8_t* src0 = static_cast<const uint8_t*>(samples);
+        int64_t done = 0, launches = 0;
+        for (int64_t i = 0; rc == ERTGPU_OK && done < total; i++) {
+            const int k = (int)(i & 1);
+            const int64_t c = h->in.next_chunk(total - done);
+            if (i >= 2 && cudaEventSynchronize(h->ev_done[k]) != cudaSuccess) { rc = fail(h, ERTGPU_ECUDA, "measure_channel: event wait failed"); break; }
+            const uint8_t* src = src0 + (size_t)done * s;
+            if (pageable) {
+                h->copy_pool->copy(h->h_stage[k], src, (size_t)c * s);
+                src = h->h_stage[k];
+            }
+            if (cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * s, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) {
+                rc = fail(h, ERTGPU_ECUDA, "measure_channel: copy failed");
+                break;
+            }
+            InputStep st = h->in.plan(h->d_stage[k], c);
+            st.rs.level = h->in.d_clevel;
+            if ((rc = h->in.launch(st, h->stream, &launches))) break;
+            if (cudaEventRecord(h->ev_done[k], h->stream) != cudaSuccess) { rc = fail(h, ERTGPU_ECUDA, "measure_channel: event record failed"); break; }
+            outputs += st.rs.count;
+            h->in.commit(st);
+            done += c;
+        }
+    }
+    unsigned long long cnt[ERTRS_GAIN_BINS];
+    const cudaError_t e1 = cudaMemcpyAsync(cnt, h->in.d_clevel, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream);
+    const cudaError_t e2 = cudaStreamSynchronize(h->stream);
+    h->in.end_measure(pos);
+    if (rc) return rc;
+    CUDA_TRY(h, e1);
+    CUDA_TRY(h, e2);
+    memset(out, 0, sizeof(*out));
+    out->components = 2 * outputs;
+    int64_t nonzero = 0;
+    for (int b = 0; b < ERTRS_GAIN_BINS; b++) nonzero += out->bins[b] = (int64_t)cnt[b];
+    out->zeros = out->components - nonzero;
+    out->k = ertrs_channel_gain(out->bins, out->components);
+    return ERTGPU_OK;
 }
 
 // Each chunk is copied to d_stage[k] and counted by level_kernel on the handle's stream; pageable input is staged through

@@ -3,8 +3,10 @@
 // resampler's plan, tables and stream position, and it launches the one kernel in front of the pipeline:
 // convert_kernel<F> (convert.cuh) or resample_kernel<F, TUNED> (resample.cuh), or the two of a decimating handle:
 // decimate_kernel<F> (decimate.cuh) into resample_kernel<cu8, false>.  The first stage of several decimating channels of
-// one capture can run as one decimate_channels_kernel<F> (launch_channels).  It also measures the level of its input with
-// level_kernel<F> (level.cuh) for ertgpu_measure_input.  Host code only.
+// one capture can run as one decimate_channels_kernel<F> (launch_channels).  A tuned handle on the wide channel path
+// (ertgpu_set_channel_gain) runs resample_wide_kernel<F>, or decimate_wide_kernel<F> into resample_wide_kernel<kFmtMid>,
+// instead.  It also measures the level of its input with level_kernel<F> (level.cuh) for ertgpu_measure_input, and that
+// of its channel with the wide kernels (begin_measure) for ertgpu_measure_channel.  Host code only.
 #pragma once
 
 #include <algorithm>
@@ -73,6 +75,8 @@ struct InputStage {
     int64_t capture_hz = 0, center_hz = 0;
     uint32_t nco_step = 0;      // W at the input rate in effect
     bool decimation = false;    // allow_decimation: a tuned handle may take up to 256:1
+    bool wide = false;          // set_channel_gain before allocate: the wide channel path (include/ertgpu_resample.h)
+    int32_t gain = 0;           // its channel gain k
     Mode mode = kPass;
     ertgpu_resampler_info rs{};  // the resampler (the second stage in kDecimate)
     std::vector<int16_t> table;
@@ -109,6 +113,10 @@ struct InputStage {
     int grid1 = 0, per1 = 0;
     size_t smem1c = 0;          // the same for decimate_channels_kernel
     int grid1c = 0, per1c = 0;
+    // the wide path's channel measurement: its own input histories, swapped in by begin_measure, and its counters
+    uint8_t* d_mhist[2] = {nullptr, nullptr};
+    uint8_t* d_mhist1[2] = {nullptr, nullptr};
+    unsigned long long* d_clevel = nullptr;
 
     bool resamples() const { return mode >= kResample; }
     // Input samples received since the stream start.
@@ -163,8 +171,23 @@ struct InputStage {
         return ERTGPU_OK;
     }
 
-    // At allocate: a tuned handle at the decoder's own rate gets its plan here, and the channel must lie inside it.
-    int plan_native(int64_t rate_out) { return tuned && !rate_in ? configure_rate(rate_out, rate_out) : ERTGPU_OK; }
+    // At allocate: a tuned handle at the decoder's own rate gets its plan here, and the channel must lie inside it.  A
+    // wide handle's plan is made again here, whenever set_channel_gain came: it always filters.
+    int plan_native(int64_t rate_out) {
+        if (!tuned || (rate_in && !wide)) return ERTGPU_OK;
+        return configure_rate(rate_in ? rate_in : rate_out, rate_out);
+    }
+
+    // The wide channel path with gain 2^k: before allocate (which plans it), or at a stream start of a wide handle (the
+    // caller checks which).
+    int set_channel_gain(int32_t k, bool allocated) {
+        if (!tuned) return fail(err_, ERTGPU_EINVAL, "set_channel_gain on an untuned handle: it needs set_input_tuning");
+        if (allocated && !wide) return fail(err_, ERTGPU_EINVAL, "set_channel_gain: the handle was allocated without the wide channel path");
+        if (k < 0 || k > ERTRS_GAIN_K_MAX) return fail(err_, ERTGPU_EINVAL, "channel gain 2^%d: k must be within 0 ... %d", k, ERTRS_GAIN_K_MAX);
+        wide = true;
+        gain = k;
+        return ERTGPU_OK;
+    }
 
     int tuning(ertgpu_tuning_info* info) const {
         if (!tuned) return ERTGPU_EINVAL;
@@ -224,11 +247,13 @@ struct InputStage {
             CUDA_TRY(err_, cudaMalloc(&d_E, E.size() * sizeof(uint32_t)));
             CUDA_TRY(err_, cudaMemcpy(d_E, E.data(), E.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
         }
+        const size_t hb = wide ? 4 : 2;  // bytes per carried sample: s_w words on the wide path
         for (int k = 0; k < 2; k++) {
-            CUDA_TRY(err_, cudaMalloc(&d_hist[k], (size_t)rs.T * 2 + 16));
+            CUDA_TRY(err_, cudaMalloc(&d_hist[k], (size_t)rs.T * hb + 16));
             // a step completes at most max_blocks blocks: less than (max_blocks + 1) * BS outputs are buffered
             CUDA_TRY(err_, cudaMalloc(&d_out[k], (size_t)(max_blocks + 1) * block * 2 + 64));
         }
+        if (wide) return allocate_wide(device, sm_count);
         smem = rs_smem_bytes(rs.P, rs.T, rs.L, rs.M, mix);
         {   // a property of the kernel, not of the handle: every handle on the device gets the largest any table needs
             static OncePerDevice once;
@@ -253,10 +278,13 @@ struct InputStage {
         dfree(d_level);
         dfree(d_taps);
         dfree(d_mid);
+        dfree(d_clevel);
         for (int k = 0; k < 2; k++) {
             dfree(d_hist[k]);
             dfree(d_out[k]);
             dfree(d_hist1[k]);
+            dfree(d_mhist[k]);
+            dfree(d_mhist1[k]);
         }
     }
 
@@ -357,6 +385,8 @@ struct InputStage {
         a->E = d_E;
         a->W = nco_step;
         a->P = rs.P;
+        a->gain = gain;
+        a->level = nullptr;
         const int64_t Q = (int64_t)rs.P << ERTRS_F, step = kRsThreads * M;
         a->step_k = step / L;
         a->step_phi = step % L;
@@ -367,6 +397,7 @@ struct InputStage {
 
     // Enqueue the step's kernel on st, if it has one, and count it in *launches.
     int launch(const InputStep& s, cudaStream_t st, int64_t* launches) const {
+        if (wide) return launch_wide(s, st, launches);
         if (mode == kDecimate) {
             if (!s.shared_first && (s.dc.count > 0 || s.dc.carry_n > 0)) {
                 const long long tiles = (s.dc.count + (long long)kDcThreads * per1 - 1) / ((long long)kDcThreads * per1);
@@ -463,6 +494,9 @@ struct InputStage {
     // decimate_channels_kernel.
     std::string label(bool shared = false) const {
         const char* f = fmt_name(fmt);
+        if (wide)
+            return mode == kDecimate ? std::string("decimate_kernel<") + f + ",wide>;resample_kernel<mid16,tuned,wide>"
+                                     : std::string("resample_kernel<") + f + ",tuned,wide>";
         switch (mode) {
             case kPass: return "";
             case kConvert: return std::string("convert_kernel<") + f + ">";
@@ -472,8 +506,96 @@ struct InputStage {
         }
     }
 
+    // The stream position begin_measure sets aside.
+    struct Position {
+        int64_t in_total, out_next, hist_first, hist_n, pend, in1_total, hist1_first, hist1_n;
+        int cur_hist, cur_out, cur_hist1;
+    };
+
+    // A channel measurement (wide path) runs the stage's own steps from a stream start, with the measurement's input
+    // histories in place of the stream's and rs.level = d_clevel in every step; end_measure puts the stream back.
+    Position begin_measure() {
+        const Position p{in_total, out_next, hist_first, hist_n, pend, in1_total, hist1_first, hist1_n, cur_hist, cur_out, cur_hist1};
+        for (int k = 0; k < 2; k++) {
+            std::swap(d_hist[k], d_mhist[k]);
+            std::swap(d_hist1[k], d_mhist1[k]);
+        }
+        reset_stream();
+        return p;
+    }
+
+    void end_measure(const Position& p) {
+        for (int k = 0; k < 2; k++) {
+            std::swap(d_hist[k], d_mhist[k]);
+            std::swap(d_hist1[k], d_mhist1[k]);
+        }
+        in_total = p.in_total;
+        out_next = p.out_next;
+        hist_first = p.hist_first;
+        hist_n = p.hist_n;
+        pend = p.pend;
+        in1_total = p.in1_total;
+        hist1_first = p.hist1_first;
+        hist1_n = p.hist1_n;
+        cur_hist = p.cur_hist;
+        cur_out = p.cur_out;
+        cur_hist1 = p.cur_hist1;
+    }
+
 private:
     std::string& err_;  // the handle's last error
+
+    // The wide path's kernels: decimate_wide_kernel<F> (kDecimate) into resample_wide_kernel<kFmtMid>, or
+    // resample_wide_kernel<F> alone.
+    int launch_wide(const InputStep& s, cudaStream_t st, int64_t* launches) const {
+        if (mode == kDecimate && (s.dc.count > 0 || s.dc.carry_n > 0)) {
+            const long long tiles = (s.dc.count + (long long)kDcThreads * per1 - 1) / ((long long)kDcThreads * per1);
+            const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid1));
+            fmt_visit(fmt, [&](auto f) { decimate_wide_kernel<f()><<<g, kDcThreads, smem1, st>>>(d_taps, s.dc); });
+            CUDA_TRY(err_, cudaGetLastError());
+            ++*launches;
+        }
+        if (s.rs.count > 0 || s.rs.carry_n > 0) {
+            const long long tiles = (s.rs.count + kRsTile - 1) / kRsTile;
+            const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid));
+            resample_wide_kernel_of(mode == kDecimate ? kFmtMid : fmt)<<<g, kRsThreads, smem, st>>>(d_A, d_D, s.rs);
+            CUDA_TRY(err_, cudaGetLastError());
+            ++*launches;
+        }
+        return ERTGPU_OK;
+    }
+
+    // allocate's end for the wide path: the last stage's launch shape, the measurement's buffers, and the first stage.
+    int allocate_wide(int device, int sm_count) {
+        const bool mid = mode == kDecimate;
+        smem = rs_wide_smem_bytes(rs.P, rs.T, rs.L, rs.M, mid);
+        {
+            static OncePerDevice once;
+            if (once.first(device)) {
+                CUDA_TRY(err_, cudaFuncSetAttribute(resample_wide_kernel_of(kFmtMid), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF64BE; f++)
+                    if (fmt_name(f))
+                        CUDA_TRY(err_, cudaFuncSetAttribute(resample_wide_kernel_of(f), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            }
+        }
+        if (smem > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", smem);
+        int per_sm = 0;
+        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_wide_kernel_of(mid ? kFmtMid : fmt), kRsThreads, smem));
+        grid = std::max(1, per_sm) * sm_count;
+        CUDA_TRY(err_, cudaMalloc(&d_clevel, ERTRS_GAIN_BINS * sizeof(unsigned long long)));
+        for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_mhist[k], (size_t)rs.T * 4 + 16));
+        if (!mid) return ERTGPU_OK;
+        if (const int rc = allocate_first(device, sm_count)) return rc;
+        for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_mhist1[k], (size_t)(dec.T1 + dec.D + 16) * 4));
+        return ERTGPU_OK;
+    }
+
+    static decltype(&resample_wide_kernel<ERTGPU_FORMAT_CU8>) resample_wide_kernel_of(int f) {
+        if (f == kFmtMid) return resample_wide_kernel<kFmtMid>;
+        decltype(&resample_wide_kernel<ERTGPU_FORMAT_CU8>) k = nullptr;
+        fmt_visit(f, [&](auto F) { k = resample_wide_kernel<F()>; });
+        return k;
+    }
 
     // The resampler for input at hz: ertrs_plan, or ertrs_plan_tuned and the NCO step on a tuned handle.  It runs when
     // the rates differ or a tuned handle mixes; the tuned instance when it mixes or its plan has P != ERTRS_P.
@@ -506,13 +628,13 @@ private:
             return fail(err_, ERTGPU_EINVAL, "input rate %lld Hz: the decoder rate %lld Hz must be within 1/4 ... 4 times it",
                         (long long)hz, (long long)rate_out);
         }
-        const bool on = hz != rate_out || w != 0;
+        const bool on = hz != rate_out || w != 0 || wide;
         std::vector<int16_t> t;
         if (on) {
             t.resize((size_t)(info.P + 1) * info.T);
             if (ertrs_build_table(&info, t.data()) != 0) return fail(err_, ERTGPU_EINVAL, "resampler table does not fit int16");
         }
-        mode = !on ? (fmt == ERTGPU_FORMAT_CU8 ? kPass : kConvert) : w != 0 || info.P != ERTRS_P ? kResampleTuned : kResample;
+        mode = !on ? (fmt == ERTGPU_FORMAT_CU8 ? kPass : kConvert) : w != 0 || info.P != ERTRS_P || wide ? kResampleTuned : kResample;
         if (d.D > 1) mode = kDecimate;
         nco_step = w;
         rs = info;
@@ -552,11 +674,12 @@ private:
     int allocate_first(int device, int sm_count) {
         CUDA_TRY(err_, cudaMalloc(&d_taps, taps.size() * sizeof(int16_t)));
         CUDA_TRY(err_, cudaMemcpy(d_taps, taps.data(), taps.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
-        for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_hist1[k], (size_t)(dec.T1 + dec.D + 16) * 2));
+        const size_t hb = wide ? 4 : 2;  // bytes per carried sample, and per stage-1 output
+        for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_hist1[k], (size_t)(dec.T1 + dec.D + 16) * hb));
         // A step hands the second stage fewer than (max_blocks + 1) * block * M / L + M / L + T samples (the blocks a
         // step may complete, plus the look-ahead).
         const int64_t mid = (int64_t)(((__int128)(max_blocks + 1) * block * rs.M + rs.L - 1) / rs.L) + rs.M / rs.L + rs.T + 64;
-        CUDA_TRY(err_, cudaMalloc(&d_mid, (size_t)mid * 2));
+        CUDA_TRY(err_, cudaMalloc(&d_mid, (size_t)mid * hb));
         per1 = dc_per_thread(dec.D, dec.T1);
         smem1 = dc_smem_bytes(dec.D, dec.T1, per1);
         {
@@ -568,6 +691,14 @@ private:
         }
         if (smem1 > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "decimator needs %zu B of shared memory", smem1);
         int per_sm = 0;
+        if (wide) {  // decimate_wide_kernel: decimate_kernel's tiles; groups run it per channel (DESIGN §3.12)
+            const void* kw = nullptr;
+            fmt_visit(fmt, [&](auto f) { kw = (const void*)decimate_wide_kernel<f()>; });
+            CUDA_TRY(err_, cudaFuncSetAttribute(kw, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kw, kDcThreads, smem1));
+            grid1 = std::max(1, per_sm) * sm_count;
+            return ERTGPU_OK;
+        }
         CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decimate_kernel_of(fmt), kDcThreads, smem1));
         grid1 = std::max(1, per_sm) * sm_count;
         per1c = dc_per_thread(dec.D, dec.T1, kDcChannelsSpanWords);

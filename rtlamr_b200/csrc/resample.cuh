@@ -38,7 +38,14 @@ struct RsArgs {
     const uint32_t* E;
     uint32_t W;
     int P;
+    // wide instances only (resample_wide_kernel): the channel gain k, and the histogram that replaces the output bytes
+    // when not null (ertgpu_measure_channel)
+    int gain;
+    unsigned long long* level;
 };
+
+// The input format of a wide cascade's second stage: the first stage's s_w pairs (ertrs_wide_mid), already mixed.
+constexpr int kFmtMid = -1;
 
 // The table as the kernel reads it: A[p][t] = h0 * 2^F + 2^(F-1) (int32), D[p][m] = the int16 pair
 // (h1 - h0 of taps 2m, 2m+1), so that c_t = (A + d * w) >> F.  P rows each.
@@ -65,23 +72,53 @@ __device__ __forceinline__ uchar2 rs_input(const RsArgs& a, long long g) {  // g
     }
 }
 
+// Input sample g of a wide instance as one word of int16 s_w,I | s_w,Q << 16 (include/ertgpu_resample.h): the history
+// and the first stage's output hold such words, cur is converted from format F.
+template <int F, class Args>
+__device__ __forceinline__ uint32_t wide_input(const Args& a, long long g) {  // g >= 0
+    const long long e = a.hist_first + a.hist_n;
+    if (g < e) return reinterpret_cast<const uint32_t*>(a.hist)[g - a.hist_first];
+    if constexpr (F == kFmtMid) return reinterpret_cast<const uint32_t*>(a.cur)[g - e];
+    else return fmt_wide_sample<F>(a.cur, g - e, a.scale);
+}
+
+// s' = s * conj(E[ph >> (32 - NCO_BITS)]) for the int16 pair s, as one word of int16 s'_I | s'_Q << 16 (ertrs_mix).
+__device__ __forceinline__ uint32_t rs_mix(int si, int sq, const uint32_t* tabE, uint32_t ph) {
+    const uint32_t e = tabE[ph >> (32 - ERTRS_NCO_BITS)];
+    const int c = (int)(short)(e & 0xffffu), s = (int)e >> 16;
+    const int mi = (si * c + sq * s + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
+    const int mq = (sq * c - si * s + (1 << (ERTRS_E_S - 1))) >> ERTRS_E_S;
+    return ((uint32_t)mi & 0xffffu) | ((uint32_t)mq << 16);
+}
+
 // The tuned resampler (ertrs_plan_tuned): as below, but every staged sample is mixed by E[k_g] first, so X[j] holds
 // the int16 pair (s'_I[j], s'_Q[j]) with s' = 0 before the stream start, and the taps are plain multiply-adds (dp2a
 // takes only 8-bit samples).  One path serves every output.  P is the plan's (a.P).
-template <int F>
+// WIDE: the channel path of include/ertgpu_resample.h.  The staged and carried samples are s_w words (wide_input), the
+// byte is ertrs_wide_byte at k = a.gain, or, with a.level, floor(log2 |acc|) is counted there instead.  F = kFmtMid
+// reads a first stage's output at W = 0 without mixing (E[0] = (2^14, 0) mixes s to s) and keeps no E.
+template <int F, bool WIDE = false>
 __device__ __forceinline__ void resample_tuned(const int32_t* __restrict__ g_A, const uint32_t* __restrict__ g_D,
                                                const RsArgs& a, int32_t* smem) {
     const int T = a.T, T2 = a.T / 2, P = a.P;
-    int32_t* tabA = smem;
-    uint32_t* tabD = reinterpret_cast<uint32_t*>(smem + P * T);
+    unsigned int* lv = reinterpret_cast<unsigned int*>(smem);  // WIDE: the CTA's level counters, in front of the table
+    int32_t* tabA = WIDE ? smem + ERTRS_GAIN_BINS : smem;
+    uint32_t* tabD = reinterpret_cast<uint32_t*>(tabA + P * T);
     uint32_t* tabE = tabD + P * T2;
-    uint32_t* X = tabE + ERTRS_NCO_N;
+    uint32_t* X = F == kFmtMid ? tabE : tabE + ERTRS_NCO_N;
     for (int i = threadIdx.x; i < P * T; i += kRsThreads) tabA[i] = g_A[i];
     for (int i = threadIdx.x; i < P * T2; i += kRsThreads) tabD[i] = g_D[i];
-    for (int i = threadIdx.x; i < ERTRS_NCO_N; i += kRsThreads) tabE[i] = a.E[i];
-    if (blockIdx.x == 0)
+    if constexpr (F != kFmtMid)
+        for (int i = threadIdx.x; i < ERTRS_NCO_N; i += kRsThreads) tabE[i] = a.E[i];
+    if constexpr (WIDE) {
+        if (threadIdx.x < ERTRS_GAIN_BINS) lv[threadIdx.x] = 0;
+        if (blockIdx.x == 0)
+            for (long long i = threadIdx.x; i < a.carry_n; i += kRsThreads)
+                reinterpret_cast<uint32_t*>(a.carry_dst)[i] = wide_input<F>(a, a.carry_first + i);
+    } else if (blockIdx.x == 0) {
         for (long long i = threadIdx.x; i < a.carry_n; i += kRsThreads)
             *reinterpret_cast<uchar2*>(a.carry_dst + 2 * i) = rs_input<F>(a, a.carry_first + i);  // carry_first >= 0
+    }
     const long long Q = (long long)P << ERTRS_F;
     const long long ntiles = (a.count + kRsTile - 1) / kRsTile;
     const uint32_t dph = (uint32_t)kRsThreads * a.W;  // phase accumulator step between a thread's staged samples
@@ -97,7 +134,12 @@ __device__ __forceinline__ void resample_tuned(const int32_t* __restrict__ g_A, 
         for (int i = threadIdx.x; i < nspan; i += kRsThreads, ph += dph) {
             const long long g = j_lo + i;
             uint32_t xw = 0;
-            if (g >= 0) {
+            if constexpr (WIDE) {
+                if (g >= 0) {
+                    const uint32_t w = wide_input<F>(a, g);
+                    xw = F == kFmtMid ? w : rs_mix((int)(short)(w & 0xffffu), (int)w >> 16, tabE, ph);
+                }
+            } else if (g >= 0) {
                 const uchar2 u = rs_input<F>(a, g);
                 const uint32_t e = tabE[ph >> (32 - ERTRS_NCO_BITS)];
                 const int c = (int)(short)(e & 0xffffu), s = (int)e >> 16;
@@ -141,12 +183,27 @@ __device__ __forceinline__ void resample_tuned(const int32_t* __restrict__ g_A, 
                 const uint32_t xc = x[tc];
                 ai += delta * (int)(short)(xc & 0xffffu);
                 aq += delta * ((int)xc >> 16);
-                const int ui = min(255, max(0, (ai + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
-                const int uq = min(255, max(0, (aq + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
-                const uchar2 o = make_uchar2((unsigned char)ui, (unsigned char)uq);
-                const long long i = n - a.n0;
-                *reinterpret_cast<uchar2*>(a.out + 2 * i) = o;
-                if (i >= a.split) *reinterpret_cast<uchar2*>(a.out2 + 2 * (i - a.split)) = o;
+                if constexpr (WIDE) {
+                    if (a.level) {
+                        if (ai) atomicAdd(&lv[31 - __clz(abs(ai))], 1u);
+                        if (aq) atomicAdd(&lv[31 - __clz(abs(aq))], 1u);
+                    } else {
+                        const int sh = ERTRS_S + ERTRS_WIDE_BITS - a.gain;
+                        const int ui = min(255, max(0, ((ai + (1 << (sh - 1)) - 1) >> sh) + 128));
+                        const int uq = min(255, max(0, ((aq + (1 << (sh - 1)) - 1) >> sh) + 128));
+                        const uchar2 o = make_uchar2((unsigned char)ui, (unsigned char)uq);
+                        const long long i = n - a.n0;
+                        *reinterpret_cast<uchar2*>(a.out + 2 * i) = o;
+                        if (i >= a.split) *reinterpret_cast<uchar2*>(a.out2 + 2 * (i - a.split)) = o;
+                    }
+                } else {
+                    const int ui = min(255, max(0, (ai + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
+                    const int uq = min(255, max(0, (aq + (1 << (ERTRS_S + 8))) >> (ERTRS_S + 1)));
+                    const uchar2 o = make_uchar2((unsigned char)ui, (unsigned char)uq);
+                    const long long i = n - a.n0;
+                    *reinterpret_cast<uchar2*>(a.out + 2 * i) = o;
+                    if (i >= a.split) *reinterpret_cast<uchar2*>(a.out2 + 2 * (i - a.split)) = o;
+                }
                 n += kRsThreads;
                 k += a.step_k;
                 phi += a.step_phi;
@@ -155,6 +212,12 @@ __device__ __forceinline__ void resample_tuned(const int32_t* __restrict__ g_A, 
                 if (r >= a.L) { r -= a.L; q++; }
                 if (phi >= a.L) { phi -= a.L; k++; q -= Q; }
             }
+        }
+    }
+    if constexpr (WIDE) {
+        if (a.level) {
+            __syncthreads();
+            if (threadIdx.x < ERTRS_GAIN_BINS && lv[threadIdx.x]) atomicAdd(a.level + threadIdx.x, (unsigned long long)lv[threadIdx.x]);
         }
     }
 }
@@ -279,6 +342,20 @@ __global__ void __launch_bounds__(kRsThreads) resample_kernel(const int32_t* __r
 inline size_t rs_smem_bytes(int P, int T, long long L, long long M, bool tuned) {
     const long long span = ((kRsTile - 1) * M + L - 1) / L + 1 + T + 1;
     return (size_t)P * T * 6 + (size_t)span * 4 + (tuned ? (size_t)ERTRS_NCO_N * 4 : 0);
+}
+
+// The wide channel path's resampler (include/ertgpu_resample.h): resample_tuned<F, true>, the one stage of a wide tuned
+// handle or, with F = kFmtMid, the second stage of a wide decimating one.
+template <int F>
+__global__ void __launch_bounds__(kRsThreads) resample_wide_kernel(const int32_t* __restrict__ g_A,
+                                                                   const uint32_t* __restrict__ g_D, RsArgs a) {
+    extern __shared__ __align__(16) int32_t rs_smem[];
+    resample_tuned<F, true>(g_A, g_D, a, rs_smem);
+}
+
+// Its shared memory: rs_smem_bytes of a tuned instance (without E for kFmtMid), and the level counters.
+inline size_t rs_wide_smem_bytes(int P, int T, long long L, long long M, bool mid) {
+    return rs_smem_bytes(P, T, L, M, !mid) + ERTRS_GAIN_BINS * 4;
 }
 
 }  // namespace ert

@@ -41,7 +41,8 @@ def lib():
         L = C.CDLL(LIB_PATH)
         L.erthost_new.restype = C.c_void_p
         L.erthost_new.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_int, C.c_float,
-                                  C.c_longlong, C.c_longlong, C.c_int, C.c_char_p, C.c_int]
+                                  C.c_longlong, C.c_longlong, C.c_int, C.c_int, C.c_char_p, C.c_int]
+        L.erthost_channel_gain.argtypes = [C.c_void_p]
         L.erthost_level.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_longlong),
                                     C.POINTER(C.c_longlong)]
         L.erthost_wav_probe.argtypes = [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
@@ -228,21 +229,26 @@ class Receiver:
 
     def __init__(self, msgtypes: str, chip_length: int = 72, device: int = 0, max_blocks: int = 0, max_cands: int = 0,
                  input_rate: int = 0, input_format: int = 0, input_scale: float | str = 0.0, capture_freq: int = 0,
-                 center_freq: int = 0):
+                 center_freq: int = 0, channel_gain: int | str | None = None):
         """The input arguments are protocol::Decoder::SetInput's.  input_rate > 0: the IQ given to decode() is sampled at
         that rate; any rate other than DataRate * ChipLength is resampled on the GPU and decode() then takes any whole
         number of IQ samples.  input_format / input_scale: the IQ's sample format (capi.FORMAT_*) and gain.
         capture_freq > 0: the IQ was recorded centred there; the channel at center_freq (0: the protocols' CenterFreq) is
         decoded.  input_scale="auto": the gain of each stream (until reset()) is measured from the first
         min(len, 2^22) samples of its first decode() call (ertgpu_measure_input) and stays fixed for the stream;
-        input_level() tells which."""
+        input_level() tells which.  channel_gain=k: the wide channel path of a tuned input with gain 2^k
+        (ertgpu_set_channel_gain); "auto": k of each stream is measured from the same samples after the input gain
+        (ertgpu_measure_channel), and channel_gain() tells which."""
         self._L = lib()
         err = C.create_string_buffer(512)
         auto = isinstance(input_scale, str)
         if auto and input_scale != "auto":
             raise ValueError(f"input_scale {input_scale!r}: a gain or 'auto'")
+        if isinstance(channel_gain, str) and channel_gain != "auto":
+            raise ValueError(f"channel_gain {channel_gain!r}: k or 'auto'")
+        cg = -1 if channel_gain is None else -2 if channel_gain == "auto" else int(channel_gain)
         self._h = self._L.erthost_new(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate, input_format,
-                                      0.0 if auto else input_scale, capture_freq, center_freq, 1 if auto else 0, err, 512)
+                                      0.0 if auto else input_scale, capture_freq, center_freq, 1 if auto else 0, cg, err, 512)
         if not self._h:
             raise RuntimeError(err.value.decode())
         v = (C.c_int32 * 12)()
@@ -273,6 +279,11 @@ class Receiver:
         if self._L.erthost_level(self._h, C.byref(k), C.byref(g), C.byref(n), bins) != 0:
             return None
         return {"exponent": k.value, "scale": g.value, "components": n.value, "bins": np.array(bins[:], dtype=np.int64)}
+
+    def channel_gain(self) -> int | None:
+        """k of the wide channel path (for "auto": once the first decode() measured it), or None without it."""
+        k = self._L.erthost_channel_gain(self._h)
+        return None if k < 0 else k
 
     def log(self) -> str:
         b = C.create_string_buffer(2048)

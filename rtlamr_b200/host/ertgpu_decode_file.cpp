@@ -31,7 +31,12 @@
 // a WAV header or SigMF core:header_bytes: the largest k in [-120, 120] at which at most one component in 65 536 clips
 // (include/ertgpu_level.h).  The gain then stays fixed for the whole stream; it does not follow the level the way a tuner's
 // AGC does.  k, G and the number of samples measured go to stderr; stdout is exactly that of -samplescale=G.  A WAV or
-// SigMF file is never detected by its content or name.  -samplefile takes only untuned uint8 input at
+// SigMF file is never detected by its content or name.
+// -channelgain=G (a power of two, 1 ... 2^14) or auto takes the wide channel path of a tuned input (a capture frequency
+// from -capturefreq or the SigMF metadata): the input keeps 15 bits through the mixer and the channel filter, and the
+// decoder's byte is formed from the channel's filtered level times G (include/ertgpu_resample.h).  auto picks G per stream
+// and channel from the stream's first 2^22 samples, after -samplescale=auto has set the input gain from the same samples,
+// and then decodes those bytes; "channel <Hz>: 2^k = G" goes to stderr, and stdout is exactly that of -channelgain=G.  -samplefile takes only untuned uint8 input at
 // 32768 * -symbollength (an 8-bit WAV at that rate is uint8).
 // -filterid / -filtertype / -unique, -format, -samplefile, -single and -duration are rtlamr's flags of the same names
 // (flags.go:37-58,69-70,140-170; the filter chain runs before the cross-block dedup, main.go:236-260).  With -format=csv a
@@ -74,7 +79,7 @@ int main(int argc, char** argv) {
     long long blocks = 4096, samplerate = 0;
     bool block_dedup = true, quiet = false, unique = false, single = false;
     std::string filterid, filtertype, format = "plain", samplefile, duration, sampleformat = "cu8", samplescale;
-    std::string capturefreq, centerfreq;
+    std::string capturefreq, centerfreq, channelgain;
     bool have_scale = false, auto_scale = false;
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
@@ -85,6 +90,7 @@ int main(int argc, char** argv) {
         else if (a.rfind("-sampleformat=", 0) == 0) sampleformat = a.substr(14);
         else if (a.rfind("-capturefreq=", 0) == 0) capturefreq = a.substr(13);
         else if (a.rfind("-centerfreq=", 0) == 0) centerfreq = a.substr(12);
+        else if (a.rfind("-channelgain=", 0) == 0) channelgain = a.substr(13);
         else if (a.rfind("-samplescale=", 0) == 0) {
             samplescale = a.substr(13);
             have_scale = true;
@@ -107,7 +113,7 @@ int main(int argc, char** argv) {
         fprintf(stderr, "usage: %s [-msgtype=scm,scm+,idm,netidm,r900,r900bcd|all] [-symbollength=N] [-blockdedup=true|false] "
                         "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
                         "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|wav|sigmf] "
-                        "[-samplescale=G|auto] "
+                        "[-samplescale=G|auto] [-channelgain=G|auto] "
                         "[-capturefreq=HZ [-centerfreq=HZ[,HZ...]]] [-quiet] FILE|- [FILE ...]\n", argv[0]);
         return 2;
     }
@@ -171,6 +177,18 @@ int main(int argc, char** argv) {
             fprintf(stderr, "invalid value \"%s\" for flag -samplescale: a finite gain > 0, or auto\n", samplescale.c_str());
             return 2;
         }
+    }
+    int32_t channel_k = -1;   // -channelgain: k of G = 2^k
+    const bool auto_channel = channelgain == "auto";
+    if (!channelgain.empty() && !auto_channel) {
+        char* end = nullptr;
+        const long long g = strtoll(channelgain.c_str(), &end, 10);
+        if (*end || g < 1 || g > (1LL << ERTRS_GAIN_K_MAX) || (g & (g - 1))) {
+            fprintf(stderr, "invalid value \"%s\" for flag -channelgain: a power of two 1 ... %lld, or auto\n", channelgain.c_str(),
+                    1LL << ERTRS_GAIN_K_MAX);
+            return 2;
+        }
+        channel_k = 63 - __builtin_clzll((unsigned long long)g);
     }
     // wav: every file's header, before anything else (stdin's is consumed here, the files' are read again below)
     std::vector<wav::Header> wav_hdr(files.size());
@@ -255,6 +273,10 @@ int main(int argc, char** argv) {
         }
     }
     const bool tuned = capture_hz > 0;
+    if (!channelgain.empty() && !tuned) {
+        fprintf(stderr, "-channelgain needs -capturefreq (or a SigMF frequency): the channel path of a tuned capture\n");
+        return 2;
+    }
     if (have_scale && fmt == ERTGPU_FORMAT_CU8) {
         fprintf(stderr, "-samplescale does not apply to uint8 (cu8) input\n");
         return 2;
@@ -280,7 +302,7 @@ int main(int argc, char** argv) {
         }
     }
     try {
-        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale},
+        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale, channel_k, auto_channel},
                                 channels);
         std::string log = rcvr.decoder().Log();
         if (!channels.empty()) {   // the channels share everything of the log but CenterFreq, its first line: name them all
@@ -317,6 +339,13 @@ int main(int argc, char** argv) {
                 rcvr.SetLevelReport([&](const ertgpu_input_level& lv) {
                     fprintf(stderr, "%s%s-samplescale=auto: 2^%d = %.9g from %lld samples\n", files.size() > 1 ? file.c_str() : "",
                             files.size() > 1 ? ": " : "", lv.exponent, (double)lv.scale, (long long)(lv.components / 2));
+                });
+            if (auto_channel)
+                rcvr.SetChannelLevelReport([&](size_t c, const ertgpu_channel_level& lv) {
+                    ertgpu_tuning_info t{};
+                    ertgpu_get_tuning(rcvr.decoder(c).Handle(), &t);
+                    fprintf(stderr, "%s%schannel %lld: 2^%d = %lld\n", files.size() > 1 ? file.c_str() : "", files.size() > 1 ? ": " : "",
+                            (long long)t.center_hz, lv.k, 1LL << lv.k);
                 });
             if (wav_in && in != stdin) wav_hdr[fi] = wav::ReadHeader(in);   // the same header as above: to the samples
             auto st = rcvr.Run(in, block_dedup, [&](const protocol::Message& m, int64_t offset, int length) {

@@ -39,9 +39,11 @@ struct erthost {
 // protocol::Input's (all 0: uint8 IQ at the decoder's own rate): IQ sampled at input_rate Hz, in sample format `format`
 // (ERTGPU_FORMAT_*) with gain `scale`, recorded centred at capture_freq Hz with the channel at center_freq.  auto_scale:
 // the gain of each stream is measured from the first min(len, ERTLV_WINDOW) samples of its first erthost_decode call.
+// channel_gain: k of the wide channel path (0 ... 14), -1 none, -2 measured like auto_scale (after it) from the same
+// samples (ertgpu_measure_channel).
 erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
                      long long input_rate, int format, float scale, long long capture_freq, long long center_freq,
-                     int auto_scale, char* errbuf, int errcap) {
+                     int auto_scale, int channel_gain, char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;   // released only on success: a throwing NewParser / Allocate must not leak the handle
     try {
         protocol::RegisterStockParsers();
@@ -52,7 +54,8 @@ erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long
             if (name.empty()) continue;
             h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
         }
-        h->d.SetInput({input_rate, format, scale, capture_freq, center_freq, auto_scale != 0});
+        h->d.SetInput({input_rate, format, scale, capture_freq, center_freq, auto_scale != 0, channel_gain < 0 ? -1 : channel_gain,
+                       channel_gain == -2});
         h->d.Allocate(device, max_blocks, max_cands);
         return h.release();
     } catch (const std::exception& e) {
@@ -262,6 +265,10 @@ long long erthost_decode(erthost* h, const uint8_t* iq, size_t len, erthost_msg*
             h->measured = true;
             h->d.SetScale(h->level.scale);
         }
+        if (h->d.AutoChannelGain() && !h->started && len % h->d.InputQuantum() == 0) {
+            const size_t s = (size_t)h->d.BytesPerSample();
+            h->d.SetChannelGain(h->d.MeasureChannel(iq, std::min(len / s, (size_t)ERTLV_WINDOW) * s).k);
+        }
         h->started = true;
         auto msgs = h->d.Decode(iq, len);
         return fill_msgs(msgs, out, cap);
@@ -374,6 +381,13 @@ int erthost_level(const erthost* h, int* exponent, float* scale, long long* comp
     *components = h->level.components;
     if (bins) memcpy(bins, h->level.bins, sizeof(h->level.bins));
     return 0;
+}
+
+// k of a handle on the wide channel path (channel_gain >= 0, or -2 once its first erthost_decode measured it); -1
+// when the handle does not take it.
+int erthost_channel_gain(const erthost* h) {
+    int32_t k = -1;
+    return ertgpu_get_channel_gain(h->d.Handle(), &k) == ERTGPU_OK ? k : -1;
 }
 
 int erthost_log(const erthost* h, char* buf, int cap) {

@@ -620,6 +620,25 @@ void Decoder::SetInput(const Input& in) {
         sample_bytes_ = FormatBytes(in.Format);
     }
     auto_scale_ = in.AutoScale;
+    if (in.ChannelGain >= 0 || in.AutoChannelGain) {
+        if (in.CaptureFreq <= 0) throw std::invalid_argument("the channel gain needs a tuned input: a capture frequency");
+        check(ertgpu_set_channel_gain(h_, in.AutoChannelGain ? 0 : in.ChannelGain));
+    }
+    auto_channel_gain_ = in.AutoChannelGain;
+}
+
+ertgpu_channel_level Decoder::MeasureChannel(const uint8_t* samples, size_t len) {
+    if (!allocated_) throw std::logic_error("MeasureChannel before Allocate");
+    ertgpu_channel_level lv{};
+    const int rc = ertgpu_measure_channel(h_, samples, len, &lv);
+    if (rc != ERTGPU_OK) raise(h_, rc, "MeasureChannel");
+    return lv;
+}
+
+void Decoder::SetChannelGain(int32_t k) {
+    const int rc = ertgpu_set_channel_gain(h_, k);
+    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
+    if (rc != ERTGPU_OK) raise(h_, rc, "SetChannelGain");
 }
 
 ertgpu_input_level Decoder::Measure(const uint8_t* samples, size_t len) {

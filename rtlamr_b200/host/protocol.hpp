@@ -146,6 +146,11 @@ struct Input {
     // (ertgpu_set_input_scale); Scale is the gain until then.  Not for cu8.  The Decoder only carries the flag: whoever
     // feeds it (receiver::Receiver::Run, erthost_decode) measures and sets the gain.
     bool AutoScale = false;
+    // The wide channel path of a tuned input (ertgpu_set_channel_gain) with gain 2^ChannelGain; -1: not taken.  With
+    // AutoChannelGain the path is taken and k of each stream is measured from its first samples (ertgpu_measure_channel,
+    // after the automatic input gain) and set before its first Decode; as with AutoScale, whoever feeds the Decoder does it.
+    int32_t ChannelGain = -1;
+    bool AutoChannelGain = false;
 };
 
 // decode.go:45-63.  Signal/Quantized are not materialised on the host: the parity taps of the C ABI
@@ -171,6 +176,11 @@ public:
     ertgpu_input_level Measure(const uint8_t* samples, size_t len);
     // ertgpu_set_input_scale: the gain of the stream that starts now (after Allocate or Reset, before Decode).
     void SetScale(float scale);
+    bool AutoChannelGain() const { return auto_channel_gain_; }
+    // ertgpu_measure_channel on len bytes of whole IQ samples (a wide channel path): the channel's level and k.
+    ertgpu_channel_level MeasureChannel(const uint8_t* samples, size_t len);
+    // ertgpu_set_channel_gain after Allocate: k of the stream that starts now (after Allocate or Reset, before Decode).
+    void SetChannelGain(int32_t k);
     // Decode takes multiples of this many bytes: whole IQ samples when resampling, whole blocks otherwise.
     size_t InputQuantum() const { return (size_t)sample_bytes_ * (resampling_ ? 1 : (size_t)Cfg.BlockSize); }
     void Allocate(int device = 0, int64_t maxBlocksPerCall = 0, int64_t maxCandidates = 0);  // decode.go:131-160
@@ -204,6 +214,7 @@ private:
     int64_t input_samples_ = 0;  // since Allocate / Reset
     int sample_bytes_ = 2;       // bytes per input IQ sample
     bool auto_scale_ = false;
+    bool auto_channel_gain_ = false;
 };
 
 void RegisterStockParsers();  // the effect of the reference's blank imports (main.go:37-44)

@@ -234,7 +234,8 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
     // and the window does not depend on the size of a Decode call.
     std::vector<uint8_t> window;
     size_t window_pos = 0;
-    if (d0.AutoScale()) {   // every channel would pick the gain of the same samples: measured once, set on each
+    // The channel gain (Input::AutoChannelGain) is measured per channel from the same window, after the input gain.
+    if (d0.AutoScale() || d0.AutoChannelGain()) {
         window.resize((size_t)std::min<uint64_t>((uint64_t)ERTLV_WINDOW * s, left));
         size_t have = 0;
         while (have < window.size()) {
@@ -243,9 +244,17 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
             have += n;
         }
         window.resize(have);
-        level_ = d0.Measure(window.data(), have / s * s);
-        for (auto& d : d_) d->SetScale(level_.scale);
-        if (level_report_) level_report_(level_);
+        if (d0.AutoScale()) {   // every channel would pick the gain of the same samples: measured once, set on each
+            level_ = d0.Measure(window.data(), have / s * s);
+            for (auto& d : d_) d->SetScale(level_.scale);
+            if (level_report_) level_report_(level_);
+        }
+        if (d0.AutoChannelGain())
+            for (size_t c = 0; c < d_.size(); c++) {
+                const ertgpu_channel_level lv = d_[c]->MeasureChannel(window.data(), have / s * s);
+                d_[c]->SetChannelGain(lv.k);
+                if (channel_report_) channel_report_(c, lv);
+            }
     }
     const auto read = [&](uint8_t* dst, size_t n) -> size_t {
         if (window_pos < window.size()) {

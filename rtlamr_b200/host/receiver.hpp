@@ -106,6 +106,11 @@ public:
     void SetLevelReport(std::function<void(const ertgpu_input_level&)> report) { level_report_ = std::move(report); }
     // The level measured at the start of the last stream (Input::AutoScale; all zero otherwise).
     const ertgpu_input_level& Level() const { return level_; }
+    // Input::AutoChannelGain: `report` sees each channel's level and k once they are measured, before the stream is
+    // decoded (after the input gain of Input::AutoScale is set).
+    void SetChannelLevelReport(std::function<void(size_t, const ertgpu_channel_level&)> report) {
+        channel_report_ = std::move(report);
+    }
 
     // Run over a FILE* until EOF, -single or the deadline.  With Input::AutoScale the stream's gain is set from its first
     // min(stream, ERTLV_WINDOW) samples (include/ertgpu_level.h) before anything is decoded; it stays for the stream.  `emit` is called once per reported message (after the
@@ -140,6 +145,7 @@ private:
     std::chrono::steady_clock::time_point deadline_ = std::chrono::steady_clock::time_point::max();
     std::function<void(const ertgpu_input_level&)> level_report_;
     ertgpu_input_level level_{};
+    std::function<void(size_t, const ertgpu_channel_level&)> channel_report_;
 
     void DumpSampleBuf(const uint8_t* call, int64_t call_first, int64_t block);
     void KeepHistory(const uint8_t* call, size_t nblocks);
