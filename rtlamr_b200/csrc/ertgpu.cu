@@ -563,6 +563,44 @@ int prepare_staging(ertgpu_handle* h, size_t bytes, const void* iq, bool* pageab
     return ERTGPU_OK;
 }
 
+// Stream `total` host samples of s bytes at src through h's two staging slots, chunk i into slot k = i & 1: it is copied
+// to d_stage[k] on h->copy_stream (through h_stage[k] when the input is pageable), and its work is enqueued on h->stream
+// behind that copy, so that the copy of chunk i + 1 overlaps chunk i's kernels.  The callbacks:
+//   next(left)        the samples of the next chunk when `left` remain; 0 ends the call with ERTGPU_EINVAL, the
+//                     message already in place;
+//   between()         before the work of every chunk but the first (collect the previous one's);
+//   enqueue(d_in, n)  enqueue the work on the n samples at d_in on h->stream.
+// Staging buffers of `bytes` each (prepare_staging).
+template <class Next, class Between, class Enqueue>
+int upload(ertgpu_handle* h, const void* src, int64_t total, size_t s, size_t bytes, Next next, Between between,
+           Enqueue enqueue) {
+    if (total == 0) return ERTGPU_OK;
+    bool pageable = true;
+    if (const int rc = prepare_staging(h, bytes, src, &pageable)) return rc;
+    const uint8_t* src0 = static_cast<const uint8_t*>(src);
+    int64_t done = 0;
+    for (int64_t i = 0; done < total; i++) {
+        const int k = (int)(i & 1);
+        const int64_t c = next(total - done);
+        if (c <= 0) return ERTGPU_EINVAL;
+        if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // the kernels that read d_stage[k] (and its H2D) are done
+        const uint8_t* p = src0 + (size_t)done * s;
+        if (pageable) {
+            h->copy_pool->copy(h->h_stage[k], p, (size_t)c * s);
+            p = h->h_stage[k];
+        }
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], p, (size_t)c * s, cudaMemcpyHostToDevice, h->copy_stream));
+        CUDA_TRY(h, cudaEventRecord(h->ev_h2d[k], h->copy_stream));
+        if (i >= 1)
+            if (const int rc = between()) return rc;
+        CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[k], 0));
+        if (const int rc = enqueue(h->d_stage[k], c)) return rc;
+        CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
+        done += c;
+    }
+    return ERTGPU_OK;
+}
+
 // Enqueue the work for the next n input samples, at d_in on the device, on st: the input stage's step and the pipeline
 // over the whole blocks it completes.
 int run_step(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaStream_t st) {
@@ -935,7 +973,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->device);
     if (h->sm_count < 1) h->sm_count = 132;
 
-    if (const int rc = h->in.allocate(h->device, c.block_size, max_blocks_per_call, h->sm_count)) return rc;
+    if (const int rc = h->in.allocate(c.block_size, max_blocks_per_call, h->sm_count)) return rc;
     h->cur_plane = h->cur_hist = 0;
     h->hist_valid = 0;
     h->block_counter = 0;
@@ -1028,7 +1066,8 @@ int ertgpu_get_channel_gain(const ertgpu_handle* h, int32_t* k) {
 }
 
 // ertgpu_measure_input's staging, with the input stage's own steps (begin_measure: from a stream start, on the
-// measurement's histories) counting into d_clevel.  The steps end on the handle's stream before the position comes back.
+// measurement's histories) counting into d_clevel.  The steps end on the handle's stream before the position comes back,
+// whether the call succeeds or not.
 int ertgpu_measure_channel(ertgpu_handle* h, const void* samples, size_t nbytes, ertgpu_channel_level* out) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     if (!h->in.wide) return fail(h, ERTGPU_EINVAL, "measure_channel: the handle does not take the wide channel path");
@@ -1038,41 +1077,22 @@ int ertgpu_measure_channel(ertgpu_handle* h, const void* samples, size_t nbytes,
     CUDA_TRY(h, cudaSetDevice(h->device));
     if (const int rc = collect_sync(h)) return rc;  // the stream's own last step is done with the histories
     CUDA_TRY(h, cudaMemsetAsync(h->in.d_clevel, 0, ERTRS_GAIN_BINS * sizeof(unsigned long long), h->stream));
-    const int64_t total = (int64_t)(nbytes / s);
-    int64_t outputs = 0;
-    int rc = ERTGPU_OK;
-    const InputStage::Position pos = h->in.begin_measure();
-    if (total) {
-        bool pageable = true;
-        rc = prepare_staging(h, (size_t)h->in.chunk() * s, samples, &pageable);
-        const uint8_t* src0 = static_cast<const uint8_t*>(samples);
-        int64_t done = 0, launches = 0;
-        for (int64_t i = 0; rc == ERTGPU_OK && done < total; i++) {
-            const int k = (int)(i & 1);
-            const int64_t c = h->in.next_chunk(total - done);
-            if (i >= 2 && cudaEventSynchronize(h->ev_done[k]) != cudaSuccess) { rc = fail(h, ERTGPU_ECUDA, "measure_channel: event wait failed"); break; }
-            const uint8_t* src = src0 + (size_t)done * s;
-            if (pageable) {
-                h->copy_pool->copy(h->h_stage[k], src, (size_t)c * s);
-                src = h->h_stage[k];
-            }
-            if (cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * s, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) {
-                rc = fail(h, ERTGPU_ECUDA, "measure_channel: copy failed");
-                break;
-            }
-            InputStep st = h->in.plan(h->d_stage[k], c);
-            st.rs.level = h->in.d_clevel;
-            if ((rc = h->in.launch(st, h->stream, &launches))) break;
-            if (cudaEventRecord(h->ev_done[k], h->stream) != cudaSuccess) { rc = fail(h, ERTGPU_ECUDA, "measure_channel: event record failed"); break; }
-            outputs += st.rs.count;
-            h->in.commit(st);
-            done += c;
-        }
-    }
+    int64_t outputs = 0, launches = 0;
+    h->in.begin_measure();
+    const int rc = upload(h, samples, (int64_t)(nbytes / s), s, (size_t)h->in.chunk() * s,
+                          [&](int64_t left) { return h->in.next_chunk(left); }, [] { return ERTGPU_OK; },
+                          [&](const uint8_t* d_in, int64_t c) {
+                              InputStep st = h->in.plan(d_in, c);
+                              st.rs.level = h->in.d_clevel;
+                              if (const int rc = h->in.launch(st, h->stream, &launches)) return rc;
+                              outputs += st.rs.count;
+                              h->in.commit(st);
+                              return ERTGPU_OK;
+                          });
     unsigned long long cnt[ERTRS_GAIN_BINS];
     const cudaError_t e1 = cudaMemcpyAsync(cnt, h->in.d_clevel, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream);
     const cudaError_t e2 = cudaStreamSynchronize(h->stream);
-    h->in.end_measure(pos);
+    h->in.end_measure();
     if (rc) return rc;
     CUDA_TRY(h, e1);
     CUDA_TRY(h, e2);
@@ -1085,9 +1105,9 @@ int ertgpu_measure_channel(ertgpu_handle* h, const void* samples, size_t nbytes,
     return ERTGPU_OK;
 }
 
-// Each chunk is copied to d_stage[k] and counted by level_kernel on the handle's stream; pageable input is staged through
-// h_stage[k] as in ertgpu_decode.  The counters live in the input stage and are zeroed first; nothing the decode reads
-// or keeps between calls is touched.
+// The samples go through ertgpu_decode's staging in chunks of a whole staging buffer, each counted by level_kernel on the
+// handle's stream.  The counters live in the input stage and are zeroed first; nothing the decode reads or keeps between
+// calls is touched.
 int ertgpu_measure_input(ertgpu_handle* h, const void* samples, size_t nbytes, ertgpu_input_level* out) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     if (h->in.fmt == ERTGPU_FORMAT_CU8) return fail(h, ERTGPU_EINVAL, "cu8 input is not measured: it takes no gain");
@@ -1097,27 +1117,11 @@ int ertgpu_measure_input(ertgpu_handle* h, const void* samples, size_t nbytes, e
     CUDA_TRY(h, cudaSetDevice(h->device));
     CUDA_TRY(h, cudaMemsetAsync(h->in.d_level, 0, kLvCounters * sizeof(unsigned long long), h->stream));
     const int64_t total = (int64_t)(nbytes / s);
-    if (total) {
-        bool pageable = true;
-        if (const int rc = prepare_staging(h, (size_t)h->in.chunk() * s, samples, &pageable)) return rc;
-        const int64_t chunk = (int64_t)(h->stage_bytes / s);
-        const uint8_t* src0 = static_cast<const uint8_t*>(samples);
-        int64_t done = 0;
-        for (int64_t i = 0; done < total; i++) {
-            const int k = (int)(i & 1);
-            const int64_t c = std::min(chunk, total - done);
-            if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // d_stage[k] and h_stage[k] are free again
-            const uint8_t* src = src0 + (size_t)done * s;
-            if (pageable) {
-                h->copy_pool->copy(h->h_stage[k], src, (size_t)c * s);
-                src = h->h_stage[k];
-            }
-            CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * s, cudaMemcpyHostToDevice, h->stream));
-            if (const int rc = h->in.launch_level(h->d_stage[k], c, h->stream)) return rc;
-            CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
-            done += c;
-        }
-    }
+    if (const int rc = upload(h, samples, total, s, (size_t)h->in.chunk() * s,
+                              [&](int64_t left) { return std::min((int64_t)(h->stage_bytes / s), left); },
+                              [] { return ERTGPU_OK; },
+                              [&](const uint8_t* d_in, int64_t c) { return h->in.launch_level(d_in, c, h->stream); }))
+        return rc;
     unsigned long long cnt[kLvCounters];
     CUDA_TRY(h, cudaMemcpyAsync(cnt, h->in.d_level, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
@@ -1167,34 +1171,15 @@ int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t f
     const size_t s = (size_t)h->in.sample_bytes;
     const int64_t total = (int64_t)(nbytes / s);
     if (total == 0) return deliver(h, out, cap, n_out);
-
-    // Staging chunks of s bytes per sample (allocated on first use): the H2D copy of chunk i+1 overlaps chunk i's kernels.
-    bool pageable = true;
-    rc = prepare_staging(h, (size_t)h->in.chunk() * s, iq, &pageable);
+    int64_t launches = 0;
+    rc = upload(h, iq, total, s, (size_t)h->in.chunk() * s, [&](int64_t left) { return h->in.next_chunk(left); },
+                [&] { return collect(h); },
+                [&](const uint8_t* d_in, int64_t c) {
+                    if (const int rc = enqueue_step(h, d_in, c, flags, h->stream)) return rc;
+                    launches += h->launches;
+                    return ERTGPU_OK;
+                });
     if (rc) return rc;
-    int64_t done = 0, launches = 0;
-    for (int64_t i = 0; done < total; i++) {
-        const int k = (int)(i & 1);
-        const int64_t c = h->in.next_chunk(total - done);
-        if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // the kernels that read d_stage[k] (and its H2D) are done
-        const uint8_t* src = iq + (size_t)done * s;
-        if (pageable) {
-            h->copy_pool->copy(h->h_stage[k], src, (size_t)c * s);
-            src = h->h_stage[k];
-        }
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * s, cudaMemcpyHostToDevice, h->copy_stream));
-        CUDA_TRY(h, cudaEventRecord(h->ev_h2d[k], h->copy_stream));
-        if (i >= 1) {
-            rc = collect(h);
-            if (rc) return rc;
-        }
-        CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[k], 0));
-        rc = enqueue_step(h, h->d_stage[k], c, flags, h->stream);
-        if (rc) return rc;
-        launches += h->launches;
-        CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
-        done += c;
-    }
     rc = collect(h);  // also waits for a last step that completed no block (ertgpu_decode is synchronous)
     if (rc) return rc;
     CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));  // a step that launched nothing still copied from iq
@@ -1223,39 +1208,30 @@ int ertgpu_decode_channels(ertgpu_handle* const* hs, int32_t n, const uint8_t* i
     if (total == 0) return ERTGPU_OK;
     int64_t chunk = 0;
     for (int k = 0; k < n; k++) chunk = std::max(chunk, hs[k]->in.chunk());
-    bool pageable = true;
-    int rc = prepare_staging(h, (size_t)chunk * s, iq, &pageable);
-    if (rc) return rc;
     // At the decoder's own rate the channel at the capture's centre is not resampled (it only converts, if anything) and
     // takes whole blocks: then every step does.
     bool whole_blocks = false;
     for (int j = 0; j < n; j++) whole_blocks |= !hs[j]->in.resamples();
     const int64_t block = h->dcfg.BS;
     int64_t launches[ERTGPU_MAX_CHANNELS] = {};
-    int64_t done = 0;
-    for (int64_t i = 0; done < total; i++) {
-        const int k = (int)(i & 1);
-        int64_t c = total - done;
-        for (int j = 0; j < n; j++) c = std::min(c, hs[j]->in.next_chunk(total - done));  // a step every channel takes
+    auto next = [&](int64_t left) {
+        int64_t c = left;
+        for (int j = 0; j < n; j++) c = std::min(c, hs[j]->in.next_chunk(left));  // a step every channel takes
         if (whole_blocks) c -= c % block;
-        if (c <= 0) return fail(h, ERTGPU_EINVAL, "no step of whole blocks fits every channel's buffers");
-        if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));
-        const uint8_t* src = iq + (size_t)done * s;
-        if (pageable) {
-            h->copy_pool->copy(h->h_stage[k], src, (size_t)c * s);
-            src = h->h_stage[k];
-        }
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], src, (size_t)c * s, cudaMemcpyHostToDevice, h->copy_stream));
-        CUDA_TRY(h, cudaEventRecord(h->ev_h2d[k], h->copy_stream));
-        if (i >= 1)
-            for (int j = 0; j < n; j++)
-                if ((rc = collect(hs[j]))) return rc;
-        CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[k], 0));
-        if ((rc = enqueue_channels(hs, n, h->d_stage[k], c, flags, h->stream))) return rc;
+        if (c <= 0) fail(h, ERTGPU_EINVAL, "no step of whole blocks fits every channel's buffers");
+        return c;
+    };
+    auto collect_all = [&] {
+        for (int j = 0; j < n; j++)
+            if (const int rc = collect(hs[j])) return rc;
+        return ERTGPU_OK;
+    };
+    int rc = upload(h, iq, total, s, (size_t)chunk * s, next, collect_all, [&](const uint8_t* d_in, int64_t c) {
+        if (const int rc = enqueue_channels(hs, n, d_in, c, flags, h->stream)) return rc;
         for (int j = 0; j < n; j++) launches[j] += hs[j]->launches;
-        CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
-        done += c;
-    }
+        return ERTGPU_OK;
+    });
+    if (rc) return rc;
     for (int j = 0; j < n; j++) {
         if ((rc = collect(hs[j]))) return rc;
         hs[j]->launches = launches[j];

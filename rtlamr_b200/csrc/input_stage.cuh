@@ -5,8 +5,10 @@
 // decimate_kernel<F> (decimate.cuh) into resample_kernel<cu8, false>.  The first stage of several decimating channels of
 // one capture can run as one decimate_channels_kernel<F> (launch_channels).  A tuned handle on the wide channel path
 // (ertgpu_set_channel_gain) runs resample_wide_kernel<F>, or decimate_wide_kernel<F> into resample_wide_kernel<kFmtMid>,
-// instead.  It also measures the level of its input with level_kernel<F> (level.cuh) for ertgpu_measure_input, and that
-// of its channel with the wide kernels (begin_measure) for ertgpu_measure_channel.  Host code only.
+// instead.  allocate chooses a handle's first- and last-stage kernels once, from its format, mode and path, and launch
+// runs whichever it chose.  It also measures the level of its input with level_kernel<F> (level.cuh) for
+// ertgpu_measure_input, and that of its channel with the wide kernels (begin_measure) for ertgpu_measure_channel.  Host
+// code only.
 #pragma once
 
 #include <algorithm>
@@ -16,11 +18,11 @@
 #include <cstdio>
 #include <cstring>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "convert.cuh"
 #include "decimate.cuh"
-#include "demod_fast.cuh"  // OncePerDevice
 #include "level.cuh"
 #include "resample.cuh"
 
@@ -86,41 +88,55 @@ struct InputStage {
     // decoder geometry (allocate)
     int64_t block = 0, max_blocks = 0;
 
+    // The stream position of both stages: all that a stream start resets.
+    struct StreamPos {
+        int64_t in_total = 0;   // input samples received since the stream start (the second stage's in kDecimate)
+        int64_t out_next = 0;   // first output not yet computed
+        int64_t hist_first = 0, hist_n = 0;  // the input samples held in d_hist[cur_hist]
+        int64_t pend = 0;       // outputs at the front of d_out[cur_out] that wait for a whole block
+        int cur_hist = 0, cur_out = 0;
+        // the first stage of kDecimate (its next output is the second stage's in_total)
+        int64_t in1_total = 0;  // input samples received since the stream start
+        int64_t hist1_first = 0, hist1_n = 0;  // the input samples held in d_hist1[cur_hist1]
+        int cur_hist1 = 0;
+    };
+    StreamPos pos;
+
+    // The kernels allocate chose: the first stage of kDecimate, and the last stage of every resampling mode.
+    using FirstKernel = void (*)(const int16_t*, DcArgs);  // decimate_kernel<F>, decimate_wide_kernel<F>
+    using LastKernel = void (*)(const int32_t*, const uint32_t*, RsArgs);  // resample_kernel<F, T>, resample_wide_kernel<F>
+    FirstKernel first_kernel = nullptr;
+    LastKernel last_kernel = nullptr;
+    decltype(&decimate_channels_kernel<ERTGPU_FORMAT_CU8>) channels_kernel = nullptr;  // kDecimate's, for launch_channels
+
     // device state
     int32_t* d_A = nullptr;     // the table as the kernel reads it (rs_pack_table)
     uint32_t* d_D = nullptr;
     uint32_t* d_E = nullptr;    // the mixer table (ertrs_nco_table)
     uint8_t* d_hist[2] = {nullptr, nullptr};  // input samples the next outputs still read
-    int cur_hist = 0;
     uint8_t* d_out[2] = {nullptr, nullptr};   // [partial block | new outputs]; the demod reads whole blocks of it
-    int cur_out = 0;
-    int64_t in_total = 0;       // input samples received since the stream start (the second stage's in kDecimate)
-    int64_t out_next = 0;       // first output not yet computed
-    int64_t hist_first = 0, hist_n = 0;  // the input samples held in d_hist[cur_hist]
-    int64_t pend = 0;           // outputs at the front of d_out[cur_out] that wait for a whole block
     size_t smem = 0;
     int grid = 0;               // most CTAs of one launch
     unsigned long long* d_level = nullptr;  // level_kernel's kLvCounters counters (converted input only)
     int level_grid = 0;
-    // the first stage of kDecimate: its taps, input history and output (the second stage's input), and stream position
+    // the first stage of kDecimate: its taps, input history and output (the second stage's input)
     int16_t* d_taps = nullptr;
     uint8_t* d_hist1[2] = {nullptr, nullptr};
-    int cur_hist1 = 0;
     uint8_t* d_mid = nullptr;
-    int64_t in1_total = 0;      // input samples received since the stream start
-    int64_t hist1_first = 0, hist1_n = 0;  // (the first stage's next output is the second stage's in_total)
     size_t smem1 = 0;
     int grid1 = 0, per1 = 0;
     size_t smem1c = 0;          // the same for decimate_channels_kernel
     int grid1c = 0, per1c = 0;
-    // the wide path's channel measurement: its own input histories, swapped in by begin_measure, and its counters
+    // the wide path's channel measurement: its own input histories and stream position, which begin_measure and
+    // end_measure swap with the stream's, and its counters
     uint8_t* d_mhist[2] = {nullptr, nullptr};
     uint8_t* d_mhist1[2] = {nullptr, nullptr};
+    StreamPos mpos;
     unsigned long long* d_clevel = nullptr;
 
     bool resamples() const { return mode >= kResample; }
     // Input samples received since the stream start.
-    int64_t received() const { return mode == kDecimate ? in1_total : in_total; }
+    int64_t received() const { return mode == kDecimate ? pos.in1_total : pos.in_total; }
 
     // ---- configuration (the handle is not allocated; rate_out = DataRate * ChipLength) ----
     int set_rate(int64_t hz, int64_t rate_out) {
@@ -219,7 +235,7 @@ struct InputStage {
 
     // ---- device buffers ----
     // Blocks of block_size samples, a step completes at most max_blocks_per_step of them; sm_count SMs.
-    int allocate(int device, int64_t block_size, int64_t max_blocks_per_step, int sm_count) {
+    int allocate(int64_t block_size, int64_t max_blocks_per_step, int sm_count) {
         block = block_size;
         max_blocks = max_blocks_per_step;
         reset_stream();
@@ -253,21 +269,22 @@ struct InputStage {
             // a step completes at most max_blocks blocks: less than (max_blocks + 1) * BS outputs are buffered
             CUDA_TRY(err_, cudaMalloc(&d_out[k], (size_t)(max_blocks + 1) * block * 2 + 64));
         }
-        if (wide) return allocate_wide(device, sm_count);
-        smem = rs_smem_bytes(rs.P, rs.T, rs.L, rs.M, mix);
-        {   // a property of the kernel, not of the handle: every handle on the device gets the largest any table needs
-            static OncePerDevice once;
-            if (once.first(device))
-                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF64BE; f++)
-                    for (int t = 0; t < 2 && fmt_name(f); t++)
-                        CUDA_TRY(err_, cudaFuncSetAttribute(resample_kernel_of(f, t), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        fmt_visit(fmt, [&](auto f) {
+            if (mode == kDecimate) {  // the second stage reads the first stage's bytes, or its s_w words on the wide path
+                first_kernel = wide ? decimate_wide_kernel<f()> : decimate_kernel<f()>;
+                last_kernel = wide ? resample_wide_kernel<kFmtMid> : resample_kernel<ERTGPU_FORMAT_CU8, false>;
+                channels_kernel = decimate_channels_kernel<f()>;
+            } else {
+                last_kernel = wide ? resample_wide_kernel<f()> : mix ? resample_kernel<f(), true> : resample_kernel<f(), false>;
+            }
+        });
+        smem = wide ? rs_wide_smem_bytes(rs.P, rs.T, rs.L, rs.M, mode == kDecimate) : rs_smem_bytes(rs.P, rs.T, rs.L, rs.M, mix);
+        if (const int rc = fit((const void*)last_kernel, kRsThreads, smem, "resampler", sm_count, &grid)) return rc;
+        if (wide) {
+            CUDA_TRY(err_, cudaMalloc(&d_clevel, ERTRS_GAIN_BINS * sizeof(unsigned long long)));
+            for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_mhist[k], (size_t)rs.T * 4 + 16));
         }
-        if (smem > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", smem);
-        int per_sm = 0;
-        const int fmt2 = mode == kDecimate ? ERTGPU_FORMAT_CU8 : fmt;  // the second stage reads the first stage's bytes
-        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_kernel_of(fmt2, mix), kRsThreads, smem));
-        grid = std::max(1, per_sm) * sm_count;
-        return mode == kDecimate ? allocate_first(device, sm_count) : ERTGPU_OK;
+        return mode == kDecimate ? allocate_first(sm_count) : ERTGPU_OK;
     }
 
     void release() {
@@ -288,10 +305,7 @@ struct InputStage {
         }
     }
 
-    void reset_stream() {
-        in_total = out_next = hist_first = hist_n = pend = cur_hist = cur_out = 0;
-        in1_total = hist1_first = hist1_n = cur_hist1 = 0;
-    }
+    void reset_stream() { pos = {}; }
 
     // ---- calls ----
     // Before anything else of a decode call: a resampling stage takes whole IQ samples of s bytes.
@@ -357,25 +371,25 @@ struct InputStage {
         }
         // every output whose window is complete
         const int64_t L = rs.L, M = rs.M, T = rs.T;
-        const int64_t in_new = in_total + n;
+        const int64_t in_new = pos.in_total + n;
         const int64_t ne = ertrs_out_end(&rs, in_new);
-        const int64_t cnt = ne - out_next;
-        s.nblocks = (pend + cnt) / block;
-        s.iq = d_out[cur_out];
+        const int64_t cnt = ne - pos.out_next;
+        s.nblocks = (pos.pend + cnt) / block;
+        s.iq = d_out[pos.cur_out];
         RsArgs* a = &s.rs;
-        a->hist = d_hist[cur_hist];
-        a->hist_first = hist_first;
-        a->hist_n = hist_n;
+        a->hist = d_hist[pos.cur_hist];
+        a->hist_first = pos.hist_first;
+        a->hist_n = pos.hist_n;
         a->cur_n = n;
-        a->n0 = out_next;
+        a->n0 = pos.out_next;
         a->count = cnt;
-        a->split = s.nblocks > 0 ? s.nblocks * block - pend : LLONG_MAX;
-        a->base_n = (out_next / L) * L;
-        a->base_k = (out_next / L) * M;
-        a->out = d_out[cur_out] + 2 * pend;
-        a->out2 = d_out[cur_out ^ 1];
+        a->split = s.nblocks > 0 ? s.nblocks * block - pos.pend : LLONG_MAX;
+        a->base_n = (pos.out_next / L) * L;
+        a->base_k = (pos.out_next / L) * M;
+        a->out = d_out[pos.cur_out] + 2 * pos.pend;
+        a->out2 = d_out[pos.cur_out ^ 1];
         const int64_t first = std::min(in_new, std::max<int64_t>(0, k_of(ne) - T / 2 + 1));
-        a->carry_dst = d_hist[cur_hist ^ 1];
+        a->carry_dst = d_hist[pos.cur_hist ^ 1];
         a->carry_first = first;
         a->carry_n = in_new - first;
         a->L = L;
@@ -395,41 +409,29 @@ struct InputStage {
         return s;
     }
 
-    // Enqueue the step's kernel on st, if it has one, and count it in *launches.
+    // Enqueue the step's kernels on st, if it has any, and count them in *launches.
     int launch(const InputStep& s, cudaStream_t st, int64_t* launches) const {
-        if (wide) return launch_wide(s, st, launches);
-        if (mode == kDecimate) {
-            if (!s.shared_first && (s.dc.count > 0 || s.dc.carry_n > 0)) {
-                const long long tiles = (s.dc.count + (long long)kDcThreads * per1 - 1) / ((long long)kDcThreads * per1);
-                const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid1));
-                decimate_kernel_of(fmt)<<<g, kDcThreads, smem1, st>>>(d_taps, s.dc);
-                CUDA_TRY(err_, cudaGetLastError());
-                ++*launches;
-            }
-            if (s.rs.count > 0 || s.rs.carry_n > 0) {
-                const long long tiles = (s.rs.count + kRsTile - 1) / kRsTile;
-                const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid));
-                resample_kernel<ERTGPU_FORMAT_CU8, false><<<g, kRsThreads, smem, st>>>(d_A, d_D, s.rs);
-                CUDA_TRY(err_, cudaGetLastError());
-                ++*launches;
-            }
-            return ERTGPU_OK;
-        }
-        if (mode == kPass || (resamples() && s.rs.count <= 0 && s.rs.carry_n <= 0)) return ERTGPU_OK;
         if (mode == kConvert) {
             const long long groups = s.nblocks * block / 8;
-            const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>((groups + kCvtThreads - 1) / kCvtThreads, grid));
+            const unsigned g = grid_of(groups, kCvtThreads, grid);
             fmt_visit(fmt, [&](auto f) {
                 if constexpr (f() != ERTGPU_FORMAT_CU8)
                     convert_kernel<f()><<<g, kCvtThreads, 0, st>>>(s.rs.cur, d_out[0], groups, scale);
             });
-        } else {
-            const long long tiles = (s.rs.count + kRsTile - 1) / kRsTile;
-            const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid));
-            resample_kernel_of(fmt, mode == kResampleTuned)<<<g, kRsThreads, smem, st>>>(d_A, d_D, s.rs);
+            CUDA_TRY(err_, cudaGetLastError());
+            ++*launches;
+            return ERTGPU_OK;
         }
-        CUDA_TRY(err_, cudaGetLastError());
-        ++*launches;
+        if (first_kernel && !s.shared_first && (s.dc.count > 0 || s.dc.carry_n > 0)) {
+            first_kernel<<<grid_of(s.dc.count, (long long)kDcThreads * per1, grid1), kDcThreads, smem1, st>>>(d_taps, s.dc);
+            CUDA_TRY(err_, cudaGetLastError());
+            ++*launches;
+        }
+        if (last_kernel && (s.rs.count > 0 || s.rs.carry_n > 0)) {
+            last_kernel<<<grid_of(s.rs.count, kRsTile, grid), kRsThreads, smem, st>>>(d_A, d_D, s.rs);
+            CUDA_TRY(err_, cudaGetLastError());
+            ++*launches;
+        }
         return ERTGPU_OK;
     }
 
@@ -449,9 +451,7 @@ struct InputStage {
         if (a.count <= 0 && a.carry_n <= 0) return ERTGPU_OK;
         DcArgs ac = a;
         ac.per = per1c;
-        const long long tiles = (a.count + (long long)kDcThreads * per1c - 1) / ((long long)kDcThreads * per1c);
-        const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid1c));
-        fmt_visit(fmt, [&](auto f) { decimate_channels_kernel<f()><<<g, kDcThreads, smem1c, st>>>(d_taps, ac, ch); });
+        channels_kernel<<<grid_of(a.count, (long long)kDcThreads * per1c, grid1c), kDcThreads, smem1c, st>>>(d_taps, ac, ch);
         CUDA_TRY(err_, cudaGetLastError());
         ++*launches;
         return ERTGPU_OK;
@@ -460,7 +460,7 @@ struct InputStage {
     // Enqueue level_kernel over n input samples at d_in (device, 16-byte aligned) on st: their counts are added to d_level.
     int launch_level(const uint8_t* d_in, int64_t n, cudaStream_t st) const {
         const long long nbytes = n * sample_bytes, groups = (nbytes + 15) / 16;
-        const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>((groups + kLvThreads - 1) / kLvThreads, level_grid));
+        const unsigned g = grid_of(groups, kLvThreads, level_grid);
         fmt_visit(fmt, [&](auto f) {
             if constexpr (f() != ERTGPU_FORMAT_CU8) level_kernel<f()><<<g, kLvThreads, 0, st>>>(d_in, nbytes, d_level);
         });
@@ -471,23 +471,23 @@ struct InputStage {
     // The step's kernel is enqueued: advance the stream position.
     void commit(const InputStep& s) {
         if (!resamples()) {  // whole blocks only (check_call)
-            in_total += s.nblocks * block;
+            pos.in_total += s.nblocks * block;
             return;
         }
         if (mode == kDecimate) {
-            in1_total += s.dc.cur_n;
-            hist1_first = s.dc.carry_first;
-            hist1_n = s.dc.carry_n;
-            cur_hist1 ^= 1;
+            pos.in1_total += s.dc.cur_n;
+            pos.hist1_first = s.dc.carry_first;
+            pos.hist1_n = s.dc.carry_n;
+            pos.cur_hist1 ^= 1;
         }
         const RsArgs& a = s.rs;
-        in_total += a.cur_n;
-        out_next += a.count;
-        hist_first = a.carry_first;
-        hist_n = a.carry_n;
-        cur_hist ^= 1;
-        pend += a.count - s.nblocks * block;
-        if (s.nblocks > 0) cur_out ^= 1;  // the outputs past the last whole block are already at the front of the other buffer
+        pos.in_total += a.cur_n;
+        pos.out_next += a.count;
+        pos.hist_first = a.carry_first;
+        pos.hist_n = a.carry_n;
+        pos.cur_hist ^= 1;
+        pos.pend += a.count - s.nblocks * block;
+        if (s.nblocks > 0) pos.cur_out ^= 1;  // the outputs past the last whole block are already at the front of the other buffer
     }
 
     // The stage's kernels as ertgpu_last_kernels names them ("" in pass-through mode); `shared`: the first stage ran as
@@ -506,95 +506,39 @@ struct InputStage {
         }
     }
 
-    // The stream position begin_measure sets aside.
-    struct Position {
-        int64_t in_total, out_next, hist_first, hist_n, pend, in1_total, hist1_first, hist1_n;
-        int cur_hist, cur_out, cur_hist1;
-    };
-
-    // A channel measurement (wide path) runs the stage's own steps from a stream start, with the measurement's input
-    // histories in place of the stream's and rs.level = d_clevel in every step; end_measure puts the stream back.
-    Position begin_measure() {
-        const Position p{in_total, out_next, hist_first, hist_n, pend, in1_total, hist1_first, hist1_n, cur_hist, cur_out, cur_hist1};
-        for (int k = 0; k < 2; k++) {
-            std::swap(d_hist[k], d_mhist[k]);
-            std::swap(d_hist1[k], d_mhist1[k]);
-        }
+    // A channel measurement (wide path) runs the stage's own steps from a stream start, with rs.level = d_clevel in every
+    // step.  begin_measure swaps the measurement's input histories and stream position in for the stream's, and
+    // end_measure swaps them back.
+    void begin_measure() {
+        swap_measure();
         reset_stream();
-        return p;
     }
 
-    void end_measure(const Position& p) {
-        for (int k = 0; k < 2; k++) {
-            std::swap(d_hist[k], d_mhist[k]);
-            std::swap(d_hist1[k], d_mhist1[k]);
-        }
-        in_total = p.in_total;
-        out_next = p.out_next;
-        hist_first = p.hist_first;
-        hist_n = p.hist_n;
-        pend = p.pend;
-        in1_total = p.in1_total;
-        hist1_first = p.hist1_first;
-        hist1_n = p.hist1_n;
-        cur_hist = p.cur_hist;
-        cur_out = p.cur_out;
-        cur_hist1 = p.cur_hist1;
-    }
+    void end_measure() { swap_measure(); }
 
 private:
     std::string& err_;  // the handle's last error
 
-    // The wide path's kernels: decimate_wide_kernel<F> (kDecimate) into resample_wide_kernel<kFmtMid>, or
-    // resample_wide_kernel<F> alone.
-    int launch_wide(const InputStep& s, cudaStream_t st, int64_t* launches) const {
-        if (mode == kDecimate && (s.dc.count > 0 || s.dc.carry_n > 0)) {
-            const long long tiles = (s.dc.count + (long long)kDcThreads * per1 - 1) / ((long long)kDcThreads * per1);
-            const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid1));
-            fmt_visit(fmt, [&](auto f) { decimate_wide_kernel<f()><<<g, kDcThreads, smem1, st>>>(d_taps, s.dc); });
-            CUDA_TRY(err_, cudaGetLastError());
-            ++*launches;
-        }
-        if (s.rs.count > 0 || s.rs.carry_n > 0) {
-            const long long tiles = (s.rs.count + kRsTile - 1) / kRsTile;
-            const unsigned g = (unsigned)std::max<long long>(1, std::min<long long>(tiles, grid));
-            resample_wide_kernel_of(mode == kDecimate ? kFmtMid : fmt)<<<g, kRsThreads, smem, st>>>(d_A, d_D, s.rs);
-            CUDA_TRY(err_, cudaGetLastError());
-            ++*launches;
-        }
-        return ERTGPU_OK;
+    void swap_measure() {
+        std::swap(pos, mpos);
+        std::swap(d_hist, d_mhist);
+        std::swap(d_hist1, d_mhist1);
     }
 
-    // allocate's end for the wide path: the last stage's launch shape, the measurement's buffers, and the first stage.
-    int allocate_wide(int device, int sm_count) {
-        const bool mid = mode == kDecimate;
-        smem = rs_wide_smem_bytes(rs.P, rs.T, rs.L, rs.M, mid);
-        {
-            static OncePerDevice once;
-            if (once.first(device)) {
-                CUDA_TRY(err_, cudaFuncSetAttribute(resample_wide_kernel_of(kFmtMid), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF64BE; f++)
-                    if (fmt_name(f))
-                        CUDA_TRY(err_, cudaFuncSetAttribute(resample_wide_kernel_of(f), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            }
-        }
-        if (smem > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "resampler needs %zu B of shared memory", smem);
+    // CTAs of a launch over n items, per to a tile: one per tile, at least one and at most cap.
+    static unsigned grid_of(long long n, long long per, int cap) {
+        return (unsigned)std::max<long long>(1, std::min<long long>((n + per - 1) / per, cap));
+    }
+
+    // A kernel of `threads` threads with `bytes` of dynamic shared memory: it may take the whole 227 KiB of a CTA, and
+    // *cap becomes the most CTAs of it the device runs at once.  `what` names it when it needs more.
+    int fit(const void* kernel, int threads, size_t bytes, const char* what, int sm_count, int* cap) {
+        if (bytes > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "%s needs %zu B of shared memory", what, bytes);
+        CUDA_TRY(err_, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         int per_sm = 0;
-        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resample_wide_kernel_of(mid ? kFmtMid : fmt), kRsThreads, smem));
-        grid = std::max(1, per_sm) * sm_count;
-        CUDA_TRY(err_, cudaMalloc(&d_clevel, ERTRS_GAIN_BINS * sizeof(unsigned long long)));
-        for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_mhist[k], (size_t)rs.T * 4 + 16));
-        if (!mid) return ERTGPU_OK;
-        if (const int rc = allocate_first(device, sm_count)) return rc;
-        for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_mhist1[k], (size_t)(dec.T1 + dec.D + 16) * 4));
+        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, bytes));
+        *cap = std::max(1, per_sm) * sm_count;
         return ERTGPU_OK;
-    }
-
-    static decltype(&resample_wide_kernel<ERTGPU_FORMAT_CU8>) resample_wide_kernel_of(int f) {
-        if (f == kFmtMid) return resample_wide_kernel<kFmtMid>;
-        decltype(&resample_wide_kernel<ERTGPU_FORMAT_CU8>) k = nullptr;
-        fmt_visit(f, [&](auto F) { k = resample_wide_kernel<F()>; });
-        return k;
     }
 
     // The resampler for input at hz: ertrs_plan, or ertrs_plan_tuned and the NCO step on a tuned handle.  It runs when
@@ -647,18 +591,18 @@ private:
     // The first stage's plan of the step over n new input samples at d_in; returns its number of outputs.
     int64_t plan_first(DcArgs& a, const uint8_t* d_in, int64_t n) const {
         const int64_t D = dec.D, T1 = dec.T1;
-        const int64_t in_new = in1_total + n;
+        const int64_t in_new = pos.in1_total + n;
         const int64_t ne = in_new - T1 / 2 > 0 ? (in_new - T1 / 2 + D - 1) / D : 0;  // ertrs_out_end at L = 1, M = D
-        a.hist = d_hist1[cur_hist1];
+        a.hist = d_hist1[pos.cur_hist1];
         a.cur = d_in;
-        a.hist_first = hist1_first;
-        a.hist_n = hist1_n;
+        a.hist_first = pos.hist1_first;
+        a.hist_n = pos.hist1_n;
         a.cur_n = n;
-        a.n0 = in_total;  // the first stage's next output is the second stage's next input
-        a.count = ne - in_total;
+        a.n0 = pos.in_total;  // the first stage's next output is the second stage's next input
+        a.count = ne - pos.in_total;
         a.out = d_mid;
         const int64_t first = std::min(in_new, std::max<int64_t>(0, ne * D - T1 / 2 + 1));
-        a.carry_dst = d_hist1[cur_hist1 ^ 1];
+        a.carry_dst = d_hist1[pos.cur_hist1 ^ 1];
         a.carry_first = first;
         a.carry_n = in_new - first;
         a.D = (int)D;
@@ -671,7 +615,7 @@ private:
     }
 
     // The first stage's device buffers, after the second stage's.
-    int allocate_first(int device, int sm_count) {
+    int allocate_first(int sm_count) {
         CUDA_TRY(err_, cudaMalloc(&d_taps, taps.size() * sizeof(int16_t)));
         CUDA_TRY(err_, cudaMemcpy(d_taps, taps.data(), taps.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
         const size_t hb = wide ? 4 : 2;  // bytes per carried sample, and per stage-1 output
@@ -682,57 +626,24 @@ private:
         CUDA_TRY(err_, cudaMalloc(&d_mid, (size_t)mid * hb));
         per1 = dc_per_thread(dec.D, dec.T1);
         smem1 = dc_smem_bytes(dec.D, dec.T1, per1);
-        {
-            static OncePerDevice once;
-            if (once.first(device))
-                for (int f = ERTGPU_FORMAT_CU8; f <= ERTGPU_FORMAT_CF64BE; f++)
-                    if (fmt_name(f))
-                        CUDA_TRY(err_, cudaFuncSetAttribute(decimate_kernel_of(f), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        }
-        if (smem1 > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "decimator needs %zu B of shared memory", smem1);
-        int per_sm = 0;
+        if (const int rc = fit((const void*)first_kernel, kDcThreads, smem1, "decimator", sm_count, &grid1)) return rc;
         if (wide) {  // decimate_wide_kernel: decimate_kernel's tiles; groups run it per channel (DESIGN §3.12)
-            const void* kw = nullptr;
-            fmt_visit(fmt, [&](auto f) { kw = (const void*)decimate_wide_kernel<f()>; });
-            CUDA_TRY(err_, cudaFuncSetAttribute(kw, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kw, kDcThreads, smem1));
-            grid1 = std::max(1, per_sm) * sm_count;
+            for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_mhist1[k], (size_t)(dec.T1 + dec.D + 16) * 4));
             return ERTGPU_OK;
         }
-        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decimate_kernel_of(fmt), kDcThreads, smem1));
-        grid1 = std::max(1, per_sm) * sm_count;
         per1c = dc_per_thread(dec.D, dec.T1, kDcChannelsSpanWords);
         smem1c = dc_channels_smem_bytes(dec.D, dec.T1, per1c);
-        if (smem1c > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "decimator needs %zu B of shared memory", smem1c);
-        const void* kc = nullptr;
-        fmt_visit(fmt, [&](auto f) { kc = (const void*)decimate_channels_kernel<f()>; });
-        CUDA_TRY(err_, cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kc, kDcThreads, smem1c));
-        grid1c = std::max(1, per_sm) * sm_count;
-        return ERTGPU_OK;
-    }
-
-    static decltype(&decimate_kernel<ERTGPU_FORMAT_CU8>) decimate_kernel_of(int f) {
-        decltype(&decimate_kernel<ERTGPU_FORMAT_CU8>) k = nullptr;
-        fmt_visit(f, [&](auto F) { k = decimate_kernel<F()>; });
-        return k;
-    }
-
-    // The resample_kernel instance of an input format, untuned or tuned.
-    static decltype(&resample_kernel<ERTGPU_FORMAT_CU8, false>) resample_kernel_of(int f, bool mix) {
-        decltype(&resample_kernel<ERTGPU_FORMAT_CU8, false>) k = nullptr;
-        fmt_visit(f, [&](auto F) { k = mix ? resample_kernel<F(), true> : resample_kernel<F(), false>; });
-        return k;
+        return fit((const void*)channels_kernel, kDcThreads, smem1c, "decimator", sm_count, &grid1c);
     }
 
     int64_t k_of(int64_t n) const { return (int64_t)((__int128)n * rs.M / rs.L); }
 
     // Most input samples the next step may take so that it completes at most max_blocks decoder blocks.
     int64_t max_input() const {
-        const int64_t cap_out = (max_blocks + 1) * block - 1 - pend;
-        const int64_t m2 = rs.T / 2 + k_of(out_next + cap_out) - in_total;
+        const int64_t cap_out = (max_blocks + 1) * block - 1 - pos.pend;
+        const int64_t m2 = rs.T / 2 + k_of(pos.out_next + cap_out) - pos.in_total;
         // decimating: the first stage completes at most m2 outputs, ceil((in1_total + x - T1/2) / D) <= in_total + m2
-        return mode == kDecimate ? (in_total + m2) * dec.D + dec.T1 / 2 - in1_total : m2;
+        return mode == kDecimate ? (pos.in_total + m2) * dec.D + dec.T1 / 2 - pos.in1_total : m2;
     }
 };
 
