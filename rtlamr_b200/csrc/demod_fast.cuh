@@ -34,7 +34,7 @@
 
 #include <cuda.h>
 
-#include <atomic>
+#include <algorithm>
 #include <type_traits>
 
 #include "ert_common.cuh"
@@ -115,9 +115,6 @@ constexpr bool fast_block_fits(int L, int BS) { return 2 * L <= BS; }
 // bytes into the history, which must be 16-byte aligned (a shorter packet: PacketSymbols = 1; PacketLength % 8 != 0: an
 // odd PacketSymbols at chip length 78).  Geometries that do not fit take demod_generic_kernel.
 constexpr bool fast_history_fits(int L, int PacketLength) { return PacketLength >= 2 * L && PacketLength % 8 == 0; }
-constexpr bool fast_geometry_fits(int L, int BS, int PacketLength) {
-    return fast_block_fits(L, BS) && fast_history_fits(L, PacketLength);
-}
 
 template <int CL>
 struct FastGeom {
@@ -405,69 +402,25 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+// The driver's entry point, looked up once per process (null when the driver has none).
 inline EncodeTiledFn encode_tiled_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
+    static const EncodeTiledFn fn = [] {
         void* p = nullptr;
         cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
+        const bool ok = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+                        q == cudaDriverEntryPointSuccess;
+        return ok ? (EncodeTiledFn)p : nullptr;
+    }();
     return fn;
 }
 
-// Per-device caches for things that are asked on every launch (a handle's calls are serialised by its owner, but
-// handles on several GPUs or threads may share these statics: a lost update only repeats an idempotent query).
-inline int current_device() {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    return dev;
-}
-inline int sm_count_of(int dev) {
-    static std::atomic<int> cache[64];
-    if (dev < 0 || dev >= 64) {
-        int n = 132;
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        return n;
-    }
-    int n = cache[dev].load(std::memory_order_relaxed);
-    if (n == 0) {
-        n = 132;
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        cache[dev].store(n, std::memory_order_relaxed);
-    }
-    return n;
-}
-// true the first time it is asked for (this flag, device): the caller then sets its per-device function attribute
-struct OncePerDevice {
-    std::atomic<unsigned long long> mask{0};
-    bool first(int dev) {
-        if (dev < 0 || dev >= 64) return true;
-        const unsigned long long bit = 1ull << dev;
-        return (mask.fetch_or(bit, std::memory_order_relaxed) & bit) == 0;
-    }
-};
-
 // Shared-space address of the dynamic segment of a kernel without static shared memory (the first KiB
-// of the window is reserved by the system).  Asked from the device once: the demod kernel's map depends
-// on where the 64 KiB-aligned LUT lands, and the launch requests exactly the bytes the map needs so that
-// CTAs of the Search/extract kernels of another call can share the SM.
+// of the window is reserved by the system).  Asked from the device once per handle (ertgpu_allocate): the demod
+// kernel's map depends on where the 64 KiB-aligned LUT lands, and the launch requests exactly the bytes the map needs
+// so that CTAs of the Search/extract kernels of another call can share the SM.
 __global__ void smem_base_probe_kernel(uint32_t* out) {
     extern __shared__ __align__(128) uint8_t probe_smem[];
     *out = smem_u32(probe_smem);
-}
-inline uint32_t dynamic_smem_base() {
-    static uint32_t base = 0;
-    if (base) return base;
-    uint32_t* d = nullptr;
-    uint32_t h = 0;
-    if (cudaMalloc(&d, 4) != cudaSuccess) return 1024;
-    smem_base_probe_kernel<<<1, 1, 1024>>>(d);
-    if (cudaMemcpy(&h, d, 4, cudaMemcpyDeviceToHost) != cudaSuccess || h == 0) h = 1024;
-    cudaFree(d);
-    base = h;
-    return base;
 }
 
 // Dynamic shared memory the kernel's map needs for W warps when the segment starts at shared address sbase:
@@ -499,67 +452,63 @@ inline double fast_round_cost(long long ntiles, long long sms, int W) {
     return full * unit + last;
 }
 
-template <int CL, int W>
-int launch_demod_fast_cw(const uint8_t* iq, const uint8_t* hist, int hist_samples, int hist_valid,
-                         const float* lut, uint32_t* plane_out, long long nblocks, int BS,
-                         unsigned long long* tile_counter, cudaStream_t st, int* w_out) {
-    if (w_out) *w_out = W;
+// A handle's demod_fast instances, chosen once (fast_demod): <CL, fast_warps<CL>()> and, when that has 8 warps, <CL, 7>,
+// each with the dynamic shared memory its launches request; and the tensor map of the handle's last call.
+struct FastDemod {
+    using Kernel = void (*)(CUtensorMap, const uint8_t*, const uint8_t*, int, int, const float*, uint32_t*, long long, int,
+                            unsigned long long*, long long);
+    Kernel kern[2] = {nullptr, nullptr};  // [1]: the 7-warp instance, if any
+    int warps[2] = {0, 0};
+    int smem[2] = {0, 0};
+    int row_bytes = 0;                    // the map's box width, FastGeom<CL>::kRowBytes
+    // Calls that stream through the same staging buffer reuse the map.  Invariant: the key and the handle's constants are
+    // all the map contains -- a buffer freed and re-allocated at the same address with the same number of blocks gives a
+    // byte-identical descriptor (addresses and extents, no handle to the allocation), so a stale hit cannot exist.
+    const void* map_iq = nullptr;
+    long long map_nblocks = 0;
+    CUtensorMap map;
+};
+
+template <int CL>
+FastDemod fast_demod_of(uint32_t sbase) {
     using G = FastGeom<CL>;
-    auto kern = demod_fast_kernel<CL, W>;
-    const int smem = fast_smem_bytes<G>(W, dynamic_smem_base());
-    if (smem > 227 * 1024) return (int)cudaErrorInvalidValue;
-    const int dev = current_device();
-    {   // a per-device attribute (handles on several GPUs may live in one process)
-        static OncePerDevice once;
-        if (once.first(dev)) {
-            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-            if (e != cudaSuccess) return (int)e;
-        }
+    constexpr int W = fast_warps<CL>();
+    FastDemod f;
+    f.kern[0] = demod_fast_kernel<CL, W>;
+    f.warps[0] = W;
+    f.smem[0] = fast_smem_bytes<G>(W, sbase);
+    if constexpr (W == 8) {
+        f.kern[1] = demod_fast_kernel<CL, 7>;
+        f.warps[1] = 7;
+        f.smem[1] = fast_smem_bytes<G>(7, sbase);
     }
-    if (!fast_geometry_fits(G::L, BS, hist_samples)) return (int)cudaErrorInvalidValue;
-    // the IQ bytes of the call as a 2D uint8 tensor: [nblocks rows][BlockSize2 bytes]
-    EncodeTiledFn enc = encode_tiled_fn();
-    if (!enc) return (int)cudaErrorNotSupported;
-    // the descriptor only depends on (base, rows, row length, box): calls that stream through the same
-    // staging buffer reuse it.  Invariant: the key is everything the encoded map contains -- a buffer that was freed and
-    // re-allocated at the same address with the same number of blocks and block size gives a byte-identical descriptor (a
-    // tensor map holds addresses and extents, no handle to the allocation), so a stale hit cannot exist; the cache is per
-    // thread and per template instantiation (the box is part of the type).
-    struct MapKey { const void* iq; long long nblocks; int BS; };
-    static thread_local MapKey last_key = {nullptr, 0, 0};
-    static thread_local CUtensorMap map;
-    if (!(last_key.iq == iq && last_key.nblocks == nblocks && last_key.BS == BS)) {
-    const cuuint64_t gdim[2] = {(cuuint64_t)(2 * BS), (cuuint64_t)nblocks};
-    const cuuint64_t gstride[1] = {(cuuint64_t)(2 * BS)};
-    const cuuint32_t box[2] = {(cuuint32_t)G::kRowBytes, 32u};
-    const cuuint32_t estr[2] = {1u, 1u};
-    // L2 promotion: the L2 fetches 256 B from DRAM around a box row
-    CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(iq), gdim, gstride, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return (int)cudaErrorInvalidValue;
-    last_key = {iq, nblocks, BS};
-    }
-    const long long ntiles = (nblocks + 31) / 32;
-    const int sms = sm_count_of(dev);
-    long long grid = (ntiles + W - 1) / W;
-    if (grid > sms) grid = sms;
-    if (grid < 1) grid = 1;
-    const long long dyn = fast_dynamic_tiles(ntiles, grid, W);
-    kern<<<(unsigned)grid, W * 32, smem, st>>>(map, iq, hist, hist_samples, hist_valid, lut, plane_out, nblocks, BS, tile_counter, dyn);
-    return (int)cudaGetLastError();
+    f.row_bytes = G::kRowBytes;
+    return f;
 }
 
-// chip lengths with a specialised kernel: every value the reference CLI accepts (flags.go:127-132
-// allows 8,32,40,...,96) except 8, plus 78, the rate the reference's sample.bin fixture was captured at
-// (nothing in the kernel needs CL to be a multiple of 8: only L is).  Anything else uses the generic kernel.
-// Two arguments: the instance of a chip length and block size (fast_block_fits), whatever the packet.
-inline int demod_fast_variant(int CL, int BS) {
+// The instances of a chip length when the dynamic segment starts at shared address sbase.  Chip lengths with a
+// specialised kernel: every value the reference CLI accepts (flags.go:127-132 allows 8,32,40,...,96) except 8, plus 78,
+// the rate the reference's sample.bin fixture was captured at (nothing in the kernel needs CL to be a multiple of 8: only
+// L is).  Anything else has no instance and uses the generic kernel.
+inline FastDemod fast_demod(int CL, uint32_t sbase) {
     switch (CL) {
-        case 32: case 40: case 48: case 56: case 64: case 72: case 78: case 80: case 88: case 96:
-            return fast_block_fits(fast_body_len(CL), BS) ? CL : 0;
-        default: return 0;
+        case 32: return fast_demod_of<32>(sbase);
+        case 40: return fast_demod_of<40>(sbase);
+        case 48: return fast_demod_of<48>(sbase);
+        case 56: return fast_demod_of<56>(sbase);
+        case 64: return fast_demod_of<64>(sbase);
+        case 72: return fast_demod_of<72>(sbase);
+        case 78: return fast_demod_of<78>(sbase);
+        case 80: return fast_demod_of<80>(sbase);
+        case 88: return fast_demod_of<88>(sbase);
+        case 96: return fast_demod_of<96>(sbase);
+        default: return FastDemod{};
     }
+}
+
+// The instance of a chip length and block size (fast_block_fits), whatever the packet: the chip length, or 0.
+inline int demod_fast_variant(int CL, int BS) {
+    return fast_demod(CL, 0).kern[0] && fast_block_fits(fast_body_len(CL), BS) ? CL : 0;
 }
 // The instance a decoder runs: the same, if its packet length also gives the lead-in history (fast_history_fits).
 inline int demod_fast_variant(int CL, int BS, int PacketLength) {
@@ -567,29 +516,38 @@ inline int demod_fast_variant(int CL, int BS, int PacketLength) {
     return v != 0 && fast_history_fits(fast_body_len(CL), PacketLength) ? v : 0;
 }
 
-inline int launch_demod_fast(int variant, const uint8_t* iq, const uint8_t* hist, int hist_samples,
-                             int hist_valid, const float* lut, uint32_t* plane_out, long long nblocks,
-                             int BS, unsigned long long* tile_counter, cudaStream_t st, int* w_out = nullptr) {
-#define ERT_FAST_ARGS iq, hist, hist_samples, hist_valid, lut, plane_out, nblocks, BS, tile_counter, st, w_out
-    // Work tiles are handed out in rounds of (SMs x resident warps).  With two warps per scheduler the SM's
-    // rate still grows almost linearly with the warp count, so when 7 warps need no more rounds than 8 the
-    // fuller last round of 7 wins (fast_round_cost); long calls keep 8.
-    const int sms = sm_count_of(current_device());
-    const long long T = (nblocks + 31) / 32;
-    const bool seven = fast_round_cost(T, sms, 7) < fast_round_cost(T, sms, 8);
-#define ERT_FAST_CASE(N)                                                                         \
-    case N:                                                                                      \
-        if constexpr (fast_warps<N>() == 8) {                                                    \
-            if (seven) return launch_demod_fast_cw<N, 7>(ERT_FAST_ARGS);                         \
-        }                                                                                        \
-        return launch_demod_fast_cw<N, fast_warps<N>()>(ERT_FAST_ARGS);
-    switch (variant) {
-        ERT_FAST_CASE(32) ERT_FAST_CASE(40) ERT_FAST_CASE(48) ERT_FAST_CASE(56) ERT_FAST_CASE(64)
-        ERT_FAST_CASE(72) ERT_FAST_CASE(78) ERT_FAST_CASE(80) ERT_FAST_CASE(88) ERT_FAST_CASE(96)
-        default: return (int)cudaErrorInvalidValue;
+// Launch one of f's instances over a call of nblocks blocks on a device of sms SMs; *w_out: its warps.  Work tiles are
+// handed out in rounds of (SMs x resident warps).  With two warps per scheduler the SM's rate still grows almost
+// linearly with the warp count, so when 7 warps need no more rounds than 8 the fuller last round of 7 wins
+// (fast_round_cost); long calls keep 8.
+inline cudaError_t launch_demod_fast(FastDemod& f, int sms, const uint8_t* iq, const uint8_t* hist, int hist_samples,
+                                     int hist_valid, const float* lut, uint32_t* plane_out, long long nblocks, int BS,
+                                     unsigned long long* tile_counter, cudaStream_t st, int* w_out) {
+    const long long ntiles = (nblocks + 31) / 32;
+    const int k = f.kern[1] && fast_round_cost(ntiles, sms, 7) < fast_round_cost(ntiles, sms, 8) ? 1 : 0;
+    const int W = f.warps[k];
+    *w_out = W;
+    if (f.map_iq != iq || f.map_nblocks != nblocks) {
+        // the IQ bytes of the call as a 2D uint8 tensor: [nblocks rows][BlockSize2 bytes]
+        const EncodeTiledFn enc = encode_tiled_fn();
+        if (!enc) return cudaErrorNotSupported;
+        const cuuint64_t gdim[2] = {(cuuint64_t)(2 * BS), (cuuint64_t)nblocks};
+        const cuuint64_t gstride[1] = {(cuuint64_t)(2 * BS)};
+        const cuuint32_t box[2] = {(cuuint32_t)f.row_bytes, 32u};
+        const cuuint32_t estr[2] = {1u, 1u};
+        // L2 promotion: the L2 fetches 256 B from DRAM around a box row
+        const CUresult r = enc(&f.map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(iq), gdim, gstride, box, estr,
+                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) return cudaErrorInvalidValue;
+        f.map_iq = iq;
+        f.map_nblocks = nblocks;
     }
-#undef ERT_FAST_CASE
-#undef ERT_FAST_ARGS
+    const long long grid = std::max(1ll, std::min<long long>((ntiles + W - 1) / W, sms));
+    const long long dyn = fast_dynamic_tiles(ntiles, grid, W);
+    f.kern[k]<<<(unsigned)grid, W * 32, f.smem[k], st>>>(f.map, iq, hist, hist_samples, hist_valid, lut, plane_out, nblocks,
+                                                          BS, tile_counter, dyn);
+    return cudaGetLastError();
 }
 
 }  // namespace ert

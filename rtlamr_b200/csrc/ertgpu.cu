@@ -17,7 +17,6 @@
 #include <sched.h>
 
 #include <algorithm>
-#include <atomic>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -40,6 +39,34 @@
 
 using namespace ert;
 
+// The kernels of a handle's pipeline and their launch constants, chosen from its configuration at allocate (the demod
+// again by ertgpu_set_demod_variant).  A pipeline only picks demod_fast's warp count and sizes its grids.
+struct PipelineKernels {
+    uint32_t smem_base = 0;      // shared address of a kernel's dynamic segment on the handle's device (demod_fast's map)
+    int demod_variant = 0;       // 0 generic, else specialised chip length
+    FastDemod fast;              // demod_variant != 0
+    int generic_threads = 0;     // demod_variant == 0: demod_generic_kernel's CTA size and shared memory (more than
+    size_t generic_smem = 0;     // 227 KiB: the decode call fails)
+    // Search: the sliding-window instance (none: search_generic_kernel), its constants but nwords, smem and most CTAs
+    decltype(&search_slide_kernel<1, false>) slide = nullptr;
+    SlideParams sl{};
+    int slide_smem = 0;
+    long long slide_cap = 0;
+    std::string search_label;    // ";search_slide_kernel<...>" or ";search_generic_kernel"
+    decltype(&extract_words_kernel<4>) extract = nullptr;
+    std::string extract_label;
+    bool r900_chain = false;     // PKL % 8 == 0: r900 chains start on 8-sample (16-byte) boundaries (else replay only)
+};
+
+// The decode stream position: all that a stream start resets.
+struct DecodePos {
+    int cur_plane = 0, cur_hist = 0;  // the ping-pong plane and history the next pipeline reads
+    int hist_valid = 0;
+    int64_t block_counter = 0;  // number of reference Decode calls consumed so far
+    bool fresh = true;          // next pipeline must see zeroed history
+    bool started = false;       // a decode call was accepted (ertgpu_set_input_scale)
+};
+
 struct ertgpu_handle {
     std::string err;
     std::vector<ertgpu_protocol> protos;
@@ -58,10 +85,7 @@ struct ertgpu_handle {
     uint16_t* d_crc = nullptr;
     uint32_t* d_plane[2] = {nullptr, nullptr};
     size_t plane_words = 0;
-    int cur_plane = 0;
     uint8_t* d_hist[2] = {nullptr, nullptr};
-    int cur_hist = 0;
-    int hist_valid = 0;
     uint8_t* d_stage[2] = {nullptr, nullptr};
     size_t stage_bytes = 0;
     uint8_t* h_stage[2] = {nullptr, nullptr};  // pinned staging of pageable input (allocated on first use)
@@ -76,7 +100,6 @@ struct ertgpu_handle {
     unsigned int* d_slot_count = nullptr;
     float* d_r900_scratch = nullptr;  // [slot][r900_span] running sums
     int r900_slots = 0, r900_span = 0;
-    bool r900_vec = false;            // PKL % 8 == 0: r900 chains start on 8-sample (16-byte) boundaries
     ertgpu_candidate* d_out = nullptr;
     unsigned long long cand_cap = 0;
     unsigned long long* d_counters = nullptr;  // kCntHits, kCntOut, kCntValid, kCntTile (demod work tiles), kCntWords
@@ -85,18 +108,16 @@ struct ertgpu_handle {
     size_t tap_floats = 0;
 
     int64_t max_blocks = 0;
-    int64_t block_counter = 0;  // number of reference Decode calls consumed so far
+    DecodePos pos;
     bool has_r900 = false;
-    int demod_variant = 0;      // 0 generic, else specialised chip length
     int sm_count = 132;
+    PipelineKernels pipe;
 
     // state of the last enqueued pipeline (for fetch and taps)
     bool pending = false;       // work is enqueued on pending_stream and not yet synchronised
     bool pending_counts = false;  // ... and it copies counters back (a resample_kernel launch alone does not)
     bool uncopied = false;      // a pipeline is synchronised, its candidates still only on the device
     unsigned long long uncopied_n = 0;
-    bool fresh = true;          // next pipeline must see zeroed history (start of stream / after reset)
-    bool started = false;       // a decode call was accepted since allocate / reset (ertgpu_set_input_scale)
     cudaStream_t pending_stream = nullptr;
     const uint8_t* last_iq = nullptr;
     const uint8_t* last_hist = nullptr;
@@ -271,32 +292,78 @@ cudaError_t launch_dep(bool pdl, K kern, dim3 grid, dim3 block, size_t smem, cud
     return cudaLaunchKernelEx(&cfg, kern, args...);
 }
 
-// Search by the sliding-window kernel; PAT...: the preambles' first 16 bits as compile-time constants (none: read
-// from sl).  Appends the instantiation to h->kernels, the constants spelt as in the source ("0xF953u, 0x16A3u").
+// h's demod instance for a variant (0: demod_generic_kernel), and the shared-memory limit of every instance it launches.
+int choose_demod(ertgpu_handle* h, int variant) {
+    PipelineKernels& k = h->pipe;
+    k.demod_variant = variant;
+    if (variant != 0) {
+        k.fast = fast_demod(variant, k.smem_base);
+        for (int i = 0; i < 2 && k.fast.kern[i]; i++)
+            if (const int rc = allow_dynamic_smem(h->err, (const void*)k.fast.kern[i], k.fast.smem[i], "demod_fast_kernel")) return rc;
+        return ERTGPU_OK;
+    }
+    const int CL = h->dcfg.CL;
+    int nthr = 128;
+    while (nthr > 32 && (256 + 2 * (size_t)CL * nthr) * sizeof(float) > 200 * 1024) nthr >>= 1;
+    k.generic_threads = nthr;
+    k.generic_smem = (256 + 2 * (size_t)CL * nthr) * sizeof(float);
+    if (k.generic_smem > 227 * 1024) return ERTGPU_OK;  // the decode call reports it
+    return allow_dynamic_smem(h->err, (const void*)demod_generic_kernel, k.generic_smem, "demod_generic_kernel");
+}
+
+// search_slide_kernel<NPRE, HALF, PAT...> and its label; PAT...: the preambles' first 16 bits as compile-time constants
+// (none: read from sl), spelt as in the source ("0xF953u, 0x16A3u").
 template <int NPRE, uint32_t... PAT>
-int launch_slide(ertgpu_handle* h, const uint32_t* plane, const SlideParams& sl, bool pdl, cudaStream_t st) {
-    const bool half = (h->dcfg.SL % 32) == 16;
-    const auto kern = half ? search_slide_kernel<NPRE, true, PAT...> : search_slide_kernel<NPRE, false, PAT...>;
-    static OncePerDevice once[2];
-    if (once[half].first(h->device))
-        CUDA_TRY(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (2 * kSlideMaxLoad + 4)));
-    const int smem = 2 * sl.load_words * 4 + 16;
-    const long long tiles = (sl.nwords + sl.tile_words - 1) / sl.tile_words;
-    int per_sm = (227 * 1024) / (smem + 1024);
-    if (per_sm > 2048 / kSlideThreads) per_sm = 2048 / kSlideThreads;
-    unsigned grid = (unsigned)std::min<long long>(tiles, (long long)h->sm_count * per_sm);
-    if (grid < 1) grid = 1;
-    CUDA_TRY(h, launch_dep(pdl, kern, dim3(grid), dim3(kSlideThreads), (size_t)smem, st, plane, sl, h->d_hits, h->d_words,
-                           h->cand_cap, h->d_counters));
-    h->kernels += ";search_slide_kernel<" + std::to_string(NPRE) + (half ? ",true" : ",false");
+void slide_instance(PipelineKernels& k, bool half) {
+    k.slide = half ? search_slide_kernel<NPRE, true, PAT...> : search_slide_kernel<NPRE, false, PAT...>;
+    k.search_label = ";search_slide_kernel<" + std::to_string(NPRE) + (half ? ",true" : ",false");
     const uint32_t pat[] = {PAT..., kSlideRuntimePat};
     for (int i = 0; pat[i] != kSlideRuntimePat; i++) {
         char s[16];
         snprintf(s, sizeof(s), "%s0x%04Xu", i ? ", " : ",", pat[i]);
-        h->kernels += s;
+        k.search_label += s;
     }
-    h->kernels += ">";
-    return ERTGPU_OK;
+    k.search_label += ">";
+}
+
+// h's Search: the sliding-window kernel where the geometry fits it, search_generic_kernel for every other geometry.
+int choose_search(ertgpu_handle* h) {
+    const DevCfg& c = h->dcfg;
+    PipelineKernels& k = h->pipe;
+    if (!make_slide_params(c, (long long)c.hist_words * 32 - c.PKL, 0, &k.sl)) {
+        k.search_label = ";search_generic_kernel";
+        return ERTGPU_OK;
+    }
+    const bool half = (c.SL % 32) == 16;
+    if (c.npre == 1) {
+        // single preamble: the stock protocols' first 16 bits are compile-time constants
+        // (scm 0xF953, scm+ 0x16A3, idm/netidm 0x5555, r900 0x0000), anything else runs the generic probe
+        switch (slide_pattern(c, 0)) {
+            case 0xF953u: slide_instance<1, 0xF953u>(k, half); break;
+            case 0x16A3u: slide_instance<1, 0x16A3u>(k, half); break;
+            case 0x5555u: slide_instance<1, 0x5555u>(k, half); break;
+            case 0x0000u: slide_instance<1, 0x0000u>(k, half); break;
+            default: slide_instance<1>(k, half); break;
+        }
+    } else if (c.npre == 2) {
+        slide_instance<2>(k, half);
+    } else if (c.npre == 3) {
+        // scm, scm+, idm (or netidm) registered in that order: BASELINE.json configs[2]
+        if (slide_pattern(c, 0) == 0xF953u && slide_pattern(c, 1) == 0x16A3u && slide_pattern(c, 2) == 0x5555u)
+            slide_instance<3, 0xF953u, 0x16A3u, 0x5555u>(k, half);
+        else
+            slide_instance<3>(k, half);
+    } else {
+        // "-msgtype=all" = scm, scm+, idm, r900 (main.go:67-73)
+        if (c.npre == 4 && slide_pattern(c, 0) == 0xF953u && slide_pattern(c, 1) == 0x16A3u &&
+            slide_pattern(c, 2) == 0x5555u && slide_pattern(c, 3) == 0x0000u)
+            slide_instance<4, 0xF953u, 0x16A3u, 0x5555u, 0x0000u>(k, half);
+        else
+            slide_instance<4>(k, half);
+    }
+    k.slide_smem = 2 * k.sl.load_words * 4 + 16;
+    k.slide_cap = (long long)h->sm_count * std::min((227 * 1024) / (k.slide_smem + 1024), 2048 / kSlideThreads);
+    return allow_dynamic_smem(h->err, (const void*)k.slide, k.slide_smem, "search_slide_kernel");
 }
 
 // Enqueue the whole per-call pipeline for the s.nblocks blocks whose IQ bytes are at s.iq, behind the input stage's
@@ -305,18 +372,19 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
     const uint8_t* d_iq = s.iq;
     const int64_t nblocks = s.nblocks;
     const DevCfg& c = h->dcfg;
-    uint32_t* plane = h->d_plane[h->cur_plane];
-    uint32_t* plane_next = h->d_plane[h->cur_plane ^ 1];
-    const uint8_t* hist = h->d_hist[h->cur_hist];
-    uint8_t* hist_next = h->d_hist[h->cur_hist ^ 1];
+    DecodePos& pos = h->pos;
+    uint32_t* plane = h->d_plane[pos.cur_plane];
+    uint32_t* plane_next = h->d_plane[pos.cur_plane ^ 1];
+    const uint8_t* hist = h->d_hist[pos.cur_hist];
+    uint8_t* hist_next = h->d_hist[pos.cur_hist ^ 1];
     const long long nwords = nblocks * c.words_per_block;
     const long long p0 = (long long)c.hist_words * 32 - c.PKL;
     h->launches = 0;
 
     CUDA_TRY(h, cudaMemsetAsync(h->d_counters, 0, kCntN * sizeof(unsigned long long), st));
-    if (h->fresh) {  // Quantized starts as zeros (decode.go:145); only the history in front of the call is read
+    if (pos.fresh) {  // Quantized starts as zeros (decode.go:145); only the history in front of the call is read
         CUDA_TRY(h, cudaMemsetAsync(plane, 0, (size_t)c.hist_words * sizeof(uint32_t), st));
-        h->fresh = false;
+        pos.fresh = false;
     }
 
     const bool tm = h->stage_timing;
@@ -330,22 +398,19 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[0], st));
     if (const int rc = h->in.launch(s, st, &h->launches)) return rc;
     // 1. magnitude + matched filter + quantize + pack
-    if (h->demod_variant != 0) {
+    PipelineKernels& k = h->pipe;
+    if (k.demod_variant != 0) {
         int w_used = 0;
-        int rc = launch_demod_fast(h->demod_variant, d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut,
-                                   plane + c.hist_words, nblocks, c.BS, h->d_counters + kCntTile, st, &w_used);
-        if (rc != 0) return fail(h, ERTGPU_ECUDA, "demod_fast launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-        h->kernels = "demod_fast_kernel<" + std::to_string(h->demod_variant) + "," + std::to_string(w_used) + ">";
+        const cudaError_t e = launch_demod_fast(k.fast, h->sm_count, d_iq, hist, c.hist_samples, pos.hist_valid, h->d_lut,
+                                                plane + c.hist_words, nblocks, c.BS, h->d_counters + kCntTile, st, &w_used);
+        if (e != cudaSuccess) return fail(h, ERTGPU_ECUDA, "demod_fast launch failed: %s", cudaGetErrorString(e));
+        h->kernels = "demod_fast_kernel<" + std::to_string(k.demod_variant) + "," + std::to_string(w_used) + ">";
     } else {
         h->kernels = "demod_generic_kernel";
-        int nthr = 128;
-        while (nthr > 32 && (256 + 2 * (size_t)c.CL * nthr) * sizeof(float) > 200 * 1024) nthr >>= 1;
-        const size_t smem = (256 + 2 * (size_t)c.CL * nthr) * sizeof(float);
-        if (smem > 227 * 1024) return fail(h, ERTGPU_EINVAL, "chip length %d too large for the generic kernel", c.CL);
-        CUDA_TRY(h, cudaFuncSetAttribute(demod_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const unsigned grid = (unsigned)((nblocks + nthr - 1) / nthr);
-        demod_generic_kernel<<<grid, nthr, smem, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut,
-                                                       plane + c.hist_words, nblocks, c.BS, c.CL);
+        if (k.generic_smem > 227 * 1024) return fail(h, ERTGPU_EINVAL, "chip length %d too large for the generic kernel", c.CL);
+        const unsigned grid = (unsigned)((nblocks + k.generic_threads - 1) / k.generic_threads);
+        demod_generic_kernel<<<grid, k.generic_threads, k.generic_smem, st>>>(d_iq, hist, c.hist_samples, pos.hist_valid,
+                                                                             h->d_lut, plane + c.hist_words, nblocks, c.BS, c.CL);
         CUDA_TRY(h, cudaGetLastError());
     }
     h->launches++;
@@ -353,48 +418,22 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
 
     // 2. preamble search over every start position of the call: the sliding-window kernel where the geometry fits
     //    it, search_generic_kernel for every other geometry
-    {
-        SlideParams sl;
-        int rc = ERTGPU_OK;
-        if (make_slide_params(c, p0, nwords, &sl)) {
-            if (c.npre == 1) {
-                // single preamble: the stock protocols' first 16 bits are compile-time constants
-                // (scm 0xF953, scm+ 0x16A3, idm/netidm 0x5555, r900 0x0000), anything else runs the generic probe
-                switch (slide_pattern(c, 0)) {
-                    case 0xF953u: rc = launch_slide<1, 0xF953u>(h, plane, sl, pdl, st); break;
-                    case 0x16A3u: rc = launch_slide<1, 0x16A3u>(h, plane, sl, pdl, st); break;
-                    case 0x5555u: rc = launch_slide<1, 0x5555u>(h, plane, sl, pdl, st); break;
-                    case 0x0000u: rc = launch_slide<1, 0x0000u>(h, plane, sl, pdl, st); break;
-                    default: rc = launch_slide<1>(h, plane, sl, pdl, st); break;
-                }
-            } else if (c.npre == 2) {
-                rc = launch_slide<2>(h, plane, sl, pdl, st);
-            } else if (c.npre == 3) {
-                // scm, scm+, idm (or netidm) registered in that order: BASELINE.json configs[2]
-                if (slide_pattern(c, 0) == 0xF953u && slide_pattern(c, 1) == 0x16A3u && slide_pattern(c, 2) == 0x5555u)
-                    rc = launch_slide<3, 0xF953u, 0x16A3u, 0x5555u>(h, plane, sl, pdl, st);
-                else
-                    rc = launch_slide<3>(h, plane, sl, pdl, st);
-            } else {
-                // "-msgtype=all" = scm, scm+, idm, r900 (main.go:67-73)
-                if (c.npre == 4 && slide_pattern(c, 0) == 0xF953u && slide_pattern(c, 1) == 0x16A3u &&
-                    slide_pattern(c, 2) == 0x5555u && slide_pattern(c, 3) == 0x0000u)
-                    rc = launch_slide<4, 0xF953u, 0x16A3u, 0x5555u, 0x0000u>(h, plane, sl, pdl, st);
-                else
-                    rc = launch_slide<4>(h, plane, sl, pdl, st);
-            }
-        } else {
-            const int nthr = 256;
-            long long blocks = std::min<long long>((nwords + nthr - 1) / nthr, (long long)h->sm_count * 16);
-            if (blocks < 1) blocks = 1;
-            CUDA_TRY(h, launch_dep(pdl, search_generic_kernel, dim3((unsigned)blocks), dim3(nthr), 0, st, (const uint32_t*)plane, p0, nwords, c,
-                                   h->d_hits, h->d_words, h->cand_cap, h->d_counters));
-            h->kernels += ";search_generic_kernel";
-        }
-        if (rc) return rc;
-        CUDA_TRY(h, cudaGetLastError());
-        h->launches++;
+    if (k.slide) {
+        SlideParams sl = k.sl;
+        sl.nwords = nwords;
+        const long long tiles = (nwords + sl.tile_words - 1) / sl.tile_words;
+        const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(tiles, k.slide_cap));
+        CUDA_TRY(h, launch_dep(pdl, k.slide, dim3(grid), dim3(kSlideThreads), (size_t)k.slide_smem, st, (const uint32_t*)plane, sl,
+                               h->d_hits, h->d_words, h->cand_cap, h->d_counters));
+    } else {
+        const int nthr = 256;
+        const long long blocks = std::max(1ll, std::min<long long>((nwords + nthr - 1) / nthr, (long long)h->sm_count * 16));
+        CUDA_TRY(h, launch_dep(pdl, search_generic_kernel, dim3((unsigned)blocks), dim3(nthr), 0, st, (const uint32_t*)plane, p0, nwords, c,
+                               h->d_hits, h->d_words, h->cand_cap, h->d_counters));
     }
+    h->kernels += k.search_label;
+    CUDA_TRY(h, cudaGetLastError());
+    h->launches++;
 
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[2], st));
     // 3. r900 payload digits for hits of an r900 preamble
@@ -404,12 +443,12 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
         CUDA_TRY(h, cudaMemsetAsync(h->d_slot_count, 0, sizeof(unsigned int), st));
         // the chain kernel loads 8 samples (16 bytes) at a time from chain starts (b + 1) * BS - BUF: without that
         // alignment no block gets a scratch slot and every r900 hit takes the exact per-candidate replay
-        const int slots = h->r900_vec ? h->r900_slots : 0;
+        const int slots = k.r900_chain ? h->r900_slots : 0;
         r900_mark_kernel<<<(unsigned)h->sm_count, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->d_slot_block,
                                               slots, h->d_slot_count);
         CUDA_TRY(h, cudaGetLastError());
-        if (h->r900_vec) {   // producer warps + one consumer warp per 16 chains, hand-offs through shared memory
-            r900_chain2_kernel<<<(unsigned)h->sm_count * 2, (kChainProducers + 1) * 32, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, c, h->d_slot_block,
+        if (k.r900_chain) {   // producer warps + one consumer warp per 16 chains, hand-offs through shared memory
+            r900_chain2_kernel<<<(unsigned)h->sm_count * 2, (kChainProducers + 1) * 32, 0, st>>>(d_iq, hist, c.hist_samples, pos.hist_valid, c, h->d_slot_block,
                                                         slots, h->d_slot_count, h->r900_span, h->d_r900_scratch);
             CUDA_TRY(h, cudaGetLastError());
             r900_digits_kernel<<<(unsigned)h->sm_count * 16, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->r900_span,
@@ -421,7 +460,7 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
             h->kernels += ";r900_replay_kernel";
         }
         // blocks that found no scratch slot: exact per-candidate replay
-        r900_replay_kernel<<<(unsigned)h->sm_count, 64, 0, st>>>(d_iq, hist, c.hist_samples, h->hist_valid, h->d_lut, c, h->d_hits,
+        r900_replay_kernel<<<(unsigned)h->sm_count, 64, 0, st>>>(d_iq, hist, c.hist_samples, pos.hist_valid, h->d_lut, c, h->d_hits,
                                                h->cand_cap, h->d_counters, h->d_block_slot, h->d_digits, h->d_slot_count, slots);
         CUDA_TRY(h, cudaGetLastError());
         h->launches += 2;
@@ -437,15 +476,12 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
         ca.nsamples = nblocks * c.BS;
         const unsigned grid = (unsigned)h->sm_count * 4;
         const bool dep = pdl && !h->has_r900;   // the r900 kernels between Search and Slice are ordinary launches
-        constexpr int kFullK = (ERTGPU_MAX_PACKET_BYTES * 8 + 31) / 32;
-        const bool short_packets = c.PK <= 128;
-        const auto kern = short_packets ? extract_words_kernel<4> : extract_words_kernel<kFullK>;
-        CUDA_TRY(h, launch_dep(dep, kern, dim3(grid), dim3(kExtractWarps * 32), 0, st, (const uint32_t*)plane, p0, c,
-                               (const HitWord*)h->d_words, h->cand_cap, (const uint16_t*)h->d_crc, h->gf, digits, (long long)h->block_counter,
+        CUDA_TRY(h, launch_dep(dep, k.extract, dim3(grid), dim3(kExtractWarps * 32), 0, st, (const uint32_t*)plane, p0, c,
+                               (const HitWord*)h->d_words, h->cand_cap, (const uint16_t*)h->d_crc, h->gf, digits, (long long)pos.block_counter,
                                flags, h->d_out, h->cand_cap, h->d_counters, ca));
         CUDA_TRY(h, cudaGetLastError());
         h->launches++;
-        h->kernels += ";extract_words_kernel<" + std::to_string(short_packets ? 4 : kFullK) + ">";
+        h->kernels += k.extract_label;
     }
     if (h->in.mode != InputStage::kPass) h->kernels += ";" + h->in.label(s.shared_first);
 
@@ -456,18 +492,17 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
 
     h->last_iq = d_iq;
     h->last_hist = hist;
-    h->last_hist_valid = h->hist_valid;
+    h->last_hist_valid = pos.hist_valid;
     h->last_plane = plane;
-    h->last_first_block = h->block_counter;
+    h->last_first_block = pos.block_counter;
     h->last_nblocks = nblocks;
     h->pending = h->pending_counts = true;
     h->pending_stream = st;
 
-    h->cur_plane ^= 1;
-    h->cur_hist ^= 1;
-    long long hv = (long long)h->hist_valid + nblocks * c.BS;
-    h->hist_valid = (int)std::min<long long>(hv, c.hist_samples);
-    h->block_counter += nblocks;
+    pos.cur_plane ^= 1;
+    pos.cur_hist ^= 1;
+    pos.hist_valid = (int)std::min<long long>((long long)pos.hist_valid + nblocks * c.BS, c.hist_samples);
+    pos.block_counter += nblocks;
     return ERTGPU_OK;
 }
 
@@ -601,6 +636,13 @@ int upload(ertgpu_handle* h, const void* src, int64_t total, size_t s, size_t by
     return ERTGPU_OK;
 }
 
+// Only an input stage launch is pending on st: it is waited for like a pipeline, with no counters to read.
+void stage_pending(ertgpu_handle* h, cudaStream_t st) {
+    h->pending = true;
+    h->pending_counts = false;
+    h->pending_stream = st;
+}
+
 // Enqueue the work for the next n input samples, at d_in on the device, on st: the input stage's step and the pipeline
 // over the whole blocks it completes.
 int run_step(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaStream_t st) {
@@ -611,9 +653,7 @@ int run_step(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaStream_t 
         h->launches = 0;
         rc = h->in.launch(s, st, &h->launches);
         if (rc == ERTGPU_OK && h->launches) {
-            h->pending = true;
-            h->pending_counts = false;
-            h->pending_stream = st;
+            stage_pending(h, st);
             if (h->kernels.empty()) h->kernels = h->in.label(s.shared_first);  // otherwise the last pipeline's list stays
         }
     }
@@ -642,11 +682,7 @@ int enqueue_channels(ertgpu_handle* const* hs, int n, const uint8_t* d_in, int64
         if (const int rc = run_step(hs[k], steps[k], flags, st)) return rc;
     ertgpu_handle* h = hs[0];
     h->launches += shared;
-    if (shared && !h->pending) {  // the shared launch wrote every channel's history: wait for it like a stage launch
-        h->pending = true;
-        h->pending_counts = false;
-        h->pending_stream = st;
-    }
+    if (shared && !h->pending) stage_pending(h, st);  // the shared launch wrote every channel's history
     return ERTGPU_OK;
 }
 
@@ -671,7 +707,7 @@ int check_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
 int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
     if (const int rc = check_decode(h, iq, nbytes, device)) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    h->started = true;
+    h->pos.started = true;
     if (h->pending) {
         int rc = collect(h);
         if (rc) return rc;
@@ -919,7 +955,6 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     }
     for (auto& set : h->ev_pool) for (int k = 0; k < 5; k++) CUDA_TRY(h, cudaEventCreate(&set[k]));
     h->ev_stage = h->ev_pool[0];
-    (void)dynamic_smem_base();  // asked once, before the first launch needs it
     make_maglut(h->h_lut);
     make_gf32(&h->gf);
     CUDA_TRY(h, cudaMalloc(&h->d_lut, 256 * sizeof(float)));
@@ -947,9 +982,6 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
         CUDA_TRY(h, cudaMalloc(&h->d_digits, h->cand_cap * ERTGPU_R900_DIGITS));
         h->r900_span = d.BS + d.PL - d.SL + 4 * ERTGPU_R900_DIGITS * d.CL + 1;
         if (h->r900_span > d.BUF + 1) h->r900_span = d.BUF + 1;
-        // BS is a power of two >= 32 and the call's bytes are 16-byte aligned: chain starts (b + 1) * BS - BUF are
-        // multiples of 8 samples when PKL is (BUF = PKL + BS, the history holds PKL samples)
-        h->r900_vec = d.PKL % 8 == 0;
         // scratch slots: one per block that holds an r900 hit.  Sized for one packet per 16 blocks
         // (at least 64 slots), at most 1 GiB; blocks beyond that use the per-candidate replay.
         {
@@ -969,15 +1001,27 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     h->tap_floats = (size_t)std::max(d.BS + d.SL, d.BUF) * 2 + 16;
     CUDA_TRY(h, cudaMalloc(&h->d_tap, h->tap_floats * sizeof(float)));
 
-    h->demod_variant = demod_fast_variant(d.CL, d.BS, d.PKL);
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->device);
     if (h->sm_count < 1) h->sm_count = 132;
 
+    h->pipe = {};
+    // where the dynamic shared memory of a kernel starts on this device, through the tap scratch
+    smem_base_probe_kernel<<<1, 1, 1024, h->stream>>>(reinterpret_cast<uint32_t*>(h->d_tap));
+    CUDA_TRY(h, cudaGetLastError());
+    CUDA_TRY(h, cudaMemcpyAsync(&h->pipe.smem_base, h->d_tap, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    if (const int rc = choose_demod(h, demod_fast_variant(d.CL, d.BS, d.PKL))) return rc;
+    if (const int rc = choose_search(h)) return rc;
+    constexpr int kFullK = (ERTGPU_MAX_PACKET_BYTES * 8 + 31) / 32;
+    const bool short_packets = d.PK <= 128;
+    h->pipe.extract = short_packets ? extract_words_kernel<4> : extract_words_kernel<kFullK>;
+    h->pipe.extract_label = ";extract_words_kernel<" + std::to_string(short_packets ? 4 : kFullK) + ">";
+    // BS is a power of two >= 32 and the call's bytes are 16-byte aligned: chain starts (b + 1) * BS - BUF are
+    // multiples of 8 samples when PKL is (BUF = PKL + BS, the history holds PKL samples)
+    h->pipe.r900_chain = d.PKL % 8 == 0;
+
     if (const int rc = h->in.allocate(c.block_size, max_blocks_per_call, h->sm_count)) return rc;
-    h->cur_plane = h->cur_hist = 0;
-    h->hist_valid = 0;
-    h->block_counter = 0;
-    h->started = false;
+    h->pos = {};
     return ERTGPU_OK;
 }
 
@@ -994,11 +1038,7 @@ int ertgpu_reset(ertgpu_handle* h) {
     int rc = collect_sync(h);
     if (rc) return rc;
     h->uncopied = false;
-    // the history in front of the next call is zeroed on that call's stream (enqueue_pipeline)
-    h->fresh = true;
-    h->hist_valid = 0;
-    h->block_counter = 0;
-    h->started = false;
+    h->pos = {};  // the history in front of the next call is zeroed on that call's stream (enqueue_pipeline)
     h->in.reset_stream();
     begin_call(h);
     return ERTGPU_OK;
@@ -1048,13 +1088,13 @@ int ertgpu_get_input_format(const ertgpu_handle* h, int32_t* format, float* scal
 int ertgpu_set_input_scale(ertgpu_handle* h, float scale) {
     if (!h) return ERTGPU_EINVAL;
     if (!h->allocated) return fail(h, ERTGPU_EINVAL, "set_input_scale before allocate: ertgpu_set_input_format takes the scale");
-    if (h->started) return fail(h, ERTGPU_EINVAL, "set_input_scale after a decode call: the gain changes only at a stream start");
+    if (h->pos.started) return fail(h, ERTGPU_EINVAL, "set_input_scale after a decode call: the gain changes only at a stream start");
     return h->in.set_scale(scale);
 }
 
 int ertgpu_set_channel_gain(ertgpu_handle* h, int32_t k) {
     if (!h) return ERTGPU_EINVAL;
-    if (h->allocated && h->started)
+    if (h->allocated && h->pos.started)
         return fail(h, ERTGPU_EINVAL, "set_channel_gain after a decode call: the gain changes only at a stream start");
     return h->in.set_channel_gain(k, h->allocated);
 }
@@ -1142,11 +1182,9 @@ int ertgpu_get_resampler(const ertgpu_handle* h, ertgpu_resampler_info* info, in
 
 int ertgpu_set_demod_variant(ertgpu_handle* h, int32_t variant) {
     // test hook: 0 forces the generic kernel, -1 restores the automatic choice
-    if (!h || !h->allocated) return ERTGPU_EINVAL;
-    if (variant < 0) h->demod_variant = demod_fast_variant(h->dcfg.CL, h->dcfg.BS, h->dcfg.PKL);
-    else if (variant == 0) h->demod_variant = 0;
-    else return ERTGPU_EINVAL;
-    return ERTGPU_OK;
+    if (!h || !h->allocated || variant > 0) return ERTGPU_EINVAL;
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    return choose_demod(h, variant < 0 ? demod_fast_variant(h->dcfg.CL, h->dcfg.BS, h->dcfg.PKL) : 0);
 }
 
 int ertgpu_decode_device_async(ertgpu_handle* h, const void* d_iq, size_t nbytes, uint32_t flags, void* stream) {
@@ -1448,8 +1486,10 @@ int ertgpu_synth_fill(int32_t device, void* d_out, int64_t first_sample, int64_t
         cudaFree(d_pk);
         return ERTGPU_ECUDA;
     }
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     long long groups = (nsamples + 7) / 8;
-    long long blocks = std::min<long long>((groups + 255) / 256, (long long)sm_count_of(current_device()) * 32);
+    long long blocks = std::min<long long>((groups + 255) / 256, (long long)sms * 32);
     if (blocks < 1) blocks = 1;
     synth_kernel<<<(unsigned)blocks, 256, 0, st>>>(static_cast<uint8_t*>(d_out), first_sample, nsamples, seed, d_pk, n);
     cudaError_t e = cudaGetLastError();

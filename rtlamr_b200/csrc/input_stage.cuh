@@ -50,6 +50,14 @@ inline int fail(std::string& err, int code, const char* fmt, ...) {
         }                                                                                       \
     } while (0)
 
+// A kernel whose launches request `bytes` of dynamic shared memory may take the whole 227 KiB of a CTA: set on each kernel
+// a handle may launch, when the handle is allocated.  `what` names the kernel when it needs more.
+inline int allow_dynamic_smem(std::string& err, const void* kernel, size_t bytes, const char* what) {
+    if (bytes > 227 * 1024) return fail(err, ERTGPU_EINVAL, "%s needs %zu B of shared memory", what, bytes);
+    CUDA_TRY(err, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    return ERTGPU_OK;
+}
+
 // One step of the stage: input samples at rs.cur on the device, and the whole uint8 blocks they complete.
 struct InputStep {
     const uint8_t* iq = nullptr;  // the blocks the pipeline reads: rs.cur itself in pass-through mode
@@ -530,11 +538,10 @@ private:
         return (unsigned)std::max<long long>(1, std::min<long long>((n + per - 1) / per, cap));
     }
 
-    // A kernel of `threads` threads with `bytes` of dynamic shared memory: it may take the whole 227 KiB of a CTA, and
-    // *cap becomes the most CTAs of it the device runs at once.  `what` names it when it needs more.
+    // A kernel of `threads` threads with `bytes` of dynamic shared memory (allow_dynamic_smem): *cap becomes the most CTAs
+    // of it the device runs at once.
     int fit(const void* kernel, int threads, size_t bytes, const char* what, int sm_count, int* cap) {
-        if (bytes > 227 * 1024) return fail(err_, ERTGPU_EINVAL, "%s needs %zu B of shared memory", what, bytes);
-        CUDA_TRY(err_, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        if (const int rc = allow_dynamic_smem(err_, kernel, bytes, what)) return rc;
         int per_sm = 0;
         CUDA_TRY(err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, bytes));
         *cap = std::max(1, per_sm) * sm_count;

@@ -11,7 +11,7 @@ their less travelled code paths run:
   * call seams: host-path splits and max_blocks_per_call chunking, packets placed across block, tile and call seams;
   * adversarial Search inputs: near-miss preambles, constant and uniform bytes, a custom preamble, an all-ones one.
 
-The last test checks that every instance the launch switches can pick was seen."""
+The last test checks that every instance allocate can choose was seen."""
 import json
 import os
 import re
@@ -689,21 +689,21 @@ def test_constant_and_uniform_bytes(built, cl, src):
     h.close()
 
 
-# ---------------------------------------------------------------- coverage of the launch switches
+# ---------------------------------------------------------------- coverage of the instance choices
 def expected_instances():
     src = open(os.path.join(ROOT, "rtlamr_b200", "csrc", "demod_fast.cuh")).read()
-    cls = sorted({int(x) for x in re.findall(r"ERT_FAST_CASE\((\d+)\)", src)})
+    cls = sorted({int(x) for x in re.findall(r"fast_demod_of<(\d+)>\(", src)})
     demod = {f"demod_fast_kernel<{cl},{w}>" for cl in cls for w in ((8, 7) if fast_warps(cl) == 8 else (fast_warps(cl),))}
     src = open(os.path.join(ROOT, "rtlamr_b200", "csrc", "ertgpu.cu")).read()
     slide = set()
-    for n, pats in re.findall(r"launch_slide<(\d+)((?:,\s*0x[0-9A-Fa-f]+u)*)>\(", src):
+    for n, pats in re.findall(r"slide_instance<(\d+)((?:,\s*0x[0-9A-Fa-f]+u)*)>\(", src):
         pats = ", ".join("0x%04Xu" % int(p[2:-1], 16) for p in re.findall(r"0x[0-9A-Fa-f]+u", pats))
         for half in ("true", "false"):
             slide.add(f"search_slide_kernel<{n},{half}" + ("," + pats if pats else "") + ">")
     return cls, demod, slide
 
 
-def test_launch_switches_have_the_expected_shape():
+def test_instance_choices_have_the_expected_shape():
     cls, demod, slide = expected_instances()
     assert cls == FAST_CLS and len(demod) == 17 and len(slide) == 20
 
