@@ -102,6 +102,17 @@ typedef struct {
 
 #define ERTGPU_CAND_HAS_R900 1u /* r900_digits[] is filled */
 
+/* How one candidate was received (ertgpu_fetch_signal): exact integer sums over its own samples, as
+ * include/ertgpu_signal.h defines them; ertsig_summary there turns them into Level, Noise, SNR and Freq. */
+typedef struct {
+    int64_t n_on, e_on;   /* high-chip inner samples, and the sum of their sI^2 + sQ^2 (s = 2u - 255) */
+    int64_t n_off, e_off; /* the same over low-chip inner samples                                     */
+    int64_t r_re, r_im;   /* sum of s[n] conj(s[n-1]) over adjacent pairs inside one high-chip span    */
+    int64_t n_pairs;      /* pairs in r                                                                */
+    int32_t protocol;     /* registered protocol whose span was measured                              */
+    int32_t symbols;      /* symbols measured (1 .. span-1 of that protocol)                           */
+} ertgpu_signal;
+
 /* decode flags */
 #define ERTGPU_DECODE_ONLY_VALID 1u /* return only candidates with check_mask != 0 */
 
@@ -397,6 +408,17 @@ int ertgpu_decode_channels_device_async(ertgpu_handle *const *handles, int32_t n
 /* Wait for the decode enqueued last and copy its candidates out (sorted as
  * above).  May be repeated (e.g. after ERTGPU_ECAPACITY). */
 int ertgpu_fetch(ertgpu_handle *h, ertgpu_candidate *out, size_t cap, size_t *n_out);
+
+/* Per-packet signal reports.  ertgpu_enable_signal, called before ertgpu_allocate (after it: ERTGPU_EINVAL), makes
+ * every decode of the handle also measure each candidate it returns on its own samples, on the GPU behind the slice
+ * stage (packet_signal_kernel, counted in ertgpu_last_launches and named last in ertgpu_last_kernels).  The candidates
+ * themselves are exactly those of a handle without reports.  ertgpu_fetch_signal returns one ertgpu_signal per
+ * candidate the last ertgpu_decode or ertgpu_fetch returned, in the same order, with ertgpu_fetch's capacity rules
+ * (ERTGPU_ECAPACITY with *n_out = the number needed); it works after ertgpu_decode, ertgpu_decode_device_async +
+ * ertgpu_fetch and, per handle, ertgpu_decode_channels[_device_async].  ERTGPU_EINVAL on a handle without reports.
+ * ertgpu_decode_sharded rejects handles with reports. */
+int ertgpu_enable_signal(ertgpu_handle *h);
+int ertgpu_fetch_signal(ertgpu_handle *h, ertgpu_signal *out, size_t cap, size_t *n_out);
 
 /* Number of candidates of the last decode, and how many passed a screen. */
 int ertgpu_last_counts(ertgpu_handle *h, int64_t *n_candidates, int64_t *n_valid);

@@ -91,6 +91,15 @@ class SynthPacket(C.Structure):
                 ("pad", C.c_int32)]
 
 
+class Signal(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("n_on", "e_on", "n_off", "e_off", "r_re", "r_im", "n_pairs")] + \
+        [("protocol", C.c_int32), ("symbols", C.c_int32)]
+
+
+SIGNAL_DTYPE = np.dtype([(n, "<i8") for n in ("n_on", "e_on", "n_off", "e_off", "r_re", "r_im", "n_pairs")] +
+                        [("protocol", "<i4"), ("symbols", "<i4")])
+assert SIGNAL_DTYPE.itemsize == C.sizeof(Signal) == 64
+
 CAND_DTYPE = np.dtype([("block", "<i8"), ("idx", "<i4"), ("preamble_id", "<i4"),
                        ("check_mask", "<u4"), ("flags", "<u4"),
                        ("bytes", "u1", (MAX_PACKET_BYTES,)), ("r900_digits", "u1", (R900_DIGITS,)),
@@ -111,6 +120,7 @@ EXPORTS = [
     "ertgpu_allow_input_decimation", "ertgpu_get_decimator",
     "ertgpu_decode_channels", "ertgpu_decode_channels_device_async",
     "ertgpu_set_channel_gain", "ertgpu_get_channel_gain", "ertgpu_measure_channel",
+    "ertgpu_enable_signal", "ertgpu_fetch_signal",
 ]
 
 _lib = None
@@ -178,6 +188,8 @@ def lib() -> C.CDLL:
     L.ertgpu_set_channel_gain.argtypes = [vp, i32]
     L.ertgpu_get_channel_gain.argtypes = [vp, C.POINTER(i32)]
     L.ertgpu_measure_channel.argtypes = [vp, vp, sz, C.POINTER(ChannelLevel)]
+    L.ertgpu_enable_signal.argtypes = [vp]
+    L.ertgpu_fetch_signal.argtypes = [vp, vp, sz, C.POINTER(sz)]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the library does not export it
     _lib = L
@@ -298,6 +310,22 @@ class Handle:
         self._check(self._L.ertgpu_measure_channel(self._h, addr, nbytes, C.byref(lv)))
         return {"components": lv.components, "zeros": lv.zeros, "bins": np.array(lv.bins[:], dtype=np.int64), "k": lv.k}
 
+    def enable_signal(self):
+        """ertgpu_enable_signal: measure every candidate's signal (before allocate)."""
+        self._check(self._L.ertgpu_enable_signal(self._h))
+
+    def fetch_signal(self, cap: int = 4096) -> np.ndarray:
+        """ertgpu_fetch_signal: one SIGNAL_DTYPE record per candidate the last decode or fetch returned, same order."""
+        while True:
+            out = np.empty(cap, dtype=SIGNAL_DTYPE)
+            n = C.c_size_t(0)
+            rc = self._L.ertgpu_fetch_signal(self._h, out.ctypes.data, cap, C.byref(n))
+            if rc == ECAPACITY and n.value > cap and "internal" not in (self._L.ertgpu_last_error(self._h) or b"").decode():
+                cap = n.value
+                continue
+            self._check(rc)
+            return out[:n.value].copy()
+
     def resampler(self):
         """ertgpu_get_resampler: (info dict, int16 table of (P+1)*T entries)."""
         info, n = ResamplerInfo(), C.c_size_t(0)
@@ -397,14 +425,14 @@ class Handle:
 def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per_call: int = 0,
                 max_candidates: int = 0, input_rate: int = 0, input_format: int = FORMAT_CU8,
                 input_scale: float = 0.0, capture_freq: int = 0, center_freq: int = 0,
-                channel_gain: int | None = None) -> Handle:
+                channel_gain: int | None = None, signal: bool = False) -> Handle:
     """NewDecoder + RegisterProtocol(NewParser(name, chip_length)) for each name + Allocate
     (reference main.go:64-86).  input_rate > 0: the IQ is sampled at that rate (ertgpu_set_input_rate);
     input_format / input_scale: its sample format and gain (ertgpu_set_input_format, not called for plain cu8);
     capture_freq > 0: the IQ was recorded centred there, and the channel at center_freq (0: the protocols'
     CenterFreq) is decoded (ertgpu_set_input_tuning, before the rate), at up to 256 times the decoder's rate
     (ertgpu_allow_input_decimation).  channel_gain k: the wide channel path with gain 2^k (ertgpu_set_channel_gain;
-    tuned handles only)."""
+    tuned handles only).  signal: per-packet signal reports (ertgpu_enable_signal)."""
     if isinstance(msgtypes, str):
         msgtypes = [m.strip() for m in msgtypes.split(",") if m.strip()]
     h = Handle()
@@ -419,6 +447,8 @@ def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per
         h.set_input_format(input_format, input_scale)
     if channel_gain is not None:
         h.set_channel_gain(channel_gain)
+    if signal:
+        h.enable_signal()
     h.allocate(device, max_blocks_per_call, max_candidates)
     return h
 

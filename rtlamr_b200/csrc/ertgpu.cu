@@ -13,6 +13,7 @@
 //             replaces Decoder.Quantized (1 byte per bit) and Decoder.packed
 //   hits    : (start, preamble) pairs found by the Search kernel (search_slide_kernel or search_generic_kernel)
 //   out     : ertgpu_candidate records produced by extract_kernel
+//   sig     : ertgpu_signal records of the same slots (packet_signal_kernel; handles with signal reports only)
 #include <ctype.h>
 #include <sched.h>
 
@@ -35,6 +36,7 @@
 #include "ert_common.cuh"
 #include "input_stage.cuh"
 #include "search.cuh"
+#include "signal.cuh"
 #include "synth.cuh"
 
 using namespace ert;
@@ -102,6 +104,9 @@ struct ertgpu_handle {
     int r900_slots = 0, r900_span = 0;
     ertgpu_candidate* d_out = nullptr;
     unsigned long long cand_cap = 0;
+    bool signal = false;              // ertgpu_enable_signal: a record per candidate in d_sig
+    ertgpu_signal* d_sig = nullptr;
+    ertsig_geometry sig_geo{};
     unsigned long long* d_counters = nullptr;  // kCntHits, kCntOut, kCntValid, kCntTile (demod work tiles), kCntWords
     unsigned long long* h_counters = nullptr;  // pinned mirror
     float* d_tap = nullptr;                    // scratch for taps
@@ -140,6 +145,7 @@ struct ertgpu_handle {
     double stage_sum[4] = {0, 0, 0, 0};  // accumulated since ertgpu_set_stage_timing(1)
     int64_t stage_n = 0;
     std::vector<ertgpu_candidate> results;
+    std::vector<ertgpu_signal> sig_results;  // results' records, in the same order
 
     InputStage in{err};  // input format, rate and tuning, and the kernel in front of the pipeline
 };
@@ -247,6 +253,7 @@ void free_device(ertgpu_handle* h) {
     dfree(h->d_slot_count);
     dfree(h->d_r900_scratch);
     dfree(h->d_out);
+    dfree(h->d_sig);
     dfree(h->d_counters);
     dfree(h->d_tap);
     h->in.release();
@@ -484,6 +491,16 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
         h->kernels += k.extract_label;
     }
     if (h->in.mode != InputStage::kPass) h->kernels += ";" + h->in.label(s.shared_first);
+    // 5. signal reports of the emitted candidates; they read d_iq, so they are enqueued before the caller records the
+    //    event that frees its staging buffer; five CTAs per SM fill it at 48 registers, to hide the loads' latency
+    if (h->signal) {
+        packet_signal_kernel<<<(unsigned)h->sm_count * 5, kSignalWarps * 32, 0, st>>>(
+            d_iq, hist, c.hist_samples, pos.hist_valid, h->sig_geo, (long long)pos.block_counter, h->d_out, h->cand_cap,
+            h->d_counters, h->d_sig);
+        CUDA_TRY(h, cudaGetLastError());
+        h->launches++;
+        h->kernels += ";packet_signal_kernel";
+    }
 
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[3], st));
     if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[4], st));
@@ -543,7 +560,22 @@ int collect(ertgpu_handle* h) {
         // Slots are handed out by atomics, so a pipeline's records arrive unordered.  Pipelines of one
         // call cover ascending, disjoint block ranges: sorting each segment as it arrives (while the next
         // chunk's H2D copy is in flight) leaves the whole list in (block, preamble, idx) order.
-        std::sort(h->results.begin() + (std::ptrdiff_t)old, h->results.end(), cand_less);
+        if (!h->signal) {
+            std::sort(h->results.begin() + (std::ptrdiff_t)old, h->results.end(), cand_less);
+            return ERTGPU_OK;
+        }
+        // with reports, the signal records take the candidates' order (the key is unique per candidate)
+        std::vector<ertgpu_signal> sig(h->uncopied_n);
+        CUDA_TRY(h, cudaMemcpy(sig.data(), h->d_sig, sig.size() * sizeof(ertgpu_signal), cudaMemcpyDeviceToHost));
+        std::vector<uint32_t> order(sig.size());
+        for (size_t i = 0; i < order.size(); i++) order[i] = (uint32_t)i;
+        const ertgpu_candidate* seg = h->results.data() + old;
+        std::sort(order.begin(), order.end(), [seg](uint32_t a, uint32_t b) { return cand_less(seg[a], seg[b]); });
+        const std::vector<ertgpu_candidate> cands(seg, seg + order.size());
+        for (size_t i = 0; i < order.size(); i++) {
+            h->results[old + i] = cands[order[i]];
+            h->sig_results.push_back(sig[order[i]]);
+        }
     }
     return ERTGPU_OK;
 }
@@ -688,6 +720,7 @@ int enqueue_channels(ertgpu_handle* const* hs, int n, const uint8_t* d_in, int64
 
 void begin_call(ertgpu_handle* h) {
     h->results.clear();
+    h->sig_results.clear();
     h->uncopied = false;
     h->overflow = false;
     h->need = 0;
@@ -764,6 +797,13 @@ int check_channels(ertgpu_handle* const* hs, int32_t n, const void* iq, size_t n
 }
 
 }  // namespace
+
+// ertgpu_decode_sharded's rule for signal reports, with its message on h.  Shared with sharded.cpp inside the library
+// only: hidden, so libertgpu.so exports nothing beyond include/ertgpu.h.
+__attribute__((visibility("hidden"))) int sharded_reject_signal(ertgpu_handle* h) {
+    return h->signal ? fail(h, ERTGPU_EINVAL, "decode_sharded: the handle has signal reports (ertgpu_enable_signal), which sharded decodes do not keep")
+                     : ERTGPU_OK;
+}
 
 extern "C" {
 
@@ -978,6 +1018,18 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     CUDA_TRY(h, cudaMalloc(&h->d_hits, h->cand_cap * sizeof(RawHit)));
     CUDA_TRY(h, cudaMalloc(&h->d_words, h->cand_cap * sizeof(HitWord)));
     CUDA_TRY(h, cudaMalloc(&h->d_out, h->cand_cap * sizeof(ertgpu_candidate)));
+    if (h->signal) {
+        CUDA_TRY(h, cudaMalloc(&h->d_sig, h->cand_cap * sizeof(ertgpu_signal)));
+        ertsig_geometry& g = h->sig_geo;
+        g = {};
+        g.CL = d.CL; g.SL = d.SL; g.BS = d.BS; g.BUF = d.BUF; g.PK = d.PK;
+        g.nproto = d.nproto;
+        for (int i = 0; i < d.nproto; i++) {
+            const ertgpu_protocol& p = h->protos[i];
+            g.preamble_id[i] = d.proto[i].preamble_id;
+            g.span[i] = p.check_kind == ERTGPU_CHECK_R900 ? p.preamble_symbols : p.packet_symbols;
+        }
+    }
     if (h->has_r900) {
         CUDA_TRY(h, cudaMalloc(&h->d_digits, h->cand_cap * ERTGPU_R900_DIGITS));
         h->r900_span = d.BS + d.PL - d.SL + 4 * ERTGPU_R900_DIGITS * d.CL + 1;
@@ -1276,6 +1328,29 @@ int ertgpu_decode_channels(ertgpu_handle* const* hs, int32_t n, const uint8_t* i
     }
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));
+    return ERTGPU_OK;
+}
+
+int ertgpu_enable_signal(ertgpu_handle* h) {
+    if (!h) return ERTGPU_EINVAL;
+    if (h->allocated) return fail(h, ERTGPU_EINVAL, "enable_signal after allocate");
+    h->signal = true;
+    return ERTGPU_OK;
+}
+
+int ertgpu_fetch_signal(ertgpu_handle* h, ertgpu_signal* out, size_t cap, size_t* n_out) {
+    if (!h || !h->allocated) return ERTGPU_EINVAL;
+    if (!h->signal) return fail(h, ERTGPU_EINVAL, "fetch_signal: the handle was allocated without signal reports (ertgpu_enable_signal)");
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    if (const int rc = collect(h)) return rc;
+    if (h->overflow) {
+        if (n_out) *n_out = (size_t)h->need;
+        return fail(h, ERTGPU_ECAPACITY, "internal candidate capacity %llu exceeded (%llu hits): allocate with a larger max_candidates",
+                    h->cand_cap, h->need);
+    }
+    if (n_out) *n_out = h->sig_results.size();
+    if (h->sig_results.size() > cap) return fail(h, ERTGPU_ECAPACITY, "output array holds %zu records, %zu needed", cap, h->sig_results.size());
+    if (!h->sig_results.empty() && out) memcpy(out, h->sig_results.data(), h->sig_results.size() * sizeof(ertgpu_signal));
     return ERTGPU_OK;
 }
 

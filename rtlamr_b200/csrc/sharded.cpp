@@ -14,6 +14,10 @@
 
 #include "../../include/ertgpu.h"
 
+// ertgpu.cu: ERTGPU_EINVAL, with the message on h, when h has signal reports (sharded decodes do not keep them).  Hidden:
+// not exported from libertgpu.so.
+__attribute__((visibility("hidden"))) int sharded_reject_signal(ertgpu_handle* h);
+
 extern "C" {
 
 int ertgpu_plan_shards(int64_t total_blocks, int32_t nshards, int32_t block_size, int32_t packet_length,
@@ -45,6 +49,7 @@ int ertgpu_decode_sharded(ertgpu_handle* const* handles, int32_t nhandles, const
         if (ertgpu_get_tuning(handles[r], nullptr) == ERTGPU_OK) return ERTGPU_EINVAL;  // tuned, even at the native rate
         int32_t fmt = ERTGPU_FORMAT_CU8;
         if (ertgpu_get_input_format(handles[r], &fmt, nullptr) != ERTGPU_OK || fmt != ERTGPU_FORMAT_CU8) return ERTGPU_EINVAL;
+        if (const int rc = sharded_reject_signal(handles[r])) return rc;
     }
     ertgpu_decoder_config c0;
     int rc = ertgpu_get_config(handles[0], &c0);

@@ -15,7 +15,9 @@ LIB_PATH = os.path.join(_HERE, "libertgpu_host.so")
 class _Msg(C.Structure):
     _fields_ = [("block", C.c_int64), ("idx", C.c_int32), ("meter_id", C.c_uint32), ("meter_type", C.c_uint32),
                 ("nchecksum", C.c_int32), ("checksum", C.c_uint8 * 8), ("msgtype", C.c_char * 12),
-                ("text", C.c_char * 1400), ("record", C.c_char * 1400)]
+                ("text", C.c_char * 1400), ("record", C.c_char * 1400), ("signal", C.c_int32), ("reserved", C.c_int32),
+                ("channel", C.c_int64), ("freq", C.c_int64), ("level", C.c_double), ("noise", C.c_double),
+                ("snr", C.c_double)]
 
 
 @dataclass(frozen=True)
@@ -28,6 +30,9 @@ class HostMessage:
     checksum: bytes
     text: str
     record: tuple
+    # Receiver(signal=True): {"channel", "freq", "level", "noise", "snr"} (freq and the dB values None for a packet that
+    # starts before the stream); None without reports
+    signal: dict | None = None
 
 
 _lib = None
@@ -41,7 +46,7 @@ def lib():
         L = C.CDLL(LIB_PATH)
         L.erthost_new.restype = C.c_void_p
         L.erthost_new.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_int, C.c_float,
-                                  C.c_longlong, C.c_longlong, C.c_int, C.c_int, C.c_char_p, C.c_int]
+                                  C.c_longlong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_int]
         L.erthost_channel_gain.argtypes = [C.c_void_p]
         L.erthost_level.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_longlong),
                                     C.POINTER(C.c_longlong)]
@@ -75,13 +80,24 @@ def lib():
         L.erthost_encode.restype = C.c_longlong
         L.erthost_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_longlong, C.c_int, C.c_longlong, C.c_int,
                                      C.c_int, C.c_char_p, C.c_longlong]
+        L.erthost_encode_signal.restype = C.c_longlong
+        L.erthost_encode_signal.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_longlong, C.c_longlong,
+                                            C.c_int, C.c_longlong, C.c_int, C.c_char_p, C.c_longlong]
         _lib = L
     return _lib
 
 
+def _signal(m):
+    if not m.signal:
+        return None
+    full = m.signal == 2
+    return {"channel": m.channel, "freq": m.freq if full else None, "level": m.level if full else None,
+            "noise": m.noise if full else None, "snr": m.snr if full else None}
+
+
 def _messages(out, n):
     return [HostMessage(m.block, m.idx, m.msgtype.decode(), m.meter_id, m.meter_type, bytes(m.checksum[:m.nchecksum]),
-                        m.text.decode(), tuple(m.record.decode().split(","))) for m in out[:n]]
+                        m.text.decode(), tuple(m.record.decode().split(",")), _signal(m)) for m in out[:n]]
 
 
 class Parsers:
@@ -177,8 +193,24 @@ def _encode(self, cands, fmt: str = "plain", unix_seconds: int = 0, nanos: int =
     return buf.value.decode()
 
 
+def _encode_signal(self, cands, sigs, channel_hz: int, rate_out: int, fmt: str = "plain", unix_seconds: int = 0,
+                   nanos: int = 0) -> str:
+    """erthost_encode_signal: every parsed message with the signal report of its candidate (sigs: capi.SIGNAL_DTYPE, one
+    per candidate) through the encoders; "plain" is ertgpu_decode_file's plain line."""
+    cands, sigs = np.ascontiguousarray(cands), np.ascontiguousarray(sigs)
+    assert len(sigs) == len(cands)
+    cap = 1 << 22
+    buf = C.create_string_buffer(cap)
+    n = self._L.erthost_encode_signal(self._h, cands.ctypes.data, sigs.ctypes.data, len(cands), channel_hz, rate_out,
+                                      FORMATS[fmt], unix_seconds, nanos, buf, cap)
+    if n < 0 or n >= cap:
+        raise RuntimeError(self._L.erthost_error(self._h).decode() if n < 0 else "encode buffer too small")
+    return buf.value.decode()
+
+
 Parsers.parse_filtered = _parse_filtered
 Parsers.encode = _encode
+Parsers.encode_signal = _encode_signal
 
 
 def wav_probe(path) -> dict:
@@ -229,7 +261,7 @@ class Receiver:
 
     def __init__(self, msgtypes: str, chip_length: int = 72, device: int = 0, max_blocks: int = 0, max_cands: int = 0,
                  input_rate: int = 0, input_format: int = 0, input_scale: float | str = 0.0, capture_freq: int = 0,
-                 center_freq: int = 0, channel_gain: int | str | None = None):
+                 center_freq: int = 0, channel_gain: int | str | None = None, signal: bool = False):
         """The input arguments are protocol::Decoder::SetInput's.  input_rate > 0: the IQ given to decode() is sampled at
         that rate; any rate other than DataRate * ChipLength is resampled on the GPU and decode() then takes any whole
         number of IQ samples.  input_format / input_scale: the IQ's sample format (capi.FORMAT_*) and gain.
@@ -238,7 +270,8 @@ class Receiver:
         min(len, 2^22) samples of its first decode() call (ertgpu_measure_input) and stays fixed for the stream;
         input_level() tells which.  channel_gain=k: the wide channel path of a tuned input with gain 2^k
         (ertgpu_set_channel_gain); "auto": k of each stream is measured from the same samples after the input gain
-        (ertgpu_measure_channel), and channel_gain() tells which."""
+        (ertgpu_measure_channel), and channel_gain() tells which.  signal: every message carries its signal report
+        (HostMessage.signal; protocol::Decoder::EnableSignal)."""
         self._L = lib()
         err = C.create_string_buffer(512)
         auto = isinstance(input_scale, str)
@@ -248,7 +281,8 @@ class Receiver:
             raise ValueError(f"channel_gain {channel_gain!r}: k or 'auto'")
         cg = -1 if channel_gain is None else -2 if channel_gain == "auto" else int(channel_gain)
         self._h = self._L.erthost_new(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate, input_format,
-                                      0.0 if auto else input_scale, capture_freq, center_freq, 1 if auto else 0, cg, err, 512)
+                                      0.0 if auto else input_scale, capture_freq, center_freq, 1 if auto else 0, cg,
+                                      1 if signal else 0, err, 512)
         if not self._h:
             raise RuntimeError(err.value.decode())
         v = (C.c_int32 * 12)()

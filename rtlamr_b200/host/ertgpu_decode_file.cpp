@@ -4,7 +4,7 @@
 // (protocol/parse.go:119-121 StringNoOffset).
 //   ertgpu_decode_file [-msgtype=scm,idm|all] [-symbollength=72] [-blockdedup=true] [-blocks=4096] [-device=0]
 //                      [-filterid=1,2] [-filtertype=4,5] [-unique=true] [-format=plain|csv|json|xml]
-//                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ]
+//                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ] [-signal]
 //                      [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|cf64_be|wav|sigmf] [-samplescale=G|auto] [-capturefreq=HZ [-centerfreq=HZ[,HZ...]]]
 //                      FILE|- [FILE ...]
 // -capturefreq names the frequency the capture was recorded centred at; -centerfreq (rtlamr's flag) the channel to
@@ -53,6 +53,14 @@
 // channel, or for the same block in an earlier channel, so a packet where two channels overlap is printed once
 // (-blockdedup=false prints it from each).  The decoder log's CenterFreq lists every channel and the summary counts each
 // channel's messages.  -samplescale=auto measures the stream once and sets that gain on every channel.
+// -signal reports how each message was received, measured on the GPU from its packet's own samples (DESIGN.md §3.13,
+// include/ertgpu_signal.h): the channel that decoded it (the tuned channel, or the protocols' CenterFreq), the carrier's
+// frequency in Hz, and its level, the noise floor between its chips and their ratio in dB of the decoder's bytes (two
+// decimals).  plain: {Block:B Idx:I Channel:C Freq:F Level:L Noise:N SNR:S TYPE:{...}}; csv: the five fields after the
+// message's own record; json: "Signal":{"Channel":..,"Freq":..,"Level":..,"Noise":..,"SNR":..} after "Message"; xml: a
+// <Signal Channel=".." Freq=".." Level=".." Noise=".." SNR=".."> element after <Message>.  A packet that starts before
+// the stream has no report: "-" for each field (plain), five empty fields (csv), null (json), no attributes (xml).
+// Without -signal every format is exactly as above.
 // Several files are a batch of independent streams through ONE decoder (buffers, tables and kernels set up once):
 // each starts from zeroed history with block numbers from 0, exactly as if it were decoded alone.  They share the
 // sample file, whose offsets keep growing from one file to the next.
@@ -77,7 +85,7 @@ int main(int argc, char** argv) {
     std::vector<std::string> files;
     int chip = 72, device = 0;
     long long blocks = 4096, samplerate = 0;
-    bool block_dedup = true, quiet = false, unique = false, single = false;
+    bool block_dedup = true, quiet = false, unique = false, single = false, signal = false;
     std::string filterid, filtertype, format = "plain", samplefile, duration, sampleformat = "cu8", samplescale;
     std::string capturefreq, centerfreq, channelgain;
     bool have_scale = false, auto_scale = false;
@@ -104,6 +112,8 @@ int main(int argc, char** argv) {
         else if (a.rfind("-format=", 0) == 0) format = a.substr(8);
         else if (a.rfind("-samplefile=", 0) == 0) samplefile = a.substr(12);
         else if (a.rfind("-single=", 0) == 0) single = a.substr(8) == "true";
+        else if (a == "-signal" || a == "-signal=true") signal = true;
+        else if (a == "-signal=false") signal = false;
         else if (a == "-single") single = true;
         else if (a.rfind("-duration=", 0) == 0) duration = a.substr(10);
         else if (a == "-quiet") quiet = true;
@@ -113,7 +123,7 @@ int main(int argc, char** argv) {
         fprintf(stderr, "usage: %s [-msgtype=scm,scm+,idm,netidm,r900,r900bcd|all] [-symbollength=N] [-blockdedup=true|false] "
                         "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
                         "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|wav|sigmf] "
-                        "[-samplescale=G|auto] [-channelgain=G|auto] "
+                        "[-samplescale=G|auto] [-channelgain=G|auto] [-signal] "
                         "[-capturefreq=HZ [-centerfreq=HZ[,HZ...]]] [-quiet] FILE|- [FILE ...]\n", argv[0]);
         return 2;
     }
@@ -302,7 +312,7 @@ int main(int argc, char** argv) {
         }
     }
     try {
-        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale, channel_k, auto_channel},
+        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale, channel_k, auto_channel, signal},
                                 channels);
         std::string log = rcvr.decoder().Log();
         if (!channels.empty()) {   // the channels share everything of the log but CenterFreq, its first line: name them all
@@ -368,7 +378,7 @@ int main(int argc, char** argv) {
                     lm.Message = &m;
                     fputs((csv ? receiver::CsvLine(lm.Record()) : json ? receiver::JsonLine(lm) : receiver::XmlLine(lm)).c_str(), stdout);
                 } else {
-                    printf("{Block:%lld Idx:%d %s:%s}\n", (long long)m.Block, m.Idx, m.MsgType().c_str(), m.String().c_str());
+                    printf("%s\n", receiver::BlockLine(m).c_str());
                 }
             }, wav_in ? wav_hdr[fi].data_size : -1);
             if (in != stdin) fclose(in);

@@ -117,12 +117,41 @@ struct LogMessage {
     std::string StringNoOffset() const {   // parse.go:119-121
         return "{Time:" + time_layout(false) + " " + Message->MsgType() + ":" + Message->String() + "}";
     }
-    std::vector<std::string> Record() const {   // parse.go:123-129
+    std::vector<std::string> Record() const {   // parse.go:123-129, then the signal report's five fields (-signal)
         std::vector<std::string> r = {time_layout(true), std::to_string(Offset), std::to_string(Length)};
         for (auto& f : Message->Record()) r.push_back(f);
+        if (Message->Signal) {
+            const protocol::SignalReport& s = *Message->Signal;
+            if (s.Valid)
+                for (auto& f : {std::to_string(s.Channel), std::to_string(s.Freq), Decibels(s.Level), Decibels(s.Noise), Decibels(s.SNR)})
+                    r.push_back(f);
+            else
+                r.insert(r.end(), 5, "");
+        }
         return r;
     }
+    // A level in dB with two decimals, as the signal report prints it.
+    static std::string Decibels(double v) {
+        char b[32];
+        snprintf(b, sizeof(b), "%.2f", v);
+        return b;
+    }
 };
+
+// ertgpu_decode_file's plain line: {Block:B Idx:I TYPE:{...}}, with -signal {Block:B Idx:I Channel:C Freq:F Level:L
+// Noise:N SNR:S TYPE:{...}} ("-" for each of the five when the packet has no summary).
+inline std::string BlockLine(const protocol::Message& m) {
+    std::string s = "{Block:" + std::to_string(m.Block) + " Idx:" + std::to_string(m.Idx) + " ";
+    if (m.Signal) {
+        const protocol::SignalReport& r = *m.Signal;
+        if (r.Valid)
+            s += "Channel:" + std::to_string(r.Channel) + " Freq:" + std::to_string(r.Freq) + " Level:" + LogMessage::Decibels(r.Level) +
+                 " Noise:" + LogMessage::Decibels(r.Noise) + " SNR:" + LogMessage::Decibels(r.SNR) + " ";
+        else
+            s += "Channel:- Freq:- Level:- Noise:- SNR:- ";
+    }
+    return s + m.MsgType() + ":" + m.String() + "}";
+}
 
 // flags.go:261-272: StringNoOffset when the sample file is os.DevNull (the default), String otherwise
 inline std::string PlainLine(const LogMessage& m, bool sample_file_is_devnull) {
@@ -197,7 +226,16 @@ inline std::string JsonLine(const LogMessage& m) {
             s += ']';
         }
     }
-    return s + "}}\n";
+    s += '}';
+    if (m.Message->Signal) {   // -signal: the report after the message, null without a summary
+        const protocol::SignalReport& r = *m.Message->Signal;
+        s += ",\"Signal\":";
+        s += r.Valid ? "{\"Channel\":" + std::to_string(r.Channel) + ",\"Freq\":" + std::to_string(r.Freq) + ",\"Level\":" +
+                           LogMessage::Decibels(r.Level) + ",\"Noise\":" + LogMessage::Decibels(r.Noise) + ",\"SNR\":" +
+                           LogMessage::Decibels(r.SNR) + "}"
+                     : "null";
+    }
+    return s + "}\n";
 }
 
 // xml.EscapeText / printer.EscapeString: the five markup characters, tab, LF and CR become character references; a byte
@@ -268,7 +306,17 @@ inline std::string XmlLine(const LogMessage& m) {
         else
             for (uint16_t v : f.Uint16s) s += open + std::to_string(v) + close;
     }
-    return s + "</Message></LogMessage>\n";
+    s += "</Message>";
+    if (m.Message->Signal) {   // -signal: a child element after the message, without attributes when there is no summary
+        const protocol::SignalReport& r = *m.Message->Signal;
+        s += "<Signal";
+        if (r.Valid)
+            s += " Channel=\"" + std::to_string(r.Channel) + "\" Freq=\"" + std::to_string(r.Freq) + "\" Level=\"" +
+                 LogMessage::Decibels(r.Level) + "\" Noise=\"" + LogMessage::Decibels(r.Noise) + "\" SNR=\"" +
+                 LogMessage::Decibels(r.SNR) + "\"";
+        s += "></Signal>";
+    }
+    return s + "</LogMessage>\n";
 }
 
 }  // namespace receiver

@@ -25,6 +25,10 @@ struct erthost_msg {
     char msgtype[12];
     char text[1400];    // Message.String()
     char record[1400];  // Message.Record() joined with ','
+    int32_t signal;     // 0: no report (the decoder has none), 1: a report without a summary, 2: with one
+    int32_t reserved;
+    int64_t channel, freq;
+    double level, noise, snr;
 };
 
 struct erthost {
@@ -40,10 +44,10 @@ struct erthost {
 // (ERTGPU_FORMAT_*) with gain `scale`, recorded centred at capture_freq Hz with the channel at center_freq.  auto_scale:
 // the gain of each stream is measured from the first min(len, ERTLV_WINDOW) samples of its first erthost_decode call.
 // channel_gain: k of the wide channel path (0 ... 14), -1 none, -2 measured like auto_scale (after it) from the same
-// samples (ertgpu_measure_channel).
+// samples (ertgpu_measure_channel).  signal: every message carries its signal report (protocol::Decoder::EnableSignal).
 erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
                      long long input_rate, int format, float scale, long long capture_freq, long long center_freq,
-                     int auto_scale, int channel_gain, char* errbuf, int errcap) {
+                     int auto_scale, int channel_gain, int signal, char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;   // released only on success: a throwing NewParser / Allocate must not leak the handle
     try {
         protocol::RegisterStockParsers();
@@ -55,7 +59,7 @@ erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long
             h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
         }
         h->d.SetInput({input_rate, format, scale, capture_freq, center_freq, auto_scale != 0, channel_gain < 0 ? -1 : channel_gain,
-                       channel_gain == -2});
+                       channel_gain == -2, signal != 0});
         h->d.Allocate(device, max_blocks, max_cands);
         return h.release();
     } catch (const std::exception& e) {
@@ -257,6 +261,36 @@ long long erthost_encode(erthost* h, const ertgpu_candidate* cands, long long n,
     }
 }
 
+// erthost_encode with the candidates' signal records sigs[0..n) (ertgpu_fetch_signal), summarised for a decoder on
+// channel_hz at rate_out, and format 0 the plain line of ertgpu_decode_file (receiver::BlockLine).
+long long erthost_encode_signal(erthost* h, const ertgpu_candidate* cands, const ertgpu_signal* sigs, long long n,
+                                long long channel_hz, long long rate_out, int format, long long unix_seconds, int nanos,
+                                char* buf, long long cap) {
+    try {
+        std::vector<protocol::MessagePtr> msgs;
+        h->d.SetSignalChannel(channel_hz, rate_out);
+        h->d.Dispatch(cands, (size_t)n, msgs, sigs);
+        std::string all;
+        for (auto& m : msgs) {
+            receiver::LogMessage lm;
+            lm.unix_seconds = unix_seconds;
+            lm.nanos = nanos;
+            lm.Message = m.get();
+            switch (format) {
+            case 1: all += receiver::CsvLine(lm.Record()); break;
+            case 2: all += receiver::JsonLine(lm); break;
+            case 3: all += receiver::XmlLine(lm); break;
+            default: all += receiver::BlockLine(*m) + "\n";
+            }
+        }
+        if ((long long)all.size() < cap && buf) memcpy(buf, all.c_str(), all.size() + 1);
+        return (long long)all.size();
+    } catch (const std::exception& e) {
+        h->err = e.what();
+        return -1;
+    }
+}
+
 long long erthost_decode(erthost* h, const uint8_t* iq, size_t len, erthost_msg* out, long long cap) {
     try {
         if (h->d.AutoScale() && !h->started && len % h->d.InputQuantum() == 0) {
@@ -300,6 +334,15 @@ static long long fill_msgs(const std::vector<protocol::MessagePtr>& msgs, erthos
                 std::string rec;
                 for (auto& f : m->Record()) rec += (rec.empty() ? "" : ",") + f;
                 snprintf(o.record, sizeof(o.record), "%s", rec.c_str());
+                if (m->Signal) {
+                    const protocol::SignalReport& r = *m->Signal;
+                    o.signal = r.Valid ? 2 : 1;
+                    o.channel = r.Channel;
+                    o.freq = r.Freq;
+                    o.level = r.Level;
+                    o.noise = r.Noise;
+                    o.snr = r.SNR;
+                }
             }
             n++;
         }

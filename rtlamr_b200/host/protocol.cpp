@@ -9,6 +9,7 @@
 #include <set>
 
 #include "../../include/ertgpu_resample.h"
+#include "../../include/ertgpu_signal.h"
 
 namespace {
 
@@ -594,7 +595,26 @@ void Decoder::Allocate(int device, int64_t maxBlocksPerCall, int64_t maxCandidat
     Cfg.BlockSize = c.block_size;
     Cfg.BlockSize2 = c.block_size2;
     Cfg.BufferLength = c.buffer_length;
+    ertgpu_tuning_info t{};
+    SetSignalChannel(ertgpu_get_tuning(h_, &t) == ERTGPU_OK ? t.center_hz : (int64_t)Cfg.CenterFreq, c.sample_rate);
     allocated_ = true;
+}
+
+void Decoder::EnableSignal() {
+    if (allocated_) throw std::logic_error("EnableSignal after Allocate");
+    const int rc = ertgpu_enable_signal(h_);
+    if (rc != ERTGPU_OK) raise(h_, rc, "EnableSignal");
+    signal_ = true;
+}
+
+const ertgpu_signal* Decoder::FetchSignal(size_t n) {
+    if (!signal_) return nullptr;
+    sigs_.resize(std::max<size_t>(n, 1));
+    size_t got = 0;
+    const int rc = ertgpu_fetch_signal(h_, sigs_.data(), sigs_.size(), &got);
+    if (rc != ERTGPU_OK) raise(h_, rc, "FetchSignal");
+    if (got != n) throw std::logic_error("FetchSignal: the records do not match the candidates");
+    return sigs_.data();
 }
 
 void Decoder::Reset() {
@@ -625,6 +645,7 @@ void Decoder::SetInput(const Input& in) {
         check(ertgpu_set_channel_gain(h_, in.AutoChannelGain ? 0 : in.ChannelGain));
     }
     auto_channel_gain_ = in.AutoChannelGain;
+    if (in.Signal) EnableSignal();
 }
 
 ertgpu_channel_level Decoder::MeasureChannel(const uint8_t* samples, size_t len) {
@@ -683,7 +704,7 @@ std::vector<std::vector<MessagePtr>> Decoder::DecodeChannels(const std::vector<D
         }
         if (rc != ERTGPU_OK) raise(d.h_, rc, "DecodeChannels");
         d.input_samples_ += (int64_t)(len / d.sample_bytes_);
-        d.Dispatch(d.cands_.data(), n, out[c]);
+        d.Dispatch(d.cands_.data(), n, out[c], d.FetchSignal(n));
     }
     return out;
 }
@@ -705,7 +726,7 @@ std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
     input_samples_ += (int64_t)(len / sample_bytes_);
 
     std::vector<MessagePtr> out;
-    Dispatch(cands_.data(), n, out);
+    Dispatch(cands_.data(), n, out, FetchSignal(n));
     return out;
 }
 
@@ -713,7 +734,7 @@ std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
 // the parsers filed under that preamble.  Candidates arrive sorted by (block, preamble, idx).
 // Decode only fetches candidates that passed a GPU screen: a parser would reject the others at its own
 // checksum test, after the same `seen` bookkeeping, so the emitted messages are identical.
-void Decoder::Dispatch(const ertgpu_candidate* cands, size_t n, std::vector<MessagePtr>& out) {
+void Decoder::Dispatch(const ertgpu_candidate* cands, size_t n, std::vector<MessagePtr>& out, const ertgpu_signal* sigs) {
     const size_t nbytes = (size_t)((Cfg.PacketSymbols + 7) >> 3);
     size_t i = 0;
     while (i < n) {
@@ -732,7 +753,23 @@ void Decoder::Dispatch(const ertgpu_candidate* cands, size_t n, std::vector<Mess
             pkts.push_back(std::move(d));
             j++;
         }
+        const size_t first = out.size();
         for (size_t pi : by_pre_[(size_t)cands[i].preamble_id]) parsers_[pi]->Parse(pkts, out);
+        for (size_t k = first; sigs && k < out.size(); k++) {  // this block and preamble: the candidate with the message's Idx
+            size_t c = i;
+            while (c < j && cands[c].idx != out[k]->Idx) c++;
+            if (c == j) throw std::logic_error("a message without its candidate");
+            SignalReport r;
+            r.Channel = signal_channel_;
+            ertsig_summary_t s;
+            if ((r.Valid = ertsig_summary(&sigs[c], signal_channel_, signal_rate_, &s) != 0)) {
+                r.Freq = s.freq_hz;
+                r.Level = s.level_db;
+                r.Noise = s.noise_db;
+                r.SNR = s.snr_db;
+            }
+            out[k]->Signal = r;
+        }
         i = j;
     }
 }

@@ -20,6 +20,7 @@
 #include <functional>
 #include <map>
 #include <memory>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -93,6 +94,15 @@ struct Field {
     std::vector<uint16_t> Uint16s;
 };
 
+// How a message was received (include/ertgpu_signal.h), from the record of the candidate it was parsed from: the
+// channel the decoder was tuned to (its CenterFreq when untuned) and, when the record has one, its summary.
+struct SignalReport {
+    int64_t Channel = 0;
+    bool Valid = false;   // false: the packet starts before the stream, no summary
+    int64_t Freq = 0;
+    double Level = 0, Noise = 0, SNR = 0;
+};
+
 // parse.go:78-84 (csv.Recorder folded in)
 struct Message {
     virtual ~Message() = default;
@@ -105,6 +115,7 @@ struct Message {
     virtual std::vector<Field> Fields() const = 0;  // exported fields in Go declaration order (embedded structs flattened)
     int64_t Block = 0;  // bookkeeping for the parity tests (not in the reference)
     int Idx = 0;
+    std::optional<SignalReport> Signal;  // set by a Decoder with signal reports (Decoder::EnableSignal)
 };
 using MessagePtr = std::unique_ptr<Message>;
 
@@ -151,6 +162,7 @@ struct Input {
     // after the automatic input gain) and set before its first Decode; as with AutoScale, whoever feeds the Decoder does it.
     int32_t ChannelGain = -1;
     bool AutoChannelGain = false;
+    bool Signal = false;  // per-packet signal reports (Decoder::EnableSignal)
 };
 
 // decode.go:45-63.  Signal/Quantized are not materialised on the host: the parity taps of the C ABI
@@ -181,6 +193,14 @@ public:
     ertgpu_channel_level MeasureChannel(const uint8_t* samples, size_t len);
     // ertgpu_set_channel_gain after Allocate: k of the stream that starts now (after Allocate or Reset, before Decode).
     void SetChannelGain(int32_t k);
+    // ertgpu_enable_signal, before Allocate: every message then carries a SignalReport.
+    void EnableSignal();
+    bool SignalEnabled() const { return signal_; }
+    // The channel and rate the summaries of Dispatch use (set by Allocate; for a Decoder that is never allocated).
+    void SetSignalChannel(int64_t channel_hz, int64_t rate_out) {
+        signal_channel_ = channel_hz;
+        signal_rate_ = rate_out;
+    }
     // Decode takes multiples of this many bytes: whole IQ samples when resampling, whole blocks otherwise.
     size_t InputQuantum() const { return (size_t)sample_bytes_ * (resampling_ ? 1 : (size_t)Cfg.BlockSize); }
     void Allocate(int device = 0, int64_t maxBlocksPerCall = 0, int64_t maxCandidates = 0);  // decode.go:131-160
@@ -197,7 +217,9 @@ public:
     // The second half of Decode (decode.go:177-187 + parse.go): candidates sorted by (block, preamble, idx) are
     // regrouped into per-block, per-preamble []Data and handed to the parsers filed under that preamble.  Needs
     // RegisterProtocol only (no device), so the parsers can be exercised on candidates from any source.
-    void Dispatch(const ertgpu_candidate* cands, size_t n, std::vector<MessagePtr>& out);
+    // sigs: the candidates' signal records (ertgpu_fetch_signal), or nullptr.  Each message then gets the report of the
+    // candidate it was parsed from, found by (block, preamble, idx).
+    void Dispatch(const ertgpu_candidate* cands, size_t n, std::vector<MessagePtr>& out, const ertgpu_signal* sigs = nullptr);
     std::string Log() const;  // decode.go:73-90
     void Reset();
     ertgpu_handle* Handle() const { return h_; }
@@ -208,6 +230,10 @@ private:
     std::vector<std::string> preambles_;        // distinct, registration order
     std::vector<std::vector<size_t>> by_pre_;   // parser indices per preamble (decode.go:124)
     std::vector<ertgpu_candidate> cands_;
+    std::vector<ertgpu_signal> sigs_;
+    bool signal_ = false;
+    int64_t signal_channel_ = 0, signal_rate_ = 0;
+    const ertgpu_signal* FetchSignal(size_t n);   // the last call's records (nullptr without reports)
     bool allocated_ = false;
     bool resampling_ = false;
     ertgpu_resampler_info rs_{};
