@@ -113,6 +113,12 @@ typedef struct {
     int32_t symbols;      /* symbols measured (1 .. span-1 of that protocol)                           */
 } ertgpu_signal;
 
+/* One row of a handle's input spectrum (ertgpu_fetch_spectrum; include/ertgpu_spectrum.h defines it). */
+typedef struct {
+    int64_t first_sample; /* input sample of the stream at which its first frame starts */
+    int64_t frames;       /* frames in it: frames_per_row, or fewer for the open row     */
+} ertgpu_spectrum_row;
+
 /* decode flags */
 #define ERTGPU_DECODE_ONLY_VALID 1u /* return only candidates with check_mask != 0 */
 
@@ -419,6 +425,27 @@ int ertgpu_fetch(ertgpu_handle *h, ertgpu_candidate *out, size_t cap, size_t *n_
  * ertgpu_decode_sharded rejects handles with reports. */
 int ertgpu_enable_signal(ertgpu_handle *h);
 int ertgpu_fetch_signal(ertgpu_handle *h, ertgpu_signal *out, size_t cap, size_t *n_out);
+
+/* The power spectrum of the input (include/ertgpu_spectrum.h).  ertgpu_enable_spectrum, called before ertgpu_allocate
+ * (after it: ERTGPU_EINVAL), makes every decode of the handle also measure its input samples, as the caller passed them,
+ * in frames of N = 2^log2_n samples (ERTSPEC_LOG2_MIN <= log2_n <= ERTSPEC_LOG2_MAX), frames_per_row F frames to a row,
+ * N F >= ERTSPEC_ROW_MIN_SAMPLES (else ERTGPU_EINVAL).  Any handle takes it, whatever its format, rate and tuning.  The
+ * kernel (spectrum_kernel<F>) runs on the handle's stream behind each step of the decode, is counted in
+ * ertgpu_last_launches and named last in ertgpu_last_kernels; candidates and signal reports are those of a handle
+ * without a spectrum.  Rows do not depend on how the stream is cut into calls.
+ * Rows wait on the device until they are fetched.  allocate sizes that buffer for the rows of one call of up to
+ * max_blocks_per_call blocks of the decoder, times the input rate over the decoder's rate (rounded up) input samples,
+ * plus two; a decode call whose rows would not fit beside the rows not yet fetched returns ERTGPU_ECAPACITY before it
+ * enqueues anything (fetch, then repeat the call).
+ * ertgpu_fetch_spectrum waits for the handle's work and returns the rows completed since the last fetch, in order:
+ * rows[i], and mean[i * N .. (i+1) * N) and peak[i * N ..] by ascending bin.  With partial = 1 it also returns the open
+ * row, when it has at least one frame, last and without consuming it.  *n_out = the rows returned, or, with
+ * ERTGPU_ECAPACITY, the rows needed (nothing is consumed).  ERTGPU_EINVAL on a handle without a spectrum.  ertgpu_reset
+ * restarts frames, rows and the carried samples.  ertgpu_decode_channels[_device_async] takes at most one handle with a
+ * spectrum, which measures the group's input once; ertgpu_decode_sharded rejects handles with a spectrum. */
+int ertgpu_enable_spectrum(ertgpu_handle *h, int32_t log2_n, int64_t frames_per_row);
+int ertgpu_fetch_spectrum(ertgpu_handle *h, int32_t partial, ertgpu_spectrum_row *rows, float *mean, float *peak,
+                          size_t cap, size_t *n_out);
 
 /* Number of candidates of the last decode, and how many passed a screen. */
 int ertgpu_last_counts(ertgpu_handle *h, int64_t *n_candidates, int64_t *n_valid);

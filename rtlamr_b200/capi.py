@@ -100,6 +100,8 @@ SIGNAL_DTYPE = np.dtype([(n, "<i8") for n in ("n_on", "e_on", "n_off", "e_off", 
                         [("protocol", "<i4"), ("symbols", "<i4")])
 assert SIGNAL_DTYPE.itemsize == C.sizeof(Signal) == 64
 
+SPECTRUM_ROW_DTYPE = np.dtype([("first_sample", "<i8"), ("frames", "<i8")])
+
 CAND_DTYPE = np.dtype([("block", "<i8"), ("idx", "<i4"), ("preamble_id", "<i4"),
                        ("check_mask", "<u4"), ("flags", "<u4"),
                        ("bytes", "u1", (MAX_PACKET_BYTES,)), ("r900_digits", "u1", (R900_DIGITS,)),
@@ -120,7 +122,7 @@ EXPORTS = [
     "ertgpu_allow_input_decimation", "ertgpu_get_decimator",
     "ertgpu_decode_channels", "ertgpu_decode_channels_device_async",
     "ertgpu_set_channel_gain", "ertgpu_get_channel_gain", "ertgpu_measure_channel",
-    "ertgpu_enable_signal", "ertgpu_fetch_signal",
+    "ertgpu_enable_signal", "ertgpu_fetch_signal", "ertgpu_enable_spectrum", "ertgpu_fetch_spectrum",
 ]
 
 _lib = None
@@ -190,6 +192,8 @@ def lib() -> C.CDLL:
     L.ertgpu_measure_channel.argtypes = [vp, vp, sz, C.POINTER(ChannelLevel)]
     L.ertgpu_enable_signal.argtypes = [vp]
     L.ertgpu_fetch_signal.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.ertgpu_enable_spectrum.argtypes = [vp, i32, C.c_int64]
+    L.ertgpu_fetch_spectrum.argtypes = [vp, i32, vp, vp, vp, sz, C.POINTER(sz)]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the library does not export it
     _lib = L
@@ -212,6 +216,7 @@ class Handle:
         self._h = C.c_void_p()
         self._check(self._L.ertgpu_create(C.byref(self._h)))
         self.cfg = None
+        self._spectrum_n = 0   # N of ertgpu_enable_spectrum
 
     def _check(self, rc: int):
         if rc != OK:
@@ -313,6 +318,17 @@ class Handle:
     def enable_signal(self):
         """ertgpu_enable_signal: measure every candidate's signal (before allocate)."""
         self._check(self._L.ertgpu_enable_signal(self._h))
+
+    def enable_spectrum(self, log2_n: int, frames_per_row: int):
+        """ertgpu_enable_spectrum: measure the input's spectrum in rows of frames_per_row frames of 2^log2_n samples
+        (before allocate)."""
+        self._check(self._L.ertgpu_enable_spectrum(self._h, log2_n, frames_per_row))
+        self._spectrum_n = 1 << log2_n
+
+    def fetch_spectrum(self, partial: bool = False):
+        """ertgpu_fetch_spectrum: (rows, mean, peak) of the rows completed since the last fetch (and the open row last,
+        not consumed, with partial): rows a SPECTRUM_ROW_DTYPE array, mean and peak float32 of shape (n_rows, N)."""
+        return fetch_spectrum(self._h, self._spectrum_n, partial)
 
     def fetch_signal(self, cap: int = 4096) -> np.ndarray:
         """ertgpu_fetch_signal: one SIGNAL_DTYPE record per candidate the last decode or fetch returned, same order."""
@@ -422,17 +438,36 @@ class Handle:
         return buf
 
 
+def fetch_spectrum(h, n_bins: int, partial: bool = False):
+    """ertgpu_fetch_spectrum on the handle h (an ertgpu_handle pointer) of a spectrum of n_bins = N bins: every row
+    there is, as Handle.fetch_spectrum returns them."""
+    L = lib()
+    n = C.c_size_t(0)
+    rc = L.ertgpu_fetch_spectrum(h, int(partial), None, None, None, 0, C.byref(n))   # how many rows
+    if rc not in (OK, ECAPACITY):
+        raise ErtGpuError(rc, (L.ertgpu_last_error(h) or b"").decode())
+    cap = n.value
+    rows = np.zeros(cap, dtype=SPECTRUM_ROW_DTYPE)
+    mean = np.zeros((cap, n_bins), dtype=np.float32)
+    peak = np.zeros((cap, n_bins), dtype=np.float32)
+    rc = L.ertgpu_fetch_spectrum(h, int(partial), rows.ctypes.data, mean.ctypes.data, peak.ctypes.data, cap, C.byref(n))
+    if rc != OK:
+        raise ErtGpuError(rc, (L.ertgpu_last_error(h) or b"").decode())
+    return rows, mean, peak
+
+
 def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per_call: int = 0,
                 max_candidates: int = 0, input_rate: int = 0, input_format: int = FORMAT_CU8,
                 input_scale: float = 0.0, capture_freq: int = 0, center_freq: int = 0,
-                channel_gain: int | None = None, signal: bool = False) -> Handle:
+                channel_gain: int | None = None, signal: bool = False, spectrum: tuple | None = None) -> Handle:
     """NewDecoder + RegisterProtocol(NewParser(name, chip_length)) for each name + Allocate
     (reference main.go:64-86).  input_rate > 0: the IQ is sampled at that rate (ertgpu_set_input_rate);
     input_format / input_scale: its sample format and gain (ertgpu_set_input_format, not called for plain cu8);
     capture_freq > 0: the IQ was recorded centred there, and the channel at center_freq (0: the protocols'
     CenterFreq) is decoded (ertgpu_set_input_tuning, before the rate), at up to 256 times the decoder's rate
     (ertgpu_allow_input_decimation).  channel_gain k: the wide channel path with gain 2^k (ertgpu_set_channel_gain;
-    tuned handles only).  signal: per-packet signal reports (ertgpu_enable_signal)."""
+    tuned handles only).  signal: per-packet signal reports (ertgpu_enable_signal).  spectrum (log2_n, frames_per_row):
+    the input's spectrum (ertgpu_enable_spectrum)."""
     if isinstance(msgtypes, str):
         msgtypes = [m.strip() for m in msgtypes.split(",") if m.strip()]
     h = Handle()
@@ -449,6 +484,8 @@ def new_decoder(msgtypes, chip_length: int = 72, device: int = 0, max_blocks_per
         h.set_channel_gain(channel_gain)
     if signal:
         h.enable_signal()
+    if spectrum is not None:
+        h.enable_spectrum(*spectrum)
     h.allocate(device, max_blocks_per_call, max_candidates)
     return h
 

@@ -14,6 +14,8 @@
 //   hits    : (start, preamble) pairs found by the Search kernel (search_slide_kernel or search_generic_kernel)
 //   out     : ertgpu_candidate records produced by extract_kernel
 //   sig     : ertgpu_signal records of the same slots (packet_signal_kernel; handles with signal reports only)
+//   spec    : the input's spectrum rows, and what spectrum_kernel carries between calls (spectrum.cuh; handles with a
+//             spectrum only)
 #include <ctype.h>
 #include <sched.h>
 
@@ -37,6 +39,7 @@
 #include "input_stage.cuh"
 #include "search.cuh"
 #include "signal.cuh"
+#include "spectrum.cuh"
 #include "synth.cuh"
 
 using namespace ert;
@@ -148,6 +151,7 @@ struct ertgpu_handle {
     std::vector<ertgpu_signal> sig_results;  // results' records, in the same order
 
     InputStage in{err};  // input format, rate and tuning, and the kernel in front of the pipeline
+    Spectrum spec;       // ertgpu_enable_spectrum
 };
 
 namespace {
@@ -257,6 +261,7 @@ void free_device(ertgpu_handle* h) {
     dfree(h->d_counters);
     dfree(h->d_tap);
     h->in.release();
+    h->spec.release();
     if (h->h_counters) cudaFreeHost(h->h_counters);
     h->h_counters = nullptr;
     if (h->stream) cudaStreamDestroy(h->stream);
@@ -675,9 +680,19 @@ void stage_pending(ertgpu_handle* h, cudaStream_t st) {
     h->pending_stream = st;
 }
 
-// Enqueue the work for the next n input samples, at d_in on the device, on st: the input stage's step and the pipeline
-// over the whole blocks it completes.
-int run_step(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaStream_t st) {
+// Enqueue spectrum_kernel over the n input samples at d_in on st, last in the step: it reads the staging buffer too.
+int launch_spectrum(ertgpu_handle* h, const uint8_t* d_in, int64_t n, cudaStream_t st) {
+    if (const int rc = h->spec.launch(h->err, d_in, n, h->in.scale, st, &h->launches)) return rc;
+    const std::string lab = ";" + h->spec.label;
+    if (h->kernels.size() < lab.size() || h->kernels.compare(h->kernels.size() - lab.size(), lab.size(), lab) != 0)
+        h->kernels += lab;  // a step without a pipeline keeps the last pipeline's list, which names it already
+    if (!h->pending) stage_pending(h, st);
+    return ERTGPU_OK;
+}
+
+// Enqueue the work for the next n input samples, at d_in on the device, on st: the input stage's step, the pipeline
+// over the whole blocks it completes and, with a spectrum, spectrum_kernel over the n samples.
+int run_step(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaStream_t st, const uint8_t* d_in, int64_t n) {
     int rc;
     if (s.nblocks > 0) {
         rc = enqueue_pipeline(h, s, flags, st);
@@ -691,11 +706,11 @@ int run_step(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaStream_t 
     }
     if (rc) return rc;
     h->in.commit(s);
-    return ERTGPU_OK;
+    return h->spec.on ? launch_spectrum(h, d_in, n, st) : ERTGPU_OK;
 }
 
 int enqueue_step(ertgpu_handle* h, const uint8_t* d_in, int64_t n, uint32_t flags, cudaStream_t st) {
-    return run_step(h, h->in.plan(d_in, n), flags, st);
+    return run_step(h, h->in.plan(d_in, n), flags, st, d_in, n);
 }
 
 // The same for the channels hs[0..n) of one capture (check_channels holds) over the same input.  Decimating channels
@@ -711,7 +726,7 @@ int enqueue_channels(ertgpu_handle* const* hs, int n, const uint8_t* d_in, int64
     int64_t shared = 0;
     if (const int rc = hs[0]->in.launch_channels(steps, n, st, &shared)) return fail(hs[0], rc, "%s", hs[0]->err.c_str());
     for (int k = 0; k < n; k++)
-        if (const int rc = run_step(hs[k], steps[k], flags, st)) return rc;
+        if (const int rc = run_step(hs[k], steps[k], flags, st, d_in, cnt)) return rc;
     ertgpu_handle* h = hs[0];
     h->launches += shared;
     if (shared && !h->pending) stage_pending(h, st);  // the shared launch wrote every channel's history
@@ -734,7 +749,15 @@ int check_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
     if (const int rc = h ? h->in.check_samples(nbytes) : ERTGPU_OK) return rc;
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     if (!iq && nbytes) return fail(h, ERTGPU_EINVAL, "null input");
-    return h->in.check_call(iq, nbytes, device);
+    if (const int rc = h->in.check_call(iq, nbytes, device)) return rc;
+    if (h->spec.on) {
+        const Spectrum& sp = h->spec;
+        const int64_t waiting = sp.rows_done() - sp.pos.rows_fetched, more = sp.rows_after((int64_t)(nbytes / h->in.sample_bytes));
+        if (waiting + more > sp.row_cap)
+            return fail(h, ERTGPU_ECAPACITY, "spectrum: %lld rows not fetched and %lld more from this call, the handle holds %lld: "
+                        "ertgpu_fetch_spectrum first, or make the call shorter", (long long)waiting, (long long)more, (long long)sp.row_cap);
+    }
+    return ERTGPU_OK;
 }
 
 int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
@@ -789,6 +812,10 @@ int check_channels(ertgpu_handle* const* hs, int32_t n, const void* iq, size_t n
                         k, (long long)h->in.received(), (long long)h0->in.received());
     }
     for (int k = 0; k < n; k++)
+        for (int j = 0; j < k; j++)
+            if (hs[k]->spec.on && hs[j]->spec.on)
+                return fail(h0, ERTGPU_EINVAL, "channels %d and %d both have a spectrum: a group measures its input once, on one handle", j, k);
+    for (int k = 0; k < n; k++)
         if (const int rc = check_decode(hs[k], iq, nbytes, device)) {
             if (k) fail(h0, rc, "channel %d: %s", k, hs[k]->err.c_str());
             return rc;
@@ -798,9 +825,10 @@ int check_channels(ertgpu_handle* const* hs, int32_t n, const void* iq, size_t n
 
 }  // namespace
 
-// ertgpu_decode_sharded's rule for signal reports, with its message on h.  Shared with sharded.cpp inside the library
-// only: hidden, so libertgpu.so exports nothing beyond include/ertgpu.h.
+// ertgpu_decode_sharded's rule for signal reports and spectra, with its message on h.  Shared with sharded.cpp inside
+// the library only: hidden, so libertgpu.so exports nothing beyond include/ertgpu.h.
 __attribute__((visibility("hidden"))) int sharded_reject_signal(ertgpu_handle* h) {
+    if (h->spec.on) return fail(h, ERTGPU_EINVAL, "decode_sharded: the handle has a spectrum (ertgpu_enable_spectrum), which sharded decodes do not measure");
     return h->signal ? fail(h, ERTGPU_EINVAL, "decode_sharded: the handle has signal reports (ertgpu_enable_signal), which sharded decodes do not keep")
                      : ERTGPU_OK;
 }
@@ -1073,6 +1101,13 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     h->pipe.r900_chain = d.PKL % 8 == 0;
 
     if (const int rc = h->in.allocate(c.block_size, max_blocks_per_call, h->sm_count)) return rc;
+    if (h->spec.on) {  // rows of the largest call: a staging chunk, or a device call of the input stage's largest step
+        const int64_t r_out = decoder_rate(h), r_in = h->in.rate_in ? h->in.rate_in : r_out;
+        const int64_t in_max = std::max({h->in.chunk(), h->in.max_call_input(),
+                                         max_blocks_per_call * c.block_size * ((r_in + r_out - 1) / r_out)});
+        if (const int rc = h->spec.allocate(h->err, h->in.fmt, h->in.sample_bytes, fmt_name(h->in.fmt), in_max, h->sm_count))
+            return rc;
+    }
     h->pos = {};
     return ERTGPU_OK;
 }
@@ -1092,6 +1127,7 @@ int ertgpu_reset(ertgpu_handle* h) {
     h->uncopied = false;
     h->pos = {};  // the history in front of the next call is zeroed on that call's stream (enqueue_pipeline)
     h->in.reset_stream();
+    h->spec.pos = {};
     begin_call(h);
     return ERTGPU_OK;
 }
@@ -1351,6 +1387,52 @@ int ertgpu_fetch_signal(ertgpu_handle* h, ertgpu_signal* out, size_t cap, size_t
     if (n_out) *n_out = h->sig_results.size();
     if (h->sig_results.size() > cap) return fail(h, ERTGPU_ECAPACITY, "output array holds %zu records, %zu needed", cap, h->sig_results.size());
     if (!h->sig_results.empty() && out) memcpy(out, h->sig_results.data(), h->sig_results.size() * sizeof(ertgpu_signal));
+    return ERTGPU_OK;
+}
+
+int ertgpu_enable_spectrum(ertgpu_handle* h, int32_t log2_n, int64_t frames_per_row) {
+    if (!h) return ERTGPU_EINVAL;
+    if (h->allocated) return fail(h, ERTGPU_EINVAL, "enable_spectrum after allocate");
+    if (log2_n < ERTSPEC_LOG2_MIN || log2_n > ERTSPEC_LOG2_MAX)
+        return fail(h, ERTGPU_EINVAL, "spectrum frames of 2^%d samples: log2_n must be within %d ... %d", log2_n, ERTSPEC_LOG2_MIN, ERTSPEC_LOG2_MAX);
+    if (frames_per_row < 1 || frames_per_row > (1ll << 40) || (frames_per_row << log2_n) < ERTSPEC_ROW_MIN_SAMPLES)
+        return fail(h, ERTGPU_EINVAL, "spectrum rows of %lld frames of 2^%d samples: N * frames_per_row must be at least %d",
+                    (long long)frames_per_row, log2_n, ERTSPEC_ROW_MIN_SAMPLES);
+    h->spec.on = true;
+    h->spec.log2n = log2_n;
+    h->spec.F = frames_per_row;
+    return ERTGPU_OK;
+}
+
+int ertgpu_fetch_spectrum(ertgpu_handle* h, int32_t partial, ertgpu_spectrum_row* rows, float* mean, float* peak, size_t cap,
+                          size_t* n_out) {
+    if (!h || !h->allocated) return ERTGPU_EINVAL;
+    Spectrum& sp = h->spec;
+    if (!sp.on) return fail(h, ERTGPU_EINVAL, "fetch_spectrum: the handle was allocated without a spectrum (ertgpu_enable_spectrum)");
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    if (const int rc = collect_sync(h)) return rc;
+    const int64_t first = sp.pos.rows_fetched, done = sp.rows_done();
+    const bool open = partial && sp.frames() % sp.F != 0;
+    const size_t need = (size_t)(done - first) + (open ? 1 : 0);
+    if (n_out) *n_out = need;
+    if (need > cap) return fail(h, ERTGPU_ECAPACITY, "output arrays hold %zu rows, %zu needed", cap, need);
+    if (need && (!rows || !mean || !peak)) return fail(h, ERTGPU_EINVAL, "null output array");
+    const size_t N = (size_t)sp.N;
+    for (int64_t r = first; r < done; r++) {
+        const size_t i = (size_t)(r - first), slot = (size_t)(r % sp.row_cap);
+        CUDA_TRY(h, cudaMemcpy(mean + i * N, sp.d_mean + slot * N, N * sizeof(float), cudaMemcpyDeviceToHost));
+        CUDA_TRY(h, cudaMemcpy(peak + i * N, sp.d_peak + slot * N, N * sizeof(float), cudaMemcpyDeviceToHost));
+        rows[i].first_sample = r * sp.F * sp.N;
+        rows[i].frames = sp.F;
+    }
+    if (open) {
+        const size_t i = (size_t)(done - first);
+        int64_t frames = 0;
+        if (const int rc = sp.open_row(h->err, mean + i * N, peak + i * N, &frames)) return rc;
+        rows[i].first_sample = done * sp.F * sp.N;
+        rows[i].frames = frames;
+    }
+    sp.pos.rows_fetched = done;
     return ERTGPU_OK;
 }
 

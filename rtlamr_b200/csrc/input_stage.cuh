@@ -364,6 +364,14 @@ struct InputStage {
         return resamples() ? std::min(c, max_input()) : c;
     }
 
+    // At least the input samples of any step that completes at most max_blocks blocks (a device call, check_call), from
+    // any stream position: max_input's bound with the history it carries at its largest.
+    int64_t max_call_input() const {
+        if (!resamples()) return max_blocks * block;
+        const int64_t m2 = k_of((max_blocks + 1) * block) + rs.T + rs.M / rs.L + 16;
+        return mode == kDecimate ? (m2 + 1) * dec.D + dec.T1 + 16 : m2;
+    }
+
     // The step over n new input samples at d_in (device).  Nothing of the stage changes until commit.
     InputStep plan(const uint8_t* d_in, int64_t n) const {
         InputStep s;

@@ -14,7 +14,7 @@
 
 #include "../../include/ertgpu.h"
 
-// ertgpu.cu: ERTGPU_EINVAL, with the message on h, when h has signal reports (sharded decodes do not keep them).  Hidden:
+// ertgpu.cu: ERTGPU_EINVAL, with the message on h, when h has signal reports or a spectrum (sharded decodes keep neither).  Hidden:
 // not exported from libertgpu.so.
 __attribute__((visibility("hidden"))) int sharded_reject_signal(ertgpu_handle* h);
 

@@ -46,7 +46,10 @@ def lib():
         L = C.CDLL(LIB_PATH)
         L.erthost_new.restype = C.c_void_p
         L.erthost_new.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong, C.c_longlong, C.c_int, C.c_float,
-                                  C.c_longlong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_int]
+                                  C.c_longlong, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_char_p,
+                                  C.c_int]
+        L.erthost_gpu_handle.restype = C.c_void_p
+        L.erthost_gpu_handle.argtypes = [C.c_void_p]
         L.erthost_channel_gain.argtypes = [C.c_void_p]
         L.erthost_level.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_longlong),
                                     C.POINTER(C.c_longlong)]
@@ -261,7 +264,8 @@ class Receiver:
 
     def __init__(self, msgtypes: str, chip_length: int = 72, device: int = 0, max_blocks: int = 0, max_cands: int = 0,
                  input_rate: int = 0, input_format: int = 0, input_scale: float | str = 0.0, capture_freq: int = 0,
-                 center_freq: int = 0, channel_gain: int | str | None = None, signal: bool = False):
+                 center_freq: int = 0, channel_gain: int | str | None = None, signal: bool = False,
+                 spectrum: tuple | None = None):
         """The input arguments are protocol::Decoder::SetInput's.  input_rate > 0: the IQ given to decode() is sampled at
         that rate; any rate other than DataRate * ChipLength is resampled on the GPU and decode() then takes any whole
         number of IQ samples.  input_format / input_scale: the IQ's sample format (capi.FORMAT_*) and gain.
@@ -271,7 +275,8 @@ class Receiver:
         input_level() tells which.  channel_gain=k: the wide channel path of a tuned input with gain 2^k
         (ertgpu_set_channel_gain); "auto": k of each stream is measured from the same samples after the input gain
         (ertgpu_measure_channel), and channel_gain() tells which.  signal: every message carries its signal report
-        (HostMessage.signal; protocol::Decoder::EnableSignal)."""
+        (HostMessage.signal; protocol::Decoder::EnableSignal).  spectrum=(log2_n, frames_per_row): the input's spectrum
+        (protocol::Decoder::EnableSpectrum), whose rows each decode() collects and spectrum() returns."""
         self._L = lib()
         err = C.create_string_buffer(512)
         auto = isinstance(input_scale, str)
@@ -282,13 +287,16 @@ class Receiver:
         cg = -1 if channel_gain is None else -2 if channel_gain == "auto" else int(channel_gain)
         self._h = self._L.erthost_new(msgtypes.encode(), chip_length, device, max_blocks, max_cands, input_rate, input_format,
                                       0.0 if auto else input_scale, capture_freq, center_freq, 1 if auto else 0, cg,
-                                      1 if signal else 0, err, 512)
+                                      1 if signal else 0, spectrum[0] if spectrum else 0, spectrum[1] if spectrum else 0,
+                                      err, 512)
         if not self._h:
             raise RuntimeError(err.value.decode())
         v = (C.c_int32 * 12)()
         self._L.erthost_config(self._h, v)
         self.cfg = dict(zip(self.CFG, [int(x) for x in v]))
         self.cfg["CenterFreq"] &= 0xFFFFFFFF
+        self._spectrum = spectrum
+        self._rows = []
 
     def close(self):
         if self._h:
@@ -302,6 +310,7 @@ class Receiver:
             pass
 
     def reset(self):
+        self._rows = []
         if self._L.erthost_reset(self._h) != 0:
             raise RuntimeError(self._L.erthost_error(self._h).decode())
 
@@ -334,4 +343,19 @@ class Receiver:
             raise RuntimeError(self._L.erthost_error(self._h).decode())
         if n > cap:
             raise OverflowError(f"{n} messages, cap {cap}")
+        if self._spectrum:
+            self._rows.append(self._fetch_spectrum(False))
         return _messages(out, n)
+
+    def _fetch_spectrum(self, partial: bool):
+        from rtlamr_b200 import capi
+        return capi.fetch_spectrum(C.c_void_p(self._L.erthost_gpu_handle(self._h)), 1 << self._spectrum[0], partial)
+
+    def spectrum(self, partial: bool = False):
+        """(rows, mean, peak) of the spectrum rows the decode() calls of the current stream completed (capi.Handle's
+        fetch_spectrum layout), and with partial the open row last."""
+        from rtlamr_b200 import capi
+        parts = self._rows + ([self._fetch_spectrum(True)] if partial else [])
+        n = 1 << self._spectrum[0]
+        empty = (np.zeros(0, capi.SPECTRUM_ROW_DTYPE), np.zeros((0, n), np.float32), np.zeros((0, n), np.float32))
+        return tuple(np.concatenate([e] + [p[k] for p in parts]) for k, e in enumerate(empty))

@@ -5,6 +5,7 @@
 //   ertgpu_decode_file [-msgtype=scm,idm|all] [-symbollength=72] [-blockdedup=true] [-blocks=4096] [-device=0]
 //                      [-filterid=1,2] [-filtertype=4,5] [-unique=true] [-format=plain|csv|json|xml]
 //                      [-samplefile=PATH] [-single] [-duration=1h5m10s] [-samplerate=HZ] [-signal]
+//                      [-spectrum=FILE [-spectrumbin=HZ] [-spectrumint=1s] [-spectrumpeak]]
 //                      [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|cf64_be|wav|sigmf] [-samplescale=G|auto] [-capturefreq=HZ [-centerfreq=HZ[,HZ...]]]
 //                      FILE|- [FILE ...]
 // -capturefreq names the frequency the capture was recorded centred at; -centerfreq (rtlamr's flag) the channel to
@@ -61,6 +62,18 @@
 // <Signal Channel=".." Freq=".." Level=".." Noise=".." SNR=".."> element after <Message>.  A packet that starts before
 // the stream has no report: "-" for each field (plain), five empty fields (csv), null (json), no attributes (xml).
 // Without -signal every format is exactly as above.
+// -spectrum=FILE also measures the power spectrum of the capture on the GPU, from the same uploaded samples as the decode
+// (DESIGN.md §3.14, include/ertgpu_spectrum.h), and appends one line per row to FILE in rtl_power's column layout, which
+// heat-map (waterfall) scripts read: date, time, Hz low, Hz high, Hz step, samples, dB, dB, ...  Hz low and Hz high are the
+// capture's centre (the capture frequency, or the protocols' CenterFreq) -+ half its rate, Hz step the bin width, samples
+// the row's input samples, and each dB a bin's mean power over the row (-spectrumpeak: its largest frame power, like
+// rtl_power -P) in dB of full scale, 0 dB for a full-scale tone.  -spectrumbin=HZ (default 10000) picks the frame length:
+// the smallest power of two N, 64 ... 16384, whose bins are at most HZ wide.  -spectrumint=DURATION (Go syntax, default 1s)
+// is a row's length, at least 2^18 samples.  The time is the recording time of the row's first sample (UTC) for a SigMF
+// recording with core:datetime, otherwise 1970-01-01 00:00:00 plus the row's offset from the start of its stream, in whole
+// seconds: rows shorter than a second may share a time, and the samples column and their order tell them apart.  At the
+// end of each stream the open row follows if it holds a frame.  Every file of a batch is its own stream with its own rows.
+// stdout is exactly what it is without -spectrum.
 // Several files are a batch of independent streams through ONE decoder (buffers, tables and kernels set up once):
 // each starts from zeroed history with block numbers from 0, exactly as if it were decoded alone.  They share the
 // sample file, whose offsets keep growing from one file to the next.
@@ -75,6 +88,7 @@
 #include <vector>
 
 #include "../../include/ertgpu_resample.h"
+#include "../../include/ertgpu_spectrum.h"
 #include "receiver.hpp"
 #include "sigmf.hpp"
 #include "wav.hpp"
@@ -88,6 +102,8 @@ int main(int argc, char** argv) {
     bool block_dedup = true, quiet = false, unique = false, single = false, signal = false;
     std::string filterid, filtertype, format = "plain", samplefile, duration, sampleformat = "cu8", samplescale;
     std::string capturefreq, centerfreq, channelgain;
+    std::string spectrum_file, spectrum_bin, spectrum_int;
+    bool spectrum_peak = false;
     bool have_scale = false, auto_scale = false;
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
@@ -117,6 +133,10 @@ int main(int argc, char** argv) {
         else if (a == "-single") single = true;
         else if (a.rfind("-duration=", 0) == 0) duration = a.substr(10);
         else if (a == "-quiet") quiet = true;
+        else if (a.rfind("-spectrum=", 0) == 0) spectrum_file = a.substr(10);
+        else if (a.rfind("-spectrumbin=", 0) == 0) spectrum_bin = a.substr(13);
+        else if (a.rfind("-spectrumint=", 0) == 0) spectrum_int = a.substr(13);
+        else if (a == "-spectrumpeak" || a == "-spectrumpeak=true") spectrum_peak = true;
         else files.push_back(a);
     }
     if (files.empty()) {
@@ -124,6 +144,7 @@ int main(int argc, char** argv) {
                         "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
                         "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|wav|sigmf] "
                         "[-samplescale=G|auto] [-channelgain=G|auto] [-signal] "
+                        "[-spectrum=FILE [-spectrumbin=HZ] [-spectrumint=D] [-spectrumpeak]] "
                         "[-capturefreq=HZ [-centerfreq=HZ[,HZ...]]] [-quiet] FILE|- [FILE ...]\n", argv[0]);
         return 2;
     }
@@ -165,6 +186,37 @@ int main(int argc, char** argv) {
         if (!duration.empty()) limit_ns = receiver::ParseDuration(duration);
     } catch (const std::exception& e) {
         fprintf(stderr, "invalid value \"%s\" for flag -duration: %s\n", duration.c_str(), e.what());
+        return 2;
+    }
+    if (spectrum_file.empty() && (!spectrum_bin.empty() || !spectrum_int.empty() || spectrum_peak)) {
+        fprintf(stderr, "-spectrumbin, -spectrumint and -spectrumpeak need -spectrum=FILE\n");
+        return 2;
+    }
+    double spectrum_hz = 10000;
+    int64_t spectrum_ns = 1000000000;
+    if (!spectrum_bin.empty()) {
+        char* end = nullptr;
+        spectrum_hz = strtod(spectrum_bin.c_str(), &end);
+        if (*end || !std::isfinite(spectrum_hz) || spectrum_hz <= 0) {
+            fprintf(stderr, "invalid value \"%s\" for flag -spectrumbin: a bin width in Hz > 0\n", spectrum_bin.c_str());
+            return 2;
+        }
+    }
+    if (!spectrum_int.empty()) {
+        try {
+            spectrum_ns = receiver::ParseDuration(spectrum_int);
+        } catch (const std::exception& e) {
+            fprintf(stderr, "invalid value \"%s\" for flag -spectrumint: %s\n", spectrum_int.c_str(), e.what());
+            return 2;
+        }
+        if (spectrum_ns < 0) {
+            fprintf(stderr, "invalid value \"%s\" for flag -spectrumint: a duration >= 0\n", spectrum_int.c_str());
+            return 2;
+        }
+    }
+    FILE* spectrum_out = nullptr;
+    if (!spectrum_file.empty() && !(spectrum_out = fopen(spectrum_file.c_str(), "w"))) {
+        fprintf(stderr, "-spectrum=%s: %s\n", spectrum_file.c_str(), strerror(errno));
         return 2;
     }
     const bool wav_in = sampleformat == "wav", sigmf_in = sampleformat == "sigmf";
@@ -311,9 +363,15 @@ int main(int argc, char** argv) {
             return 1;
         }
     }
+    const int64_t rate_in = samplerate ? samplerate : 32768LL * chip;
+    const int32_t spectrum_log2 = spectrum_out ? ertspec_log2_for_bin(rate_in, spectrum_hz) : 0;
+    const int64_t spectrum_frames = spectrum_out ? ertspec_frames_per_row(spectrum_log2, spectrum_ns, rate_in) : 0;
     try {
-        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale, channel_k, auto_channel, signal},
+        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale, channel_k, auto_channel, signal,
+                                                                spectrum_log2, spectrum_frames},
                                 channels);
+        const int64_t spectrum_centre = capture_hz ? capture_hz : (int64_t)rcvr.decoder().Cfg.CenterFreq;
+        std::vector<char> line;
         std::string log = rcvr.decoder().Log();
         if (!channels.empty()) {   // the channels share everything of the log but CenterFreq, its first line: name them all
             std::string names;
@@ -358,6 +416,20 @@ int main(int argc, char** argv) {
                             (long long)t.center_hz, lv.k, 1LL << lv.k);
                 });
             if (wav_in && in != stdin) wav_hdr[fi] = wav::ReadHeader(in);   // the same header as above: to the samples
+            const auto spectrum_rows = [&](const protocol::SpectrumRows& r) {
+                for (size_t i = 0; i < r.rows.size(); i++) {
+                    const int64_t s0 = r.rows[i].first_sample;
+                    int64_t ns = s0 / rate_in * 1000000000 + s0 % rate_in * 1000000000 / rate_in;   // stream time
+                    if (sigmf_in && sigmf::Dated(rec[fi])) ns = sigmf::BlockTime(rec[fi], s0 - 1, 1, rec[0].rate);
+                    const int64_t sec = ns / 1000000000 - (ns % 1000000000 < 0);
+                    const float* p = (spectrum_peak ? r.peak.data() : r.mean.data()) + i * (size_t)r.N;
+                    const int len = ertspec_csv_line(nullptr, 0, sec, spectrum_centre, rate_in, spectrum_log2,
+                                                     r.rows[i].frames * r.N, p);
+                    line.resize((size_t)len + 1);
+                    ertspec_csv_line(line.data(), line.size(), sec, spectrum_centre, rate_in, spectrum_log2, r.rows[i].frames * r.N, p);
+                    if (fputs(line.data(), spectrum_out) < 0) throw std::runtime_error("writing the -spectrum file failed");
+                }
+            };
             auto st = rcvr.Run(in, block_dedup, [&](const protocol::Message& m, int64_t offset, int length) {
                 if (quiet) return;
                 if (csv || json || xml) {
@@ -380,7 +452,8 @@ int main(int argc, char** argv) {
                 } else {
                     printf("%s\n", receiver::BlockLine(m).c_str());
                 }
-            }, wav_in ? wav_hdr[fi].data_size : -1);
+            }, wav_in ? wav_hdr[fi].data_size : -1, spectrum_out ? std::function<void(const protocol::SpectrumRows&)>(spectrum_rows)
+                                                                : std::function<void(const protocol::SpectrumRows&)>());
             if (in != stdin) fclose(in);
             fprintf(stderr, "%s%s%lld messages (%lld duplicates dropped) from %lld blocks, %.1f MB in %.3f s = %.1f Msamples/s\n",
                     files.size() > 1 ? file.c_str() : "", files.size() > 1 ? ": " : "", (long long)st.messages,
@@ -394,6 +467,11 @@ int main(int argc, char** argv) {
     } catch (const std::exception& e) {
         fprintf(stderr, "error: %s\n", e.what());
         if (sample) fclose(sample);
+        if (spectrum_out) fclose(spectrum_out);
+        return 1;
+    }
+    if (spectrum_out && fclose(spectrum_out) != 0) {
+        perror(spectrum_file.c_str());
         return 1;
     }
     if (sample && fclose(sample) != 0) {

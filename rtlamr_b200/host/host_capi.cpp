@@ -45,9 +45,12 @@ struct erthost {
 // the gain of each stream is measured from the first min(len, ERTLV_WINDOW) samples of its first erthost_decode call.
 // channel_gain: k of the wide channel path (0 ... 14), -1 none, -2 measured like auto_scale (after it) from the same
 // samples (ertgpu_measure_channel).  signal: every message carries its signal report (protocol::Decoder::EnableSignal).
+// spectrum_log2 > 0: the input's spectrum in rows of spectrum_frames frames of 2^spectrum_log2 samples
+// (protocol::Decoder::EnableSpectrum; erthost_gpu_handle gives the handle ertgpu_fetch_spectrum takes).
 erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long long max_blocks, long long max_cands,
                      long long input_rate, int format, float scale, long long capture_freq, long long center_freq,
-                     int auto_scale, int channel_gain, int signal, char* errbuf, int errcap) {
+                     int auto_scale, int channel_gain, int signal, int spectrum_log2, long long spectrum_frames,
+                     char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;   // released only on success: a throwing NewParser / Allocate must not leak the handle
     try {
         protocol::RegisterStockParsers();
@@ -59,7 +62,7 @@ erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long
             h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
         }
         h->d.SetInput({input_rate, format, scale, capture_freq, center_freq, auto_scale != 0, channel_gain < 0 ? -1 : channel_gain,
-                       channel_gain == -2, signal != 0});
+                       channel_gain == -2, signal != 0, spectrum_log2, spectrum_frames});
         h->d.Allocate(device, max_blocks, max_cands);
         return h.release();
     } catch (const std::exception& e) {
@@ -99,6 +102,8 @@ int erthost_config(const erthost* h, int32_t* out12) {
     memcpy(out12, v, sizeof(v));
     return 0;
 }
+
+ertgpu_handle* erthost_gpu_handle(erthost* h) { return h->d.Handle(); }
 
 int erthost_reset(erthost* h) {
     try {

@@ -607,6 +607,29 @@ void Decoder::EnableSignal() {
     signal_ = true;
 }
 
+void Decoder::EnableSpectrum(int32_t log2_n, int64_t frames_per_row) {
+    if (allocated_) throw std::logic_error("EnableSpectrum after Allocate");
+    const int rc = ertgpu_enable_spectrum(h_, log2_n, frames_per_row);
+    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
+    if (rc != ERTGPU_OK) raise(h_, rc, "EnableSpectrum");
+    spectrum_n_ = 1 << log2_n;
+}
+
+SpectrumRows Decoder::FetchSpectrum(bool partial) {
+    SpectrumRows r;
+    r.N = spectrum_n_;
+    size_t n = 0;
+    int rc = ertgpu_fetch_spectrum(h_, partial, nullptr, nullptr, nullptr, 0, &n);
+    if (rc != ERTGPU_OK && rc != ERTGPU_ECAPACITY) raise(h_, rc, "FetchSpectrum");
+    if (n == 0) return r;
+    r.rows.resize(n);
+    r.mean.resize(n * (size_t)r.N);
+    r.peak.resize(n * (size_t)r.N);
+    rc = ertgpu_fetch_spectrum(h_, partial, r.rows.data(), r.mean.data(), r.peak.data(), n, &n);
+    if (rc != ERTGPU_OK) raise(h_, rc, "FetchSpectrum");
+    return r;
+}
+
 const ertgpu_signal* Decoder::FetchSignal(size_t n) {
     if (!signal_) return nullptr;
     sigs_.resize(std::max<size_t>(n, 1));
@@ -646,6 +669,7 @@ void Decoder::SetInput(const Input& in) {
     }
     auto_channel_gain_ = in.AutoChannelGain;
     if (in.Signal) EnableSignal();
+    if (in.SpectrumLog2) EnableSpectrum(in.SpectrumLog2, in.SpectrumFrames);
 }
 
 ertgpu_channel_level Decoder::MeasureChannel(const uint8_t* samples, size_t len) {

@@ -163,6 +163,16 @@ struct Input {
     int32_t ChannelGain = -1;
     bool AutoChannelGain = false;
     bool Signal = false;  // per-packet signal reports (Decoder::EnableSignal)
+    // The input's spectrum in rows of SpectrumFrames frames of 2^SpectrumLog2 samples (Decoder::EnableSpectrum); 0: none.
+    int32_t SpectrumLog2 = 0;
+    int64_t SpectrumFrames = 0;
+};
+
+// Rows of a Decoder's input spectrum (ertgpu_fetch_spectrum): rows[i] with mean and peak [i * N, (i+1) * N) by bin.
+struct SpectrumRows {
+    int32_t N = 0;
+    std::vector<ertgpu_spectrum_row> rows;
+    std::vector<float> mean, peak;
 };
 
 // decode.go:45-63.  Signal/Quantized are not materialised on the host: the parity taps of the C ABI
@@ -220,6 +230,11 @@ public:
     // sigs: the candidates' signal records (ertgpu_fetch_signal), or nullptr.  Each message then gets the report of the
     // candidate it was parsed from, found by (block, preamble, idx).
     void Dispatch(const ertgpu_candidate* cands, size_t n, std::vector<MessagePtr>& out, const ertgpu_signal* sigs = nullptr);
+    // ertgpu_enable_spectrum, before Allocate.
+    void EnableSpectrum(int32_t log2_n, int64_t frames_per_row);
+    bool SpectrumEnabled() const { return spectrum_n_ != 0; }
+    // ertgpu_fetch_spectrum: the rows completed since the last fetch and, with partial, the open row (not consumed).
+    SpectrumRows FetchSpectrum(bool partial = false);
     std::string Log() const;  // decode.go:73-90
     void Reset();
     ertgpu_handle* Handle() const { return h_; }
@@ -232,6 +247,7 @@ private:
     std::vector<ertgpu_candidate> cands_;
     std::vector<ertgpu_signal> sigs_;
     bool signal_ = false;
+    int32_t spectrum_n_ = 0;
     int64_t signal_channel_ = 0, signal_rate_ = 0;
     const ertgpu_signal* FetchSignal(size_t n);   // the last call's records (nullptr without reports)
     bool allocated_ = false;

@@ -33,6 +33,7 @@ Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int6
             if (!name.empty()) d.RegisterProtocol(protocol::NewParser(name, chipLength));  // main.go:77-82
         protocol::Input in = input;
         if (!channels.empty()) in.CenterFreq = channels[c];
+        if (c > 0) in.SpectrumLog2 = 0;   // one spectrum of the capture, on channel 0
         d.SetInput(in);
         d.Allocate(device, blocksPerCall, 0);  // main.go:86
     }
@@ -211,7 +212,7 @@ void Receiver::KeepHistory(const uint8_t* call, size_t nblocks) {
 }
 
 Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&, int64_t, int)>& emit,
-                    int64_t max_bytes) {
+                    int64_t max_bytes, const std::function<void(const protocol::SpectrumRows&)>& rows) {
     Stats st;
     protocol::Decoder& d0 = *d_[0];
     st.channel_messages.assign(d_.size(), 0);
@@ -222,6 +223,12 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
     size_t q = 0;
     for (auto& d : d_) q = std::max(q, d->InputQuantum());
     if (q != bs2 && sample_file_) throw std::logic_error("-samplefile with converted or resampled input");
+    const bool spectrum = d0.SpectrumEnabled() && rows;
+    const auto spectrum_rows = [&](bool partial) {
+        if (!spectrum) return;
+        const protocol::SpectrumRows r = d0.FetchSpectrum(partial);
+        if (!r.rows.empty()) rows(r);
+    };
     std::vector<protocol::Decoder*> ds;
     for (auto& d : d_) ds.push_back(d.get());
     uint64_t left = max_bytes < 0 ? UINT64_MAX : (uint64_t)max_bytes;
@@ -326,6 +333,7 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
             st.bytes += (int64_t)whole;   // input bytes: s per input sample
             st.samples += (int64_t)(whole / s);
             stream_blocks_ += nblocks;
+            spectrum_rows(false);
             int64_t ready = INT64_MAX;
             for (size_t c = 0; c < per.size(); c++) {
                 for (auto& m : per[c]) held[c].push_back(std::move(m));
@@ -341,6 +349,7 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
         if (eof) break;  // EOF: the trailing partial block is dropped like main.go does
     }
     report(INT64_MAX);   // the blocks a lagging channel never completes, or those read before the deadline
+    spectrum_rows(true);
     st.seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     return st;
 }

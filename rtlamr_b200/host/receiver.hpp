@@ -115,9 +115,11 @@ public:
     // Run over a FILE* until EOF, -single or the deadline.  With Input::AutoScale the stream's gain is set from its first
     // min(stream, ERTLV_WINDOW) samples (include/ertgpu_level.h) before anything is decoded; it stays for the stream.  `emit` is called once per reported message (after the
     // cross-block dedup when block_dedup) with its LogMessage Offset and Length (0 without a sample file).  max_bytes >= 0
-    // stops reading after that many bytes (the data chunk of a WAV file).
+    // stops reading after that many bytes (the data chunk of a WAV file).  With a spectrum (Input::SpectrumLog2; with
+    // several channels, channel 0's handle measures the capture once) `rows` sees the rows each decode call completed,
+    // after the call, and at the end of the stream the open row when it has at least one frame.
     Stats Run(FILE* in, bool block_dedup, const std::function<void(const protocol::Message&, int64_t, int)>& emit,
-              int64_t max_bytes = -1);
+              int64_t max_bytes = -1, const std::function<void(const protocol::SpectrumRows&)>& rows = {});
 
     // Start a new, independent stream (the next file of a batch): zeroed Decoder history (decode.go:144-145),
     // block numbers restart at 0, empty dedup set, empty sampleBuf.
