@@ -72,6 +72,66 @@ struct DecodePos {
     bool started = false;       // a decode call was accepted (ertgpu_set_input_scale)
 };
 
+// What is enqueued and not yet read back.
+struct InFlight {
+    cudaStream_t stream = nullptr;    // work is enqueued on it and not yet synchronised (null: none)
+    bool counts = false;              // ... and it copies counters back (a resample_kernel launch alone does not)
+    unsigned long long uncopied = 0;  // candidates of a synchronised pipeline still only on the device
+};
+
+// What the last enqueued pipeline read (ertgpu_tap).
+struct LastPipeline {
+    const uint8_t* iq = nullptr;
+    const uint8_t* hist = nullptr;
+    int hist_valid = 0;
+    const uint32_t* plane = nullptr;  // null: no pipeline yet
+    int64_t first_block = 0, nblocks = 0;
+};
+
+// The results of the current decode call.
+struct CallResults {
+    std::vector<ertgpu_candidate> cands;
+    std::vector<ertgpu_signal> sigs;  // cands' records, in the same order (signal reports only)
+    bool overflow = false;            // a pipeline found more hits than the handle holds ...
+    unsigned long long need = 0;      // ... the most it found
+    int64_t hits = 0, valid = 0;      // ertgpu_last_counts
+    // Empty, with the vectors' capacity kept: a call does not grow them again.
+    void clear() {
+        cands.clear();
+        sigs.clear();
+        *this = {std::move(cands), std::move(sigs)};
+    }
+};
+
+// Stage timing: a pool of event sets so that nothing has to be read back between steps; the elapsed times of finished
+// pipelines are folded into the sums when the pool is full or when somebody asks.
+struct StageTiming {
+    static constexpr int kSets = 64;
+    bool on = false;     // ertgpu_set_stage_timing
+    bool valid = false;  // the last pipeline recorded sets[last]
+    Event sets[kSets][5];
+    int last = 0;        // the set of the last enqueued pipeline
+    int next = 0;        // set the next pipeline will use
+    int unread = 0;      // finished or pending sets not yet folded (the last `unread` sets)
+    double sum[4] = {};  // accumulated since ertgpu_set_stage_timing(1)
+    int64_t n = 0;
+
+    // Fold the sets of finished pipelines into the sums (only called with no pipeline pending).
+    void fold() {
+        for (int i = unread; i > 0; i--) {
+            const Event* set = sets[(next - i + 2 * kSets) % kSets];
+            float ms[4];
+            bool ok = true;
+            for (int k = 0; k < 4; k++) ok = ok && cudaEventElapsedTime(&ms[k], set[k], set[k + 1]) == cudaSuccess;
+            if (ok) {
+                for (int k = 0; k < 4; k++) sum[k] += ms[k];
+                n++;
+            }
+        }
+        unread = 0;
+    }
+};
+
 struct ertgpu_handle {
     std::string err;
     std::vector<ertgpu_protocol> protos;
@@ -81,39 +141,40 @@ struct ertgpu_handle {
 
     DevCfg dcfg{};
     Gf32 gf{};
-    float h_lut[256];
 
-    cudaStream_t stream = nullptr, copy_stream = nullptr;
-    cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
+    // The handle's CUDA resources but the input stage's, the spectrum's and the timing events: free_device clears them.
+    // The streams come last, so they are destroyed after the rest.
+    struct Device {
+        DeviceArray<float> lut;
+        DeviceArray<uint16_t> crc;
+        DeviceArray<uint32_t> plane[2];
+        DeviceArray<uint8_t> hist[2];
+        DeviceArray<uint8_t> stage[2];
+        size_t stage_bytes = 0;
+        PinnedArray<uint8_t> h_stage[2];  // pinned staging of pageable input (allocated on first use)
+        size_t h_stage_bytes = 0;
+        DeviceArray<RawHit> hits;
+        DeviceArray<HitWord> words;       // words of starts that hold a hit (what Slice works from)
+        DeviceArray<uint8_t> digits;
+        DeviceArray<int> block_slot;      // r900: scratch slot of each block of the call (-1 none)
+        DeviceArray<int> slot_block;
+        DeviceArray<unsigned int> slot_count;
+        DeviceArray<float> r900_scratch;  // [slot][r900_span] running sums
+        DeviceArray<ertgpu_candidate> out;
+        DeviceArray<ertgpu_signal> sig;
+        DeviceArray<unsigned long long> counters;  // kCntHits, kCntOut, kCntValid, kCntTile (demod work tiles), kCntWords
+        PinnedArray<unsigned long long> h_counters;  // pinned mirror
+        DeviceArray<float> tap;                    // scratch for taps
+        Event ev_h2d[2], ev_done[2];
+        Stream stream, copy_stream;
+    } dev;
 
-    float* d_lut = nullptr;
-    uint16_t* d_crc = nullptr;
-    uint32_t* d_plane[2] = {nullptr, nullptr};
-    size_t plane_words = 0;
-    uint8_t* d_hist[2] = {nullptr, nullptr};
-    uint8_t* d_stage[2] = {nullptr, nullptr};
-    size_t stage_bytes = 0;
-    uint8_t* h_stage[2] = {nullptr, nullptr};  // pinned staging of pageable input (allocated on first use)
-    size_t h_stage_bytes = 0;
     std::unique_ptr<CopyPool> copy_pool;   // host threads of the pageable-input staging
     std::string kernels;                        // instantiations launched by the last pipeline
-    RawHit* d_hits = nullptr;
-    HitWord* d_words = nullptr;       // words of starts that hold a hit (what Slice works from)
-    uint8_t* d_digits = nullptr;
-    int* d_block_slot = nullptr;      // r900: scratch slot of each block of the call (-1 none)
-    int* d_slot_block = nullptr;
-    unsigned int* d_slot_count = nullptr;
-    float* d_r900_scratch = nullptr;  // [slot][r900_span] running sums
     int r900_slots = 0, r900_span = 0;
-    ertgpu_candidate* d_out = nullptr;
     unsigned long long cand_cap = 0;
-    bool signal = false;              // ertgpu_enable_signal: a record per candidate in d_sig
-    ertgpu_signal* d_sig = nullptr;
+    bool signal = false;              // ertgpu_enable_signal: a record per candidate in dev.sig
     ertsig_geometry sig_geo{};
-    unsigned long long* d_counters = nullptr;  // kCntHits, kCntOut, kCntValid, kCntTile (demod work tiles), kCntWords
-    unsigned long long* h_counters = nullptr;  // pinned mirror
-    float* d_tap = nullptr;                    // scratch for taps
-    size_t tap_floats = 0;
 
     int64_t max_blocks = 0;
     DecodePos pos;
@@ -121,34 +182,11 @@ struct ertgpu_handle {
     int sm_count = 132;
     PipelineKernels pipe;
 
-    // state of the last enqueued pipeline (for fetch and taps)
-    bool pending = false;       // work is enqueued on pending_stream and not yet synchronised
-    bool pending_counts = false;  // ... and it copies counters back (a resample_kernel launch alone does not)
-    bool uncopied = false;      // a pipeline is synchronised, its candidates still only on the device
-    unsigned long long uncopied_n = 0;
-    cudaStream_t pending_stream = nullptr;
-    const uint8_t* last_iq = nullptr;
-    const uint8_t* last_hist = nullptr;
-    int last_hist_valid = 0;
-    const uint32_t* last_plane = nullptr;
-    int64_t last_first_block = 0, last_nblocks = 0;
-    bool overflow = false;
-    unsigned long long need = 0;
-    int64_t total_hits = 0, total_valid = 0;
+    InFlight fly;
+    LastPipeline last;
+    CallResults res;
     int64_t launches = 0;
-    bool stage_timing = false;
-    // stage timing: a pool of event sets so that nothing has to be read back between steps; the elapsed
-    // times of finished pipelines are folded into the sums when the pool is full or when somebody asks
-    static constexpr int kStageSets = 64;
-    cudaEvent_t ev_pool[kStageSets][5] = {};
-    cudaEvent_t* ev_stage = ev_pool[0];  // the set of the last enqueued pipeline
-    int stage_next = 0;                  // set the next pipeline will use
-    int stage_unread = 0;                // finished or pending sets not yet folded (the last stage_unread sets)
-    bool stage_valid = false;
-    double stage_sum[4] = {0, 0, 0, 0};  // accumulated since ertgpu_set_stage_timing(1)
-    int64_t stage_n = 0;
-    std::vector<ertgpu_candidate> results;
-    std::vector<ertgpu_signal> sig_results;  // results' records, in the same order
+    StageTiming timing;
 
     InputStage in{err};  // input format, rate and tuning, and the kernel in front of the pipeline
     Spectrum spec;       // ertgpu_enable_spectrum
@@ -234,63 +272,19 @@ int check_decodable(ertgpu_handle* h) {
 void free_device(ertgpu_handle* h) {
     if (!h->allocated) return;
     cudaSetDevice(h->device);
-    auto dfree = [](auto*& p) { if (p) cudaFree(p); p = nullptr; };
-    auto evfree = [](cudaEvent_t& e) { if (e) cudaEventDestroy(e); e = nullptr; };
-    for (int k = 0; k < 2; k++) {
-        dfree(h->d_plane[k]);
-        dfree(h->d_hist[k]);
-        dfree(h->d_stage[k]);
-        if (h->h_stage[k]) cudaFreeHost(h->h_stage[k]);
-        h->h_stage[k] = nullptr;
-        evfree(h->ev_h2d[k]);
-        evfree(h->ev_done[k]);
-    }
-    h->stage_bytes = h->h_stage_bytes = 0;
-    for (auto& set : h->ev_pool) for (int k = 0; k < 5; k++) evfree(set[k]);
-    dfree(h->d_lut);
-    dfree(h->d_crc);
-    dfree(h->d_hits);
-    dfree(h->d_words);
-    dfree(h->d_digits);
-    dfree(h->d_block_slot);
-    dfree(h->d_slot_block);
-    dfree(h->d_slot_count);
-    dfree(h->d_r900_scratch);
-    dfree(h->d_out);
-    dfree(h->d_sig);
-    dfree(h->d_counters);
-    dfree(h->d_tap);
-    h->in.release();
-    h->spec.release();
-    if (h->h_counters) cudaFreeHost(h->h_counters);
-    h->h_counters = nullptr;
-    if (h->stream) cudaStreamDestroy(h->stream);
-    if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-    h->stream = h->copy_stream = nullptr;
-    h->pending = h->uncopied = false;
-    h->last_plane = nullptr;
+    h->in.dev = {};
+    h->spec.dev = {};
+    h->timing = {};
+    h->dev = {};
+    h->fly = {};
+    h->last = {};
     h->allocated = false;
-}
-
-// Fold the event sets of finished pipelines into the running sums (only called with no pipeline pending).
-void fold_stage_times(ertgpu_handle* h) {
-    for (int i = h->stage_unread; i > 0; i--) {
-        cudaEvent_t* set = h->ev_pool[(h->stage_next - i + 2 * ertgpu_handle::kStageSets) % ertgpu_handle::kStageSets];
-        float ms[4];
-        bool ok = true;
-        for (int k = 0; k < 4; k++) ok = ok && cudaEventElapsedTime(&ms[k], set[k], set[k + 1]) == cudaSuccess;
-        if (ok) {
-            for (int k = 0; k < 4; k++) h->stage_sum[k] += ms[k];
-            h->stage_n++;
-        }
-    }
-    h->stage_unread = 0;
 }
 
 // Launch `kern` as a programmatic dependent of the kernel in front of it on the stream (its CTAs may become resident
 // while that kernel drains; the kernel itself calls pdl_wait() before it reads anything).  pdl == false: ordinary launch.
 template <class K, class... Args>
-cudaError_t launch_dep(bool pdl, K kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+cudaError_t launch_dep(bool pdl, K kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, const Args&... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
@@ -385,36 +379,38 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
     const int64_t nblocks = s.nblocks;
     const DevCfg& c = h->dcfg;
     DecodePos& pos = h->pos;
-    uint32_t* plane = h->d_plane[pos.cur_plane];
-    uint32_t* plane_next = h->d_plane[pos.cur_plane ^ 1];
-    const uint8_t* hist = h->d_hist[pos.cur_hist];
-    uint8_t* hist_next = h->d_hist[pos.cur_hist ^ 1];
+    uint32_t* plane = h->dev.plane[pos.cur_plane];
+    uint32_t* plane_next = h->dev.plane[pos.cur_plane ^ 1];
+    const uint8_t* hist = h->dev.hist[pos.cur_hist];
+    uint8_t* hist_next = h->dev.hist[pos.cur_hist ^ 1];
     const long long nwords = nblocks * c.words_per_block;
     const long long p0 = (long long)c.hist_words * 32 - c.PKL;
     h->launches = 0;
 
-    CUDA_TRY(h, cudaMemsetAsync(h->d_counters, 0, kCntN * sizeof(unsigned long long), st));
+    CUDA_TRY(h, cudaMemsetAsync(h->dev.counters, 0, kCntN * sizeof(unsigned long long), st));
     if (pos.fresh) {  // Quantized starts as zeros (decode.go:145); only the history in front of the call is read
         CUDA_TRY(h, cudaMemsetAsync(plane, 0, (size_t)c.hist_words * sizeof(uint32_t), st));
         pos.fresh = false;
     }
 
-    const bool tm = h->stage_timing;
+    StageTiming& t = h->timing;
+    const bool tm = t.on;
     const bool pdl = !tm;   // events recorded between the kernels would sit between primary and dependent
     if (tm) {
-        if (h->stage_unread == ertgpu_handle::kStageSets) fold_stage_times(h);  // every earlier pipeline has been waited for
-        h->ev_stage = h->ev_pool[h->stage_next];
-        h->stage_next = (h->stage_next + 1) % ertgpu_handle::kStageSets;
-        h->stage_unread++;
+        if (t.unread == StageTiming::kSets) t.fold();  // every earlier pipeline has been waited for
+        t.last = t.next;
+        t.next = (t.next + 1) % StageTiming::kSets;
+        t.unread++;
     }
-    if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[0], st));
+    const Event* ev = t.sets[t.last];
+    if (tm) CUDA_TRY(h, cudaEventRecord(ev[0], st));
     if (const int rc = h->in.launch(s, st, &h->launches)) return rc;
     // 1. magnitude + matched filter + quantize + pack
     PipelineKernels& k = h->pipe;
     if (k.demod_variant != 0) {
         int w_used = 0;
-        const cudaError_t e = launch_demod_fast(k.fast, h->sm_count, d_iq, hist, c.hist_samples, pos.hist_valid, h->d_lut,
-                                                plane + c.hist_words, nblocks, c.BS, h->d_counters + kCntTile, st, &w_used);
+        const cudaError_t e = launch_demod_fast(k.fast, h->sm_count, d_iq, hist, c.hist_samples, pos.hist_valid, h->dev.lut,
+                                                plane + c.hist_words, nblocks, c.BS, h->dev.counters + kCntTile, st, &w_used);
         if (e != cudaSuccess) return fail(h, ERTGPU_ECUDA, "demod_fast launch failed: %s", cudaGetErrorString(e));
         h->kernels = "demod_fast_kernel<" + std::to_string(k.demod_variant) + "," + std::to_string(w_used) + ">";
     } else {
@@ -422,11 +418,11 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
         if (k.generic_smem > 227 * 1024) return fail(h, ERTGPU_EINVAL, "chip length %d too large for the generic kernel", c.CL);
         const unsigned grid = (unsigned)((nblocks + k.generic_threads - 1) / k.generic_threads);
         demod_generic_kernel<<<grid, k.generic_threads, k.generic_smem, st>>>(d_iq, hist, c.hist_samples, pos.hist_valid,
-                                                                             h->d_lut, plane + c.hist_words, nblocks, c.BS, c.CL);
+                                                                             h->dev.lut, plane + c.hist_words, nblocks, c.BS, c.CL);
         CUDA_TRY(h, cudaGetLastError());
     }
     h->launches++;
-    if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[1], st));
+    if (tm) CUDA_TRY(h, cudaEventRecord(ev[1], st));
 
     // 2. preamble search over every start position of the call: the sliding-window kernel where the geometry fits
     //    it, search_generic_kernel for every other geometry
@@ -436,35 +432,35 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
         const long long tiles = (nwords + sl.tile_words - 1) / sl.tile_words;
         const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(tiles, k.slide_cap));
         CUDA_TRY(h, launch_dep(pdl, k.slide, dim3(grid), dim3(kSlideThreads), (size_t)k.slide_smem, st, (const uint32_t*)plane, sl,
-                               h->d_hits, h->d_words, h->cand_cap, h->d_counters));
+                               h->dev.hits, h->dev.words, h->cand_cap, h->dev.counters));
     } else {
         const int nthr = 256;
         const long long blocks = std::max(1ll, std::min<long long>((nwords + nthr - 1) / nthr, (long long)h->sm_count * 16));
         CUDA_TRY(h, launch_dep(pdl, search_generic_kernel, dim3((unsigned)blocks), dim3(nthr), 0, st, (const uint32_t*)plane, p0, nwords, c,
-                               h->d_hits, h->d_words, h->cand_cap, h->d_counters));
+                               h->dev.hits, h->dev.words, h->cand_cap, h->dev.counters));
     }
     h->kernels += k.search_label;
     CUDA_TRY(h, cudaGetLastError());
     h->launches++;
 
-    if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[2], st));
+    if (tm) CUDA_TRY(h, cudaEventRecord(ev[2], st));
     // 3. r900 payload digits for hits of an r900 preamble
     const uint8_t* digits = nullptr;
     if (h->has_r900) {
-        CUDA_TRY(h, cudaMemsetAsync(h->d_block_slot, 0xFF, (size_t)nblocks * sizeof(int), st));
-        CUDA_TRY(h, cudaMemsetAsync(h->d_slot_count, 0, sizeof(unsigned int), st));
+        CUDA_TRY(h, cudaMemsetAsync(h->dev.block_slot, 0xFF, (size_t)nblocks * sizeof(int), st));
+        CUDA_TRY(h, cudaMemsetAsync(h->dev.slot_count, 0, sizeof(unsigned int), st));
         // the chain kernel loads 8 samples (16 bytes) at a time from chain starts (b + 1) * BS - BUF: without that
         // alignment no block gets a scratch slot and every r900 hit takes the exact per-candidate replay
         const int slots = k.r900_chain ? h->r900_slots : 0;
-        r900_mark_kernel<<<(unsigned)h->sm_count, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->d_slot_block,
-                                              slots, h->d_slot_count);
+        r900_mark_kernel<<<(unsigned)h->sm_count, 256, 0, st>>>(c, h->dev.hits, h->cand_cap, h->dev.counters, h->dev.block_slot, h->dev.slot_block,
+                                              slots, h->dev.slot_count);
         CUDA_TRY(h, cudaGetLastError());
         if (k.r900_chain) {   // producer warps + one consumer warp per 16 chains, hand-offs through shared memory
-            r900_chain2_kernel<<<(unsigned)h->sm_count * 2, (kChainProducers + 1) * 32, 0, st>>>(d_iq, hist, c.hist_samples, pos.hist_valid, c, h->d_slot_block,
-                                                        slots, h->d_slot_count, h->r900_span, h->d_r900_scratch);
+            r900_chain2_kernel<<<(unsigned)h->sm_count * 2, (kChainProducers + 1) * 32, 0, st>>>(d_iq, hist, c.hist_samples, pos.hist_valid, c, h->dev.slot_block,
+                                                        slots, h->dev.slot_count, h->r900_span, h->dev.r900_scratch);
             CUDA_TRY(h, cudaGetLastError());
-            r900_digits_kernel<<<(unsigned)h->sm_count * 16, 256, 0, st>>>(c, h->d_hits, h->cand_cap, h->d_counters, h->d_block_slot, h->r900_span,
-                                                        h->d_r900_scratch, h->d_digits);
+            r900_digits_kernel<<<(unsigned)h->sm_count * 16, 256, 0, st>>>(c, h->dev.hits, h->cand_cap, h->dev.counters, h->dev.block_slot, h->r900_span,
+                                                        h->dev.r900_scratch, h->dev.digits);
             CUDA_TRY(h, cudaGetLastError());
             h->launches += 2;
             h->kernels += ";r900_chain2_kernel";
@@ -472,11 +468,11 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
             h->kernels += ";r900_replay_kernel";
         }
         // blocks that found no scratch slot: exact per-candidate replay
-        r900_replay_kernel<<<(unsigned)h->sm_count, 64, 0, st>>>(d_iq, hist, c.hist_samples, pos.hist_valid, h->d_lut, c, h->d_hits,
-                                               h->cand_cap, h->d_counters, h->d_block_slot, h->d_digits, h->d_slot_count, slots);
+        r900_replay_kernel<<<(unsigned)h->sm_count, 64, 0, st>>>(d_iq, hist, c.hist_samples, pos.hist_valid, h->dev.lut, c, h->dev.hits,
+                                               h->cand_cap, h->dev.counters, h->dev.block_slot, h->dev.digits, h->dev.slot_count, slots);
         CUDA_TRY(h, cudaGetLastError());
         h->launches += 2;
-        digits = h->d_digits;
+        digits = h->dev.digits;
     }
 
     // 4. slice + integrity screens, one warp per word of starts with a hit; the same kernel carries the history to
@@ -489,8 +485,8 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
         const unsigned grid = (unsigned)h->sm_count * 4;
         const bool dep = pdl && !h->has_r900;   // the r900 kernels between Search and Slice are ordinary launches
         CUDA_TRY(h, launch_dep(dep, k.extract, dim3(grid), dim3(kExtractWarps * 32), 0, st, (const uint32_t*)plane, p0, c,
-                               (const HitWord*)h->d_words, h->cand_cap, (const uint16_t*)h->d_crc, h->gf, digits, (long long)pos.block_counter,
-                               flags, h->d_out, h->cand_cap, h->d_counters, ca));
+                               (const HitWord*)h->dev.words, h->cand_cap, (const uint16_t*)h->dev.crc, h->gf, digits, (long long)pos.block_counter,
+                               flags, h->dev.out, h->cand_cap, h->dev.counters, ca));
         CUDA_TRY(h, cudaGetLastError());
         h->launches++;
         h->kernels += k.extract_label;
@@ -500,26 +496,21 @@ int enqueue_pipeline(ertgpu_handle* h, const InputStep& s, uint32_t flags, cudaS
     //    event that frees its staging buffer; five CTAs per SM fill it at 48 registers, to hide the loads' latency
     if (h->signal) {
         packet_signal_kernel<<<(unsigned)h->sm_count * 5, kSignalWarps * 32, 0, st>>>(
-            d_iq, hist, c.hist_samples, pos.hist_valid, h->sig_geo, (long long)pos.block_counter, h->d_out, h->cand_cap,
-            h->d_counters, h->d_sig);
+            d_iq, hist, c.hist_samples, pos.hist_valid, h->sig_geo, (long long)pos.block_counter, h->dev.out, h->cand_cap,
+            h->dev.counters, h->dev.sig);
         CUDA_TRY(h, cudaGetLastError());
         h->launches++;
         h->kernels += ";packet_signal_kernel";
     }
 
-    if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[3], st));
-    if (tm) CUDA_TRY(h, cudaEventRecord(h->ev_stage[4], st));
-    h->stage_valid = tm;
-    CUDA_TRY(h, cudaMemcpyAsync(h->h_counters, h->d_counters, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    if (tm) CUDA_TRY(h, cudaEventRecord(ev[3], st));
+    if (tm) CUDA_TRY(h, cudaEventRecord(ev[4], st));
+    t.valid = tm;
+    CUDA_TRY(h, cudaMemcpyAsync(h->dev.h_counters, h->dev.counters, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
 
-    h->last_iq = d_iq;
-    h->last_hist = hist;
-    h->last_hist_valid = pos.hist_valid;
-    h->last_plane = plane;
-    h->last_first_block = pos.block_counter;
-    h->last_nblocks = nblocks;
-    h->pending = h->pending_counts = true;
-    h->pending_stream = st;
+    h->last = {d_iq, hist, pos.hist_valid, plane, pos.block_counter, nblocks};
+    h->fly.stream = st;
+    h->fly.counts = true;
 
     pos.cur_plane ^= 1;
     pos.cur_hist ^= 1;
@@ -537,77 +528,77 @@ bool cand_less(const ertgpu_candidate& a, const ertgpu_candidate& b) {
 // Wait for the pending work and read the counters of its pipeline (candidates stay on the device).  A resample_kernel
 // launch alone is waited for too: it read the caller's input and wrote the resampler state the next call reads.
 int collect_sync(ertgpu_handle* h) {
-    if (!h->pending) return ERTGPU_OK;
-    CUDA_TRY(h, cudaStreamSynchronize(h->pending_stream));
-    h->pending = false;
-    if (!h->pending_counts) return ERTGPU_OK;
-    const unsigned long long nh = h->h_counters[0], no = h->h_counters[1], nv = h->h_counters[2];
-    h->total_hits += (int64_t)nh;
-    h->total_valid += (int64_t)nv;
+    if (!h->fly.stream) return ERTGPU_OK;
+    CUDA_TRY(h, cudaStreamSynchronize(h->fly.stream));
+    h->fly.stream = nullptr;
+    if (!h->fly.counts) return ERTGPU_OK;
+    const unsigned long long nh = h->dev.h_counters[0], no = h->dev.h_counters[1], nv = h->dev.h_counters[2];
+    CallResults& r = h->res;
+    r.hits += (int64_t)nh;
+    r.valid += (int64_t)nv;
     if (nh > h->cand_cap) {
-        h->overflow = true;
-        h->need = std::max(h->need, nh);
+        r.overflow = true;
+        r.need = std::max(r.need, nh);
     }
-    h->uncopied_n = std::min(no, h->cand_cap);
-    h->uncopied = h->uncopied_n > 0;
-    return ERTGPU_OK;  // stage times are folded lazily (fold_stage_times)
+    h->fly.uncopied = std::min(no, h->cand_cap);
+    return ERTGPU_OK;  // stage times are folded lazily (StageTiming::fold)
 }
 
-// ... and append its candidates to h->results.
+// ... and append its candidates to h->res.
 int collect(ertgpu_handle* h) {
     int rc = collect_sync(h);
     if (rc) return rc;
-    if (h->uncopied) {
-        const size_t old = h->results.size();
-        h->results.resize(old + h->uncopied_n);
-        CUDA_TRY(h, cudaMemcpy(h->results.data() + old, h->d_out, h->uncopied_n * sizeof(ertgpu_candidate), cudaMemcpyDeviceToHost));
-        h->uncopied = false;
+    if (const unsigned long long n = h->fly.uncopied) {
+        std::vector<ertgpu_candidate>& res = h->res.cands;
+        const size_t old = res.size();
+        res.resize(old + n);
+        CUDA_TRY(h, cudaMemcpy(res.data() + old, h->dev.out, n * sizeof(ertgpu_candidate), cudaMemcpyDeviceToHost));
+        h->fly.uncopied = 0;
         // Slots are handed out by atomics, so a pipeline's records arrive unordered.  Pipelines of one
         // call cover ascending, disjoint block ranges: sorting each segment as it arrives (while the next
         // chunk's H2D copy is in flight) leaves the whole list in (block, preamble, idx) order.
         if (!h->signal) {
-            std::sort(h->results.begin() + (std::ptrdiff_t)old, h->results.end(), cand_less);
+            std::sort(res.begin() + (std::ptrdiff_t)old, res.end(), cand_less);
             return ERTGPU_OK;
         }
         // with reports, the signal records take the candidates' order (the key is unique per candidate)
-        std::vector<ertgpu_signal> sig(h->uncopied_n);
-        CUDA_TRY(h, cudaMemcpy(sig.data(), h->d_sig, sig.size() * sizeof(ertgpu_signal), cudaMemcpyDeviceToHost));
+        std::vector<ertgpu_signal> sig(n);
+        CUDA_TRY(h, cudaMemcpy(sig.data(), h->dev.sig, sig.size() * sizeof(ertgpu_signal), cudaMemcpyDeviceToHost));
         std::vector<uint32_t> order(sig.size());
         for (size_t i = 0; i < order.size(); i++) order[i] = (uint32_t)i;
-        const ertgpu_candidate* seg = h->results.data() + old;
+        const ertgpu_candidate* seg = res.data() + old;
         std::sort(order.begin(), order.end(), [seg](uint32_t a, uint32_t b) { return cand_less(seg[a], seg[b]); });
         const std::vector<ertgpu_candidate> cands(seg, seg + order.size());
         for (size_t i = 0; i < order.size(); i++) {
-            h->results[old + i] = cands[order[i]];
-            h->sig_results.push_back(sig[order[i]]);
+            res[old + i] = cands[order[i]];
+            h->res.sigs.push_back(sig[order[i]]);
         }
     }
     return ERTGPU_OK;
 }
 
-int deliver(ertgpu_handle* h, ertgpu_candidate* out, size_t cap, size_t* n_out) {
-    if (h->overflow) {
-        if (n_out) *n_out = (size_t)h->need;
+// The call's records v (candidates, or their signal reports: `what`) into out[0..cap), unless a pipeline found more hits
+// than the handle holds.
+template <class T>
+int deliver(ertgpu_handle* h, const std::vector<T>& v, T* out, size_t cap, size_t* n_out, const char* what) {
+    if (h->res.overflow) {
+        if (n_out) *n_out = (size_t)h->res.need;
         return fail(h, ERTGPU_ECAPACITY, "internal candidate capacity %llu exceeded (%llu hits): allocate with a larger max_candidates",
-                    h->cand_cap, h->need);
+                    h->cand_cap, h->res.need);
     }
-    if (n_out) *n_out = h->results.size();  // already sorted segment by segment in collect()
-    if (h->results.size() > cap) return fail(h, ERTGPU_ECAPACITY, "output array holds %zu candidates, %zu needed", cap, h->results.size());
-    if (!h->results.empty() && out) memcpy(out, h->results.data(), h->results.size() * sizeof(ertgpu_candidate));
+    if (n_out) *n_out = v.size();  // in order already (collect)
+    if (v.size() > cap) return fail(h, ERTGPU_ECAPACITY, "output array holds %zu %s, %zu needed", cap, what, v.size());
+    if (!v.empty() && out) memcpy(out, v.data(), v.size() * sizeof(T));
     return ERTGPU_OK;
 }
 
 // Device staging buffers of `bytes` each (kept when large enough) and, for pageable input, the pinned staging
 // buffers and the copy threads.
 int prepare_staging(ertgpu_handle* h, size_t bytes, const void* iq, bool* pageable) {
-    if (h->stage_bytes < bytes) {
-        for (int k = 0; k < 2; k++) {
-            cudaFree(h->d_stage[k]);
-            h->d_stage[k] = nullptr;
-        }
-        h->stage_bytes = 0;
-        for (int k = 0; k < 2; k++) CUDA_TRY(h, cudaMalloc(&h->d_stage[k], bytes));
-        h->stage_bytes = bytes;
+    if (h->dev.stage_bytes < bytes) {
+        h->dev.stage_bytes = 0;
+        for (int k = 0; k < 2; k++) CUDA_TRY(h, h->dev.stage[k].alloc(bytes));
+        h->dev.stage_bytes = bytes;
     }
     // Pinned (or registered / managed) input goes to the device directly.  Ordinary pageable memory -- a Go slice,
     // main.go:166's block buffer -- would make every cudaMemcpyAsync a synchronous driver-staged copy: it is staged
@@ -618,14 +609,10 @@ int prepare_staging(ertgpu_handle* h, size_t bytes, const void* iq, bool* pageab
         if (cudaPointerGetAttributes(&at, iq) == cudaSuccess) *pageable = at.type == cudaMemoryTypeUnregistered;
         else cudaGetLastError();
     }
-    if (*pageable && h->h_stage_bytes < h->stage_bytes) {
-        for (int k = 0; k < 2; k++) {
-            if (h->h_stage[k]) cudaFreeHost(h->h_stage[k]);
-            h->h_stage[k] = nullptr;
-        }
-        h->h_stage_bytes = 0;
-        for (int k = 0; k < 2; k++) CUDA_TRY(h, cudaHostAlloc(&h->h_stage[k], h->stage_bytes, cudaHostAllocDefault));
-        h->h_stage_bytes = h->stage_bytes;
+    if (*pageable && h->dev.h_stage_bytes < h->dev.stage_bytes) {
+        h->dev.h_stage_bytes = 0;
+        for (int k = 0; k < 2; k++) CUDA_TRY(h, h->dev.h_stage[k].alloc(h->dev.stage_bytes));
+        h->dev.h_stage_bytes = h->dev.stage_bytes;
     }
     if (*pageable) {
         int copy_threads = (int)std::min(8u, std::max(1u, std::thread::hardware_concurrency() / 4));  // ~6 GB/s per memcpy stream; 8 fill a PCIe 5 x16 link
@@ -636,12 +623,12 @@ int prepare_staging(ertgpu_handle* h, size_t bytes, const void* iq, bool* pageab
 }
 
 // Stream `total` host samples of s bytes at src through h's two staging slots, chunk i into slot k = i & 1: it is copied
-// to d_stage[k] on h->copy_stream (through h_stage[k] when the input is pageable), and its work is enqueued on h->stream
+// to dev.stage[k] on dev.copy_stream (through dev.h_stage[k] when the input is pageable), and its work is enqueued on dev.stream
 // behind that copy, so that the copy of chunk i + 1 overlaps chunk i's kernels.  The callbacks:
 //   next(left)        the samples of the next chunk when `left` remain; 0 ends the call with ERTGPU_EINVAL, the
 //                     message already in place;
 //   between()         before the work of every chunk but the first (collect the previous one's);
-//   enqueue(d_in, n)  enqueue the work on the n samples at d_in on h->stream.
+//   enqueue(d_in, n)  enqueue the work on the n samples at d_in on dev.stream.
 // Staging buffers of `bytes` each (prepare_staging).
 template <class Next, class Between, class Enqueue>
 int upload(ertgpu_handle* h, const void* src, int64_t total, size_t s, size_t bytes, Next next, Between between,
@@ -655,19 +642,19 @@ int upload(ertgpu_handle* h, const void* src, int64_t total, size_t s, size_t by
         const int k = (int)(i & 1);
         const int64_t c = next(total - done);
         if (c <= 0) return ERTGPU_EINVAL;
-        if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->ev_done[k]));  // the kernels that read d_stage[k] (and its H2D) are done
+        if (i >= 2) CUDA_TRY(h, cudaEventSynchronize(h->dev.ev_done[k]));  // the kernels that read dev.stage[k] (and its H2D) are done
         const uint8_t* p = src0 + (size_t)done * s;
         if (pageable) {
-            h->copy_pool->copy(h->h_stage[k], p, (size_t)c * s);
-            p = h->h_stage[k];
+            h->copy_pool->copy(h->dev.h_stage[k], p, (size_t)c * s);
+            p = h->dev.h_stage[k];
         }
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_stage[k], p, (size_t)c * s, cudaMemcpyHostToDevice, h->copy_stream));
-        CUDA_TRY(h, cudaEventRecord(h->ev_h2d[k], h->copy_stream));
+        CUDA_TRY(h, cudaMemcpyAsync(h->dev.stage[k], p, (size_t)c * s, cudaMemcpyHostToDevice, h->dev.copy_stream));
+        CUDA_TRY(h, cudaEventRecord(h->dev.ev_h2d[k], h->dev.copy_stream));
         if (i >= 1)
             if (const int rc = between()) return rc;
-        CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[k], 0));
-        if (const int rc = enqueue(h->d_stage[k], c)) return rc;
-        CUDA_TRY(h, cudaEventRecord(h->ev_done[k], h->stream));
+        CUDA_TRY(h, cudaStreamWaitEvent(h->dev.stream, h->dev.ev_h2d[k], 0));
+        if (const int rc = enqueue(h->dev.stage[k], c)) return rc;
+        CUDA_TRY(h, cudaEventRecord(h->dev.ev_done[k], h->dev.stream));
         done += c;
     }
     return ERTGPU_OK;
@@ -675,9 +662,8 @@ int upload(ertgpu_handle* h, const void* src, int64_t total, size_t s, size_t by
 
 // Only an input stage launch is pending on st: it is waited for like a pipeline, with no counters to read.
 void stage_pending(ertgpu_handle* h, cudaStream_t st) {
-    h->pending = true;
-    h->pending_counts = false;
-    h->pending_stream = st;
+    h->fly.stream = st;
+    h->fly.counts = false;
 }
 
 // Enqueue spectrum_kernel over the n input samples at d_in on st, last in the step: it reads the staging buffer too.
@@ -686,7 +672,7 @@ int launch_spectrum(ertgpu_handle* h, const uint8_t* d_in, int64_t n, cudaStream
     const std::string lab = ";" + h->spec.label;
     if (h->kernels.size() < lab.size() || h->kernels.compare(h->kernels.size() - lab.size(), lab.size(), lab) != 0)
         h->kernels += lab;  // a step without a pipeline keeps the last pipeline's list, which names it already
-    if (!h->pending) stage_pending(h, st);
+    if (!h->fly.stream) stage_pending(h, st);
     return ERTGPU_OK;
 }
 
@@ -729,17 +715,13 @@ int enqueue_channels(ertgpu_handle* const* hs, int n, const uint8_t* d_in, int64
         if (const int rc = run_step(hs[k], steps[k], flags, st, d_in, cnt)) return rc;
     ertgpu_handle* h = hs[0];
     h->launches += shared;
-    if (shared && !h->pending) stage_pending(h, st);  // the shared launch wrote every channel's history
+    if (shared && !h->fly.stream) stage_pending(h, st);  // the shared launch wrote every channel's history
     return ERTGPU_OK;
 }
 
 void begin_call(ertgpu_handle* h) {
-    h->results.clear();
-    h->sig_results.clear();
-    h->uncopied = false;
-    h->overflow = false;
-    h->need = 0;
-    h->total_hits = h->total_valid = 0;
+    h->res.clear();
+    h->fly.uncopied = 0;
 }
 
 // The start of both decode calls.  The input is checked by the input stage's rules before anything is collected, so
@@ -764,7 +746,7 @@ int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
     if (const int rc = check_decode(h, iq, nbytes, device)) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
     h->pos.started = true;
-    if (h->pending) {
+    if (h->fly.stream) {
         int rc = collect(h);
         if (rc) return rc;
     }
@@ -1015,20 +997,18 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     h->cand_cap = (unsigned long long)max_candidates;
     h->allocated = true;  // from here free_device() cleans up on failure
 
-    CUDA_TRY(h, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    CUDA_TRY(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
+    CUDA_TRY(h, h->dev.stream.create(cudaStreamNonBlocking));
+    CUDA_TRY(h, h->dev.copy_stream.create(cudaStreamNonBlocking));
     for (int k = 0; k < 2; k++) {
-        CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_h2d[k], cudaEventDisableTiming));
-        CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_done[k], cudaEventDisableTiming));
+        CUDA_TRY(h, h->dev.ev_h2d[k].create(cudaEventDisableTiming));
+        CUDA_TRY(h, h->dev.ev_done[k].create(cudaEventDisableTiming));
     }
-    for (auto& set : h->ev_pool) for (int k = 0; k < 5; k++) CUDA_TRY(h, cudaEventCreate(&set[k]));
-    h->ev_stage = h->ev_pool[0];
-    make_maglut(h->h_lut);
+    for (auto& set : h->timing.sets) for (Event& e : set) CUDA_TRY(h, e.create(cudaEventDefault));
+    std::vector<float> lut(256);
+    make_maglut(lut.data());
     make_gf32(&h->gf);
-    CUDA_TRY(h, cudaMalloc(&h->d_lut, 256 * sizeof(float)));
-    CUDA_TRY(h, cudaMemcpy(h->d_lut, h->h_lut, 256 * sizeof(float), cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMalloc(&h->d_crc, tables.size() * sizeof(uint16_t)));
-    CUDA_TRY(h, cudaMemcpy(h->d_crc, tables.data(), tables.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, h->dev.lut.upload(lut));
+    CUDA_TRY(h, h->dev.crc.upload(tables));
 
     // Slack behind the largest call's words, for the Search kernels' reads past the call's last word:
     //  * search_slide_kernel's last tile starts at a word below nwords and loads load_words <= kSlideMaxLoad words;
@@ -1036,18 +1016,18 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
     //    one, w < nwords; with p0 + PKL = 32*hist_words the bits they use lie inside the call's words while k <= PK
     //    (the next word may be the first one behind them).  Rule R2 (check_decodable) keeps every preamble at most
     //    PK + 1 bits long, so no Search result depends on bits past the call's words.
-    h->plane_words = (size_t)d.hist_words + (size_t)max_blocks_per_call * d.words_per_block + kSlideMaxLoad + 8;
+    const size_t plane_words = (size_t)d.hist_words + (size_t)max_blocks_per_call * d.words_per_block + kSlideMaxLoad + 8;
     for (int k = 0; k < 2; k++) {
-        CUDA_TRY(h, cudaMalloc(&h->d_plane[k], h->plane_words * sizeof(uint32_t)));
-        CUDA_TRY(h, cudaMemset(h->d_plane[k], 0, h->plane_words * sizeof(uint32_t)));
-        CUDA_TRY(h, cudaMalloc(&h->d_hist[k], (size_t)d.hist_samples * 2 + 16));
-        CUDA_TRY(h, cudaMemset(h->d_hist[k], 0, (size_t)d.hist_samples * 2 + 16));
+        CUDA_TRY(h, h->dev.plane[k].alloc(plane_words));
+        CUDA_TRY(h, cudaMemset(h->dev.plane[k], 0, plane_words * sizeof(uint32_t)));
+        CUDA_TRY(h, h->dev.hist[k].alloc((size_t)d.hist_samples * 2 + 16));
+        CUDA_TRY(h, cudaMemset(h->dev.hist[k], 0, (size_t)d.hist_samples * 2 + 16));
     }
-    CUDA_TRY(h, cudaMalloc(&h->d_hits, h->cand_cap * sizeof(RawHit)));
-    CUDA_TRY(h, cudaMalloc(&h->d_words, h->cand_cap * sizeof(HitWord)));
-    CUDA_TRY(h, cudaMalloc(&h->d_out, h->cand_cap * sizeof(ertgpu_candidate)));
+    CUDA_TRY(h, h->dev.hits.alloc(h->cand_cap));
+    CUDA_TRY(h, h->dev.words.alloc(h->cand_cap));
+    CUDA_TRY(h, h->dev.out.alloc(h->cand_cap));
     if (h->signal) {
-        CUDA_TRY(h, cudaMalloc(&h->d_sig, h->cand_cap * sizeof(ertgpu_signal)));
+        CUDA_TRY(h, h->dev.sig.alloc(h->cand_cap));
         ertsig_geometry& g = h->sig_geo;
         g = {};
         g.CL = d.CL; g.SL = d.SL; g.BS = d.BS; g.BUF = d.BUF; g.PK = d.PK;
@@ -1059,7 +1039,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
         }
     }
     if (h->has_r900) {
-        CUDA_TRY(h, cudaMalloc(&h->d_digits, h->cand_cap * ERTGPU_R900_DIGITS));
+        CUDA_TRY(h, h->dev.digits.alloc(h->cand_cap * ERTGPU_R900_DIGITS));
         h->r900_span = d.BS + d.PL - d.SL + 4 * ERTGPU_R900_DIGITS * d.CL + 1;
         if (h->r900_span > d.BUF + 1) h->r900_span = d.BUF + 1;
         // scratch slots: one per block that holds an r900 hit.  Sized for one packet per 16 blocks
@@ -1071,25 +1051,24 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
             h->r900_slots = (int)std::max<int64_t>(1, std::min<int64_t>(want, max_blocks_per_call));
         }
         if (const char* e = getenv("ERTGPU_R900_SLOTS")) h->r900_slots = std::max(1, atoi(e));  // test hook: force the replay fallback
-        CUDA_TRY(h, cudaMalloc(&h->d_block_slot, (size_t)max_blocks_per_call * sizeof(int)));
-        CUDA_TRY(h, cudaMalloc(&h->d_slot_block, (size_t)h->r900_slots * sizeof(int)));
-        CUDA_TRY(h, cudaMalloc(&h->d_slot_count, sizeof(unsigned int)));
-        CUDA_TRY(h, cudaMalloc(&h->d_r900_scratch, (size_t)h->r900_slots * r900_pitch(h->r900_span) * sizeof(float) + 64));
+        CUDA_TRY(h, h->dev.block_slot.alloc((size_t)max_blocks_per_call));
+        CUDA_TRY(h, h->dev.slot_block.alloc((size_t)h->r900_slots));
+        CUDA_TRY(h, h->dev.slot_count.alloc(1));
+        CUDA_TRY(h, h->dev.r900_scratch.alloc((size_t)h->r900_slots * r900_pitch(h->r900_span) + 16));
     }
-    CUDA_TRY(h, cudaMalloc(&h->d_counters, kCntN * sizeof(unsigned long long)));
-    CUDA_TRY(h, cudaHostAlloc(&h->h_counters, kCntN * sizeof(unsigned long long), cudaHostAllocDefault));
-    h->tap_floats = (size_t)std::max(d.BS + d.SL, d.BUF) * 2 + 16;
-    CUDA_TRY(h, cudaMalloc(&h->d_tap, h->tap_floats * sizeof(float)));
+    CUDA_TRY(h, h->dev.counters.alloc(kCntN));
+    CUDA_TRY(h, h->dev.h_counters.alloc(kCntN));
+    CUDA_TRY(h, h->dev.tap.alloc((size_t)std::max(d.BS + d.SL, d.BUF) * 2 + 16));
 
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->device);
     if (h->sm_count < 1) h->sm_count = 132;
 
     h->pipe = {};
     // where the dynamic shared memory of a kernel starts on this device, through the tap scratch
-    smem_base_probe_kernel<<<1, 1, 1024, h->stream>>>(reinterpret_cast<uint32_t*>(h->d_tap));
+    smem_base_probe_kernel<<<1, 1, 1024, h->dev.stream>>>(reinterpret_cast<uint32_t*>(h->dev.tap.get()));
     CUDA_TRY(h, cudaGetLastError());
-    CUDA_TRY(h, cudaMemcpyAsync(&h->pipe.smem_base, h->d_tap, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(&h->pipe.smem_base, h->dev.tap, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->dev.stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->dev.stream));
     if (const int rc = choose_demod(h, demod_fast_variant(d.CL, d.BS, d.PKL))) return rc;
     if (const int rc = choose_search(h)) return rc;
     constexpr int kFullK = (ERTGPU_MAX_PACKET_BYTES * 8 + 31) / 32;
@@ -1124,7 +1103,6 @@ int ertgpu_reset(ertgpu_handle* h) {
     CUDA_TRY(h, cudaSetDevice(h->device));
     int rc = collect_sync(h);
     if (rc) return rc;
-    h->uncopied = false;
     h->pos = {};  // the history in front of the next call is zeroed on that call's stream (enqueue_pipeline)
     h->in.reset_stream();
     h->spec.pos = {};
@@ -1204,22 +1182,22 @@ int ertgpu_measure_channel(ertgpu_handle* h, const void* samples, size_t nbytes,
     if (nbytes % s) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of %zu-byte IQ samples", nbytes, s);
     CUDA_TRY(h, cudaSetDevice(h->device));
     if (const int rc = collect_sync(h)) return rc;  // the stream's own last step is done with the histories
-    CUDA_TRY(h, cudaMemsetAsync(h->in.d_clevel, 0, ERTRS_GAIN_BINS * sizeof(unsigned long long), h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->in.dev.clevel, 0, ERTRS_GAIN_BINS * sizeof(unsigned long long), h->dev.stream));
     int64_t outputs = 0, launches = 0;
     h->in.begin_measure();
     const int rc = upload(h, samples, (int64_t)(nbytes / s), s, (size_t)h->in.chunk() * s,
                           [&](int64_t left) { return h->in.next_chunk(left); }, [] { return ERTGPU_OK; },
                           [&](const uint8_t* d_in, int64_t c) {
                               InputStep st = h->in.plan(d_in, c);
-                              st.rs.level = h->in.d_clevel;
-                              if (const int rc = h->in.launch(st, h->stream, &launches)) return rc;
+                              st.rs.level = h->in.dev.clevel;
+                              if (const int rc = h->in.launch(st, h->dev.stream, &launches)) return rc;
                               outputs += st.rs.count;
                               h->in.commit(st);
                               return ERTGPU_OK;
                           });
     unsigned long long cnt[ERTRS_GAIN_BINS];
-    const cudaError_t e1 = cudaMemcpyAsync(cnt, h->in.d_clevel, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream);
-    const cudaError_t e2 = cudaStreamSynchronize(h->stream);
+    const cudaError_t e1 = cudaMemcpyAsync(cnt, h->in.dev.clevel, sizeof(cnt), cudaMemcpyDeviceToHost, h->dev.stream);
+    const cudaError_t e2 = cudaStreamSynchronize(h->dev.stream);
     h->in.end_measure();
     if (rc) return rc;
     CUDA_TRY(h, e1);
@@ -1243,16 +1221,16 @@ int ertgpu_measure_input(ertgpu_handle* h, const void* samples, size_t nbytes, e
     const size_t s = (size_t)h->in.sample_bytes;
     if (nbytes % s) return fail(h, ERTGPU_ESIZE, "nbytes %zu is not a whole number of %zu-byte IQ samples", nbytes, s);
     CUDA_TRY(h, cudaSetDevice(h->device));
-    CUDA_TRY(h, cudaMemsetAsync(h->in.d_level, 0, kLvCounters * sizeof(unsigned long long), h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->in.dev.level, 0, kLvCounters * sizeof(unsigned long long), h->dev.stream));
     const int64_t total = (int64_t)(nbytes / s);
     if (const int rc = upload(h, samples, total, s, (size_t)h->in.chunk() * s,
-                              [&](int64_t left) { return std::min((int64_t)(h->stage_bytes / s), left); },
+                              [&](int64_t left) { return std::min((int64_t)(h->dev.stage_bytes / s), left); },
                               [] { return ERTGPU_OK; },
-                              [&](const uint8_t* d_in, int64_t c) { return h->in.launch_level(d_in, c, h->stream); }))
+                              [&](const uint8_t* d_in, int64_t c) { return h->in.launch_level(d_in, c, h->dev.stream); }))
         return rc;
     unsigned long long cnt[kLvCounters];
-    CUDA_TRY(h, cudaMemcpyAsync(cnt, h->in.d_level, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(cnt, h->in.dev.level, sizeof(cnt), cudaMemcpyDeviceToHost, h->dev.stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->dev.stream));
     memset(out, 0, sizeof(*out));
     out->components = 2 * total;
     out->zeros = (int64_t)cnt[kLvZero];
@@ -1279,7 +1257,7 @@ int ertgpu_decode_device_async(ertgpu_handle* h, const void* d_iq, size_t nbytes
     const int rc = begin_decode(h, d_iq, nbytes, true);
     if (rc || nbytes == 0) return rc;
     return enqueue_step(h, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / h->in.sample_bytes), flags,
-                        stream ? (cudaStream_t)stream : h->stream);
+                        stream ? (cudaStream_t)stream : h->dev.stream);
 }
 
 int ertgpu_fetch(ertgpu_handle* h, ertgpu_candidate* out, size_t cap, size_t* n_out) {
@@ -1287,7 +1265,7 @@ int ertgpu_fetch(ertgpu_handle* h, ertgpu_candidate* out, size_t cap, size_t* n_
     CUDA_TRY(h, cudaSetDevice(h->device));
     int rc = collect(h);
     if (rc) return rc;
-    return deliver(h, out, cap, n_out);
+    return deliver(h, h->res.cands, out, cap, n_out, "candidates");
 }
 
 int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t flags, ertgpu_candidate* out,
@@ -1296,21 +1274,21 @@ int ertgpu_decode(ertgpu_handle* h, const uint8_t* iq, size_t nbytes, uint32_t f
     if (rc) return rc;
     const size_t s = (size_t)h->in.sample_bytes;
     const int64_t total = (int64_t)(nbytes / s);
-    if (total == 0) return deliver(h, out, cap, n_out);
+    if (total == 0) return deliver(h, h->res.cands, out, cap, n_out, "candidates");
     int64_t launches = 0;
     rc = upload(h, iq, total, s, (size_t)h->in.chunk() * s, [&](int64_t left) { return h->in.next_chunk(left); },
                 [&] { return collect(h); },
                 [&](const uint8_t* d_in, int64_t c) {
-                    if (const int rc = enqueue_step(h, d_in, c, flags, h->stream)) return rc;
+                    if (const int rc = enqueue_step(h, d_in, c, flags, h->dev.stream)) return rc;
                     launches += h->launches;
                     return ERTGPU_OK;
                 });
     if (rc) return rc;
     rc = collect(h);  // also waits for a last step that completed no block (ertgpu_decode is synchronous)
     if (rc) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));  // a step that launched nothing still copied from iq
+    CUDA_TRY(h, cudaStreamSynchronize(h->dev.copy_stream));  // a step that launched nothing still copied from iq
     h->launches = launches;
-    return deliver(h, out, cap, n_out);
+    return deliver(h, h->res.cands, out, cap, n_out, "candidates");
 }
 
 int ertgpu_decode_channels_device_async(ertgpu_handle* const* hs, int32_t n, const void* d_iq, size_t nbytes, uint32_t flags,
@@ -1320,7 +1298,7 @@ int ertgpu_decode_channels_device_async(ertgpu_handle* const* hs, int32_t n, con
         if (const int rc = begin_decode(hs[k], d_iq, nbytes, true)) return rc;
     if (nbytes == 0) return ERTGPU_OK;
     return enqueue_channels(hs, n, static_cast<const uint8_t*>(d_iq), (int64_t)(nbytes / hs[0]->in.sample_bytes), flags,
-                            stream ? (cudaStream_t)stream : hs[0]->stream);
+                            stream ? (cudaStream_t)stream : hs[0]->dev.stream);
 }
 
 // ertgpu_decode's loop over hs[0]'s staging buffers and streams, with every channel's step behind each chunk's copy.
@@ -1353,7 +1331,7 @@ int ertgpu_decode_channels(ertgpu_handle* const* hs, int32_t n, const uint8_t* i
         return ERTGPU_OK;
     };
     int rc = upload(h, iq, total, s, (size_t)chunk * s, next, collect_all, [&](const uint8_t* d_in, int64_t c) {
-        if (const int rc = enqueue_channels(hs, n, d_in, c, flags, h->stream)) return rc;
+        if (const int rc = enqueue_channels(hs, n, d_in, c, flags, h->dev.stream)) return rc;
         for (int j = 0; j < n; j++) launches[j] += hs[j]->launches;
         return ERTGPU_OK;
     });
@@ -1362,8 +1340,8 @@ int ertgpu_decode_channels(ertgpu_handle* const* hs, int32_t n, const uint8_t* i
         if ((rc = collect(hs[j]))) return rc;
         hs[j]->launches = launches[j];
     }
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->dev.stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->dev.copy_stream));
     return ERTGPU_OK;
 }
 
@@ -1379,15 +1357,7 @@ int ertgpu_fetch_signal(ertgpu_handle* h, ertgpu_signal* out, size_t cap, size_t
     if (!h->signal) return fail(h, ERTGPU_EINVAL, "fetch_signal: the handle was allocated without signal reports (ertgpu_enable_signal)");
     CUDA_TRY(h, cudaSetDevice(h->device));
     if (const int rc = collect(h)) return rc;
-    if (h->overflow) {
-        if (n_out) *n_out = (size_t)h->need;
-        return fail(h, ERTGPU_ECAPACITY, "internal candidate capacity %llu exceeded (%llu hits): allocate with a larger max_candidates",
-                    h->cand_cap, h->need);
-    }
-    if (n_out) *n_out = h->sig_results.size();
-    if (h->sig_results.size() > cap) return fail(h, ERTGPU_ECAPACITY, "output array holds %zu records, %zu needed", cap, h->sig_results.size());
-    if (!h->sig_results.empty() && out) memcpy(out, h->sig_results.data(), h->sig_results.size() * sizeof(ertgpu_signal));
-    return ERTGPU_OK;
+    return deliver(h, h->res.sigs, out, cap, n_out, "records");
 }
 
 int ertgpu_enable_spectrum(ertgpu_handle* h, int32_t log2_n, int64_t frames_per_row) {
@@ -1420,8 +1390,8 @@ int ertgpu_fetch_spectrum(ertgpu_handle* h, int32_t partial, ertgpu_spectrum_row
     const size_t N = (size_t)sp.N;
     for (int64_t r = first; r < done; r++) {
         const size_t i = (size_t)(r - first), slot = (size_t)(r % sp.row_cap);
-        CUDA_TRY(h, cudaMemcpy(mean + i * N, sp.d_mean + slot * N, N * sizeof(float), cudaMemcpyDeviceToHost));
-        CUDA_TRY(h, cudaMemcpy(peak + i * N, sp.d_peak + slot * N, N * sizeof(float), cudaMemcpyDeviceToHost));
+        CUDA_TRY(h, cudaMemcpy(mean + i * N, sp.dev.mean + slot * N, N * sizeof(float), cudaMemcpyDeviceToHost));
+        CUDA_TRY(h, cudaMemcpy(peak + i * N, sp.dev.peak + slot * N, N * sizeof(float), cudaMemcpyDeviceToHost));
         rows[i].first_sample = r * sp.F * sp.N;
         rows[i].frames = sp.F;
     }
@@ -1438,13 +1408,13 @@ int ertgpu_fetch_spectrum(ertgpu_handle* h, int32_t partial, ertgpu_spectrum_row
 
 int ertgpu_last_counts(ertgpu_handle* h, int64_t* n_candidates, int64_t* n_valid) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
-    if (h->pending) {
+    if (h->fly.stream) {
         CUDA_TRY(h, cudaSetDevice(h->device));
         int rc = collect_sync(h);  // counters only; ertgpu_fetch copies the candidates if wanted
         if (rc) return rc;
     }
-    if (n_candidates) *n_candidates = h->total_hits;
-    if (n_valid) *n_valid = h->total_valid;
+    if (n_candidates) *n_candidates = h->res.hits;
+    if (n_valid) *n_valid = h->res.valid;
     return ERTGPU_OK;
 }
 
@@ -1453,33 +1423,33 @@ int64_t ertgpu_last_launches(const ertgpu_handle* h) { return h ? h->launches : 
 int ertgpu_tap(ertgpu_handle* h, int32_t which, int64_t block, void* dst, size_t cap, size_t* n_out) {
     if (!h || !h->allocated) return ERTGPU_EINVAL;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    if (h->pending) {
+    if (h->fly.stream) {
         int rc = collect(h);
         if (rc) return rc;
     }
-    if (!h->last_plane) return fail(h, ERTGPU_EINVAL, "no decode call yet");
+    const LastPipeline& l = h->last;
+    if (!l.plane) return fail(h, ERTGPU_EINVAL, "no decode call yet");
     const DevCfg& c = h->dcfg;
-    const int64_t b = block - h->last_first_block;
-    if (b < 0 || b >= h->last_nblocks) return fail(h, ERTGPU_EINVAL, "block %lld outside the last (chunk of the) call [%lld,%lld)",
-                                                   (long long)block, (long long)h->last_first_block,
-                                                   (long long)(h->last_first_block + h->last_nblocks));
+    const int64_t b = block - l.first_block;
+    if (b < 0 || b >= l.nblocks) return fail(h, ERTGPU_EINVAL, "block %lld outside the last (chunk of the) call [%lld,%lld)",
+                                             (long long)block, (long long)l.first_block, (long long)(l.first_block + l.nblocks));
     std::vector<uint8_t> bytes;
     if (which == ERTGPU_TAP_SIGNAL || which == ERTGPU_TAP_CSUM) {
-        float* sig = h->d_tap;
-        float* cs = h->d_tap + (c.BS + c.SL);
-        tap_signal_csum_kernel<<<1, 32, 0, h->stream>>>(h->last_iq, h->last_hist, c.hist_samples, h->last_hist_valid, h->d_lut,
+        float* sig = h->dev.tap;
+        float* cs = h->dev.tap + (c.BS + c.SL);
+        tap_signal_csum_kernel<<<1, 32, 0, h->dev.stream>>>(l.iq, l.hist, c.hist_samples, l.hist_valid, h->dev.lut,
                                                         b, c.BS, c.SL, sig, cs);
         CUDA_TRY(h, cudaGetLastError());
         const size_t n = which == ERTGPU_TAP_SIGNAL ? (size_t)(c.BS + c.SL) : (size_t)(c.BS + c.SL + 1);
         bytes.resize(n * sizeof(float));
-        CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), which == ERTGPU_TAP_SIGNAL ? sig : cs, bytes.size(), cudaMemcpyDeviceToHost, h->stream));
-        CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+        CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), which == ERTGPU_TAP_SIGNAL ? sig : cs, bytes.size(), cudaMemcpyDeviceToHost, h->dev.stream));
+        CUDA_TRY(h, cudaStreamSynchronize(h->dev.stream));
     } else if (which == ERTGPU_TAP_QUANTIZED || which == ERTGPU_TAP_PACKED) {
         // Quantized after block b = stream bits [(b+1)*BS - BUF, (b+1)*BS)  (decode.go:166,172)
         const long long first_bit = (long long)c.hist_words * 32 + (b + 1) * c.BS - c.BUF;
         const long long w0 = first_bit >> 5, w1 = (first_bit + c.BUF + 31) >> 5;
         std::vector<uint32_t> words((size_t)(w1 - w0));
-        CUDA_TRY(h, cudaMemcpy(words.data(), h->last_plane + w0, words.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        CUDA_TRY(h, cudaMemcpy(words.data(), l.plane + w0, words.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
         std::vector<uint8_t> q((size_t)c.BUF);
         for (long long i = 0; i < c.BUF; i++) {
             const long long pos = first_bit + i - (w0 << 5);
@@ -1496,21 +1466,21 @@ int ertgpu_tap(ertgpu_handle* h, int32_t which, int64_t block, void* dst, size_t
             }
         }
     } else if (which == ERTGPU_TAP_R900_QUANTIZED) {
-        float* cs = h->d_tap;
-        uint8_t* qd = reinterpret_cast<uint8_t*>(h->d_tap + c.BUF + 4);
-        tap_r900_csum_kernel<<<1, 32, 0, h->stream>>>(h->last_iq, h->last_hist, c.hist_samples, h->last_hist_valid, h->d_lut, b,
+        float* cs = h->dev.tap;
+        uint8_t* qd = reinterpret_cast<uint8_t*>(h->dev.tap + c.BUF + 4);
+        tap_r900_csum_kernel<<<1, 32, 0, h->dev.stream>>>(l.iq, l.hist, c.hist_samples, l.hist_valid, h->dev.lut, b,
                                                       c.BS, c.BUF, cs);
         CUDA_TRY(h, cudaGetLastError());
-        tap_r900_digits_kernel<<<(c.BUF + 255) / 256, 256, 0, h->stream>>>(cs, c.BUF, c.CL, qd);
+        tap_r900_digits_kernel<<<(c.BUF + 255) / 256, 256, 0, h->dev.stream>>>(cs, c.BUF, c.CL, qd);
         CUDA_TRY(h, cudaGetLastError());
         bytes.resize((size_t)c.BUF);
-        CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), qd, bytes.size(), cudaMemcpyDeviceToHost, h->stream));
-        CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+        CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), qd, bytes.size(), cudaMemcpyDeviceToHost, h->dev.stream));
+        CUDA_TRY(h, cudaStreamSynchronize(h->dev.stream));
     } else if (which == ERTGPU_TAP_RESAMPLED) {
         if (h->in.mode == InputStage::kPass) return fail(h, ERTGPU_EINVAL, "the handle neither resamples nor converts its input");
         bytes.resize((size_t)c.BS * 2);
-        CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), h->last_iq + (size_t)b * c.BS * 2, bytes.size(), cudaMemcpyDeviceToHost, h->stream));
-        CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+        CUDA_TRY(h, cudaMemcpyAsync(bytes.data(), l.iq + (size_t)b * c.BS * 2, bytes.size(), cudaMemcpyDeviceToHost, h->dev.stream));
+        CUDA_TRY(h, cudaStreamSynchronize(h->dev.stream));
     } else {
         return fail(h, ERTGPU_EINVAL, "unknown tap %d", which);
     }
@@ -1524,11 +1494,12 @@ int ertgpu_set_stage_timing(ertgpu_handle* h, int32_t enable) {
     CUDA_TRY(h, cudaSetDevice(h->device));
     const int rc = collect_sync(h);
     if (rc) return rc;
-    h->stage_timing = enable != 0;
+    StageTiming& t = h->timing;
+    t.on = enable != 0;
     if (enable) {
-        for (int k = 0; k < 4; k++) h->stage_sum[k] = 0;
-        h->stage_n = 0;
-        h->stage_unread = 0;
+        for (int k = 0; k < 4; k++) t.sum[k] = 0;
+        t.n = 0;
+        t.unread = 0;
     }
     return ERTGPU_OK;
 }
@@ -1538,8 +1509,9 @@ int ertgpu_last_stage_ms(ertgpu_handle* h, float* ms4) {
     CUDA_TRY(h, cudaSetDevice(h->device));
     const int rc = collect_sync(h);
     if (rc) return rc;
-    if (!h->stage_valid) return fail(h, ERTGPU_EINVAL, "stage timing was not enabled for the last decode");
-    for (int k = 0; k < 4; k++) CUDA_TRY(h, cudaEventElapsedTime(&ms4[k], h->ev_stage[k], h->ev_stage[k + 1]));
+    const StageTiming& t = h->timing;
+    if (!t.valid) return fail(h, ERTGPU_EINVAL, "stage timing was not enabled for the last decode");
+    for (int k = 0; k < 4; k++) CUDA_TRY(h, cudaEventElapsedTime(&ms4[k], t.sets[t.last][k], t.sets[t.last][k + 1]));
     return ERTGPU_OK;
 }
 
@@ -1548,9 +1520,10 @@ int ertgpu_stage_ms_mean(ertgpu_handle* h, float* ms4, int64_t* n_pipelines) {
     CUDA_TRY(h, cudaSetDevice(h->device));
     const int rc = collect_sync(h);
     if (rc) return rc;
-    fold_stage_times(h);
-    for (int k = 0; k < 4; k++) ms4[k] = h->stage_n ? (float)(h->stage_sum[k] / (double)h->stage_n) : 0.0f;
-    if (n_pipelines) *n_pipelines = h->stage_n;
+    StageTiming& t = h->timing;
+    t.fold();
+    for (int k = 0; k < 4; k++) ms4[k] = t.n ? (float)(t.sum[k] / (double)t.n) : 0.0f;
+    if (n_pipelines) *n_pipelines = t.n;
     return ERTGPU_OK;
 }
 

@@ -14,49 +14,18 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
 #include <cstring>
 #include <string>
 #include <utility>
 #include <vector>
 
 #include "convert.cuh"
+#include "cuda_owned.hpp"
 #include "decimate.cuh"
 #include "level.cuh"
 #include "resample.cuh"
 
 namespace ert {
-
-// The message goes to err; returns code.
-inline int fail(std::string& err, int code, const char* fmt, ...) {
-    char buf[512];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof(buf), fmt, ap);
-    va_end(ap);
-    err = buf;
-    return code;
-}
-
-// `sink`: whatever fail() takes (a handle, an error string)
-#define CUDA_TRY(sink, expr)                                                                    \
-    do {                                                                                        \
-        cudaError_t e__ = (expr);                                                               \
-        if (e__ != cudaSuccess) {                                                               \
-            cudaGetLastError();                                                                 \
-            return fail(sink, e__ == cudaErrorMemoryAllocation ? ERTGPU_ENOMEM : ERTGPU_ECUDA,  \
-                        "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-        }                                                                                       \
-    } while (0)
-
-// A kernel whose launches request `bytes` of dynamic shared memory may take the whole 227 KiB of a CTA: set on each kernel
-// a handle may launch, when the handle is allocated.  `what` names the kernel when it needs more.
-inline int allow_dynamic_smem(std::string& err, const void* kernel, size_t bytes, const char* what) {
-    if (bytes > 227 * 1024) return fail(err, ERTGPU_EINVAL, "%s needs %zu B of shared memory", what, bytes);
-    CUDA_TRY(err, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    return ERTGPU_OK;
-}
 
 // One step of the stage: input samples at rs.cur on the device, and the whole uint8 blocks they complete.
 struct InputStep {
@@ -69,9 +38,9 @@ struct InputStep {
 
 struct InputStage {
     // kPass: uint8 IQ at the decoder's rate, read where the caller put it.  kConvert: another format at that rate,
-    // convert_kernel<F> into d_out[0].  kResample(Tuned): resample_kernel<F, false (true)> into d_out[cur_out]; the tuned
-    // instance runs for a tuned capture or a plan with P != ERTRS_P.  kDecimate: decimate_kernel<F> into d_mid, then
-    // resample_kernel<cu8, false> from d_mid into d_out[cur_out] (a tuned handle that allows decimation, above 10:1).
+    // convert_kernel<F> into dev.out[0].  kResample(Tuned): resample_kernel<F, false (true)> into dev.out[cur_out]; the tuned
+    // instance runs for a tuned capture or a plan with P != ERTRS_P.  kDecimate: decimate_kernel<F> into dev.mid, then
+    // resample_kernel<cu8, false> from dev.mid into dev.out[cur_out] (a tuned handle that allows decimation, above 10:1).
     enum Mode { kPass, kConvert, kResample, kResampleTuned, kDecimate };
 
     explicit InputStage(std::string& err) : err_(err) {}
@@ -100,12 +69,12 @@ struct InputStage {
     struct StreamPos {
         int64_t in_total = 0;   // input samples received since the stream start (the second stage's in kDecimate)
         int64_t out_next = 0;   // first output not yet computed
-        int64_t hist_first = 0, hist_n = 0;  // the input samples held in d_hist[cur_hist]
-        int64_t pend = 0;       // outputs at the front of d_out[cur_out] that wait for a whole block
+        int64_t hist_first = 0, hist_n = 0;  // the input samples held in dev.hist[cur_hist]
+        int64_t pend = 0;       // outputs at the front of dev.out[cur_out] that wait for a whole block
         int cur_hist = 0, cur_out = 0;
         // the first stage of kDecimate (its next output is the second stage's in_total)
         int64_t in1_total = 0;  // input samples received since the stream start
-        int64_t hist1_first = 0, hist1_n = 0;  // the input samples held in d_hist1[cur_hist1]
+        int64_t hist1_first = 0, hist1_n = 0;  // the input samples held in dev.hist1[cur_hist1]
         int cur_hist1 = 0;
     };
     StreamPos pos;
@@ -118,29 +87,32 @@ struct InputStage {
     decltype(&decimate_channels_kernel<ERTGPU_FORMAT_CU8>) channels_kernel = nullptr;  // kDecimate's, for launch_channels
 
     // device state
-    int32_t* d_A = nullptr;     // the table as the kernel reads it (rs_pack_table)
-    uint32_t* d_D = nullptr;
-    uint32_t* d_E = nullptr;    // the mixer table (ertrs_nco_table)
-    uint8_t* d_hist[2] = {nullptr, nullptr};  // input samples the next outputs still read
-    uint8_t* d_out[2] = {nullptr, nullptr};   // [partial block | new outputs]; the demod reads whole blocks of it
     size_t smem = 0;
     int grid = 0;               // most CTAs of one launch
-    unsigned long long* d_level = nullptr;  // level_kernel's kLvCounters counters (converted input only)
     int level_grid = 0;
-    // the first stage of kDecimate: its taps, input history and output (the second stage's input)
-    int16_t* d_taps = nullptr;
-    uint8_t* d_hist1[2] = {nullptr, nullptr};
-    uint8_t* d_mid = nullptr;
-    size_t smem1 = 0;
+    size_t smem1 = 0;           // the first stage of kDecimate
     int grid1 = 0, per1 = 0;
     size_t smem1c = 0;          // the same for decimate_channels_kernel
     int grid1c = 0, per1c = 0;
-    // the wide path's channel measurement: its own input histories and stream position, which begin_measure and
-    // end_measure swap with the stream's, and its counters
-    uint8_t* d_mhist[2] = {nullptr, nullptr};
-    uint8_t* d_mhist1[2] = {nullptr, nullptr};
-    StreamPos mpos;
-    unsigned long long* d_clevel = nullptr;
+    StreamPos mpos;             // the wide path's channel measurement (begin_measure)
+    // The stage's device tables and buffers: the handle clears them (= {}) when it releases its own.
+    struct Device {
+        DeviceArray<int32_t> A;     // the table as the kernel reads it (rs_pack_table)
+        DeviceArray<uint32_t> D;
+        DeviceArray<uint32_t> E;    // the mixer table (ertrs_nco_table)
+        DeviceArray<uint8_t> hist[2];  // input samples the next outputs still read
+        DeviceArray<uint8_t> out[2];   // [partial block | new outputs]; the demod reads whole blocks of it
+        DeviceArray<unsigned long long> level;  // level_kernel's kLvCounters counters (converted input only)
+        // the first stage of kDecimate: its taps, input history and output (the second stage's input)
+        DeviceArray<int16_t> taps;
+        DeviceArray<uint8_t> hist1[2];
+        DeviceArray<uint8_t> mid;
+        // the wide path's channel measurement: its own input histories (with mpos), which begin_measure and end_measure
+        // swap with the stream's, and its counters
+        DeviceArray<uint8_t> mhist[2];
+        DeviceArray<uint8_t> mhist1[2];
+        DeviceArray<unsigned long long> clevel;
+    } dev;
 
     bool resamples() const { return mode >= kResample; }
     // Input samples received since the stream start.
@@ -248,34 +220,31 @@ struct InputStage {
         max_blocks = max_blocks_per_step;
         reset_stream();
         if (fmt != ERTGPU_FORMAT_CU8) {
-            CUDA_TRY(err_, cudaMalloc(&d_level, kLvCounters * sizeof(unsigned long long)));
+            CUDA_TRY(err_, dev.level.alloc(kLvCounters));
             level_grid = sm_count * 4;
         }
         if (mode == kPass) return ERTGPU_OK;
         if (mode == kConvert) {
             grid = sm_count * 8;
-            CUDA_TRY(err_, cudaMalloc(&d_out[0], (size_t)max_blocks * block * 2));  // 256-byte aligned
+            CUDA_TRY(err_, dev.out[0].alloc((size_t)max_blocks * block * 2));  // 256-byte aligned
             return ERTGPU_OK;
         }
         const bool mix = mode == kResampleTuned;
         std::vector<int32_t> A((size_t)rs.P * rs.T);
         std::vector<uint32_t> D((size_t)rs.P * (rs.T / 2));
         rs_pack_table(table.data(), rs.P, rs.T, A.data(), D.data());
-        CUDA_TRY(err_, cudaMalloc(&d_A, A.size() * sizeof(int32_t)));
-        CUDA_TRY(err_, cudaMemcpy(d_A, A.data(), A.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-        CUDA_TRY(err_, cudaMalloc(&d_D, D.size() * sizeof(uint32_t)));
-        CUDA_TRY(err_, cudaMemcpy(d_D, D.data(), D.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        CUDA_TRY(err_, dev.A.upload(A));
+        CUDA_TRY(err_, dev.D.upload(D));
         if (mix || mode == kDecimate) {
             std::vector<uint32_t> E(ERTRS_NCO_N);
             ertrs_nco_table(E.data());
-            CUDA_TRY(err_, cudaMalloc(&d_E, E.size() * sizeof(uint32_t)));
-            CUDA_TRY(err_, cudaMemcpy(d_E, E.data(), E.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+            CUDA_TRY(err_, dev.E.upload(E));
         }
         const size_t hb = wide ? 4 : 2;  // bytes per carried sample: s_w words on the wide path
         for (int k = 0; k < 2; k++) {
-            CUDA_TRY(err_, cudaMalloc(&d_hist[k], (size_t)rs.T * hb + 16));
+            CUDA_TRY(err_, dev.hist[k].alloc((size_t)rs.T * hb + 16));
             // a step completes at most max_blocks blocks: less than (max_blocks + 1) * BS outputs are buffered
-            CUDA_TRY(err_, cudaMalloc(&d_out[k], (size_t)(max_blocks + 1) * block * 2 + 64));
+            CUDA_TRY(err_, dev.out[k].alloc((size_t)(max_blocks + 1) * block * 2 + 64));
         }
         fmt_visit(fmt, [&](auto f) {
             if (mode == kDecimate) {  // the second stage reads the first stage's bytes, or its s_w words on the wide path
@@ -289,28 +258,10 @@ struct InputStage {
         smem = wide ? rs_wide_smem_bytes(rs.P, rs.T, rs.L, rs.M, mode == kDecimate) : rs_smem_bytes(rs.P, rs.T, rs.L, rs.M, mix);
         if (const int rc = fit((const void*)last_kernel, kRsThreads, smem, "resampler", sm_count, &grid)) return rc;
         if (wide) {
-            CUDA_TRY(err_, cudaMalloc(&d_clevel, ERTRS_GAIN_BINS * sizeof(unsigned long long)));
-            for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_mhist[k], (size_t)rs.T * 4 + 16));
+            CUDA_TRY(err_, dev.clevel.alloc(ERTRS_GAIN_BINS));
+            for (int k = 0; k < 2; k++) CUDA_TRY(err_, dev.mhist[k].alloc((size_t)rs.T * 4 + 16));
         }
         return mode == kDecimate ? allocate_first(sm_count) : ERTGPU_OK;
-    }
-
-    void release() {
-        auto dfree = [](auto*& p) { if (p) cudaFree(p); p = nullptr; };
-        dfree(d_A);
-        dfree(d_D);
-        dfree(d_E);
-        dfree(d_level);
-        dfree(d_taps);
-        dfree(d_mid);
-        dfree(d_clevel);
-        for (int k = 0; k < 2; k++) {
-            dfree(d_hist[k]);
-            dfree(d_out[k]);
-            dfree(d_hist1[k]);
-            dfree(d_mhist[k]);
-            dfree(d_mhist1[k]);
-        }
     }
 
     void reset_stream() { pos = {}; }
@@ -377,13 +328,13 @@ struct InputStage {
         InputStep s;
         s.rs.cur = d_in;
         if (!resamples()) {
-            s.iq = mode == kPass ? d_in : d_out[0];
+            s.iq = mode == kPass ? d_in : dev.out[0];
             s.nblocks = n / block;
             return s;
         }
         if (mode == kDecimate) {  // the second stage takes the first stage's outputs of this step
             n = plan_first(s.dc, d_in, n);
-            s.rs.cur = d_mid;
+            s.rs.cur = dev.mid;
         }
         // every output whose window is complete
         const int64_t L = rs.L, M = rs.M, T = rs.T;
@@ -391,9 +342,9 @@ struct InputStage {
         const int64_t ne = ertrs_out_end(&rs, in_new);
         const int64_t cnt = ne - pos.out_next;
         s.nblocks = (pos.pend + cnt) / block;
-        s.iq = d_out[pos.cur_out];
+        s.iq = dev.out[pos.cur_out];
         RsArgs* a = &s.rs;
-        a->hist = d_hist[pos.cur_hist];
+        a->hist = dev.hist[pos.cur_hist];
         a->hist_first = pos.hist_first;
         a->hist_n = pos.hist_n;
         a->cur_n = n;
@@ -402,17 +353,17 @@ struct InputStage {
         a->split = s.nblocks > 0 ? s.nblocks * block - pos.pend : LLONG_MAX;
         a->base_n = (pos.out_next / L) * L;
         a->base_k = (pos.out_next / L) * M;
-        a->out = d_out[pos.cur_out] + 2 * pos.pend;
-        a->out2 = d_out[pos.cur_out ^ 1];
+        a->out = dev.out[pos.cur_out] + 2 * pos.pend;
+        a->out2 = dev.out[pos.cur_out ^ 1];
         const int64_t first = std::min(in_new, std::max<int64_t>(0, k_of(ne) - T / 2 + 1));
-        a->carry_dst = d_hist[pos.cur_hist ^ 1];
+        a->carry_dst = dev.hist[pos.cur_hist ^ 1];
         a->carry_first = first;
         a->carry_n = in_new - first;
         a->L = L;
         a->M = M;
         a->T = (int)T;
         a->scale = scale;
-        a->E = d_E;
+        a->E = dev.E;
         a->W = nco_step;
         a->P = rs.P;
         a->gain = gain;
@@ -432,19 +383,19 @@ struct InputStage {
             const unsigned g = grid_of(groups, kCvtThreads, grid);
             fmt_visit(fmt, [&](auto f) {
                 if constexpr (f() != ERTGPU_FORMAT_CU8)
-                    convert_kernel<f()><<<g, kCvtThreads, 0, st>>>(s.rs.cur, d_out[0], groups, scale);
+                    convert_kernel<f()><<<g, kCvtThreads, 0, st>>>(s.rs.cur, dev.out[0], groups, scale);
             });
             CUDA_TRY(err_, cudaGetLastError());
             ++*launches;
             return ERTGPU_OK;
         }
         if (first_kernel && !s.shared_first && (s.dc.count > 0 || s.dc.carry_n > 0)) {
-            first_kernel<<<grid_of(s.dc.count, (long long)kDcThreads * per1, grid1), kDcThreads, smem1, st>>>(d_taps, s.dc);
+            first_kernel<<<grid_of(s.dc.count, (long long)kDcThreads * per1, grid1), kDcThreads, smem1, st>>>(dev.taps, s.dc);
             CUDA_TRY(err_, cudaGetLastError());
             ++*launches;
         }
         if (last_kernel && (s.rs.count > 0 || s.rs.carry_n > 0)) {
-            last_kernel<<<grid_of(s.rs.count, kRsTile, grid), kRsThreads, smem, st>>>(d_A, d_D, s.rs);
+            last_kernel<<<grid_of(s.rs.count, kRsTile, grid), kRsThreads, smem, st>>>(dev.A, dev.D, s.rs);
             CUDA_TRY(err_, cudaGetLastError());
             ++*launches;
         }
@@ -467,18 +418,18 @@ struct InputStage {
         if (a.count <= 0 && a.carry_n <= 0) return ERTGPU_OK;
         DcArgs ac = a;
         ac.per = per1c;
-        channels_kernel<<<grid_of(a.count, (long long)kDcThreads * per1c, grid1c), kDcThreads, smem1c, st>>>(d_taps, ac, ch);
+        channels_kernel<<<grid_of(a.count, (long long)kDcThreads * per1c, grid1c), kDcThreads, smem1c, st>>>(dev.taps, ac, ch);
         CUDA_TRY(err_, cudaGetLastError());
         ++*launches;
         return ERTGPU_OK;
     }
 
-    // Enqueue level_kernel over n input samples at d_in (device, 16-byte aligned) on st: their counts are added to d_level.
+    // Enqueue level_kernel over n input samples at d_in (device, 16-byte aligned) on st: their counts are added to dev.level.
     int launch_level(const uint8_t* d_in, int64_t n, cudaStream_t st) const {
         const long long nbytes = n * sample_bytes, groups = (nbytes + 15) / 16;
         const unsigned g = grid_of(groups, kLvThreads, level_grid);
         fmt_visit(fmt, [&](auto f) {
-            if constexpr (f() != ERTGPU_FORMAT_CU8) level_kernel<f()><<<g, kLvThreads, 0, st>>>(d_in, nbytes, d_level);
+            if constexpr (f() != ERTGPU_FORMAT_CU8) level_kernel<f()><<<g, kLvThreads, 0, st>>>(d_in, nbytes, dev.level);
         });
         CUDA_TRY(err_, cudaGetLastError());
         return ERTGPU_OK;
@@ -522,7 +473,7 @@ struct InputStage {
         }
     }
 
-    // A channel measurement (wide path) runs the stage's own steps from a stream start, with rs.level = d_clevel in every
+    // A channel measurement (wide path) runs the stage's own steps from a stream start, with rs.level = dev.clevel in every
     // step.  begin_measure swaps the measurement's input histories and stream position in for the stream's, and
     // end_measure swaps them back.
     void begin_measure() {
@@ -537,8 +488,8 @@ private:
 
     void swap_measure() {
         std::swap(pos, mpos);
-        std::swap(d_hist, d_mhist);
-        std::swap(d_hist1, d_mhist1);
+        std::swap(dev.hist, dev.mhist);
+        std::swap(dev.hist1, dev.mhist1);
     }
 
     // CTAs of a launch over n items, per to a tile: one per tile, at least one and at most cap.
@@ -608,42 +559,41 @@ private:
         const int64_t D = dec.D, T1 = dec.T1;
         const int64_t in_new = pos.in1_total + n;
         const int64_t ne = in_new - T1 / 2 > 0 ? (in_new - T1 / 2 + D - 1) / D : 0;  // ertrs_out_end at L = 1, M = D
-        a.hist = d_hist1[pos.cur_hist1];
+        a.hist = dev.hist1[pos.cur_hist1];
         a.cur = d_in;
         a.hist_first = pos.hist1_first;
         a.hist_n = pos.hist1_n;
         a.cur_n = n;
         a.n0 = pos.in_total;  // the first stage's next output is the second stage's next input
         a.count = ne - pos.in_total;
-        a.out = d_mid;
+        a.out = dev.mid;
         const int64_t first = std::min(in_new, std::max<int64_t>(0, ne * D - T1 / 2 + 1));
-        a.carry_dst = d_hist1[pos.cur_hist1 ^ 1];
+        a.carry_dst = dev.hist1[pos.cur_hist1 ^ 1];
         a.carry_first = first;
         a.carry_n = in_new - first;
         a.D = (int)D;
         a.T1 = (int)T1;
         a.per = per1;
         a.scale = scale;
-        a.E = d_E;
+        a.E = dev.E;
         a.W = nco_step;
         return a.count;
     }
 
     // The first stage's device buffers, after the second stage's.
     int allocate_first(int sm_count) {
-        CUDA_TRY(err_, cudaMalloc(&d_taps, taps.size() * sizeof(int16_t)));
-        CUDA_TRY(err_, cudaMemcpy(d_taps, taps.data(), taps.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
+        CUDA_TRY(err_, dev.taps.upload(taps));
         const size_t hb = wide ? 4 : 2;  // bytes per carried sample, and per stage-1 output
-        for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_hist1[k], (size_t)(dec.T1 + dec.D + 16) * hb));
+        for (int k = 0; k < 2; k++) CUDA_TRY(err_, dev.hist1[k].alloc((size_t)(dec.T1 + dec.D + 16) * hb));
         // A step hands the second stage fewer than (max_blocks + 1) * block * M / L + M / L + T samples (the blocks a
         // step may complete, plus the look-ahead).
         const int64_t mid = (int64_t)(((__int128)(max_blocks + 1) * block * rs.M + rs.L - 1) / rs.L) + rs.M / rs.L + rs.T + 64;
-        CUDA_TRY(err_, cudaMalloc(&d_mid, (size_t)mid * hb));
+        CUDA_TRY(err_, dev.mid.alloc((size_t)mid * hb));
         per1 = dc_per_thread(dec.D, dec.T1);
         smem1 = dc_smem_bytes(dec.D, dec.T1, per1);
         if (const int rc = fit((const void*)first_kernel, kDcThreads, smem1, "decimator", sm_count, &grid1)) return rc;
         if (wide) {  // decimate_wide_kernel: decimate_kernel's tiles; groups run it per channel (DESIGN §3.12)
-            for (int k = 0; k < 2; k++) CUDA_TRY(err_, cudaMalloc(&d_mhist1[k], (size_t)(dec.T1 + dec.D + 16) * 4));
+            for (int k = 0; k < 2; k++) CUDA_TRY(err_, dev.mhist1[k].alloc((size_t)(dec.T1 + dec.D + 16) * 4));
             return ERTGPU_OK;
         }
         per1c = dc_per_thread(dec.D, dec.T1, kDcChannelsSpanWords);

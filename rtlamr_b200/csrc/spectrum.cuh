@@ -22,6 +22,7 @@
 
 #include "../../include/ertgpu_spectrum.h"
 #include "convert.cuh"
+#include "cuda_owned.hpp"
 
 namespace ert {
 
@@ -228,22 +229,23 @@ struct Spectrum {
     std::string label;  // "spectrum_kernel<fmt>"
     decltype(&spectrum_kernel<ERTGPU_FORMAT_CU8>) kern = nullptr;
 
-    float* d_win = nullptr;
-    float2* d_tw = nullptr;
-    uint8_t* d_carry[2] = {nullptr, nullptr};
-    float* d_gpart[2] = {nullptr, nullptr};
-    float* d_open[2] = {nullptr, nullptr};
-    float* d_grp = nullptr;
-    unsigned int* d_cnt = nullptr;
-    float* d_mean = nullptr;
-    float* d_peak = nullptr;
+    // The device tables and buffers: the handle clears them (= {}) when it releases its own.
+    struct Device {
+        DeviceArray<float> win;
+        DeviceArray<float2> tw;
+        DeviceArray<uint8_t> carry[2];
+        DeviceArray<float> gpart[2], open[2];
+        DeviceArray<float> grp;
+        DeviceArray<unsigned int> cnt;
+        DeviceArray<float> mean, peak;
+    } dev;
 
     // The stream position: all that a stream start resets.
     struct Pos {
         int64_t samples = 0;       // input samples since the stream start
         int64_t rows_fetched = 0;  // rows ertgpu_fetch_spectrum returned
-        int cc = 0, gc = 0, oc = 0;  // which of d_carry, d_gpart, d_open the next launch reads
-        bool open_valid = false;     // d_open[oc] holds the open row's completed groups
+        int cc = 0, gc = 0, oc = 0;  // which of dev.carry, dev.gpart, dev.open the next launch reads
+        bool open_valid = false;     // dev.open[oc] holds the open row's completed groups
     } pos;
 
     int64_t frames() const { return pos.samples / N; }
@@ -277,37 +279,20 @@ struct Spectrum {
             const double ph = -2.0 * ERTSPEC_PI * (double)m / (double)N;
             tw[(size_t)m] = make_float2((float)cos(ph), (float)sin(ph));
         }
-        CUDA_TRY(err, cudaMalloc(&d_win, (size_t)N * sizeof(float)));
-        CUDA_TRY(err, cudaMemcpy(d_win, w.data(), (size_t)N * sizeof(float), cudaMemcpyHostToDevice));
-        CUDA_TRY(err, cudaMalloc(&d_tw, (size_t)N * sizeof(float2)));
-        CUDA_TRY(err, cudaMemcpy(d_tw, tw.data(), (size_t)N * sizeof(float2), cudaMemcpyHostToDevice));
+        CUDA_TRY(err, dev.win.upload(w));
+        CUDA_TRY(err, dev.tw.upload(tw));
         for (int k = 0; k < 2; k++) {
-            CUDA_TRY(err, cudaMalloc(&d_carry[k], (size_t)N * 16));
-            CUDA_TRY(err, cudaMalloc(&d_gpart[k], (size_t)2 * N * sizeof(float)));
-            CUDA_TRY(err, cudaMalloc(&d_open[k], (size_t)2 * N * sizeof(float)));
+            CUDA_TRY(err, dev.carry[k].alloc((size_t)N * 16));
+            CUDA_TRY(err, dev.gpart[k].alloc((size_t)2 * N));
+            CUDA_TRY(err, dev.open[k].alloc((size_t)2 * N));
         }
-        CUDA_TRY(err, cudaMalloc(&d_grp, (size_t)item_cap * 2 * N * sizeof(float)));
-        CUDA_TRY(err, cudaMalloc(&d_cnt, (size_t)cnt_cap * sizeof(unsigned int)));
-        CUDA_TRY(err, cudaMemset(d_cnt, 0, (size_t)cnt_cap * sizeof(unsigned int)));
-        CUDA_TRY(err, cudaMalloc(&d_mean, (size_t)row_cap * N * sizeof(float)));
-        CUDA_TRY(err, cudaMalloc(&d_peak, (size_t)row_cap * N * sizeof(float)));
+        CUDA_TRY(err, dev.grp.alloc((size_t)item_cap * 2 * N));
+        CUDA_TRY(err, dev.cnt.alloc((size_t)cnt_cap));
+        CUDA_TRY(err, cudaMemset(dev.cnt, 0, (size_t)cnt_cap * sizeof(unsigned int)));
+        CUDA_TRY(err, dev.mean.alloc((size_t)row_cap * N));
+        CUDA_TRY(err, dev.peak.alloc((size_t)row_cap * N));
         pos = {};
         return ERTGPU_OK;
-    }
-
-    void release() {
-        auto dfree = [](auto*& p) { if (p) cudaFree(p); p = nullptr; };
-        dfree(d_win);
-        dfree(d_tw);
-        for (int k = 0; k < 2; k++) {
-            dfree(d_carry[k]);
-            dfree(d_gpart[k]);
-            dfree(d_open[k]);
-        }
-        dfree(d_grp);
-        dfree(d_cnt);
-        dfree(d_mean);
-        dfree(d_peak);
     }
 
     // Enqueue the kernel over n input samples at d_in (device) on st, with input gain g, and advance the position: one
@@ -332,8 +317,8 @@ struct Spectrum {
         SpecArgs a{};
         a.in = d_in;
         a.n = n;
-        a.carry_src = d_carry[pos.cc];
-        a.carry_dst = d_carry[pos.cc ^ 1];
+        a.carry_src = dev.carry[pos.cc];
+        a.carry_dst = dev.carry[pos.cc ^ 1];
         a.carry_n = (int)carry_n;
         a.g = g;
         a.log2n = log2n;
@@ -342,18 +327,18 @@ struct Spectrum {
         a.G = G;
         a.f0 = f0;
         a.nf = nf;
-        a.win = d_win;
-        a.tw = d_tw;
+        a.win = dev.win;
+        a.tw = dev.tw;
         a.scale = ertspec_power_scale(log2n);
-        a.gpart_src = d_gpart[pos.gc];
-        a.gpart_dst = d_gpart[pos.gc ^ 1];
-        a.open_src = d_open[pos.oc];
-        a.open_dst = d_open[pos.oc ^ 1];
+        a.gpart_src = dev.gpart[pos.gc];
+        a.gpart_dst = dev.gpart[pos.gc ^ 1];
+        a.open_src = dev.open[pos.oc];
+        a.open_dst = dev.open[pos.oc ^ 1];
         a.open_valid = pos.open_valid;
-        a.grp = d_grp;
-        a.cnt = d_cnt;
-        a.rows_mean = d_mean;
-        a.rows_peak = d_peak;
+        a.grp = dev.grp;
+        a.cnt = dev.cnt;
+        a.rows_mean = dev.mean;
+        a.rows_peak = dev.peak;
         a.row_cap = row_cap;
         const int64_t carry_bytes = (carry_n + n - nf * N) * 16;
         const int64_t want = std::max<int64_t>(items, (carry_bytes + threads - 1) / threads);
@@ -381,9 +366,9 @@ struct Spectrum {
         *frames_in_row = fr;
         if (fr == 0) return ERTGPU_OK;
         std::vector<float> m((size_t)2 * N, 0.0f), gp((size_t)2 * N, 0.0f);
-        if (pos.open_valid) CUDA_TRY(err, cudaMemcpy(m.data(), d_open[pos.oc], m.size() * sizeof(float), cudaMemcpyDeviceToHost));
+        if (pos.open_valid) CUDA_TRY(err, cudaMemcpy(m.data(), dev.open[pos.oc], m.size() * sizeof(float), cudaMemcpyDeviceToHost));
         const bool mid_group = fr % G != 0;
-        if (mid_group) CUDA_TRY(err, cudaMemcpy(gp.data(), d_gpart[pos.gc], gp.size() * sizeof(float), cudaMemcpyDeviceToHost));
+        if (mid_group) CUDA_TRY(err, cudaMemcpy(gp.data(), dev.gpart[pos.gc], gp.size() * sizeof(float), cudaMemcpyDeviceToHost));
         for (int p = 0; p < N; p++) {
             volatile float s = m[(size_t)p];
             float pk = m[(size_t)N + p];
