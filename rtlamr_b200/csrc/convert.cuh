@@ -12,16 +12,9 @@
 #include <utility>
 
 #include "../../include/ertgpu.h"
+#include "../../include/ertgpu_format.h"
 
 namespace ert {
-
-// bytes per IQ sample of a format
-__host__ __device__ constexpr int fmt_sample_bytes(int f) {
-    return f == ERTGPU_FORMAT_CS16 || f == ERTGPU_FORMAT_CS16BE || f == ERTGPU_FORMAT_CU16 || f == ERTGPU_FORMAT_CU16BE ? 4
-           : f == ERTGPU_FORMAT_CF64 || f == ERTGPU_FORMAT_CF64BE                                                      ? 16
-           : f == ERTGPU_FORMAT_CF32 || f >= ERTGPU_FORMAT_CF32BE                                                      ? 8
-                                                                                                                      : 2;
-}
 
 // Every input format, and f(std::integral_constant<int, F>{}) for the one equal to `format`; false when none is.
 using AllFormats = std::integer_sequence<int, ERTGPU_FORMAT_CU8, ERTGPU_FORMAT_CS8, ERTGPU_FORMAT_CS16, ERTGPU_FORMAT_CF32,
@@ -34,38 +27,6 @@ bool fmt_visit_in(int format, Fn&& f, std::integer_sequence<int, Fs...>) {
 }
 template <typename Fn>
 bool fmt_visit(int format, Fn&& f) { return fmt_visit_in(format, f, AllFormats{}); }
-
-// The name of a format: its SigMF datatype, or cu8 / cs8 / cs16 / cf32 for the first four.
-inline const char* fmt_name(int f) {
-    switch (f) {
-        case ERTGPU_FORMAT_CU8: return "cu8";
-        case ERTGPU_FORMAT_CS8: return "cs8";
-        case ERTGPU_FORMAT_CS16: return "cs16";
-        case ERTGPU_FORMAT_CF32: return "cf32";
-        case ERTGPU_FORMAT_CS16BE: return "ci16_be";
-        case ERTGPU_FORMAT_CF32BE: return "cf32_be";
-        case ERTGPU_FORMAT_CU16: return "cu16_le";
-        case ERTGPU_FORMAT_CU16BE: return "cu16_be";
-        case ERTGPU_FORMAT_CS32: return "ci32_le";
-        case ERTGPU_FORMAT_CS32BE: return "ci32_be";
-        case ERTGPU_FORMAT_CU32: return "cu32_le";
-        case ERTGPU_FORMAT_CU32BE: return "cu32_be";
-        case ERTGPU_FORMAT_CF64: return "cf64_le";
-        case ERTGPU_FORMAT_CF64BE: return "cf64_be";
-        default: return nullptr;
-    }
-}
-
-// The default gain of a format, which maps full scale to full scale (0 for cu8, which is not scaled).
-inline float fmt_default_scale(int f) {
-    switch (f) {
-        case ERTGPU_FORMAT_CU8: return 0.0f;
-        case ERTGPU_FORMAT_CS8: return 1.0f;
-        case ERTGPU_FORMAT_CS16: case ERTGPU_FORMAT_CS16BE: case ERTGPU_FORMAT_CU16: case ERTGPU_FORMAT_CU16BE: return 1.0f / 256.0f;
-        case ERTGPU_FORMAT_CS32: case ERTGPU_FORMAT_CS32BE: case ERTGPU_FORMAT_CU32: case ERTGPU_FORMAT_CU32BE: return 1.0f / 16777216.0f;
-        default: return 128.0f;   // float32 and float64
-    }
-}
 
 // One IQ component x (int8, int16 or float32, exact in float32) times g as the decoder's byte.  The product is one
 // float32 multiply rounded to nearest even (__fmul_rn: never contracted).  NaN is decided here, before fmaxf (which
@@ -93,7 +54,7 @@ __device__ __forceinline__ auto fmt_x(const uint32_t* x, int c) {
     constexpr bool be = F == ERTGPU_FORMAT_CS16BE || F == ERTGPU_FORMAT_CF32BE || F == ERTGPU_FORMAT_CU16BE ||
                         F == ERTGPU_FORMAT_CS32BE || F == ERTGPU_FORMAT_CU32BE || F == ERTGPU_FORMAT_CF64BE;
     constexpr bool un = F == ERTGPU_FORMAT_CU16 || F == ERTGPU_FORMAT_CU16BE || F == ERTGPU_FORMAT_CU32 || F == ERTGPU_FORMAT_CU32BE;
-    constexpr int S = fmt_sample_bytes(F);
+    constexpr int S = ertfmt_bytes(F);
     static_assert(F != ERTGPU_FORMAT_CU8, "cu8 is not converted");
     if constexpr (S == 2) {         // cs8: four components per word
         return (int8_t)(x[c >> 2] >> (8 * (c & 3)));
@@ -135,7 +96,7 @@ __device__ __forceinline__ uint32_t fmt_comp(const uint32_t* x, int c, float g) 
 // The bytes of IQ sample j of format F (F != cu8) at src: I in the low byte, Q in the high byte.
 template <int F>
 __device__ __forceinline__ uchar2 fmt_sample(const uint8_t* src, long long j, float g) {
-    constexpr int S = fmt_sample_bytes(F);
+    constexpr int S = ertfmt_bytes(F);
     uint32_t x[(S + 3) / 4];
     // cs8, cs16 and cf32 are loaded as the vector of their components, which the compiler reads in place
     if constexpr (F == ERTGPU_FORMAT_CS8) {
@@ -189,7 +150,7 @@ __device__ __forceinline__ uint32_t fmt_wide_sample(const uint8_t* src, long lon
         const uchar2 u = *reinterpret_cast<const uchar2*>(src + 2 * j);
         return ((uint32_t)(64 * (2 * (int)u.x - 255)) & 0xffffu) | ((uint32_t)(64 * (2 * (int)u.y - 255)) << 16);
     } else {
-        constexpr int S = fmt_sample_bytes(F);
+        constexpr int S = ertfmt_bytes(F);
         uint32_t x[(S + 3) / 4];
         if constexpr (S == 2) {
             x[0] = *reinterpret_cast<const uint16_t*>(src + 2 * j);
@@ -218,7 +179,7 @@ constexpr int kCvtThreads = 256;
 template <int F>
 __global__ void __launch_bounds__(kCvtThreads) convert_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out,
                                                               long long ngroups, float g) {
-    constexpr int kLoads = fmt_sample_bytes(F) * 8 / 16;
+    constexpr int kLoads = ertfmt_bytes(F) * 8 / 16;
     for (long long grp = (long long)blockIdx.x * blockDim.x + threadIdx.x; grp < ngroups;
          grp += (long long)gridDim.x * blockDim.x) {
         const uint4* src = reinterpret_cast<const uint4*>(in) + grp * kLoads;

@@ -1084,7 +1084,7 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
         const int64_t r_out = decoder_rate(h), r_in = h->in.rate_in ? h->in.rate_in : r_out;
         const int64_t in_max = std::max({h->in.chunk(), h->in.max_call_input(),
                                          max_blocks_per_call * c.block_size * ((r_in + r_out - 1) / r_out)});
-        if (const int rc = h->spec.allocate(h->err, h->in.fmt, h->in.sample_bytes, fmt_name(h->in.fmt), in_max, h->sm_count))
+        if (const int rc = h->spec.allocate(h->err, h->in.fmt, h->in.sample_bytes, ertfmt_name(h->in.fmt), in_max, h->sm_count))
             return rc;
     }
     h->pos = {};
@@ -1236,7 +1236,7 @@ int ertgpu_measure_input(ertgpu_handle* h, const void* samples, size_t nbytes, e
     out->zeros = (int64_t)cnt[kLvZero];
     out->nans = (int64_t)cnt[kLvNan];
     for (int b = 0; b < ERTLV_BINS; b++) out->bins[b] = (int64_t)cnt[b];
-    out->exponent = ertlv_exponent(out->bins, out->components, out->zeros, out->nans, ilogbf(fmt_default_scale(h->in.fmt)));
+    out->exponent = ertlv_exponent(out->bins, out->components, out->zeros, out->nans, ilogbf(ertfmt_default_scale(h->in.fmt)));
     out->scale = ldexpf(1.0f, out->exponent);
     return ERTGPU_OK;
 }

@@ -148,13 +148,13 @@ struct InputStage {
     }
 
     int set_format(int32_t format, float g) {
-        if (!fmt_name(format)) return fail(err_, ERTGPU_EINVAL, "unknown input format %d", format);
+        if (!ertfmt_name(format)) return fail(err_, ERTGPU_EINVAL, "unknown input format %d", format);
         if (!std::isfinite(g) || g < 0.0f) return fail(err_, ERTGPU_EINVAL, "input scale %g is not a finite value >= 0", (double)g);
         if (format == ERTGPU_FORMAT_CU8 && g != 0.0f) return fail(err_, ERTGPU_EINVAL, "cu8 input is not scaled (scale %g)", (double)g);
-        if (g == 0.0f) g = fmt_default_scale(format);
+        if (g == 0.0f) g = ertfmt_default_scale(format);
         fmt = format;
         scale = g;
-        sample_bytes = fmt_sample_bytes(format);
+        sample_bytes = ertfmt_bytes(format);
         if (!resamples()) mode = fmt == ERTGPU_FORMAT_CU8 ? kPass : kConvert;
         return ERTGPU_OK;
     }
@@ -163,7 +163,7 @@ struct InputStage {
     int set_scale(float g) {
         if (fmt == ERTGPU_FORMAT_CU8) return fail(err_, ERTGPU_EINVAL, "cu8 input is not scaled");
         if (!std::isfinite(g) || g < 0.0f) return fail(err_, ERTGPU_EINVAL, "input scale %g is not a finite value >= 0", (double)g);
-        scale = g == 0.0f ? fmt_default_scale(fmt) : g;
+        scale = g == 0.0f ? ertfmt_default_scale(fmt) : g;
         return ERTGPU_OK;
     }
 
@@ -460,7 +460,7 @@ struct InputStage {
     // The stage's kernels as ertgpu_last_kernels names them ("" in pass-through mode); `shared`: the first stage ran as
     // decimate_channels_kernel.
     std::string label(bool shared = false) const {
-        const char* f = fmt_name(fmt);
+        const char* f = ertfmt_name(fmt);
         if (wide)
             return mode == kDecimate ? std::string("decimate_kernel<") + f + ",wide>;resample_kernel<mid16,tuned,wide>"
                                      : std::string("resample_kernel<") + f + ",tuned,wide>";

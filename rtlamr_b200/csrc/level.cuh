@@ -53,7 +53,7 @@ __device__ __forceinline__ void lv_count(unsigned int* s, int bin) {
 template <int F>
 __global__ void __launch_bounds__(kLvThreads) level_kernel(const uint8_t* __restrict__ in, long long nbytes,
                                                            unsigned long long* __restrict__ counters) {
-    constexpr int S = fmt_sample_bytes(F), kComps = 32 / S;  // components per 16 bytes
+    constexpr int S = ertfmt_bytes(F), kComps = 32 / S;  // components per 16 bytes
     __shared__ unsigned int s[kLvCounters];
     for (int i = threadIdx.x; i < kLvCounters; i += kLvThreads) s[i] = 0;
     __syncthreads();

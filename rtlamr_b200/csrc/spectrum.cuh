@@ -129,7 +129,7 @@ template <int F>
 __global__ void __launch_bounds__(kSpecMaxThreads) spectrum_kernel(SpecArgs a) {
     extern __shared__ float2 x[];
     int& s_last = *reinterpret_cast<int*>(x + a.N);  // (all of a CTA's shared memory is dynamic: allow_dynamic_smem)
-    constexpr int S = fmt_sample_bytes(F);
+    constexpr int S = ertfmt_bytes(F);
     const int T = blockDim.x, t = threadIdx.x, N = a.N;
 
     // the raw bytes after the last whole frame, for the next call

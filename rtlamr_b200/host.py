@@ -71,9 +71,6 @@ def lib():
         L.erthost_new_parse_only.argtypes = [C.c_char_p, C.c_int, C.c_char_p, C.c_int]
         L.erthost_parse.restype = C.c_longlong
         L.erthost_parse.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.POINTER(_Msg), C.c_longlong]
-        L.erthost_parse_dedup.restype = C.c_longlong
-        L.erthost_parse_dedup.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.POINTER(_Msg), C.c_longlong,
-                                          C.POINTER(C.c_longlong)]
         L.erthost_parse_dedup_channels.restype = C.c_longlong
         L.erthost_parse_dedup_channels.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_int,
                                                    C.POINTER(_Msg), C.POINTER(C.c_int), C.c_longlong, C.POINTER(C.c_longlong)]
@@ -103,6 +100,9 @@ def _messages(out, n):
                         m.text.decode(), tuple(m.record.decode().split(",")), _signal(m)) for m in out[:n]]
 
 
+FORMATS = {"plain": 0, "csv": 1, "json": 2, "xml": 3}
+
+
 class Parsers:
     """NewDecoder + RegisterProtocol(NewParser(..)) WITHOUT Allocate: no device is touched.  parse() is the second
     half of Decode (decode.go:177-187 and every parser's Parse) on candidate records from any source."""
@@ -119,101 +119,80 @@ class Parsers:
             self._L.erthost_free(self._h)
             self._h = None
 
+    def _check(self, n):
+        """n, the count an erthost_* call returned; a negative one raises with the handle's message."""
+        if n < 0:
+            raise RuntimeError(self._L.erthost_error(self._h).decode())
+        return n
+
     def parse(self, cands: np.ndarray, cap: int = 4096) -> list[HostMessage]:
         """cands: structured array with capi.CAND_DTYPE, sorted by (block, preamble_id, idx)."""
         cands = np.ascontiguousarray(cands)
         assert cands.dtype.itemsize == 160
         out = (_Msg * cap)()
-        n = self._L.erthost_parse(self._h, cands.ctypes.data, len(cands), out, cap)
-        if n < 0:
-            raise RuntimeError(self._L.erthost_error(self._h).decode())
+        n = self._check(self._L.erthost_parse(self._h, cands.ctypes.data, len(cands), out, cap))
         if n > cap:
             raise OverflowError(f"{n} messages, cap {cap}")
         return _messages(out, n)
 
+    def parse_dedup(self, cands: np.ndarray, block_dedup: bool = True, cap: int = 4096):
+        """parse() followed by the receive loop's cross-block dedup (main.go:244-260,292): (messages, duplicates
+        dropped)."""
+        msgs, dup, _ = self.parse_filtered(cands, block_dedup=block_dedup, cap=cap)
+        return msgs, dup
 
-def _parse_dedup(self, cands: np.ndarray, block_dedup: bool = True, cap: int = 4096):
-    """parse() followed by the receive loop's cross-block dedup (main.go:244-260,292): (messages, duplicates dropped)."""
-    cands = np.ascontiguousarray(cands)
-    out = (_Msg * cap)()
-    dup = C.c_longlong(0)
-    n = self._L.erthost_parse_dedup(self._h, cands.ctypes.data, len(cands), 1 if block_dedup else 0, out, cap, C.byref(dup))
-    if n < 0:
-        raise RuntimeError(self._L.erthost_error(self._h).decode())
-    return _messages(out, min(n, cap)), int(dup.value)
+    def parse_dedup_channels(self, per_channel, block_dedup: bool = True, cap: int = 4096):
+        """parse() of each channel's candidates (a list of arrays, one per channel of one capture), then the receiver's
+        cross-channel dedup in its print order (ascending block, then channel): ([(channel, message)], duplicates
+        dropped)."""
+        cands = np.ascontiguousarray(np.concatenate(per_channel)) if per_channel else np.zeros(0, np.uint8)
+        counts = (C.c_longlong * len(per_channel))(*[len(c) for c in per_channel])
+        out, chan = (_Msg * cap)(), (C.c_int * cap)()
+        dup = C.c_longlong(0)
+        n = self._check(self._L.erthost_parse_dedup_channels(self._h, cands.ctypes.data, counts, len(per_channel),
+                                                             1 if block_dedup else 0, out, chan, cap, C.byref(dup)))
+        n = min(n, cap)
+        return list(zip(chan[:n], _messages(out, n))), int(dup.value)
 
+    def parse_filtered(self, cands, filterid: str = "", filtertype: str = "", unique: bool = False,
+                       block_dedup: bool = True, cap: int = 1 << 16):
+        """erthost_parse_filtered: parsers, then the receive loop's filter chain (-filterid, -filtertype, -unique in the
+        order flag.Visit adds them, main.go:97-113) and the cross-block dedup (main.go:236-260).  Returns (messages,
+        dropped by the dedup, rejected by the filters)."""
+        cands = np.ascontiguousarray(cands)
+        out = (_Msg * cap)()
+        dup, flt = C.c_longlong(0), C.c_longlong(0)
+        n = self._check(self._L.erthost_parse_filtered(self._h, cands.ctypes.data, len(cands), filterid.encode(),
+                                                       filtertype.encode(), 1 if unique else 0, 1 if block_dedup else 0,
+                                                       out, cap, C.byref(dup), C.byref(flt)))
+        return _messages(out, min(n, cap)), int(dup.value), int(flt.value)
 
-Parsers.parse_dedup = _parse_dedup
+    def encode(self, cands, fmt: str = "plain", unix_seconds: int = 0, nanos: int = 0, offset: int = 0, length: int = 0,
+               sample_file_is_devnull: bool = True) -> str:
+        """erthost_encode: every parsed message through the plain, csv, json or xml encoder (flags.go:140-170) as one
+        string of lines."""
+        cands = np.ascontiguousarray(cands)
+        cap = 1 << 22
+        buf = C.create_string_buffer(cap)
+        n = self._L.erthost_encode(self._h, cands.ctypes.data, len(cands), FORMATS[fmt], unix_seconds, nanos, offset,
+                                   length, 1 if sample_file_is_devnull else 0, buf, cap)
+        if n < 0 or n >= cap:
+            raise RuntimeError("erthost_encode failed" if n < 0 else "encode buffer too small")
+        return buf.value.decode()
 
-
-def _parse_dedup_channels(self, per_channel, block_dedup: bool = True, cap: int = 4096):
-    """parse() of each channel's candidates (a list of arrays, one per channel of one capture), then the receiver's
-    cross-channel dedup in its print order (ascending block, then channel): ([(channel, message)], duplicates dropped)."""
-    cands = np.ascontiguousarray(np.concatenate(per_channel)) if per_channel else np.zeros(0, np.uint8)
-    counts = (C.c_longlong * len(per_channel))(*[len(c) for c in per_channel])
-    out, chan = (_Msg * cap)(), (C.c_int * cap)()
-    dup = C.c_longlong(0)
-    n = self._L.erthost_parse_dedup_channels(self._h, cands.ctypes.data, counts, len(per_channel), 1 if block_dedup else 0,
-                                             out, chan, cap, C.byref(dup))
-    if n < 0:
-        raise RuntimeError(self._L.erthost_error(self._h).decode())
-    n = min(n, cap)
-    return list(zip(chan[:n], _messages(out, n))), int(dup.value)
-
-
-Parsers.parse_dedup_channels = _parse_dedup_channels
-
-
-def _parse_filtered(self, cands, filterid: str = "", filtertype: str = "", unique: bool = False, block_dedup: bool = True,
-                    cap: int = 1 << 16):
-    """erthost_parse_filtered: parsers, then the receive loop's filter chain (-filterid, -filtertype, -unique in the order
-    flag.Visit adds them, main.go:97-113) and the cross-block dedup (main.go:236-260).  Returns (messages, dropped by the
-    dedup, rejected by the filters)."""
-    cands = np.ascontiguousarray(cands)
-    out = (_Msg * cap)()
-    dup, flt = C.c_longlong(0), C.c_longlong(0)
-    n = self._L.erthost_parse_filtered(self._h, cands.ctypes.data, len(cands), filterid.encode(), filtertype.encode(),
-                                       1 if unique else 0, 1 if block_dedup else 0, out, cap, C.byref(dup), C.byref(flt))
-    if n < 0:
-        raise RuntimeError(self._L.erthost_error(self._h).decode())
-    return _messages(out, min(n, cap)), int(dup.value), int(flt.value)
-
-
-FORMATS = {"plain": 0, "csv": 1, "json": 2, "xml": 3}
-
-
-def _encode(self, cands, fmt: str = "plain", unix_seconds: int = 0, nanos: int = 0, offset: int = 0, length: int = 0,
-            sample_file_is_devnull: bool = True) -> str:
-    """erthost_encode: every parsed message through the plain, csv, json or xml encoder (flags.go:140-170) as one string
-    of lines."""
-    cands = np.ascontiguousarray(cands)
-    cap = 1 << 22
-    buf = C.create_string_buffer(cap)
-    n = self._L.erthost_encode(self._h, cands.ctypes.data, len(cands), FORMATS[fmt], unix_seconds, nanos, offset, length,
-                               1 if sample_file_is_devnull else 0, buf, cap)
-    if n < 0 or n >= cap:
-        raise RuntimeError("erthost_encode failed" if n < 0 else "encode buffer too small")
-    return buf.value.decode()
-
-
-def _encode_signal(self, cands, sigs, channel_hz: int, rate_out: int, fmt: str = "plain", unix_seconds: int = 0,
-                   nanos: int = 0) -> str:
-    """erthost_encode_signal: every parsed message with the signal report of its candidate (sigs: capi.SIGNAL_DTYPE, one
-    per candidate) through the encoders; "plain" is ertgpu_decode_file's plain line."""
-    cands, sigs = np.ascontiguousarray(cands), np.ascontiguousarray(sigs)
-    assert len(sigs) == len(cands)
-    cap = 1 << 22
-    buf = C.create_string_buffer(cap)
-    n = self._L.erthost_encode_signal(self._h, cands.ctypes.data, sigs.ctypes.data, len(cands), channel_hz, rate_out,
-                                      FORMATS[fmt], unix_seconds, nanos, buf, cap)
-    if n < 0 or n >= cap:
-        raise RuntimeError(self._L.erthost_error(self._h).decode() if n < 0 else "encode buffer too small")
-    return buf.value.decode()
-
-
-Parsers.parse_filtered = _parse_filtered
-Parsers.encode = _encode
-Parsers.encode_signal = _encode_signal
+    def encode_signal(self, cands, sigs, channel_hz: int, rate_out: int, fmt: str = "plain", unix_seconds: int = 0,
+                      nanos: int = 0) -> str:
+        """erthost_encode_signal: every parsed message with the signal report of its candidate (sigs:
+        capi.SIGNAL_DTYPE, one per candidate) through the encoders; "plain" is ertgpu_decode_file's plain line."""
+        cands, sigs = np.ascontiguousarray(cands), np.ascontiguousarray(sigs)
+        assert len(sigs) == len(cands)
+        cap = 1 << 22
+        buf = C.create_string_buffer(cap)
+        n = self._check(self._L.erthost_encode_signal(self._h, cands.ctypes.data, sigs.ctypes.data, len(cands), channel_hz,
+                                                      rate_out, FORMATS[fmt], unix_seconds, nanos, buf, cap))
+        if n >= cap:
+            raise RuntimeError("encode buffer too small")
+        return buf.value.decode()
 
 
 def wav_probe(path) -> dict:

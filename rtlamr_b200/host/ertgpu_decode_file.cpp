@@ -80,403 +80,398 @@
 #include <cerrno>
 #include <chrono>
 #include <cmath>
+#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <ctime>
-#include <iostream>
-#include <tuple>
+#include <functional>
+#include <string>
 #include <vector>
 
+#include "../../include/ertgpu_format.h"
 #include "../../include/ertgpu_resample.h"
 #include "../../include/ertgpu_spectrum.h"
 #include "receiver.hpp"
 #include "sigmf.hpp"
 #include "wav.hpp"
 
-int main(int argc, char** argv) {
-    const auto start = std::chrono::steady_clock::now();   // main.go:350-353: the time limit covers the whole run
-    std::string msgtype = "scm";
+namespace {
+
+// An end of the program before the run: main writes the message and a newline to stderr and returns the code, 2 for a
+// usage error and 1 for a file that cannot be read.
+struct Exit {
+    int code;
+    std::string message;
+};
+
+[[noreturn]] __attribute__((format(printf, 1, 2))) void usage(const char* fmt, ...) {
+    va_list ap, ap2;
+    va_start(ap, fmt);
+    va_copy(ap2, ap);
+    std::string msg((size_t)vsnprintf(nullptr, 0, fmt, ap), '\0');
+    va_end(ap);
+    vsnprintf(&msg[0], msg.size() + 1, fmt, ap2);
+    va_end(ap2);
+    throw Exit{2, msg};
+}
+
+// perror(name)'s line for errno, with status 1.
+Exit file_error(const std::string& name) {
+    const std::string reason = strerror(errno);
+    return Exit{1, (name.empty() ? "" : name + ": ") + reason};
+}
+
+// The command line as given: every -flag=value spelling the CLI takes, and anything else as a file name.
+struct Options {
     std::vector<std::string> files;
+    std::string msgtype = "scm", format = "plain", sampleformat = "cu8";
     int chip = 72, device = 0;
     long long blocks = 4096, samplerate = 0;
-    bool block_dedup = true, quiet = false, unique = false, single = false, signal = false;
-    std::string filterid, filtertype, format = "plain", samplefile, duration, sampleformat = "cu8", samplescale;
-    std::string capturefreq, centerfreq, channelgain;
+    bool block_dedup = true, quiet = false, unique = false, single = false, signal = false, spectrum_peak = false;
+    bool have_scale = false;
+    std::string filterid, filtertype, samplefile, duration, samplescale, capturefreq, centerfreq, channelgain;
     std::string spectrum_file, spectrum_bin, spectrum_int;
-    bool spectrum_peak = false;
-    bool have_scale = false, auto_scale = false;
+};
+
+Options parse_flags(int argc, char** argv) {
+    Options o;
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i];
-        if (a.rfind("-msgtype=", 0) == 0) msgtype = a.substr(9);
-        else if (a.rfind("-symbollength=", 0) == 0) chip = atoi(a.c_str() + 14);
-        else if (a.rfind("-device=", 0) == 0) device = atoi(a.c_str() + 8);
-        else if (a.rfind("-samplerate=", 0) == 0) samplerate = atoll(a.c_str() + 12);
-        else if (a.rfind("-sampleformat=", 0) == 0) sampleformat = a.substr(14);
-        else if (a.rfind("-capturefreq=", 0) == 0) capturefreq = a.substr(13);
-        else if (a.rfind("-centerfreq=", 0) == 0) centerfreq = a.substr(12);
-        else if (a.rfind("-channelgain=", 0) == 0) channelgain = a.substr(13);
+        if (a.rfind("-msgtype=", 0) == 0) o.msgtype = a.substr(9);
+        else if (a.rfind("-symbollength=", 0) == 0) o.chip = atoi(a.c_str() + 14);
+        else if (a.rfind("-device=", 0) == 0) o.device = atoi(a.c_str() + 8);
+        else if (a.rfind("-samplerate=", 0) == 0) o.samplerate = atoll(a.c_str() + 12);
+        else if (a.rfind("-sampleformat=", 0) == 0) o.sampleformat = a.substr(14);
+        else if (a.rfind("-capturefreq=", 0) == 0) o.capturefreq = a.substr(13);
+        else if (a.rfind("-centerfreq=", 0) == 0) o.centerfreq = a.substr(12);
+        else if (a.rfind("-channelgain=", 0) == 0) o.channelgain = a.substr(13);
         else if (a.rfind("-samplescale=", 0) == 0) {
-            samplescale = a.substr(13);
-            have_scale = true;
+            o.samplescale = a.substr(13);
+            o.have_scale = true;
         }
-        else if (a.rfind("-blocks=", 0) == 0) blocks = atoll(a.c_str() + 8);
-        else if (a.rfind("-blockdedup=", 0) == 0) block_dedup = a.substr(12) != "false";
-        else if (a.rfind("-filterid=", 0) == 0) filterid = a.substr(10);
-        else if (a.rfind("-filtertype=", 0) == 0) filtertype = a.substr(12);
-        else if (a.rfind("-unique=", 0) == 0) unique = a.substr(8) == "true";
-        else if (a == "-unique") unique = true;
-        else if (a.rfind("-format=", 0) == 0) format = a.substr(8);
-        else if (a.rfind("-samplefile=", 0) == 0) samplefile = a.substr(12);
-        else if (a.rfind("-single=", 0) == 0) single = a.substr(8) == "true";
-        else if (a == "-signal" || a == "-signal=true") signal = true;
-        else if (a == "-signal=false") signal = false;
-        else if (a == "-single") single = true;
-        else if (a.rfind("-duration=", 0) == 0) duration = a.substr(10);
-        else if (a == "-quiet") quiet = true;
-        else if (a.rfind("-spectrum=", 0) == 0) spectrum_file = a.substr(10);
-        else if (a.rfind("-spectrumbin=", 0) == 0) spectrum_bin = a.substr(13);
-        else if (a.rfind("-spectrumint=", 0) == 0) spectrum_int = a.substr(13);
-        else if (a == "-spectrumpeak" || a == "-spectrumpeak=true") spectrum_peak = true;
-        else files.push_back(a);
+        else if (a.rfind("-blocks=", 0) == 0) o.blocks = atoll(a.c_str() + 8);
+        else if (a.rfind("-blockdedup=", 0) == 0) o.block_dedup = a.substr(12) != "false";
+        else if (a.rfind("-filterid=", 0) == 0) o.filterid = a.substr(10);
+        else if (a.rfind("-filtertype=", 0) == 0) o.filtertype = a.substr(12);
+        else if (a.rfind("-unique=", 0) == 0) o.unique = a.substr(8) == "true";
+        else if (a == "-unique") o.unique = true;
+        else if (a.rfind("-format=", 0) == 0) o.format = a.substr(8);
+        else if (a.rfind("-samplefile=", 0) == 0) o.samplefile = a.substr(12);
+        else if (a.rfind("-single=", 0) == 0) o.single = a.substr(8) == "true";
+        else if (a == "-signal" || a == "-signal=true") o.signal = true;
+        else if (a == "-signal=false") o.signal = false;
+        else if (a == "-single") o.single = true;
+        else if (a.rfind("-duration=", 0) == 0) o.duration = a.substr(10);
+        else if (a == "-quiet") o.quiet = true;
+        else if (a.rfind("-spectrum=", 0) == 0) o.spectrum_file = a.substr(10);
+        else if (a.rfind("-spectrumbin=", 0) == 0) o.spectrum_bin = a.substr(13);
+        else if (a.rfind("-spectrumint=", 0) == 0) o.spectrum_int = a.substr(13);
+        else if (a == "-spectrumpeak" || a == "-spectrumpeak=true") o.spectrum_peak = true;
+        else o.files.push_back(a);
     }
-    if (files.empty()) {
-        fprintf(stderr, "usage: %s [-msgtype=scm,scm+,idm,netidm,r900,r900bcd|all] [-symbollength=N] [-blockdedup=true|false] "
-                        "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
-                        "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|wav|sigmf] "
-                        "[-samplescale=G|auto] [-channelgain=G|auto] [-signal] "
-                        "[-spectrum=FILE [-spectrumbin=HZ] [-spectrumint=D] [-spectrumpeak]] "
-                        "[-capturefreq=HZ [-centerfreq=HZ[,HZ...]]] [-quiet] FILE|- [FILE ...]\n", argv[0]);
-        return 2;
-    }
+    if (o.files.empty())
+        usage("usage: %s [-msgtype=scm,scm+,idm,netidm,r900,r900bcd|all] [-symbollength=N] [-blockdedup=true|false] "
+              "[-blocks=K] [-device=D] [-filterid=ID,..] [-filtertype=T,..] [-unique=true|false] [-format=plain|csv|json|xml] "
+              "[-samplefile=PATH] [-single] [-duration=D] [-samplerate=HZ] [-sampleformat=cu8|cs8|cs16|cf32|ci16_be|...|wav|sigmf] "
+              "[-samplescale=G|auto] [-channelgain=G|auto] [-signal] "
+              "[-spectrum=FILE [-spectrumbin=HZ] [-spectrumint=D] [-spectrumpeak]] "
+              "[-capturefreq=HZ [-centerfreq=HZ[,HZ...]]] [-quiet] FILE|- [FILE ...]", argv[0]);
+    return o;
+}
+
+// What the flags and the files' headers say about the capture, checked.
+struct Capture {
+    int64_t decoder_rate = 0;   // DataRate * ChipLength = 32768 * -symbollength
+    int64_t rate = 0;           // the capture's: -samplerate, the WAV header or the SigMF metadata, or decoder_rate
+    bool resampling = false;    // rate != decoder_rate
+    bool wav_in = false, sigmf_in = false;
+    int32_t fmt = ERTGPU_FORMAT_CU8;
+    float scale = 0.0f;
+    bool auto_scale = false, auto_channel = false;
+    int32_t channel_k = -1;    // -channelgain: k of G = 2^k
+    long long capture_hz = 0, center_hz = 0;
+    std::vector<int64_t> channels;   // -centerfreq=F1,F2,...
+    int64_t limit_ns = 0;
+    bool writes_samples = false;   // -samplefile names a file: os.DevNull, the default, is never opened (flags.go:136-141)
+    receiver::Format out = receiver::PLAIN;
+    FILE* spectrum_out = nullptr;
+    int32_t spectrum_log2 = 0;
+    int64_t spectrum_frames = 0;
+    std::vector<wav::Header> wav_hdr;
+    std::vector<sigmf::Recording> rec;
+};
+
+Capture resolve(const Options& o) {
+    Capture c;
+    c.decoder_rate = 32768LL * o.chip;
     // -capturefreq / -centerfreq: whole Hz, > 0 and >= 0; -centerfreq may be a comma list of channels
     std::vector<std::string> centers;
-    for (size_t p = 0; !centerfreq.empty();) {
-        const size_t q = centerfreq.find(',', p);
-        centers.push_back(centerfreq.substr(p, q == std::string::npos ? std::string::npos : q - p));
+    for (size_t p = 0; !o.centerfreq.empty();) {
+        const size_t q = o.centerfreq.find(',', p);
+        centers.push_back(o.centerfreq.substr(p, q == std::string::npos ? std::string::npos : q - p));
         if (q == std::string::npos) break;
         p = q + 1;
     }
-    long long capture_hz = 0, center_hz = 0;
-    std::vector<long long> list;
-    std::vector<std::tuple<const char*, const std::string*, long long*, long long>> freqs = {
-        std::make_tuple("-capturefreq", &capturefreq, &capture_hz, 1LL)};
-    if (centers.size() == 1) freqs.push_back(std::make_tuple("-centerfreq", &centerfreq, &center_hz, 0LL));
-    list.resize(centers.size() > 1 ? centers.size() : 0);
-    for (size_t c = 0; c < list.size(); c++) freqs.push_back(std::make_tuple("-centerfreq", &centers[c], &list[c], 1LL));
-    for (auto [flag, text, out, min] : freqs) {
-        if (text->empty() && text == &capturefreq) continue;
+    const auto hz = [](const char* flag, const std::string& text, long long min) {
         char* end = nullptr;
         errno = 0;
-        *out = strtoll(text->c_str(), &end, 10);
-        if (text->empty() || *end || errno || *out < min) {
-            fprintf(stderr, "invalid value \"%s\" for flag %s: a frequency in Hz%s\n", text->c_str(), flag, min ? " > 0" : "");
-            return 2;
-        }
-    }
-    const std::vector<int64_t> channels(list.begin(), list.end());
-    for (size_t c = 0; c < channels.size(); c++)
-        for (size_t j = 0; j < c; j++)
-            if (channels[c] == channels[j]) {
-                fprintf(stderr, "-centerfreq names the channel %lld Hz twice\n", (long long)channels[c]);
-                return 2;
-            }
-    const bool csv = format == "csv", json = format == "json", xml = format == "xml";
-    int64_t limit_ns = 0;
+        const long long v = strtoll(text.c_str(), &end, 10);
+        if (text.empty() || *end || errno || v < min)
+            usage("invalid value \"%s\" for flag %s: a frequency in Hz%s", text.c_str(), flag, min ? " > 0" : "");
+        return v;
+    };
+    if (!o.capturefreq.empty()) c.capture_hz = hz("-capturefreq", o.capturefreq, 1);
+    if (centers.size() == 1) c.center_hz = hz("-centerfreq", o.centerfreq, 0);
+    else
+        for (const std::string& t : centers) c.channels.push_back(hz("-centerfreq", t, 1));
+    for (size_t i = 0; i < c.channels.size(); i++)
+        for (size_t j = 0; j < i; j++)
+            if (c.channels[i] == c.channels[j]) usage("-centerfreq names the channel %lld Hz twice", (long long)c.channels[i]);
+    c.out = o.format == "csv" ? receiver::CSV : o.format == "json" ? receiver::JSON : o.format == "xml" ? receiver::XML : receiver::PLAIN;
     try {
-        if (!duration.empty()) limit_ns = receiver::ParseDuration(duration);
+        if (!o.duration.empty()) c.limit_ns = receiver::ParseDuration(o.duration);
     } catch (const std::exception& e) {
-        fprintf(stderr, "invalid value \"%s\" for flag -duration: %s\n", duration.c_str(), e.what());
-        return 2;
+        usage("invalid value \"%s\" for flag -duration: %s", o.duration.c_str(), e.what());
     }
-    if (spectrum_file.empty() && (!spectrum_bin.empty() || !spectrum_int.empty() || spectrum_peak)) {
-        fprintf(stderr, "-spectrumbin, -spectrumint and -spectrumpeak need -spectrum=FILE\n");
-        return 2;
-    }
+    if (o.spectrum_file.empty() && (!o.spectrum_bin.empty() || !o.spectrum_int.empty() || o.spectrum_peak))
+        usage("-spectrumbin, -spectrumint and -spectrumpeak need -spectrum=FILE");
     double spectrum_hz = 10000;
     int64_t spectrum_ns = 1000000000;
-    if (!spectrum_bin.empty()) {
+    if (!o.spectrum_bin.empty()) {
         char* end = nullptr;
-        spectrum_hz = strtod(spectrum_bin.c_str(), &end);
-        if (*end || !std::isfinite(spectrum_hz) || spectrum_hz <= 0) {
-            fprintf(stderr, "invalid value \"%s\" for flag -spectrumbin: a bin width in Hz > 0\n", spectrum_bin.c_str());
-            return 2;
-        }
+        spectrum_hz = strtod(o.spectrum_bin.c_str(), &end);
+        if (*end || !std::isfinite(spectrum_hz) || spectrum_hz <= 0)
+            usage("invalid value \"%s\" for flag -spectrumbin: a bin width in Hz > 0", o.spectrum_bin.c_str());
     }
-    if (!spectrum_int.empty()) {
+    if (!o.spectrum_int.empty()) {
         try {
-            spectrum_ns = receiver::ParseDuration(spectrum_int);
+            spectrum_ns = receiver::ParseDuration(o.spectrum_int);
         } catch (const std::exception& e) {
-            fprintf(stderr, "invalid value \"%s\" for flag -spectrumint: %s\n", spectrum_int.c_str(), e.what());
-            return 2;
+            usage("invalid value \"%s\" for flag -spectrumint: %s", o.spectrum_int.c_str(), e.what());
         }
-        if (spectrum_ns < 0) {
-            fprintf(stderr, "invalid value \"%s\" for flag -spectrumint: a duration >= 0\n", spectrum_int.c_str());
-            return 2;
-        }
+        if (spectrum_ns < 0) usage("invalid value \"%s\" for flag -spectrumint: a duration >= 0", o.spectrum_int.c_str());
     }
-    FILE* spectrum_out = nullptr;
-    if (!spectrum_file.empty() && !(spectrum_out = fopen(spectrum_file.c_str(), "w"))) {
-        fprintf(stderr, "-spectrum=%s: %s\n", spectrum_file.c_str(), strerror(errno));
-        return 2;
-    }
-    const bool wav_in = sampleformat == "wav", sigmf_in = sampleformat == "sigmf";
-    int32_t fmt = ERTGPU_FORMAT_CU8;
-    if (sampleformat == "cs8") fmt = ERTGPU_FORMAT_CS8;
-    else if (sampleformat == "cs16") fmt = ERTGPU_FORMAT_CS16;
-    else if (sampleformat == "cf32") fmt = ERTGPU_FORMAT_CF32;
-    else if (!wav_in && !sigmf_in && (fmt = sigmf::FormatOf(sampleformat)) < 0) {
-        fprintf(stderr, "invalid value \"%s\" for flag -sampleformat: cu8, cs8, cs16, cf32, a complex SigMF datatype "
-                        "(ci16_be, cf64_le, ...), wav or sigmf\n", sampleformat.c_str());
-        return 2;
-    }
-    float scale = 0.0f;
-    if (samplescale == "auto") {
-        auto_scale = true;
-    } else if (have_scale) {
+    if (!o.spectrum_file.empty() && !(c.spectrum_out = fopen(o.spectrum_file.c_str(), "w")))
+        usage("-spectrum=%s: %s", o.spectrum_file.c_str(), strerror(errno));
+    c.wav_in = o.sampleformat == "wav";
+    c.sigmf_in = o.sampleformat == "sigmf";
+    if (!c.wav_in && !c.sigmf_in && (c.fmt = ertfmt_from_name(o.sampleformat.c_str())) < 0)
+        usage("invalid value \"%s\" for flag -sampleformat: cu8, cs8, cs16, cf32, a complex SigMF datatype "
+              "(ci16_be, cf64_le, ...), wav or sigmf", o.sampleformat.c_str());
+    if (o.samplescale == "auto") {
+        c.auto_scale = true;
+    } else if (o.have_scale) {
         char* end = nullptr;
-        scale = strtof(samplescale.c_str(), &end);
-        if (samplescale.empty() || *end || !std::isfinite(scale) || scale <= 0.0f) {
-            fprintf(stderr, "invalid value \"%s\" for flag -samplescale: a finite gain > 0, or auto\n", samplescale.c_str());
-            return 2;
-        }
+        c.scale = strtof(o.samplescale.c_str(), &end);
+        if (o.samplescale.empty() || *end || !std::isfinite(c.scale) || c.scale <= 0.0f)
+            usage("invalid value \"%s\" for flag -samplescale: a finite gain > 0, or auto", o.samplescale.c_str());
     }
-    int32_t channel_k = -1;   // -channelgain: k of G = 2^k
-    const bool auto_channel = channelgain == "auto";
-    if (!channelgain.empty() && !auto_channel) {
+    c.auto_channel = o.channelgain == "auto";
+    if (!o.channelgain.empty() && !c.auto_channel) {
         char* end = nullptr;
-        const long long g = strtoll(channelgain.c_str(), &end, 10);
-        if (*end || g < 1 || g > (1LL << ERTRS_GAIN_K_MAX) || (g & (g - 1))) {
-            fprintf(stderr, "invalid value \"%s\" for flag -channelgain: a power of two 1 ... %lld, or auto\n", channelgain.c_str(),
-                    1LL << ERTRS_GAIN_K_MAX);
-            return 2;
-        }
-        channel_k = 63 - __builtin_clzll((unsigned long long)g);
+        const long long g = strtoll(o.channelgain.c_str(), &end, 10);
+        if (*end || g < 1 || g > (1LL << ERTRS_GAIN_K_MAX) || (g & (g - 1)))
+            usage("invalid value \"%s\" for flag -channelgain: a power of two 1 ... %lld, or auto", o.channelgain.c_str(),
+                  1LL << ERTRS_GAIN_K_MAX);
+        c.channel_k = 63 - __builtin_clzll((unsigned long long)g);
     }
-    // wav: every file's header, before anything else (stdin's is consumed here, the files' are read again below)
-    std::vector<wav::Header> wav_hdr(files.size());
-    if (wav_in) {
+    const std::vector<std::string>& files = o.files;
+    long long samplerate = o.samplerate;
+    // wav: every file's header, before anything else (stdin's is consumed here, the files' are read again by the run)
+    c.wav_hdr.resize(files.size());
+    if (c.wav_in) {
         for (size_t fi = 0; fi < files.size(); fi++) {
             FILE* in = files[fi] == "-" ? stdin : fopen(files[fi].c_str(), "rb");
-            if (!in) {
-                perror(files[fi].c_str());
-                return 1;
-            }
+            if (!in) throw file_error(files[fi]);
             try {
-                wav_hdr[fi] = wav::ReadHeader(in);
+                c.wav_hdr[fi] = wav::ReadHeader(in);
             } catch (const std::exception& e) {
-                fprintf(stderr, "%s: %s\n", files[fi].c_str(), e.what());
                 if (in != stdin) fclose(in);
-                return 1;
+                throw Exit{1, files[fi] + ": " + e.what()};
             }
             if (in != stdin) fclose(in);
-            if (wav_hdr[fi].rate != wav_hdr[0].rate || wav_hdr[fi].format != wav_hdr[0].format) {
-                fprintf(stderr, "%s: %lld Hz, format %d, but %s: %lld Hz, format %d: the files of a batch share one decoder\n",
-                        files[0].c_str(), (long long)wav_hdr[0].rate, wav_hdr[0].format, files[fi].c_str(),
-                        (long long)wav_hdr[fi].rate, wav_hdr[fi].format);
-                return 2;
-            }
+            const wav::Header &h0 = c.wav_hdr[0], &h = c.wav_hdr[fi];
+            if (h.rate != h0.rate || h.format != h0.format)
+                usage("%s: %lld Hz, format %d, but %s: %lld Hz, format %d: the files of a batch share one decoder", files[0].c_str(),
+                      (long long)h0.rate, h0.format, files[fi].c_str(), (long long)h.rate, h.format);
         }
-        if (samplerate != 0 && samplerate != wav_hdr[0].rate) {
-            fprintf(stderr, "-samplerate=%lld disagrees with the WAV header's %lld Hz\n", samplerate, (long long)wav_hdr[0].rate);
-            return 2;
-        }
-        samplerate = wav_hdr[0].rate;
-        fmt = wav_hdr[0].format;
+        if (samplerate != 0 && samplerate != c.wav_hdr[0].rate)
+            usage("-samplerate=%lld disagrees with the WAV header's %lld Hz", samplerate, (long long)c.wav_hdr[0].rate);
+        samplerate = c.wav_hdr[0].rate;
+        c.fmt = c.wav_hdr[0].format;
     }
     // sigmf: every recording's metadata, before anything else
-    std::vector<sigmf::Recording> rec(files.size());
-    if (sigmf_in) {
+    c.rec.resize(files.size());
+    if (c.sigmf_in) {
         for (size_t fi = 0; fi < files.size(); fi++) {
-            if (files[fi] == "-") {
-                fprintf(stderr, "-sampleformat=sigmf reads NAME.sigmf-meta beside NAME.sigmf-data, not stdin\n");
-                return 2;
-            }
+            if (files[fi] == "-") usage("-sampleformat=sigmf reads NAME.sigmf-meta beside NAME.sigmf-data, not stdin");
             try {
-                rec[fi] = sigmf::Read(files[fi]);
+                c.rec[fi] = sigmf::Read(files[fi]);
             } catch (const std::exception& e) {
-                fprintf(stderr, "%s: %s\n", files[fi].c_str(), e.what());
-                return 1;
+                throw Exit{1, files[fi] + ": " + e.what()};
             }
-            if (rec[fi].rate != rec[0].rate || rec[fi].format != rec[0].format || rec[fi].frequency != rec[0].frequency) {
-                fprintf(stderr, "%s: %s at %lld Hz, %lld Hz, but %s: %s at %lld Hz, %lld Hz: the files of a batch share one decoder\n",
-                        files[0].c_str(), sigmf::FormatName(rec[0].format), (long long)rec[0].rate, (long long)rec[0].frequency,
-                        files[fi].c_str(), sigmf::FormatName(rec[fi].format), (long long)rec[fi].rate, (long long)rec[fi].frequency);
-                return 2;
-            }
+            const sigmf::Recording &r0 = c.rec[0], &r = c.rec[fi];
+            if (r.rate != r0.rate || r.format != r0.format || r.frequency != r0.frequency)
+                usage("%s: %s at %lld Hz, %lld Hz, but %s: %s at %lld Hz, %lld Hz: the files of a batch share one decoder",
+                      files[0].c_str(), ertfmt_name(r0.format), (long long)r0.rate, (long long)r0.frequency, files[fi].c_str(),
+                      ertfmt_name(r.format), (long long)r.rate, (long long)r.frequency);
         }
-        if (samplerate != 0 && samplerate != rec[0].rate) {
-            fprintf(stderr, "-samplerate=%lld disagrees with the SigMF core:sample_rate %lld Hz\n", samplerate, (long long)rec[0].rate);
-            return 2;
-        }
-        if (capture_hz != 0 && rec[0].frequency != 0 && capture_hz != rec[0].frequency) {
-            fprintf(stderr, "-capturefreq=%lld disagrees with the SigMF core:frequency %lld Hz\n", capture_hz, (long long)rec[0].frequency);
-            return 2;
-        }
-        samplerate = rec[0].rate;
-        fmt = rec[0].format;
-        if (rec[0].frequency) capture_hz = rec[0].frequency;
+        const sigmf::Recording& r0 = c.rec[0];
+        if (samplerate != 0 && samplerate != r0.rate)
+            usage("-samplerate=%lld disagrees with the SigMF core:sample_rate %lld Hz", samplerate, (long long)r0.rate);
+        if (c.capture_hz != 0 && r0.frequency != 0 && c.capture_hz != r0.frequency)
+            usage("-capturefreq=%lld disagrees with the SigMF core:frequency %lld Hz", c.capture_hz, (long long)r0.frequency);
+        samplerate = r0.rate;
+        c.fmt = r0.format;
+        if (r0.frequency) c.capture_hz = r0.frequency;
     }
-    if (!centerfreq.empty() && capture_hz == 0) {
-        fprintf(stderr, "-centerfreq needs -capturefreq: the frequency at the centre of the capture\n");
-        return 2;
-    }
-    if (!channels.empty() && !samplefile.empty() && samplefile != "/dev/null") {
-        fprintf(stderr, "-samplefile takes one channel, not a -centerfreq list\n");
-        return 2;
-    }
-    for (const int64_t ch : channels) {   // each channel of a list lies inside the capture (ertrs_plan_decimated's rule)
-        const int64_t rate = samplerate ? samplerate : 32768LL * chip;
+    c.rate = samplerate ? samplerate : c.decoder_rate;
+    // -samplerate names the capture's rate; the default DataRate*ChipLength (32768 * -symbollength) resamples nothing
+    c.resampling = samplerate != 0 && samplerate != c.decoder_rate;
+    c.writes_samples = !o.samplefile.empty() && o.samplefile != "/dev/null";
+    if (!o.centerfreq.empty() && c.capture_hz == 0) usage("-centerfreq needs -capturefreq: the frequency at the centre of the capture");
+    if (!c.channels.empty() && c.writes_samples) usage("-samplefile takes one channel, not a -centerfreq list");
+    for (const int64_t ch : c.channels) {   // each channel of a list lies inside the capture (ertrs_plan_decimated's rule)
         ertgpu_decimator_info d{};
         ertgpu_resampler_info info{};
-        if (ertrs_plan_decimated(rate, 32768LL * chip, ch - capture_hz, &d, &info) != 0) {
-            fprintf(stderr, "-centerfreq channel %lld Hz does not fit a %lld Hz capture at %lld Hz: |offset| + 0.4 * %lld Hz "
-                            "must be at most half the capture's rate\n", (long long)ch, (long long)rate, capture_hz, 32768LL * chip);
-            return 2;
-        }
+        if (ertrs_plan_decimated(c.rate, c.decoder_rate, ch - c.capture_hz, &d, &info) != 0)
+            usage("-centerfreq channel %lld Hz does not fit a %lld Hz capture at %lld Hz: |offset| + 0.4 * %lld Hz "
+                  "must be at most half the capture's rate", (long long)ch, (long long)c.rate, c.capture_hz, (long long)c.decoder_rate);
     }
-    const bool tuned = capture_hz > 0;
-    if (!channelgain.empty() && !tuned) {
-        fprintf(stderr, "-channelgain needs -capturefreq (or a SigMF frequency): the channel path of a tuned capture\n");
-        return 2;
+    const bool tuned = c.capture_hz > 0;
+    if (!o.channelgain.empty() && !tuned)
+        usage("-channelgain needs -capturefreq (or a SigMF frequency): the channel path of a tuned capture");
+    if (o.have_scale && c.fmt == ERTGPU_FORMAT_CU8) usage("-samplescale does not apply to uint8 (cu8) input");
+    if (tuned && c.writes_samples) usage("-samplefile does not take tuned (-capturefreq) input");
+    if ((c.resampling || c.fmt != ERTGPU_FORMAT_CU8) && c.writes_samples)
+        usage("-samplefile needs uint8 (cu8) input at 32768 * -symbollength = %lld Hz; this input is %s at %lld Hz",
+              (long long)c.decoder_rate, ertfmt_name(c.fmt), (long long)c.rate);
+    if (c.spectrum_out) {
+        c.spectrum_log2 = ertspec_log2_for_bin(c.rate, spectrum_hz);
+        c.spectrum_frames = ertspec_frames_per_row(c.spectrum_log2, spectrum_ns, c.rate);
     }
-    if (have_scale && fmt == ERTGPU_FORMAT_CU8) {
-        fprintf(stderr, "-samplescale does not apply to uint8 (cu8) input\n");
-        return 2;
-    }
-    // -samplerate names the capture's rate; the default DataRate*ChipLength (32768 * -symbollength) resamples nothing
-    const bool resampling = samplerate != 0 && samplerate != 32768LL * chip;
-    if (tuned && !samplefile.empty() && samplefile != "/dev/null") {
-        fprintf(stderr, "-samplefile does not take tuned (-capturefreq) input\n");
-        return 2;
-    }
-    if ((resampling || fmt != ERTGPU_FORMAT_CU8) && !samplefile.empty() && samplefile != "/dev/null") {
-        fprintf(stderr, "-samplefile needs uint8 (cu8) input at 32768 * -symbollength = %lld Hz; this input is %s at %lld Hz\n",
-                32768LL * chip, sigmf::FormatName(fmt),
-                samplerate ? samplerate : 32768LL * chip);
-        return 2;
-    }
-    FILE* sample = nullptr;   // os.DevNull, the default, is never opened (flags.go:136-141)
-    if (!samplefile.empty() && samplefile != "/dev/null") {
-        sample = fopen(samplefile.c_str(), "wb");
-        if (!sample) {
-            perror(samplefile.c_str());
-            return 1;
-        }
-    }
-    const int64_t rate_in = samplerate ? samplerate : 32768LL * chip;
-    const int32_t spectrum_log2 = spectrum_out ? ertspec_log2_for_bin(rate_in, spectrum_hz) : 0;
-    const int64_t spectrum_frames = spectrum_out ? ertspec_frames_per_row(spectrum_log2, spectrum_ns, rate_in) : 0;
+    return c;
+}
+
+// The batch: every file through one receiver, then the files closed.  Returns the exit status.
+int run(const Options& o, Capture& c, std::chrono::steady_clock::time_point start) {
+    FILE* sample = nullptr;
+    if (c.writes_samples && !(sample = fopen(o.samplefile.c_str(), "wb"))) throw file_error(o.samplefile);
+    const std::vector<std::string>& files = o.files;
     try {
-        receiver::Receiver rcvr(msgtype, chip, device, blocks, {resampling ? samplerate : 0, fmt, scale, capture_hz, center_hz, auto_scale, channel_k, auto_channel, signal,
-                                                                spectrum_log2, spectrum_frames},
-                                channels);
-        const int64_t spectrum_centre = capture_hz ? capture_hz : (int64_t)rcvr.decoder().Cfg.CenterFreq;
+        receiver::Receiver rcvr(o.msgtype, o.chip, o.device, o.blocks,
+                                {c.resampling ? c.rate : 0, c.fmt, c.scale, c.capture_hz, c.center_hz, c.auto_scale, c.channel_k,
+                                 c.auto_channel, o.signal, c.spectrum_log2, c.spectrum_frames},
+                                c.channels);
+        const protocol::PacketConfig& cfg = rcvr.decoder().Cfg;
+        const int64_t spectrum_centre = c.capture_hz ? c.capture_hz : (int64_t)cfg.CenterFreq;
         std::vector<char> line;
         std::string log = rcvr.decoder().Log();
-        if (!channels.empty()) {   // the channels share everything of the log but CenterFreq, its first line: name them all
+        if (!c.channels.empty()) {   // the channels share everything of the log but CenterFreq, its first line: name them all
             std::string names;
-            for (size_t c = 0; c < channels.size(); c++) names += (c ? "," : "") + std::to_string(channels[c]);
+            for (size_t i = 0; i < c.channels.size(); i++) names += (i ? "," : "") + std::to_string(c.channels[i]);
             log = "CenterFreq: " + names + log.substr(log.find('\n'));
         }
         fputs(log.c_str(), stderr);
         if (sample) rcvr.SetSampleFile(sample);
-        if (limit_ns) rcvr.SetDeadline(start + std::chrono::nanoseconds(limit_ns));
-        if (single) rcvr.SetSingle(nullptr);
-        // the order flag.Visit gives the chain (main.go:97-113): filterid, filtertype, unique
-        if (!filterid.empty()) {
-            auto f = std::make_shared<receiver::MeterIDFilter>();
-            f->ids.Set(filterid);
-            rcvr.filters().Add(f);
-            if (single) rcvr.SetSingle(&f->ids);   // main.go:278: -single empties the filter's own set
-        }
-        if (!filtertype.empty()) {
-            auto f = std::make_shared<receiver::MeterTypeFilter>();
-            f->types.Set(filtertype);
-            rcvr.filters().Add(f);
-        }
-        if (unique) rcvr.filters().Add(std::make_shared<receiver::UniqueFilter>());
+        if (c.limit_ns) rcvr.SetDeadline(start + std::chrono::nanoseconds(c.limit_ns));
+        receiver::UintMap* ids = nullptr;
+        rcvr.filters() = receiver::NewFilterChain(o.filterid, o.filtertype, o.unique, &ids);
+        if (o.single) rcvr.SetSingle(ids);   // main.go:278: -single empties the -filterid filter's own set
         for (size_t fi = 0; fi < files.size(); fi++) {
             const std::string& file = files[fi];
-            FILE* in = sigmf_in ? sigmf::OpenSamples(rec[fi]) : file == "-" ? stdin : fopen(file.c_str(), "rb");
-            if (!in) {
-                perror(file.c_str());
-                return 1;
-            }
+            const std::string prefix = files.size() > 1 ? file + ": " : "";
+            const bool dated = c.sigmf_in && sigmf::Dated(c.rec[fi]);
+            FILE* in = c.sigmf_in ? sigmf::OpenSamples(c.rec[fi]) : file == "-" ? stdin : fopen(file.c_str(), "rb");
+            if (!in) throw file_error(file);
             if (fi) rcvr.Reset();
-            if (auto_scale)
+            if (c.auto_scale)
                 rcvr.SetLevelReport([&](const ertgpu_input_level& lv) {
-                    fprintf(stderr, "%s%s-samplescale=auto: 2^%d = %.9g from %lld samples\n", files.size() > 1 ? file.c_str() : "",
-                            files.size() > 1 ? ": " : "", lv.exponent, (double)lv.scale, (long long)(lv.components / 2));
+                    fprintf(stderr, "%s-samplescale=auto: 2^%d = %.9g from %lld samples\n", prefix.c_str(), lv.exponent,
+                            (double)lv.scale, (long long)(lv.components / 2));
                 });
-            if (auto_channel)
-                rcvr.SetChannelLevelReport([&](size_t c, const ertgpu_channel_level& lv) {
+            if (c.auto_channel)
+                rcvr.SetChannelLevelReport([&](size_t ch, const ertgpu_channel_level& lv) {
                     ertgpu_tuning_info t{};
-                    ertgpu_get_tuning(rcvr.decoder(c).Handle(), &t);
-                    fprintf(stderr, "%s%schannel %lld: 2^%d = %lld\n", files.size() > 1 ? file.c_str() : "", files.size() > 1 ? ": " : "",
-                            (long long)t.center_hz, lv.k, 1LL << lv.k);
+                    ertgpu_get_tuning(rcvr.decoder(ch).Handle(), &t);
+                    fprintf(stderr, "%schannel %lld: 2^%d = %lld\n", prefix.c_str(), (long long)t.center_hz, lv.k, 1LL << lv.k);
                 });
-            if (wav_in && in != stdin) wav_hdr[fi] = wav::ReadHeader(in);   // the same header as above: to the samples
-            const auto spectrum_rows = [&](const protocol::SpectrumRows& r) {
-                for (size_t i = 0; i < r.rows.size(); i++) {
-                    const int64_t s0 = r.rows[i].first_sample;
-                    int64_t ns = s0 / rate_in * 1000000000 + s0 % rate_in * 1000000000 / rate_in;   // stream time
-                    if (sigmf_in && sigmf::Dated(rec[fi])) ns = sigmf::BlockTime(rec[fi], s0 - 1, 1, rec[0].rate);
-                    const int64_t sec = ns / 1000000000 - (ns % 1000000000 < 0);
-                    const float* p = (spectrum_peak ? r.peak.data() : r.mean.data()) + i * (size_t)r.N;
-                    const int len = ertspec_csv_line(nullptr, 0, sec, spectrum_centre, rate_in, spectrum_log2,
-                                                     r.rows[i].frames * r.N, p);
-                    line.resize((size_t)len + 1);
-                    ertspec_csv_line(line.data(), line.size(), sec, spectrum_centre, rate_in, spectrum_log2, r.rows[i].frames * r.N, p);
-                    if (fputs(line.data(), spectrum_out) < 0) throw std::runtime_error("writing the -spectrum file failed");
-                }
-            };
-            auto st = rcvr.Run(in, block_dedup, [&](const protocol::Message& m, int64_t offset, int length) {
-                if (quiet) return;
-                if (csv || json || xml) {
-                    receiver::LogMessage lm;
-                    if (sigmf_in && sigmf::Dated(rec[fi])) {
-                        const protocol::PacketConfig& c = rcvr.decoder().Cfg;
-                        const int64_t ns = sigmf::BlockTime(rec[fi], m.Block, c.BlockSize, c.SampleRate);
-                        lm.unix_seconds = ns / 1000000000 - (ns % 1000000000 < 0);
-                        lm.nanos = (int32_t)(ns - lm.unix_seconds * 1000000000);
-                    } else {
-                        timespec ts{};
-                        clock_gettime(CLOCK_REALTIME, &ts);
-                        lm.unix_seconds = (int64_t)ts.tv_sec;
-                        lm.nanos = (int32_t)ts.tv_nsec;
+            if (c.wav_in && in != stdin) c.wav_hdr[fi] = wav::ReadHeader(in);   // the same header as before: to the samples
+            std::function<void(const protocol::SpectrumRows&)> rows;
+            if (c.spectrum_out)
+                rows = [&](const protocol::SpectrumRows& r) {
+                    for (size_t i = 0; i < r.rows.size(); i++) {
+                        const int64_t s0 = r.rows[i].first_sample;
+                        int64_t ns = s0 / c.rate * 1000000000 + s0 % c.rate * 1000000000 / c.rate;   // stream time
+                        if (dated) ns = sigmf::BlockTime(c.rec[fi], s0 - 1, 1, c.rec[0].rate);
+                        const int64_t sec = ns / 1000000000 - (ns % 1000000000 < 0);
+                        const float* p = (o.spectrum_peak ? r.peak.data() : r.mean.data()) + i * (size_t)r.N;
+                        const int len = ertspec_csv_line(nullptr, 0, sec, spectrum_centre, c.rate, c.spectrum_log2,
+                                                         r.rows[i].frames * r.N, p);
+                        line.resize((size_t)len + 1);
+                        ertspec_csv_line(line.data(), line.size(), sec, spectrum_centre, c.rate, c.spectrum_log2,
+                                         r.rows[i].frames * r.N, p);
+                        if (fputs(line.data(), c.spectrum_out) < 0) throw std::runtime_error("writing the -spectrum file failed");
                     }
-                    lm.Offset = offset;
-                    lm.Length = length;
-                    lm.Message = &m;
-                    fputs((csv ? receiver::CsvLine(lm.Record()) : json ? receiver::JsonLine(lm) : receiver::XmlLine(lm)).c_str(), stdout);
-                } else {
+                };
+            const auto st = rcvr.Run(in, o.block_dedup, [&](const protocol::Message& m, int64_t offset, int length) {
+                if (o.quiet) return;
+                if (c.out == receiver::PLAIN) {
                     printf("%s\n", receiver::BlockLine(m).c_str());
+                    return;
                 }
-            }, wav_in ? wav_hdr[fi].data_size : -1, spectrum_out ? std::function<void(const protocol::SpectrumRows&)>(spectrum_rows)
-                                                                : std::function<void(const protocol::SpectrumRows&)>());
+                receiver::LogMessage lm;
+                if (dated) {
+                    const int64_t ns = sigmf::BlockTime(c.rec[fi], m.Block, cfg.BlockSize, cfg.SampleRate);
+                    lm.unix_seconds = ns / 1000000000 - (ns % 1000000000 < 0);
+                    lm.nanos = (int32_t)(ns - lm.unix_seconds * 1000000000);
+                } else {
+                    timespec ts{};
+                    clock_gettime(CLOCK_REALTIME, &ts);
+                    lm.unix_seconds = (int64_t)ts.tv_sec;
+                    lm.nanos = (int32_t)ts.tv_nsec;
+                }
+                lm.Offset = offset;
+                lm.Length = length;
+                lm.Message = &m;
+                fputs(receiver::Line(c.out, lm).c_str(), stdout);
+            }, c.wav_in ? c.wav_hdr[fi].data_size : -1, rows);
             if (in != stdin) fclose(in);
-            fprintf(stderr, "%s%s%lld messages (%lld duplicates dropped) from %lld blocks, %.1f MB in %.3f s = %.1f Msamples/s\n",
-                    files.size() > 1 ? file.c_str() : "", files.size() > 1 ? ": " : "", (long long)st.messages,
-                    (long long)st.duplicates, (long long)st.blocks, st.bytes / 1e6, st.seconds,
-                    st.samples / 1e6 / (st.seconds > 0 ? st.seconds : 1));
-            for (size_t c = 0; c < channels.size(); c++)
-                fprintf(stderr, "%s%s%lld Hz: %lld messages\n", files.size() > 1 ? file.c_str() : "", files.size() > 1 ? ": " : "",
-                        (long long)channels[c], (long long)st.channel_messages[c]);
+            fprintf(stderr, "%s%lld messages (%lld duplicates dropped) from %lld blocks, %.1f MB in %.3f s = %.1f Msamples/s\n",
+                    prefix.c_str(), (long long)st.messages, (long long)st.duplicates, (long long)st.blocks, st.bytes / 1e6,
+                    st.seconds, st.samples / 1e6 / (st.seconds > 0 ? st.seconds : 1));
+            for (size_t ch = 0; ch < c.channels.size(); ch++)
+                fprintf(stderr, "%s%lld Hz: %lld messages\n", prefix.c_str(), (long long)c.channels[ch],
+                        (long long)st.channel_messages[ch]);
             if (st.stopped) break;
         }
     } catch (const std::exception& e) {
         fprintf(stderr, "error: %s\n", e.what());
         if (sample) fclose(sample);
-        if (spectrum_out) fclose(spectrum_out);
+        if (c.spectrum_out) fclose(c.spectrum_out);
         return 1;
     }
-    if (spectrum_out && fclose(spectrum_out) != 0) {
-        perror(spectrum_file.c_str());
+    if (c.spectrum_out && fclose(c.spectrum_out) != 0) {
+        perror(o.spectrum_file.c_str());
         return 1;
     }
     if (sample && fclose(sample) != 0) {
-        perror(samplefile.c_str());
+        perror(o.samplefile.c_str());
         return 1;
     }
     return 0;
+}
+
+}  // namespace
+
+int main(int argc, char** argv) {
+    const auto start = std::chrono::steady_clock::now();   // main.go:350-353: the time limit covers the whole run
+    try {
+        const Options o = parse_flags(argc, argv);
+        Capture c = resolve(o);
+        return run(o, c, start);
+    } catch (const Exit& e) {
+        fprintf(stderr, "%s\n", e.message.c_str());
+        return e.code;
+    }
 }

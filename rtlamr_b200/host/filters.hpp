@@ -79,6 +79,28 @@ struct FilterChain {   // parse.go:126-149
     bool empty() const { return filters.empty(); }
 };
 
+// The receive loop's filter chain from -filterid, -filtertype and -unique ("" and false: the flag is not given), in the
+// order flag.Visit builds it (main.go:97-113: filterid, filtertype, unique -- lexicographic, whatever the command line's
+// order).  *ids, when asked for, is the MeterIDFilter's set, which -single empties (main.go:278), or nullptr without one.
+inline FilterChain NewFilterChain(const std::string& filterid, const std::string& filtertype, bool unique,
+                                  UintMap** ids = nullptr) {
+    FilterChain fc;
+    if (ids) *ids = nullptr;
+    if (!filterid.empty()) {
+        auto f = std::make_shared<MeterIDFilter>();
+        f->ids.Set(filterid);
+        fc.Add(f);
+        if (ids) *ids = &f->ids;
+    }
+    if (!filtertype.empty()) {
+        auto f = std::make_shared<MeterTypeFilter>();
+        f->types.Set(filtertype);
+        fc.Add(f);
+    }
+    if (unique) fc.Add(std::make_shared<UniqueFilter>());
+    return fc;
+}
+
 // parse.go:103-125.  Time is kept as (seconds, nanoseconds) UTC; the reference formats local time with the same layouts.
 struct LogMessage {
     int64_t unix_seconds = 0;
@@ -317,6 +339,20 @@ inline std::string XmlLine(const LogMessage& m) {
         s += "></Signal>";
     }
     return s + "</LogMessage>\n";
+}
+
+// -format (flags.go:140-170), with erthost_encode's values; a fixed underlying type, so that any other int the C surface
+// is given converts to a value that is none of the four and is encoded as plain.
+enum Format : int { PLAIN = 0, CSV = 1, JSON = 2, XML = 3 };
+
+// The csv, json or xml line of a message.  The plain line is not here: each caller has its own (PlainLine, BlockLine).
+inline std::string Line(Format f, const LogMessage& m) {
+    switch (f) {
+    case CSV: return CsvLine(m.Record());
+    case JSON: return JsonLine(m);
+    case XML: return XmlLine(m);
+    default: throw std::logic_error("Line: the plain line is the caller's");
+    }
 }
 
 }  // namespace receiver

@@ -5,7 +5,6 @@
 #include <cstdio>
 #include <cstring>
 #include <memory>
-#include <sstream>
 
 #include "../../include/ertgpu_level.h"
 #include "protocol.hpp"
@@ -53,14 +52,8 @@ erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long
                      char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;   // released only on success: a throwing NewParser / Allocate must not leak the handle
     try {
-        protocol::RegisterStockParsers();
         h.reset(new erthost());
-        std::stringstream ss(msgtypes_csv);
-        std::string name;
-        while (std::getline(ss, name, ',')) {
-            if (name.empty()) continue;
-            h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
-        }
+        protocol::RegisterProtocols(h->d, msgtypes_csv, chip_length);
         h->d.SetInput({input_rate, format, scale, capture_freq, center_freq, auto_scale != 0, channel_gain < 0 ? -1 : channel_gain,
                        channel_gain == -2, signal != 0, spectrum_log2, spectrum_frames});
         h->d.Allocate(device, max_blocks, max_cands);
@@ -75,14 +68,8 @@ erthost* erthost_new(const char* msgtypes_csv, int chip_length, int device, long
 erthost* erthost_new_parse_only(const char* msgtypes_csv, int chip_length, char* errbuf, int errcap) {
     std::unique_ptr<erthost> h;
     try {
-        protocol::RegisterStockParsers();
         h.reset(new erthost());
-        std::stringstream ss(msgtypes_csv);
-        std::string name;
-        while (std::getline(ss, name, ',')) {
-            if (name.empty()) continue;
-            h->d.RegisterProtocol(protocol::NewParser(name, chip_length));
-        }
+        protocol::RegisterProtocols(h->d, msgtypes_csv, chip_length);
         return h.release();
     } catch (const std::exception& e) {
         if (errbuf && errcap > 0) snprintf(errbuf, (size_t)errcap, "%s", e.what());
@@ -118,50 +105,24 @@ int erthost_reset(erthost* h) {
 
 // rcvr.d.Decode(block) for N blocks (main.go:235); returns the number of messages (all are counted,
 // the first `cap` are written), or -1 on error / -2 when len is not a multiple of BlockSize2.
-static long long fill_msgs(const std::vector<protocol::MessagePtr>& msgs, erthost_msg* out, long long cap);
+static long long fill_msgs(const std::vector<const protocol::Message*>& msgs, erthost_msg* out, long long cap);
+static std::vector<const protocol::Message*> pointers(const std::vector<protocol::MessagePtr>& msgs);
 
 // The parsers alone (decode.go:177-187 + each Parse): candidates sorted by (block, preamble, idx) in, messages out.
 long long erthost_parse(erthost* h, const ertgpu_candidate* cands, long long n, erthost_msg* out, long long cap) {
     try {
         std::vector<protocol::MessagePtr> msgs;
         h->d.Dispatch(cands, (size_t)n, msgs);
-        return fill_msgs(msgs, out, cap);
+        return fill_msgs(pointers(msgs), out, cap);
     } catch (const std::exception& e) {
         h->err = e.what();
         return -1;
     }
 }
 
-// erthost_parse followed by the receive loop's cross-block dedup (main.go:244-260,292) with a fresh memory:
-// the messages rtlamr would print for this candidate list with -blockdedup=`unique`.
-long long erthost_parse_dedup(erthost* h, const ertgpu_candidate* cands, long long n, int block_dedup, erthost_msg* out,
-                              long long cap, long long* duplicates) {
-    try {
-        std::vector<protocol::MessagePtr> msgs, kept;
-        h->d.Dispatch(cands, (size_t)n, msgs);
-        receiver::BlockDedup dd;
-        receiver::Stats st;
-        std::vector<const protocol::Message*> order;
-        dd.Filter(msgs, block_dedup != 0, [&](const protocol::Message& m) { order.push_back(&m); }, st);
-        if (duplicates) *duplicates = st.duplicates;
-        // re-own in emit order (msgs keeps the objects alive until we return)
-        std::vector<protocol::MessagePtr> view;
-        for (const protocol::Message* m : order)
-            for (auto& p : msgs)
-                if (p.get() == m) {
-                    view.push_back(std::move(p));
-                    break;
-                }
-        return fill_msgs(view, out, cap);
-    } catch (const std::exception& e) {
-        h->err = e.what();
-        return -1;
-    }
-}
-
-// erthost_parse_dedup over the candidate lists of nch channels of one capture (counts[c] candidates of channel c, one
-// list after the other in cands): each list is parsed, and the messages go through the cross-channel dedup in the order
-// the receiver prints them (ascending block, then channel).  channel_out[i]: the channel of out[i].
+// erthost_parse_filtered without filters over the candidate lists of nch channels of one capture (counts[c] candidates
+// of channel c, one list after the other in cands): each list is parsed, and the messages go through the cross-channel
+// dedup in the order the receiver prints them (ascending block, then channel).  channel_out[i]: the channel of out[i].
 long long erthost_parse_dedup_channels(erthost* h, const ertgpu_candidate* cands, const long long* counts, int nch,
                                        int block_dedup, erthost_msg* out, int* channel_out, long long cap, long long* duplicates) {
     try {
@@ -174,19 +135,18 @@ long long erthost_parse_dedup_channels(erthost* h, const ertgpu_candidate* cands
         receiver::Stats st;
         std::vector<size_t> pos((size_t)nch, 0), cnt;
         std::vector<protocol::MessagePtr*> at;
-        std::vector<protocol::MessagePtr> view;
+        std::vector<const protocol::Message*> order;
         std::vector<int> chan;
         int64_t b = 0;
         while (receiver::NextBlock(per, pos, at, cnt, &b))
             dd.FilterChannels(at.data(), cnt.data(), (size_t)nch, block_dedup != 0, [&](const protocol::Message& m, size_t c) {
-                for (size_t i = 0; i < cnt[c]; i++)
-                    if (at[c][i].get() == &m) view.push_back(std::move(at[c][i]));
+                order.push_back(&m);
                 chan.push_back((int)c);
                 return true;
             }, st);
         if (duplicates) *duplicates = st.duplicates;
         for (size_t i = 0; i < chan.size() && (long long)i < cap; i++) channel_out[i] = chan[i];
-        return fill_msgs(view, out, cap);
+        return fill_msgs(order, out, cap);
     } catch (const std::exception& e) {
         h->err = e.what();
         return -1;
@@ -196,38 +156,21 @@ long long erthost_parse_dedup_channels(erthost* h, const ertgpu_candidate* cands
 // erthost_parse, then the receive loop of main.go:236-260 on the result with a fresh memory: the filter chain in the order
 // flag.Visit builds it (main.go:97-113: filterid, filtertype, unique -- lexicographic, whatever the command line's order),
 // then the cross-block digest dedup.  filterid / filtertype: comma lists as for the flags, NULL or "" = flag not given.
+// Without filters: the messages rtlamr would print for this candidate list with -blockdedup=`block_dedup`.
 long long erthost_parse_filtered(erthost* h, const ertgpu_candidate* cands, long long n, const char* filterid, const char* filtertype,
                                  int unique, int block_dedup, erthost_msg* out, long long cap, long long* duplicates,
                                  long long* filtered) {
     try {
         std::vector<protocol::MessagePtr> msgs;
         h->d.Dispatch(cands, (size_t)n, msgs);
-        receiver::FilterChain fc;
-        if (filterid && *filterid) {
-            auto f = std::make_shared<receiver::MeterIDFilter>();
-            f->ids.Set(filterid);
-            fc.Add(f);
-        }
-        if (filtertype && *filtertype) {
-            auto f = std::make_shared<receiver::MeterTypeFilter>();
-            f->types.Set(filtertype);
-            fc.Add(f);
-        }
-        if (unique) fc.Add(std::make_shared<receiver::UniqueFilter>());
+        receiver::FilterChain fc = receiver::NewFilterChain(filterid ? filterid : "", filtertype ? filtertype : "", unique != 0);
         receiver::BlockDedup dd;
         receiver::Stats st;
         std::vector<const protocol::Message*> order;
         dd.Filter(msgs, block_dedup != 0, [&](const protocol::Message& m) { order.push_back(&m); }, st, fc.empty() ? nullptr : &fc);
         if (duplicates) *duplicates = st.duplicates;
         if (filtered) *filtered = st.filtered;
-        std::vector<protocol::MessagePtr> view;
-        for (const protocol::Message* m : order)
-            for (auto& p : msgs)
-                if (p.get() == m) {
-                    view.push_back(std::move(p));
-                    break;
-                }
-        return fill_msgs(view, out, cap);
+        return fill_msgs(order, out, cap);
     } catch (const std::exception& e) {
         h->err = e.what();
         return -1;
@@ -243,6 +186,8 @@ long long erthost_encode(erthost* h, const ertgpu_candidate* cands, long long n,
     try {
         std::vector<protocol::MessagePtr> msgs;
         h->d.Dispatch(cands, (size_t)n, msgs);
+        const receiver::Format f = (receiver::Format)format;
+        const bool plain = f != receiver::CSV && f != receiver::JSON && f != receiver::XML;
         std::string all;
         for (auto& m : msgs) {
             receiver::LogMessage lm;
@@ -251,12 +196,7 @@ long long erthost_encode(erthost* h, const ertgpu_candidate* cands, long long n,
             lm.Offset = offset;
             lm.Length = length;
             lm.Message = m.get();
-            switch (format) {
-            case 1: all += receiver::CsvLine(lm.Record()); break;
-            case 2: all += receiver::JsonLine(lm); break;
-            case 3: all += receiver::XmlLine(lm); break;
-            default: all += receiver::PlainLine(lm, sample_file_is_devnull != 0) + "\n";
-            }
+            all += plain ? receiver::PlainLine(lm, sample_file_is_devnull != 0) + "\n" : receiver::Line(f, lm);
         }
         if ((long long)all.size() < cap && buf) memcpy(buf, all.c_str(), all.size() + 1);
         return (long long)all.size();
@@ -275,18 +215,15 @@ long long erthost_encode_signal(erthost* h, const ertgpu_candidate* cands, const
         std::vector<protocol::MessagePtr> msgs;
         h->d.SetSignalChannel(channel_hz, rate_out);
         h->d.Dispatch(cands, (size_t)n, msgs, sigs);
+        const receiver::Format f = (receiver::Format)format;
+        const bool plain = f != receiver::CSV && f != receiver::JSON && f != receiver::XML;
         std::string all;
         for (auto& m : msgs) {
             receiver::LogMessage lm;
             lm.unix_seconds = unix_seconds;
             lm.nanos = nanos;
             lm.Message = m.get();
-            switch (format) {
-            case 1: all += receiver::CsvLine(lm.Record()); break;
-            case 2: all += receiver::JsonLine(lm); break;
-            case 3: all += receiver::XmlLine(lm); break;
-            default: all += receiver::BlockLine(*m) + "\n";
-            }
+            all += plain ? receiver::BlockLine(*m) + "\n" : receiver::Line(f, lm);
         }
         if ((long long)all.size() < cap && buf) memcpy(buf, all.c_str(), all.size() + 1);
         return (long long)all.size();
@@ -298,19 +235,13 @@ long long erthost_encode_signal(erthost* h, const ertgpu_candidate* cands, const
 
 long long erthost_decode(erthost* h, const uint8_t* iq, size_t len, erthost_msg* out, long long cap) {
     try {
-        if (h->d.AutoScale() && !h->started && len % h->d.InputQuantum() == 0) {
-            const size_t s = (size_t)h->d.BytesPerSample();
-            h->level = h->d.Measure(iq, std::min(len / s, (size_t)ERTLV_WINDOW) * s);
-            h->measured = true;
-            h->d.SetScale(h->level.scale);
-        }
-        if (h->d.AutoChannelGain() && !h->started && len % h->d.InputQuantum() == 0) {
-            const size_t s = (size_t)h->d.BytesPerSample();
-            h->d.SetChannelGain(h->d.MeasureChannel(iq, std::min(len / s, (size_t)ERTLV_WINDOW) * s).k);
-        }
+        if (!h->started && len % h->d.InputQuantum() == 0)
+            receiver::StartStream({&h->d}, iq, len, [h](const ertgpu_input_level& lv) {
+                h->level = lv;
+                h->measured = true;
+            }, {});
         h->started = true;
-        auto msgs = h->d.Decode(iq, len);
-        return fill_msgs(msgs, out, cap);
+        return fill_msgs(pointers(h->d.Decode(iq, len)), out, cap);
     } catch (const std::length_error& e) {
         h->err = e.what();
         return -2;
@@ -320,10 +251,16 @@ long long erthost_decode(erthost* h, const uint8_t* iq, size_t len, erthost_msg*
     }
 }
 
-static long long fill_msgs(const std::vector<protocol::MessagePtr>& msgs, erthost_msg* out, long long cap) {
+static std::vector<const protocol::Message*> pointers(const std::vector<protocol::MessagePtr>& msgs) {
+    std::vector<const protocol::Message*> v;
+    for (const auto& m : msgs) v.push_back(m.get());
+    return v;
+}
+
+static long long fill_msgs(const std::vector<const protocol::Message*>& msgs, erthost_msg* out, long long cap) {
     {
         long long n = 0;
-        for (auto& m : msgs) {
+        for (const protocol::Message* m : msgs) {
             if (n < cap) {
                 erthost_msg& o = out[n];
                 memset(&o, 0, sizeof(o));

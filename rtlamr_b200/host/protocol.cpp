@@ -7,7 +7,9 @@
 #include <cstring>
 #include <mutex>
 #include <set>
+#include <sstream>
 
+#include "../../include/ertgpu_format.h"
 #include "../../include/ertgpu_resample.h"
 #include "../../include/ertgpu_signal.h"
 
@@ -533,6 +535,14 @@ void RegisterStockParsers() {
     });
 }
 
+void RegisterProtocols(Decoder& d, const std::string& msgtypes, int chipLength) {
+    RegisterStockParsers();
+    std::stringstream ss(msgtypes);
+    std::string name;
+    while (std::getline(ss, name, ','))
+        if (!name.empty()) d.RegisterProtocol(NewParser(name, chipLength));
+}
+
 // ----------------------------------------------------------------------- Decoder
 namespace {
 [[noreturn]] void raise(ertgpu_handle* h, int rc, const char* what) {
@@ -609,9 +619,7 @@ void Decoder::EnableSignal() {
 
 void Decoder::EnableSpectrum(int32_t log2_n, int64_t frames_per_row) {
     if (allocated_) throw std::logic_error("EnableSpectrum after Allocate");
-    const int rc = ertgpu_enable_spectrum(h_, log2_n, frames_per_row);
-    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
-    if (rc != ERTGPU_OK) raise(h_, rc, "EnableSpectrum");
+    Check(ertgpu_enable_spectrum(h_, log2_n, frames_per_row), "EnableSpectrum");
     spectrum_n_ = 1 << log2_n;
 }
 
@@ -648,24 +656,20 @@ void Decoder::Reset() {
 
 void Decoder::SetInput(const Input& in) {
     if (allocated_) throw std::logic_error("SetInput after Allocate");
-    const auto check = [this](int rc) {
-        if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
-        if (rc != ERTGPU_OK) raise(h_, rc, "SetInput");
-    };
     if (in.CaptureFreq > 0 || in.CenterFreq != 0) {
-        check(ertgpu_set_input_tuning(h_, in.CaptureFreq, in.CenterFreq));
-        check(ertgpu_allow_input_decimation(h_));  // up to 256:1; nothing changes up to 10:1
+        Check(ertgpu_set_input_tuning(h_, in.CaptureFreq, in.CenterFreq), "SetInput");
+        Check(ertgpu_allow_input_decimation(h_), "SetInput");  // up to 256:1; nothing changes up to 10:1
     }
-    if (in.SampleRate > 0) check(ertgpu_set_input_rate(h_, in.SampleRate));
+    if (in.SampleRate > 0) Check(ertgpu_set_input_rate(h_, in.SampleRate), "SetInput");
     if (in.AutoScale && in.Format == ERTGPU_FORMAT_CU8) throw std::invalid_argument("automatic gain does not apply to uint8 (cu8) input");
     if (in.Format != ERTGPU_FORMAT_CU8 || in.Scale != 0.0f) {
-        check(ertgpu_set_input_format(h_, in.Format, in.Scale));
-        sample_bytes_ = FormatBytes(in.Format);
+        Check(ertgpu_set_input_format(h_, in.Format, in.Scale), "SetInput");
+        sample_bytes_ = ertfmt_bytes(in.Format);
     }
     auto_scale_ = in.AutoScale;
     if (in.ChannelGain >= 0 || in.AutoChannelGain) {
         if (in.CaptureFreq <= 0) throw std::invalid_argument("the channel gain needs a tuned input: a capture frequency");
-        check(ertgpu_set_channel_gain(h_, in.AutoChannelGain ? 0 : in.ChannelGain));
+        Check(ertgpu_set_channel_gain(h_, in.AutoChannelGain ? 0 : in.ChannelGain), "SetInput");
     }
     auto_channel_gain_ = in.AutoChannelGain;
     if (in.Signal) EnableSignal();
@@ -681,9 +685,7 @@ ertgpu_channel_level Decoder::MeasureChannel(const uint8_t* samples, size_t len)
 }
 
 void Decoder::SetChannelGain(int32_t k) {
-    const int rc = ertgpu_set_channel_gain(h_, k);
-    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
-    if (rc != ERTGPU_OK) raise(h_, rc, "SetChannelGain");
+    Check(ertgpu_set_channel_gain(h_, k), "SetChannelGain");
 }
 
 ertgpu_input_level Decoder::Measure(const uint8_t* samples, size_t len) {
@@ -695,14 +697,36 @@ ertgpu_input_level Decoder::Measure(const uint8_t* samples, size_t len) {
 }
 
 void Decoder::SetScale(float scale) {
-    const int rc = ertgpu_set_input_scale(h_, scale);
-    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
-    if (rc != ERTGPU_OK) raise(h_, rc, "SetScale");
+    Check(ertgpu_set_input_scale(h_, scale), "SetScale");
 }
 
 int64_t Decoder::BlocksDecoded() const {
     if (!allocated_ || Cfg.BlockSize <= 0) return 0;
     return (resampling_ ? ertrs_out_end(&rs_, input_samples_) : input_samples_) / Cfg.BlockSize;
+}
+
+void Decoder::Check(int rc, const char* what) const {
+    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(h_));
+    if (rc != ERTGPU_OK) raise(h_, rc, what);
+}
+
+// The messages of the call just made on the handle: `deliver` fetches its candidates into a buffer of the size it is
+// given, which grows once to what the call found; then the input is counted and the messages dispatched with their
+// signal records.
+template <typename Deliver>
+std::vector<MessagePtr> Decoder::Collect(size_t len, const char* what, Deliver deliver) {
+    size_t n = 0;
+    if (cands_.size() < 1024) cands_.resize(1024);
+    int rc = deliver(cands_.data(), cands_.size(), &n);
+    if (rc == ERTGPU_ECAPACITY && n > cands_.size() && std::string(ertgpu_last_error(h_)).find("internal") == std::string::npos) {
+        cands_.resize(n);
+        rc = ertgpu_fetch(h_, cands_.data(), cands_.size(), &n);
+    }
+    if (rc != ERTGPU_OK) raise(h_, rc, what);
+    input_samples_ += (int64_t)(len / sample_bytes_);
+    std::vector<MessagePtr> out;
+    Dispatch(cands_.data(), n, out, FetchSignal(n));
+    return out;
 }
 
 std::vector<std::vector<MessagePtr>> Decoder::DecodeChannels(const std::vector<Decoder*>& ds, const uint8_t* input, size_t len) {
@@ -713,23 +737,10 @@ std::vector<std::vector<MessagePtr>> Decoder::DecodeChannels(const std::vector<D
     if (len % d0.InputQuantum()) throw std::length_error("input is not a whole number of IQ samples");
     std::vector<ertgpu_handle*> hs;
     for (const Decoder* d : ds) hs.push_back(d->h_);
-    int rc = ertgpu_decode_channels(hs.data(), (int32_t)hs.size(), input, len, ERTGPU_DECODE_ONLY_VALID);
-    if (rc == ERTGPU_EINVAL) throw std::invalid_argument(ertgpu_last_error(d0.h_));
-    if (rc != ERTGPU_OK) raise(d0.h_, rc, "DecodeChannels");
-    std::vector<std::vector<MessagePtr>> out(ds.size());
-    for (size_t c = 0; c < ds.size(); c++) {
-        Decoder& d = *ds[c];
-        size_t n = 0;
-        if (d.cands_.size() < 1024) d.cands_.resize(1024);
-        rc = ertgpu_fetch(d.h_, d.cands_.data(), d.cands_.size(), &n);
-        if (rc == ERTGPU_ECAPACITY && n > d.cands_.size() && std::string(ertgpu_last_error(d.h_)).find("internal") == std::string::npos) {
-            d.cands_.resize(n);
-            rc = ertgpu_fetch(d.h_, d.cands_.data(), d.cands_.size(), &n);
-        }
-        if (rc != ERTGPU_OK) raise(d.h_, rc, "DecodeChannels");
-        d.input_samples_ += (int64_t)(len / d.sample_bytes_);
-        d.Dispatch(d.cands_.data(), n, out[c], d.FetchSignal(n));
-    }
+    d0.Check(ertgpu_decode_channels(hs.data(), (int32_t)hs.size(), input, len, ERTGPU_DECODE_ONLY_VALID), "DecodeChannels");
+    std::vector<std::vector<MessagePtr>> out;
+    for (Decoder* d : ds)
+        out.push_back(d->Collect(len, "DecodeChannels", [d](ertgpu_candidate* c, size_t cap, size_t* n) { return ertgpu_fetch(d->h_, c, cap, n); }));
     return out;
 }
 
@@ -739,19 +750,9 @@ std::vector<MessagePtr> Decoder::Decode(const uint8_t* input, size_t len) {
         throw std::length_error(resampling_ ? "input is not a whole number of IQ samples"
                                             : sample_bytes_ == 2 ? "input is not a whole number of BlockSize2-byte blocks"
                                                                  : "input is not a whole number of blocks");
-    size_t n = 0;
-    if (cands_.size() < 1024) cands_.resize(1024);
-    int rc = ertgpu_decode(h_, input, len, ERTGPU_DECODE_ONLY_VALID, cands_.data(), cands_.size(), &n);
-    if (rc == ERTGPU_ECAPACITY && n > cands_.size() && std::string(ertgpu_last_error(h_)).find("internal") == std::string::npos) {
-        cands_.resize(n);
-        rc = ertgpu_fetch(h_, cands_.data(), cands_.size(), &n);
-    }
-    if (rc != ERTGPU_OK) raise(h_, rc, "Decode");
-    input_samples_ += (int64_t)(len / sample_bytes_);
-
-    std::vector<MessagePtr> out;
-    Dispatch(cands_.data(), n, out, FetchSignal(n));
-    return out;
+    return Collect(len, "Decode", [&](ertgpu_candidate* c, size_t cap, size_t* n) {
+        return ertgpu_decode(h_, input, len, ERTGPU_DECODE_ONLY_VALID, c, cap, n);
+    });
 }
 
 // Rebuild the reference's per-block, per-preamble []Data lists (decode.go:177-187) and hand each to

@@ -138,16 +138,6 @@ ParserPtr NewParser(const std::string& name, int chipLength);    // parse.go:42-
 
 // The IQ fed to Decode (not part of the reference, which decodes uint8 IQ at DataRate*ChipLength only).  Every field's
 // default leaves the input as the reference takes it.
-// Bytes per IQ sample of an ERTGPU_FORMAT_*.
-inline int FormatBytes(int32_t f) {
-    switch (f) {
-        case ERTGPU_FORMAT_CU8: case ERTGPU_FORMAT_CS8: return 2;
-        case ERTGPU_FORMAT_CS16: case ERTGPU_FORMAT_CS16BE: case ERTGPU_FORMAT_CU16: case ERTGPU_FORMAT_CU16BE: return 4;
-        case ERTGPU_FORMAT_CF64: case ERTGPU_FORMAT_CF64BE: return 16;
-        default: return 8;
-    }
-}
-
 struct Input {
     int64_t SampleRate = 0;             // Hz; another rate than DataRate*ChipLength is resampled (ertgpu_set_input_rate)
     int32_t Format = ERTGPU_FORMAT_CU8; // converted on the GPU with gain Scale, 0: the format's default (ertgpu_set_input_format)
@@ -250,6 +240,11 @@ private:
     int32_t spectrum_n_ = 0;
     int64_t signal_channel_ = 0, signal_rate_ = 0;
     const ertgpu_signal* FetchSignal(size_t n);   // the last call's records (nullptr without reports)
+    // An rc of libertgpu: ERTGPU_EINVAL throws std::invalid_argument with the handle's message, any other failure
+    // std::runtime_error naming `what`.
+    void Check(int rc, const char* what) const;
+    template <typename Deliver>
+    std::vector<MessagePtr> Collect(size_t len, const char* what, Deliver deliver);
     bool allocated_ = false;
     bool resampling_ = false;
     ertgpu_resampler_info rs_{};
@@ -260,5 +255,8 @@ private:
 };
 
 void RegisterStockParsers();  // the effect of the reference's blank imports (main.go:37-44)
+// main.go:77-82: NewParser + RegisterProtocol for each name of a comma list of message types (empty names skipped),
+// after RegisterStockParsers.
+void RegisterProtocols(Decoder& d, const std::string& msgtypes, int chipLength);
 
 }  // namespace protocol

@@ -9,7 +9,6 @@
 #include <chrono>
 #include <cstdint>
 #include <cstring>
-#include <sstream>
 #include <stdexcept>
 
 #include "../../include/ertgpu_level.h"
@@ -20,17 +19,12 @@ Digest NewDigest(const protocol::Message& m) { return Digest(m.MsgType(), m.Mete
 
 Receiver::Receiver(const std::string& msgtypes, int chipLength, int device, int64_t blocksPerCall,
                    const protocol::Input& input, const std::vector<int64_t>& channels) {
-    protocol::RegisterStockParsers();
     if (blocksPerCall <= 0) blocksPerCall = 4096;
     blocks_per_call_ = blocksPerCall;
     for (size_t c = 0; c < std::max<size_t>(1, channels.size()); c++) {
         d_.push_back(std::make_unique<protocol::Decoder>());
         protocol::Decoder& d = *d_.back();
-        std::string list = msgtypes == "all" ? "scm,scm+,idm,r900" : msgtypes;  // main.go:67-73
-        std::stringstream ss(list);
-        std::string name;
-        while (std::getline(ss, name, ','))
-            if (!name.empty()) d.RegisterProtocol(protocol::NewParser(name, chipLength));  // main.go:77-82
+        protocol::RegisterProtocols(d, msgtypes == "all" ? "scm,scm+,idm,r900" : msgtypes, chipLength);  // main.go:67-82
         protocol::Input in = input;
         if (!channels.empty()) in.CenterFreq = channels[c];
         if (c > 0) in.SpectrumLog2 = 0;   // one spectrum of the capture, on channel 0
@@ -56,25 +50,17 @@ Receiver::~Receiver() {
     for (int k = 0; k < 2; k++) ertgpu_host_free(buf_[k]);
 }
 
-void Receiver::Filter(std::vector<protocol::MessagePtr>& msgs, bool block_dedup,
-                      const std::function<void(const protocol::Message&)>& emit, Stats& st) {
-    dedup_.Filter(msgs, block_dedup, emit, st, fc_.empty() ? nullptr : &fc_);
-}
-
 void BlockDedup::Filter(std::vector<protocol::MessagePtr>& msgs, bool block_dedup,
                         const std::function<void(const protocol::Message&)>& emit, Stats& st, FilterChain* fc) {
     size_t i = 0;
     while (i < msgs.size()) {
         size_t j = i;
         while (j < msgs.size() && msgs[j]->Block == msgs[i]->Block) j++;
-        FilterBlock(msgs.data() + i, j - i, block_dedup, [&](const protocol::Message& m) { emit(m); return true; }, st, fc);
+        protocol::MessagePtr* block = msgs.data() + i;
+        const size_t n = j - i;
+        FilterChannels(&block, &n, 1, block_dedup, [&](const protocol::Message& m, size_t) { emit(m); return true; }, st, fc);
         i = j;
     }
-}
-
-bool BlockDedup::FilterBlock(protocol::MessagePtr* msgs, size_t n, bool block_dedup,
-                             const std::function<bool(const protocol::Message&)>& emit, Stats& st, FilterChain* fc) {
-    return FilterChannels(&msgs, &n, 1, block_dedup, [&](const protocol::Message& m, size_t) { return emit(m); }, st, fc);
 }
 
 bool BlockDedup::FilterChannels(protocol::MessagePtr* const* msgs, const size_t* n, size_t nch, bool block_dedup,
@@ -130,6 +116,24 @@ bool NextBlock(std::vector<std::vector<protocol::MessagePtr>>& per, std::vector<
     }
     *block = b;
     return true;
+}
+
+void StartStream(const std::vector<protocol::Decoder*>& ds, const uint8_t* window, size_t len,
+                 const std::function<void(const ertgpu_input_level&)>& level,
+                 const std::function<void(size_t, const ertgpu_channel_level&)>& channel) {
+    protocol::Decoder& d0 = *ds[0];
+    const size_t s = (size_t)d0.BytesPerSample(), n = std::min(len / s, (size_t)ERTLV_WINDOW) * s;
+    if (d0.AutoScale()) {   // every channel would pick the gain of the same samples: measured once, set on each
+        const ertgpu_input_level lv = d0.Measure(window, n);
+        for (protocol::Decoder* d : ds) d->SetScale(lv.scale);
+        if (level) level(lv);
+    }
+    if (d0.AutoChannelGain())
+        for (size_t c = 0; c < ds.size(); c++) {
+            const ertgpu_channel_level lv = ds[c]->MeasureChannel(window, n);
+            ds[c]->SetChannelGain(lv.k);
+            if (channel) channel(c, lv);
+        }
 }
 
 int64_t ParseDuration(const std::string& str) {   // time.ParseDuration
@@ -229,8 +233,6 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
         const protocol::SpectrumRows r = d0.FetchSpectrum(partial);
         if (!r.rows.empty()) rows(r);
     };
-    std::vector<protocol::Decoder*> ds;
-    for (auto& d : d_) ds.push_back(d.get());
     uint64_t left = max_bytes < 0 ? UINT64_MAX : (uint64_t)max_bytes;
     // main.go:225-230: sampleBuf grows by one block per block until it holds more than BufferLength<<1 bytes
     sample_blocks_ = 2 * (int64_t)d0.Cfg.BufferLength / (int64_t)bs2 + 1;
@@ -241,7 +243,8 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
     // and the window does not depend on the size of a Decode call.
     std::vector<uint8_t> window;
     size_t window_pos = 0;
-    // The channel gain (Input::AutoChannelGain) is measured per channel from the same window, after the input gain.
+    std::vector<protocol::Decoder*> ds;
+    for (auto& d : d_) ds.push_back(d.get());
     if (d0.AutoScale() || d0.AutoChannelGain()) {
         window.resize((size_t)std::min<uint64_t>((uint64_t)ERTLV_WINDOW * s, left));
         size_t have = 0;
@@ -251,17 +254,7 @@ Stats Receiver::Run(FILE* in, bool block_dedup, const std::function<void(const p
             have += n;
         }
         window.resize(have);
-        if (d0.AutoScale()) {   // every channel would pick the gain of the same samples: measured once, set on each
-            level_ = d0.Measure(window.data(), have / s * s);
-            for (auto& d : d_) d->SetScale(level_.scale);
-            if (level_report_) level_report_(level_);
-        }
-        if (d0.AutoChannelGain())
-            for (size_t c = 0; c < d_.size(); c++) {
-                const ertgpu_channel_level lv = d_[c]->MeasureChannel(window.data(), have / s * s);
-                d_[c]->SetChannelGain(lv.k);
-                if (channel_report_) channel_report_(c, lv);
-            }
+        StartStream(ds, window.data(), have, level_report_, channel_report_);
     }
     const auto read = [&](uint8_t* dst, size_t n) -> size_t {
         if (window_pos < window.size()) {

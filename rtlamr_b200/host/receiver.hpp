@@ -48,12 +48,9 @@ public:
     // receive loop's filter chain (main.go:236-239): a message it rejects is skipped BEFORE its digest is recorded.
     void Filter(std::vector<protocol::MessagePtr>& msgs, bool block_dedup,
                 const std::function<void(const protocol::Message&)>& emit, Stats& st, FilterChain* fc = nullptr);
-    // The same for the n messages of ONE block.  `emit` returns false to drop the rest of the block (-single's `break`,
-    // main.go:275-277); FilterBlock then returns false too.
-    bool FilterBlock(protocol::MessagePtr* msgs, size_t n, bool block_dedup,
-                     const std::function<bool(const protocol::Message&)>& emit, Stats& st, FilterChain* fc = nullptr);
     // The same for ONE block's messages of nch channels, channel c's n[c] messages at msgs[c], in the order the channels
-    // were given; `emit` also sees the channel.
+    // were given; `emit` also sees the channel, and returns false to drop the rest of the block (-single's `break`,
+    // main.go:275-277); FilterChannels then returns false too.
     bool FilterChannels(protocol::MessagePtr* const* msgs, const size_t* n, size_t nch, bool block_dedup,
                         const std::function<bool(const protocol::Message&, size_t)>& emit, Stats& st, FilterChain* fc = nullptr);
     void Reset() {
@@ -71,6 +68,14 @@ private:
 // move past it.  False when every channel is done.
 bool NextBlock(std::vector<std::vector<protocol::MessagePtr>>& per, std::vector<size_t>& pos,
                std::vector<protocol::MessagePtr*>& at, std::vector<size_t>& n, int64_t* block);
+
+// The start of a stream whose decoders ds (one per channel of a group, on the same input) take Input::AutoScale or
+// Input::AutoChannelGain, from a window of its first len bytes (at most ERTLV_WINDOW whole samples of it are measured):
+// the input gain is measured once, on ds[0], and set on every decoder; then each channel's gain is measured and set.
+// `level` and `channel` (when set) see each measurement.
+void StartStream(const std::vector<protocol::Decoder*>& ds, const uint8_t* window, size_t len,
+                 const std::function<void(const ertgpu_input_level&)>& level,
+                 const std::function<void(size_t, const ertgpu_channel_level&)>& channel);
 
 class Receiver {
 public:
@@ -104,8 +109,6 @@ public:
     void SetDeadline(std::chrono::steady_clock::time_point t) { deadline_ = t; }
     // Input::AutoScale: `report` sees each stream's level and gain once it is measured, before the stream is decoded.
     void SetLevelReport(std::function<void(const ertgpu_input_level&)> report) { level_report_ = std::move(report); }
-    // The level measured at the start of the last stream (Input::AutoScale; all zero otherwise).
-    const ertgpu_input_level& Level() const { return level_; }
     // Input::AutoChannelGain: `report` sees each channel's level and k once they are measured, before the stream is
     // decoded (after the input gain of Input::AutoScale is set).
     void SetChannelLevelReport(std::function<void(size_t, const ertgpu_channel_level&)> report) {
@@ -125,10 +128,6 @@ public:
     // block numbers restart at 0, empty dedup set, empty sampleBuf.
     void Reset();
 
-    // The dedup step on one Decode result (messages grouped by ascending Block), exposed for tests.
-    void Filter(std::vector<protocol::MessagePtr>& msgs, bool block_dedup,
-                const std::function<void(const protocol::Message&)>& emit, Stats& st);
-
 private:
     std::vector<std::unique_ptr<protocol::Decoder>> d_;   // one per channel
     int64_t blocks_per_call_;
@@ -146,7 +145,6 @@ private:
     UintMap* single_ids_ = nullptr;
     std::chrono::steady_clock::time_point deadline_ = std::chrono::steady_clock::time_point::max();
     std::function<void(const ertgpu_input_level&)> level_report_;
-    ertgpu_input_level level_{};
     std::function<void(size_t, const ertgpu_channel_level&)> channel_report_;
 
     void DumpSampleBuf(const uint8_t* call, int64_t call_first, int64_t block);

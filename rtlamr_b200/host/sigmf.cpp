@@ -14,7 +14,7 @@
 #include <utility>
 
 #include "../../include/ertgpu.h"
-#include "protocol.hpp"
+#include "../../include/ertgpu_format.h"
 
 namespace sigmf {
 
@@ -277,38 +277,6 @@ struct SampleReader {
 
 }  // namespace
 
-int32_t FormatOf(const std::string& t) {
-    static const std::pair<const char*, int32_t> names[] = {
-        {"cu8", ERTGPU_FORMAT_CU8},         {"ci8", ERTGPU_FORMAT_CS8},         {"ci16_le", ERTGPU_FORMAT_CS16},
-        {"cf32_le", ERTGPU_FORMAT_CF32},    {"ci16_be", ERTGPU_FORMAT_CS16BE},  {"cf32_be", ERTGPU_FORMAT_CF32BE},
-        {"cu16_le", ERTGPU_FORMAT_CU16},    {"cu16_be", ERTGPU_FORMAT_CU16BE},  {"ci32_le", ERTGPU_FORMAT_CS32},
-        {"ci32_be", ERTGPU_FORMAT_CS32BE},  {"cu32_le", ERTGPU_FORMAT_CU32},    {"cu32_be", ERTGPU_FORMAT_CU32BE},
-        {"cf64_le", ERTGPU_FORMAT_CF64},    {"cf64_be", ERTGPU_FORMAT_CF64BE}};
-    for (const auto& n : names)
-        if (t == n.first) return n.second;
-    return -1;
-}
-
-const char* FormatName(int32_t f) {
-    switch (f) {
-        case ERTGPU_FORMAT_CU8: return "cu8";
-        case ERTGPU_FORMAT_CS8: return "cs8";
-        case ERTGPU_FORMAT_CS16: return "cs16";
-        case ERTGPU_FORMAT_CF32: return "cf32";
-        case ERTGPU_FORMAT_CS16BE: return "ci16_be";
-        case ERTGPU_FORMAT_CF32BE: return "cf32_be";
-        case ERTGPU_FORMAT_CU16: return "cu16_le";
-        case ERTGPU_FORMAT_CU16BE: return "cu16_be";
-        case ERTGPU_FORMAT_CS32: return "ci32_le";
-        case ERTGPU_FORMAT_CS32BE: return "ci32_be";
-        case ERTGPU_FORMAT_CU32: return "cu32_le";
-        case ERTGPU_FORMAT_CU32BE: return "cu32_be";
-        case ERTGPU_FORMAT_CF64: return "cf64_le";
-        case ERTGPU_FORMAT_CF64BE: return "cf64_be";
-        default: return "?";
-    }
-}
-
 int64_t ParseDatetime(const std::string& s) {
     const auto fail = [&s]() { bad("core:datetime \"" + s + "\" is not ISO 8601 YYYY-MM-DDTHH:MM:SS[.fraction](Z|+HH:MM)"); };
     size_t i = 0;
@@ -381,7 +349,7 @@ Recording Parse(const std::string& json, const std::string& data_path) {
     const Value* dt = g->get("core:datatype");
     if (!dt) bad("global core:datatype is missing");
     if (dt->kind != Value::kString) bad("core:datatype is not a string");
-    r.format = FormatOf(dt->str);
+    r.format = ertfmt_from_sigmf(dt->str.c_str());
     if (r.format < 0) {
         if (!dt->str.empty() && dt->str[0] == 'r') bad("core:datatype \"" + dt->str + "\" is real-valued: IQ needs a complex (c...) type");
         bad("core:datatype \"" + dt->str + "\" is not a complex SigMF datatype");
@@ -443,10 +411,10 @@ Recording Read(const std::string& path) {
     if (stat(r.data_path.c_str(), &st) != 0) bad(r.data_path + ": " + strerror(errno));
     int64_t headers = 0;
     for (const Segment& s : r.segments) headers += s.header_bytes;
-    const int64_t S = protocol::FormatBytes(r.format), data = (int64_t)st.st_size - headers;
+    const int64_t S = ertfmt_bytes(r.format), data = (int64_t)st.st_size - headers;
     if (data < 0 || data % S)
         bad("core:header_bytes: the data file's " + std::to_string((long long)st.st_size) + " bytes less " + std::to_string(headers) +
-            " header bytes are not a whole number of " + std::to_string(S) + "-byte " + FormatName(r.format) + " samples");
+            " header bytes are not a whole number of " + std::to_string(S) + "-byte " + ertfmt_name(r.format) + " samples");
     r.samples = data / S;
     if (r.segments.back().sample_start > r.samples)
         bad("core:sample_start " + std::to_string(r.segments.back().sample_start) + " is past the data file's " +
@@ -478,7 +446,7 @@ FILE* OpenSamples(const Recording& r) {
     FILE* f = fopen(r.data_path.c_str(), "rb");
     if (!f) bad(r.data_path + ": " + strerror(errno));
     auto* rd = new SampleReader{f, {}};
-    const int64_t S = protocol::FormatBytes(r.format);
+    const int64_t S = ertfmt_bytes(r.format);
     int64_t h = 0;
     rd->ext.emplace_back(0, 0);
     for (const Segment& s : r.segments) {

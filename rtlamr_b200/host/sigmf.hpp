@@ -38,12 +38,6 @@ Recording Parse(const std::string& json, const std::string& data_path);
 // the fraction may have any number of digits and is truncated to nanoseconds.
 int64_t ParseDatetime(const std::string& s);
 
-// The ERTGPU_FORMAT_* of a complex SigMF datatype name (cu8, ci8, ci16_le, ..., cf64_be), or -1.
-int32_t FormatOf(const std::string& datatype);
-
-// The name of a format: its SigMF datatype, or cu8 / cs8 / cs16 / cf32 for the first four.
-const char* FormatName(int32_t format);
-
 // Whether any segment carries a core:datetime.
 bool Dated(const Recording& r);
 

@@ -226,6 +226,25 @@ def test_one_literal_line_per_format(built):
     assert encode("scm", pkt, "csv", **kw) == ["2023-11-14T22:13:20.5Z,4096,8192,17580293,8,0x1,0x1,111414,0xd005\n"]
 
 
+@pytest.mark.parametrize("fmt", [-1, 4, 1 << 30])
+def test_any_other_format_value_is_the_plain_line(built, fmt):
+    """erthost_encode and erthost_encode_signal take 1, 2 and 3 as csv, json and xml, and every other int as plain."""
+    import ctypes as C
+    from rtlamr_b200 import capi, host, synth
+    rec = records([(synth.encode_scm(17580293, 8, 1, 1, 111414), None)])
+    sig = np.zeros(len(rec), dtype=capi.SIGNAL_DTYPE)
+    p = host.Parsers("scm", 72)
+    try:
+        L, buf = p._L, C.create_string_buffer(1 << 16)
+        n = L.erthost_encode(p._h, rec.ctypes.data, len(rec), fmt, T0, 0, 4096, 8192, 1, buf, len(buf))
+        assert buf.raw[:n].decode() == p.encode(rec, "plain", unix_seconds=T0, offset=4096, length=8192)
+        n = L.erthost_encode_signal(p._h, rec.ctypes.data, sig.ctypes.data, len(rec), 912_600_000, 2_359_296, fmt, T0, 0,
+                                    buf, len(buf))
+        assert buf.raw[:n].decode() == p.encode_signal(rec, sig, 912_600_000, 2_359_296, "plain", unix_seconds=T0)
+    finally:
+        p.close()
+
+
 def test_scmplus_packet_crc_is_keyed_packetcrc_in_json_and_checksum_in_xml(built):
     """scmplus.go:101: `xml:"Checksum,attr",json:"Checksum"` -- reflect.StructTag.Get("json") stops at the comma, so only the
     xml key takes effect."""
