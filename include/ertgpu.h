@@ -53,7 +53,8 @@ extern "C" {
  * candidates every parser would reject) */
 #define ERTGPU_CHECK_NONE 0
 #define ERTGPU_CHECK_CRC16 1 /* Checksum(init, Bytes[from:to]) == residue: scm/scm.go:76, scmplus/scmplus.go:77 */
-#define ERTGPU_CHECK_IDM 2   /* packet CRC Bytes[4:92] and serial CRC Bytes[9:13]+Bytes[88:90]: idm/idm.go:77-87, netidm/netidm.go:88-98 */
+#define ERTGPU_CHECK_IDM 2   /* packet CRC Bytes[4:92] and serial CRC Bytes[9:13]+Bytes[88:90]: idm/idm.go:77-87, netidm/netidm.go:88-98;
+                              * crc_from/crc_to are ignored, crc_init/crc_poly/crc_residue apply to both CRCs */
 #define ERTGPU_CHECK_R900 3  /* base-6 digit pairs <= 31 and RS syndrome == 0: r900/r900.go:199-221 */
 
 /* One registered parser's PacketConfig (protocol/decode.go:27-42) as the parser's
@@ -66,10 +67,10 @@ typedef struct {
     int32_t preamble_symbols;               /* PacketConfig.PreambleSymbols   */
     int32_t packet_symbols;                 /* PacketConfig.PacketSymbols     */
     uint32_t center_freq;                   /* PacketConfig.CenterFreq        */
-    int32_t check_kind;                     /* ERTGPU_CHECK_*                 */
+    int32_t check_kind;                     /* ERTGPU_CHECK_* (any other value: EINVAL) */
     uint16_t crc_init, crc_poly, crc_residue; /* crc.NewCRC arguments, crc/crc.go:16-24 */
     uint16_t reserved;
-    int32_t crc_from, crc_to;               /* byte range for ERTGPU_CHECK_CRC16 */
+    int32_t crc_from, crc_to;               /* byte range for ERTGPU_CHECK_CRC16 (ignored otherwise) */
 } ertgpu_protocol;
 
 /* Decoder.Cfg after Allocate (protocol/decode.go:131-141) */
@@ -397,7 +398,8 @@ int ertgpu_decode_device_async(ertgpu_handle *h, const void *d_iq, size_t nbytes
  * are free: n calls on a group equal one call over the same bytes.  The rules, each broken one ERTGPU_EINVAL with the
  * rule named in ertgpu_last_error(handles[0]):
  *   1 <= n <= ERTGPU_MAX_CHANNELS, and no handle appears twice;
- *   every handle is allocated, on one device, with the same protocols (and so the same chip length);
+ *   every handle is allocated, on one device, with the same protocols, equal field for field even where a screen
+ *   ignores the field (and so the same chip length);
  *   every handle is tuned (ertgpu_set_input_tuning), with the same capture centre, input rate, format and scale;
  *   every handle is at the same stream position (fresh, or reset together, and fed together since);
  *   every handle takes the wide channel path (ertgpu_set_channel_gain), each with its own k, or none does.  Wide

@@ -754,6 +754,8 @@ int begin_decode(ertgpu_handle* h, const void* iq, size_t nbytes, bool device) {
     return ERTGPU_OK;
 }
 
+// Field for field, the fields a screen ignores included (crc_from/crc_to of a CHECK_IDM protocol): a group of
+// channels never mixes structs that merely screen alike.
 bool same_protocol(const ertgpu_protocol& a, const ertgpu_protocol& b) {
     return strncmp(a.name, b.name, sizeof(a.name)) == 0 && strncmp(a.preamble, b.preamble, sizeof(a.preamble)) == 0 &&
            a.data_rate == b.data_rate && a.chip_length == b.chip_length && a.preamble_symbols == b.preamble_symbols &&
@@ -888,6 +890,9 @@ int ertgpu_register_protocol(ertgpu_handle* h, const ertgpu_protocol* p) {
     if (p->chip_length <= 0 || p->preamble_symbols <= 0 || p->packet_symbols <= 0)
         return fail(h, ERTGPU_EINVAL, "non-positive geometry");
     if ((p->packet_symbols + 7) / 8 > ERTGPU_MAX_PACKET_BYTES) return fail(h, ERTGPU_EINVAL, "packet too long");
+    if (p->check_kind != ERTGPU_CHECK_NONE && p->check_kind != ERTGPU_CHECK_CRC16 && p->check_kind != ERTGPU_CHECK_IDM &&
+        p->check_kind != ERTGPU_CHECK_R900)
+        return fail(h, ERTGPU_EINVAL, "unknown check_kind %d", (int)p->check_kind);
     if (p->check_kind == ERTGPU_CHECK_CRC16 &&
         (p->crc_from < 0 || p->crc_to > (p->packet_symbols + 7) / 8 || p->crc_from >= p->crc_to))
         return fail(h, ERTGPU_EINVAL, "bad crc range");
@@ -974,7 +979,10 @@ static int allocate_impl(ertgpu_handle* h, int32_t device, int64_t max_blocks_pe
         dp.table = i;
         tables.resize((size_t)(i + 1) * 256);
         make_crc_table(p.crc_poly, tables.data() + (size_t)i * 256);
-        if (p.check_kind == ERTGPU_CHECK_IDM) dp.crc_from = 4;   // the IDM screen's first CRC starts at byte 4 whatever crc_from says (idm.go:77-87)
+        if (p.check_kind == ERTGPU_CHECK_IDM) {   // the IDM screen's packet CRC is Bytes[4:92] whatever the range fields say (idm.go:77)
+            dp.crc_from = 4;
+            dp.crc_to = 92;
+        }
         if (p.check_kind == ERTGPU_CHECK_R900) {
             d.pre_has_r900[found] = 1;
             h->has_r900 = true;

@@ -170,10 +170,15 @@ def encode_r900(meter_id: int, unkn1: int, nouse: int, backflow: int, consumptio
     digits = []
     for s in symbols:
         digits += [s // 6, s % 6]
+    return r900_chips(digits), symbols
+
+
+def r900_chips(digits) -> list[int]:
+    """The r900 preamble's Manchester chips followed by 4 chips per base-6 digit: any 42 digits, valid or not."""
     chips = manchester_chips([int(c) for c in PREAMBLE["r900"]])
     for d in digits:
-        chips += _R900_CHIPS[d]
-    return chips, symbols
+        chips += _R900_CHIPS[int(d)]
+    return chips
 
 
 # ---------------------------------------------------------------- packet table

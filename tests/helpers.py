@@ -43,14 +43,20 @@ def synth_stream(msgtypes, cl, nsamples, seed=0x5EED0001, spacing=1 << 19, pkt_s
 def screen_expected(proto, data: bytes, digits=None) -> bool:
     """What bit i of check_mask must be for a candidate filed under parser `proto` (a stock name or a capi.Protocol):
     scm/scm.go:76, scmplus/scmplus.go:77, idm/idm.go:77-87, netidm/netidm.go:88-98, r900/r900.go:199-221; a protocol
-    struct's own CRC16 (init, polynomial, residue over bytes [crc_from, crc_to)) or ERTGPU_CHECK_NONE (always set)."""
+    struct's own CRC16 (init, polynomial, residue over bytes [crc_from, crc_to)), its own IDM pair (init, polynomial,
+    residue over Bytes[4:92] and Bytes[9:13] + Bytes[88:90], whatever its range fields say) or ERTGPU_CHECK_NONE
+    (always set)."""
     if not isinstance(proto, str):
         kind = proto.check_kind
         if kind == capi.CHECK_NONE:
             return True
         if kind == capi.CHECK_CRC16:
             return oracle.crc_checksum(proto.crc_init, data[proto.crc_from:proto.crc_to], proto.crc_poly) == proto.crc_residue
-        proto = {capi.CHECK_IDM: "idm", capi.CHECK_R900: "r900"}[kind]
+        if kind == capi.CHECK_IDM:
+            init, poly, res = proto.crc_init, proto.crc_poly, proto.crc_residue
+            return (oracle.crc_checksum(init, data[4:92], poly) == res
+                    and oracle.crc_checksum(init, data[9:13] + data[88:90], poly) == res)
+        proto = {capi.CHECK_R900: "r900"}[kind]
     if proto == "scm":
         return oracle.crc_checksum(0, data[2:12], 0x6F63) == 0
     if proto == "scm+":
