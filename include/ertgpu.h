@@ -39,7 +39,8 @@ extern "C" {
 #define ERTGPU_EINVAL (-1)    /* bad argument / call order                       */
 #define ERTGPU_ECUDA (-2)     /* CUDA runtime error, no device, wrong arch       */
 #define ERTGPU_ENOMEM (-3)    /* host or device allocation failed                */
-#define ERTGPU_ECAPACITY (-4) /* output array too small: *n_out holds the need   */
+#define ERTGPU_ECAPACITY (-4) /* output array (or max_candidates) too small:    *
+                               * *n_out holds the need, see ertgpu_decode       */
 #define ERTGPU_ESIZE (-5)     /* nbytes not a multiple of BlockSize2 / too large */
 
 #define ERTGPU_MAX_PROTOCOLS 8
@@ -199,7 +200,16 @@ int ertgpu_stock_protocol(const char *msgtype, int32_t chip_length, ertgpu_proto
 /* Decoder.Allocate (decode.go:131-160): derive SymbolLength, BlockSize, ...,
  * select the CUDA device, allocate device buffers for up to
  * max_blocks_per_call blocks per decode call and max_candidates candidates.
- * max_blocks_per_call <= 0 or max_candidates <= 0 pick defaults.
+ * max_blocks_per_call <= 0 or max_candidates <= 0 pick defaults (2^18
+ * candidates).
+ *
+ * max_candidates bounds the preamble matches ("hits") of one pipeline step: a
+ * decode call runs in steps of up to max_blocks_per_call decoder blocks, and
+ * every start position of a step whose bits match a registered preamble takes
+ * one slot, whatever the decode flags are (ERTGPU_DECODE_ONLY_VALID drops
+ * candidates after their screens, so it does not lower the need).  A call
+ * with a step of more hits returns ERTGPU_ECAPACITY with "internal" in
+ * ertgpu_last_error (see ertgpu_decode).
  *
  * Before any device call it returns ERTGPU_EINVAL, with a message naming the
  * rule, for a merged configuration (PS, PK, CL, SL, PL, PKL, BS, BUF of
@@ -377,7 +387,17 @@ int ertgpu_abi_version(void);
  * (block, preamble_id, idx) order.  Synchronous; copies are pipelined with
  * the kernels internally.  If more than cap candidates exist the call returns
  * ERTGPU_ECAPACITY with *n_out = the number needed and the stream state
- * already advanced (call ertgpu_fetch with a larger array to get them). */
+ * already advanced (call ertgpu_fetch with a larger array to get them).
+ *
+ * ERTGPU_ECAPACITY has a second meaning: a step of the call found more hits
+ * than the handle's max_candidates (ertgpu_allocate), and ertgpu_last_error
+ * says "internal".  Then *n_out = the most hits of any step of the call: the
+ * smallest max_candidates at which the same call succeeds.  The call's
+ * candidates (and signal reports) are lost: ertgpu_fetch and
+ * ertgpu_fetch_signal return the same code and *n_out until the next decode
+ * call or ertgpu_reset.  The stream still advances exactly as it would have
+ * without the overflow, so the next call decodes as on a handle that never
+ * overflowed; and ertgpu_last_counts counts every hit of the call. */
 int ertgpu_decode(ertgpu_handle *h, const uint8_t *iq, size_t nbytes, uint32_t flags,
                   ertgpu_candidate *out, size_t cap, size_t *n_out);
 
@@ -414,7 +434,9 @@ int ertgpu_decode_channels_device_async(ertgpu_handle *const *handles, int32_t n
                                         uint32_t flags, void *stream);
 
 /* Wait for the decode enqueued last and copy its candidates out (sorted as
- * above).  May be repeated (e.g. after ERTGPU_ECAPACITY). */
+ * above).  May be repeated (e.g. after ERTGPU_ECAPACITY): an array too small
+ * loses nothing.  ERTGPU_ECAPACITY as ertgpu_decode returns it, in both
+ * meanings (*n_out = the candidates, or the hits of the largest step). */
 int ertgpu_fetch(ertgpu_handle *h, ertgpu_candidate *out, size_t cap, size_t *n_out);
 
 /* Per-packet signal reports.  ertgpu_enable_signal, called before ertgpu_allocate (after it: ERTGPU_EINVAL), makes
@@ -449,7 +471,10 @@ int ertgpu_enable_spectrum(ertgpu_handle *h, int32_t log2_n, int64_t frames_per_
 int ertgpu_fetch_spectrum(ertgpu_handle *h, int32_t partial, ertgpu_spectrum_row *rows, float *mean, float *peak,
                           size_t cap, size_t *n_out);
 
-/* Number of candidates of the last decode, and how many passed a screen. */
+/* Number of candidates of the last decode, and how many passed a screen.
+ * n_candidates counts every hit of the call (with flags 0, one candidate
+ * each), also after an overflow of max_candidates; n_valid then counts only
+ * the hits the handle held, and may fall short. */
 int ertgpu_last_counts(ertgpu_handle *h, int64_t *n_candidates, int64_t *n_valid);
 
 /* Kernels launched by the last decode call (for bench.py's gpu_launches). */
@@ -510,7 +535,11 @@ int ertgpu_plan_shards(int64_t total_blocks, int32_t nshards, int32_t block_size
  * dropped, block numbers are made global and the lists are concatenated in (block, preamble,
  * idx) order -- the same list one handle returns for the whole buffer after ertgpu_reset.
  * All handles must be allocated with the same protocols; each is reset first.  There is no
- * collective: shards are independent (every candidate is decided inside one shard + halo). */
+ * collective: shards are independent (every candidate is decided inside one shard + halo).
+ * The call empties every handle's ertgpu_last_error first; a shard's failure leaves its
+ * message on its handle.  When shards overflow their handle's max_candidates (shard and halo
+ * are one ertgpu_decode), it returns ERTGPU_ECAPACITY with *n_out = the largest need of those
+ * shards; when only the output array is too small, *n_out = the candidates. */
 int ertgpu_decode_sharded(ertgpu_handle *const *handles, int32_t nhandles, const uint8_t *iq, size_t nbytes,
                           uint32_t flags, ertgpu_candidate *out, size_t cap, size_t *n_out);
 

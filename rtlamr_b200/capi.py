@@ -507,7 +507,9 @@ def plan_shards(total_blocks: int, nshards: int, block_size: int, packet_length:
 
 
 def decode_sharded(handles, iq, flags: int = 0, cap: int = 1 << 16) -> np.ndarray:
-    """ertgpu_decode_sharded: one host buffer over several handles (one host thread per handle)."""
+    """ertgpu_decode_sharded: one host buffer over several handles (one host thread per handle).  Repeated with a larger
+    array when the output array was too small; an overflow of a handle's max_candidates raises at once (the call empties
+    every handle's message first, so an "internal" message names this call's overflow)."""
     if isinstance(iq, tuple):
         addr, nbytes = iq
     else:
@@ -518,11 +520,11 @@ def decode_sharded(handles, iq, flags: int = 0, cap: int = 1 << 16) -> np.ndarra
         out = np.empty(cap, dtype=CAND_DTYPE)
         n = C.c_size_t(0)
         rc = lib().ertgpu_decode_sharded(hs, len(handles), addr, nbytes, flags, out.ctypes.data, cap, C.byref(n))
-        if rc == ECAPACITY and n.value > cap:
+        msgs = [(lib().ertgpu_last_error(h._h) or b"").decode() for h in handles]
+        if rc == ECAPACITY and n.value > cap and not any("internal" in m for m in msgs):
             cap = n.value
             continue
         if rc != OK:
-            msgs = [(lib().ertgpu_last_error(h._h) or b"").decode() for h in handles]
             raise ErtGpuError(rc, "; ".join(m for m in msgs if m) or "ertgpu_decode_sharded failed")
         return out[:n.value].copy()
 

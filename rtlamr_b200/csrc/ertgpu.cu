@@ -816,6 +816,7 @@ __attribute__((visibility("hidden"))) int sharded_reject_signal(ertgpu_handle* h
     return h->signal ? fail(h, ERTGPU_EINVAL, "decode_sharded: the handle has signal reports (ertgpu_enable_signal), which sharded decodes do not keep")
                      : ERTGPU_OK;
 }
+__attribute__((visibility("hidden"))) void sharded_clear_error(ertgpu_handle* h) { h->err.clear(); }
 
 extern "C" {
 

@@ -394,7 +394,10 @@ extract_words_kernel(const uint32_t* __restrict__ plane, long long p0, const __g
         __syncwarp();
         const bool active = (hw.mask >> (31 - lane)) & 1u;
         const int rank = __popc(hw.mask >> (31 - lane)) - 1;   // set bits above this lane's = index among the word's hits
-        const bool has_dig = r900_digits != nullptr && cfg.pre_has_r900[hw.preamble_id];
+        // Hit slots and word slots come from two counters: a word below word_cap (= the hit capacity) may still hold
+        // hits whose slots are past it, with no digits computed (the call overflowed and delivers nothing).
+        const bool has_dig = r900_digits != nullptr && cfg.pre_has_r900[hw.preamble_id] &&
+                             hw.slot + (unsigned long long)rank < word_cap;
         // ---- screens
         uint32_t mask = 0;
         for (int i = 0; i < cfg.nproto; i++) {

@@ -14,9 +14,11 @@
 
 #include "../../include/ertgpu.h"
 
-// ertgpu.cu: ERTGPU_EINVAL, with the message on h, when h has signal reports or a spectrum (sharded decodes keep neither).  Hidden:
-// not exported from libertgpu.so.
+// ertgpu.cu: ERTGPU_EINVAL, with the message on h, when h has signal reports or a spectrum (sharded decodes keep neither);
+// and h's message emptied, so that after a sharded call it names a failure of that call only.  Both hidden: not exported
+// from libertgpu.so.
 __attribute__((visibility("hidden"))) int sharded_reject_signal(ertgpu_handle* h);
+__attribute__((visibility("hidden"))) void sharded_clear_error(ertgpu_handle* h);
 
 extern "C" {
 
@@ -43,6 +45,7 @@ int ertgpu_decode_sharded(ertgpu_handle* const* handles, int32_t nhandles, const
     if (!handles || nhandles < 1 || (!iq && nbytes)) return ERTGPU_EINVAL;
     for (int32_t r = 0; r < nhandles; r++)
         if (!handles[r]) return ERTGPU_EINVAL;
+    for (int32_t r = 0; r < nhandles; r++) sharded_clear_error(handles[r]);
     for (int32_t r = 0; r < nhandles; r++) {  // shards are cut at decoder blocks of uint8 input: no resampling or converting handles
         ertgpu_resampler_info ri;
         if (ertgpu_get_resampler(handles[r], &ri, nullptr, 0, nullptr) == ERTGPU_OK) return ERTGPU_EINVAL;
@@ -70,6 +73,7 @@ int ertgpu_decode_sharded(ertgpu_handle* const* handles, int32_t nhandles, const
     struct Part {
         std::vector<ertgpu_candidate> cands;
         int rc = ERTGPU_OK;
+        size_t need = 0;  // rc == ERTGPU_ECAPACITY: the max_candidates at which the shard's decode succeeds
     };
     std::vector<Part> parts((size_t)nhandles);
     auto work = [&](int32_t r) {
@@ -87,6 +91,8 @@ int ertgpu_decode_sharded(ertgpu_handle* const* handles, int32_t nhandles, const
             p.cands.resize(n);
             p.rc = ertgpu_fetch(h, p.cands.data(), p.cands.size(), &n);
         }
+        // an array of n candidates holds the call's output: ERTGPU_ECAPACITY now means the handle's max_candidates
+        if (p.rc == ERTGPU_ECAPACITY) p.need = n;
         if (p.rc != ERTGPU_OK) return;
         // drop the halo's candidates, renumber the rest (the handle counted blocks from its first fed block)
         const int64_t halo = s.first_block - s.first_fed_block;
@@ -103,8 +109,18 @@ int ertgpu_decode_sharded(ertgpu_handle* const* handles, int32_t nhandles, const
     for (int32_t r = 1; r < nhandles; r++) th.emplace_back(work, r);
     work(0);
     for (auto& t : th) t.join();
-    for (int32_t r = 0; r < nhandles; r++)
-        if (parts[(size_t)r].rc != ERTGPU_OK) return parts[(size_t)r].rc;  // ertgpu_last_error(handles[r]) has the message
+    // ertgpu_last_error(handles[r]) has the message of shard r's failure.  Any other error before a capacity overflow;
+    // an overflow reports the largest need of the shards that overflowed, the max_candidates at which every shard fits.
+    size_t need = 0;
+    for (int32_t r = 0; r < nhandles; r++) {
+        const Part& p = parts[(size_t)r];
+        if (p.rc != ERTGPU_OK && p.rc != ERTGPU_ECAPACITY) return p.rc;
+        need = std::max(need, p.need);
+    }
+    if (need) {
+        if (n_out) *n_out = need;
+        return ERTGPU_ECAPACITY;
+    }
     size_t total = 0;
     for (auto& p : parts) total += p.cands.size();
     if (n_out) *n_out = total;

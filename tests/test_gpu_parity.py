@@ -367,14 +367,7 @@ def test_edge_cases(built):
         cands, _ = o.decode(np.full(4 * bs2, v, dtype=np.uint8))
         assert len(got) == len(cands)
         assert np.array_equal(h.tap(capi.TAP_QUANTIZED, 3), o.quantized())
-    # tiny candidate capacity -> ERTGPU_ECAPACITY with the need reported
-    h2 = capi.new_decoder("scm", 72, max_candidates=4)
-    iq, _, _ = synth_stream("scm", 72, 1 << 20, spacing=1 << 18)
-    with pytest.raises(capi.ErtGpuError) as e:
-        h2.decode(whole_blocks(iq, bs2))
-    assert e.value.code == capi.ECAPACITY
-    h.close()
-    h2.close()
+    h.close()   # the candidate capacity: tests/test_gpu_capacity.py
 
 
 def test_synth_device_generator_matches_host(built):
